@@ -15,14 +15,16 @@
 // (tdq_tc.cuh tile_product) -- k_i, y1 and the error-sum prefix are BITWISE what tdq_linear_stage writes, (err/tol)^2 per
 // element bitwise what k_norm computes; only the order of the float64 sum over elements differs (tests/test_gpu_linear.py).
 //
-// Layout: G independent tile pipelines ("groups", one warpgroup each) per CTA, one CTA per SM; the weight planes (96 KB) sit
-// in shared memory once per CTA.  A tile is 16 state rows x 128 features; a thread owns 16 elements of it in the accumulator
-// layout of tdq_tc.cuh.  State per thread: k_0..k_3 in registers, y0 in shared memory; once k_0..k_3 are known the remaining
-// rows and the error estimate are running sums that each later k_j is folded into.  Per stage a group does: newest term +
-// split + st.shared, fence.proxy.async, bar.sync (its 128 threads), 96 wgmma + commit; while they run, the prefix of the next
-// row's sum; then wgmma.wait and k_{i+1} = small + big.  The chain of a tile is serial by nature (stage i+1 needs k_i); the
-// groups interleave, one hiding the other's latency.  The last block to finish adds the per-block partials of the squared
-// error norm and runs the controller step (tdq_ctrl_dev.cuh).
+// Layout: one CTA of two warpgroups per SM, persistent; the weight planes (96 KB) sit in shared memory once per CTA.  A tile
+// is 32 state rows x 128 features; warpgroup h owns output features [64 h, 64 h + 64) of it and issues m64n32k16 products
+// (tdq_tc.cuh), so every 2 KB weight operand fetched from shared memory serves 32 rows (DESIGN.md section 3c).  A thread
+// owns 16 elements of the tile in the accumulator layout of tdq_tc.cuh.  State per thread: k_0..k_3 in registers, y0 in
+// shared memory; once k_0..k_3 are known the remaining rows and the error estimate are running sums that each later k_j is
+// folded into.  Per stage: newest term + split + st.shared of the warpgroup's feature half of the B planes,
+// fence.proxy.async, bar.sync (all 256 threads: the product needs both halves), 48 wgmma + commits per warpgroup; while they
+// run, the prefix of the next row's sum; then wgmma.wait and k_{i+1} = small + big.  The chain of a tile is serial by nature
+// (stage i+1 needs k_i).  The last block to finish adds the per-block partials of the squared error norm and runs the
+// controller step (tdq_ctrl_dev.cuh).
 //
 // Stage derivatives, y1 and the error prefix are written to HBM only for attempts that can contain an output time (the
 // lazy interpolant fit needs them, tdq_interp.cu) or when the caller keeps every step (dense output, events).
@@ -36,12 +38,13 @@ namespace {
 
 using namespace tdq_tc;
 
-constexpr int AT_Y0 = TILE_ROWS * LD * 4;      // a tile's y0 (float32) stays in shared memory: read once per stage
+constexpr int AT_ROWS = 32;                    // state rows per tile = MMA N
+constexpr int AT_THREADS = 256;                // two warpgroups, one per half of the output features
+constexpr int AT_STAGE = 3 * y_plane<AT_ROWS>();   // the B planes of a tile (24 KB)
+constexpr int AT_Y0 = AT_ROWS * LD * 4;        // a tile's y0 (float32) stays in shared memory: read once per stage
 constexpr int AT_AUX = 2048;                   // flag, coefficient tables, reduction scratch
-// G: tile pipelines (warpgroups) per CTA
-constexpr int at_smem(int G) { return W_BYTES + G * (Y_STAGE + AT_Y0) + AT_AUX + 128; }
+constexpr int AT_SMEM = W_BYTES + AT_STAGE + AT_Y0 + AT_AUX + 128;
 constexpr int AT_MAX_S = 7;
-constexpr int AT_GROUPS = 2;                  // tile pipelines per CTA: 255 registers per thread (3 or 4 spill heavily)
 
 // explicit shared-space accesses with 32-bit addresses (a pointer derived from the aligned dynamic shared memory base is
 // generic to the compiler: 64-bit address registers and generic ST/LD otherwise)
@@ -67,11 +70,10 @@ __host__ __device__ constexpr int popc_below(unsigned mask, int j) {
 // a non-zero coefficient in that row.  EM: the same for the error weights of slots 0..S-1 (k_S always carries the last one).
 // CTRL: the last block to finish also runs the controller step (tdq_ctrl_dev.cuh: accept / reject, next step size, the next
 // attempt's tables, the device-side loop's condition) -- one launch per attempt instead of two.
-template <int S, unsigned long long RM, unsigned EM, int G, bool CTRL>
-__global__ void __launch_bounds__(G * 128, 1)
+template <int S, unsigned long long RM, unsigned EM, bool CTRL>
+__global__ void __launch_bounds__(AT_THREADS, 1)
 k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const uint32_t *__restrict__ wt,
                  double *partials, double *norm_out, const int64_t *seg_counts, int store_always, size_t n_rows_sz) {
-    constexpr int AT_THREADS = G * 128;
     if (c->halt) {
         // An attempt issued after the end of the solve is a no-op -- but its controller step still has to tick the mailbox:
         // a host that runs ahead (eager run_ahead, graph replay) accounts for every attempt it queued (tdq_ctrl_dev.cuh).
@@ -80,7 +82,7 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
     }
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
-    uint8_t *aux = smem + W_BYTES + G * (Y_STAGE + AT_Y0);
+    uint8_t *aux = smem + W_BYTES + AT_STAGE + AT_Y0;
     int *s_flag = reinterpret_cast<int *>(aux);
     float *s_cr = reinterpret_cast<float *>(aux + 64);                    // [S][8]: coef[i][m] as float32
     float *s_ce = s_cr + AT_MAX_S * 8;                                    // [8]:    ecoef[m]
@@ -120,23 +122,23 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
     constexpr int EK = popc_below(EM, S);                                 // index of k_S's error weight in ecoef
     const float ecS = s_ce[EK];
 
-    // group g = one tile pipeline; w = warp inside the warpgroup
-    const int g = warp >> 2, w = warp & 3;
+    // h = the warpgroup's half of the output features; w = warp inside the warpgroup
+    const int h = warp >> 2, w = warp & 3;
     const uint32_t wsm = smem_u32(smem);
-    const uint32_t stage = wsm + W_BYTES + g * Y_STAGE;
-    const uint32_t sy0 = wsm + W_BYTES + G * Y_STAGE + g * AT_Y0 + (tid & 127) * 4;   // element e at sy0 + 512 e: this thread's only
-    const int toff = thread_offset(w, lane);
+    const uint32_t wsm_h = wsm + h * 8 * SBO;                             // the weight rows of features [64 h, 64 h + 64)
+    const uint32_t stage = wsm + W_BYTES;
+    const uint32_t sy0 = stage + AT_STAGE + tid * 4;                      // element e at sy0 + 1024 e: this thread's only
+    const int toff = thread_offset(w, lane) + 64 * h;
 
-    const int tiles = (n_rows + TILE_ROWS - 1) / TILE_ROWS;
-    const int workers = (int)gridDim.x * G;
+    const int tiles = (n_rows + AT_ROWS - 1) / AT_ROWS;
     double acc = 0.0;
     int nbad = 0;
 
-    // One tile through all S stages.  FULL: all 16 rows exist (no per-row predicates); the one partial tile of a launch
+    // One tile through all S stages.  FULL: all 32 rows exist (no per-row predicates); the one partial tile of a launch
     // takes the predicated copy of the same code.
     //
     // Schedule of stage i (row i needs k_0 .. k_i, the newest one, k_i, has just come out of the accumulators):
-    //   critical path   y_i = y0 + (prefix_i + k_i c_ii)  ->  split  ->  planes  ->  fence, bar.sync, 96 wgmma + commit
+    //   critical path   y_i = y0 + (prefix_i + k_i c_ii)  ->  split  ->  planes  ->  fence, bar.sync, 48 wgmma + commits
     //   MMA window      everything that does not depend on the product in flight: the prefix of the NEXT row's sum
     //                   (sum over j <= i of k_j c_{i+1,j}: ascending j, so the newest term is always added last and the
     //                   value is bitwise the one a single ascending loop produces), the running sums, y1's bookkeeping
@@ -148,7 +150,7 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
     auto row_mask = [](int i) -> unsigned { return (unsigned)((RM >> (8 * i)) & 0xffull); };
     auto do_tile = [&](auto full_tag, const int t) {
         constexpr bool FULL = decltype(full_tag)::value;
-        const int row0 = t * TILE_ROWS;
+        const int row0 = t * AT_ROWS;
         const int rows_here = n_rows - row0;
         const size_t base = (size_t)row0 * LD + toff;
         float K[KEEP][16];
@@ -160,13 +162,13 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
             for (int e = 0; e < 16; ++e) {
                 Y0[e] = 0.f;
                 KN[e] = 0.f;
-                if (FULL || elem_row(e, lane) < rows_here) {
-                    Y0[e] = __ldcs(y0 + base + elem_offset(e));
-                    KN[e] = __ldcs(k0 + base + elem_offset(e));
+                if (FULL || elem_row<AT_ROWS>(e, lane) < rows_here) {
+                    Y0[e] = __ldcs(y0 + base + elem_offset<AT_ROWS>(e));
+                    KN[e] = __ldcs(k0 + base + elem_offset<AT_ROWS>(e));
                 }
             }
 #pragma unroll
-            for (int e = 0; e < 16; ++e) sts_f32(sy0 + e * 512, Y0[e]);   // only this thread reads it back: no barrier
+            for (int e = 0; e < 16; ++e) sts_f32(sy0 + e * 1024, Y0[e]);   // only this thread reads it back: no barrier
         }
 #pragma unroll
         for (int i = 0; i < S; ++i) {
@@ -188,18 +190,18 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
                     if (has_prefix && has_new) sum = pre + KN[e] * c_new;
                     else if (has_prefix) sum = pre;
                     else sum = KN[e] * c_new;
-                    yv[e] = lds_f32(sy0 + e * 512) + sum;
+                    yv[e] = lds_f32(sy0 + e * 1024) + sum;
                     if (last) Y1[e] = yv[e];
                 }
-                // every warp of the group is past its wait for the previous product: the planes may be overwritten
-                asm volatile("bar.sync %0, 128;" :: "r"(g + 1) : "memory");
-                store_planes(stage, yv, w, lane);
+                // every warp of both warpgroups is past its wait for the previous product: the planes may be overwritten
+                __syncthreads();
+                store_planes<AT_ROWS>(stage, yv, h, w, lane);
             }
             // ---- k_{i+1} = y_i W^T ----
             fence_async_smem();
-            asm volatile("bar.sync %0, 128;" :: "r"(g + 1) : "memory");
-            TileAcc tacc;
-            tile_product(wsm, stage, tacc);
+            __syncthreads();                                              // both feature halves of the B planes are stored
+            TileAcc<AT_ROWS> tacc;
+            tile_product(wsm_h, stage, tacc);
             // ---- MMA window ----
             if (i + 1 < KEEP && i + 1 < S) {
                 // prefix of the next row's sum over the slots known so far
@@ -289,16 +291,16 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
 #pragma unroll
                 for (int e = 0; e < 16; ++e) {
                     const float y1v = Y1[e];
-                    if (FULL || elem_row(e, lane) < rows_here) {
+                    if (FULL || elem_row<AT_ROWS>(e, lane) < rows_here) {
                         if (!isfinite(y1v)) nbad += 1;
-                        const size_t o = base + elem_offset(e);
+                        const size_t o = base + elem_offset<AT_ROWS>(e);
                         if (ycand) ycand[o] = y1v;
                         if (store) {
                             out.y1[o] = y1v;
                             out.err[o] = AE[e];
                         }
                     }
-                    Y1[e] = Ar<float>::add(atolT, Ar<float>::mul(rtolT, Ar<float>::max_nan(fabsf(lds_f32(sy0 + e * 512)), fabsf(y1v))));
+                    Y1[e] = Ar<float>::add(atolT, Ar<float>::mul(rtolT, Ar<float>::max_nan(fabsf(lds_f32(sy0 + e * 1024)), fabsf(y1v))));
                 }
                 reg_fence(Y1);
             }
@@ -307,14 +309,14 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
             if (store) {
 #pragma unroll
                 for (int e = 0; e < 16; ++e)
-                    if (FULL || elem_row(e, lane) < rows_here) out.k[i + 1][base + elem_offset(e)] = KN[e];
+                    if (FULL || elem_row<AT_ROWS>(e, lane) < rows_here) out.k[i + 1][base + elem_offset<AT_ROWS>(e)] = KN[e];
             }
             if (last) {
                 // ---- k_S: candidate commit, error ratio (misc.py:80-82 up to the mean) ----
 #pragma unroll
                 for (int e = 0; e < 16; ++e) {
-                    if (FULL || elem_row(e, lane) < rows_here) {
-                        if (kcand) kcand[base + elem_offset(e)] = KN[e];
+                    if (FULL || elem_row<AT_ROWS>(e, lane) < rows_here) {
+                        if (kcand) kcand[base + elem_offset<AT_ROWS>(e)] = KN[e];
                         if (fold) {
                             const float num = Ar<float>::add(AE[e], Ar<float>::mul(KN[e], ecS));
                             const float q = Ar<float>::div(num, Y1[e]);
@@ -326,18 +328,18 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
         }
     };
 #pragma unroll 1
-    for (int t = g * (int)gridDim.x + (int)blockIdx.x; t < tiles; t += workers) {
-        {   // the next tile's y0 / k_0 rows of this warp towards L2: lanes 0..15 -> y0 rows, 16..31 -> k_0 rows (the warp's 16
-            // features of a row are 64 contiguous bytes, two chains apart)
-            const int tn = t + workers, pr = lane & 15;
-            const long long prow = (long long)tn * TILE_ROWS + pr;
+    for (int t = (int)blockIdx.x; t < tiles; t += (int)gridDim.x) {
+        {   // the next tile's y0 / k_0 rows of this warp towards L2: lane = row (the warp's 16 features of a row are 64
+            // contiguous bytes)
+            const int tn = t + (int)gridDim.x;
+            const long long prow = (long long)tn * AT_ROWS + lane;
             if (tn < tiles && prow < (long long)n_rows) {
-                const float *pp = (lane < 16 ? y0 : k0) + (size_t)prow * LD + 16 * w;
-                asm volatile("prefetch.global.L2 [%0];" :: "l"(pp));
-                asm volatile("prefetch.global.L2 [%0];" :: "l"(pp + 64));
+                const size_t o = (size_t)prow * LD + 64 * h + 16 * w;
+                asm volatile("prefetch.global.L2 [%0];" :: "l"(y0 + o));
+                asm volatile("prefetch.global.L2 [%0];" :: "l"(k0 + o));
             }
         }
-        if (n_rows - t * TILE_ROWS >= TILE_ROWS) do_tile(std::true_type{}, t);
+        if (n_rows - t * AT_ROWS >= AT_ROWS) do_tile(std::true_type{}, t);
         else do_tile(std::false_type{}, t);
     }
     const double bad = (double)nbad;
@@ -396,27 +398,24 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
 constexpr unsigned long long RM_DOPRI5 = 0x01ull | (0x03ull << 8) | (0x07ull << 16) | (0x0full << 24) | (0x1full << 32) | (0x3dull << 40);
 constexpr unsigned long long RM_BOSH3 = 0x01ull | (0x02ull << 8) | (0x07ull << 16);
 
-template <int S, unsigned long long RM, unsigned EM, int G, bool CTRL>
-int launch_attempt_g(TdqCtrl *c, const float *y0, const float *k0, const AttOut &out, const uint32_t *wt, double *partials,
+template <int S, unsigned long long RM, unsigned EM, bool CTRL>
+int launch_attempt_c(TdqCtrl *c, const float *y0, const float *k0, const AttOut &out, const uint32_t *wt, double *partials,
                      double *norm_out, const int64_t *seg_counts, int store_always, size_t n_rows, cudaStream_t st) {
-    auto kern = k_linear_attempt<S, RM, EM, G, CTRL>;
-    constexpr int AT_SMEM = at_smem(G);
+    auto kern = k_linear_attempt<S, RM, EM, CTRL>;
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM) != cudaSuccess) return -2;
-    const size_t tiles = (n_rows + TILE_ROWS - 1) / TILE_ROWS;
-    size_t grid = (tiles + G - 1) / G;
+    size_t grid = (n_rows + AT_ROWS - 1) / AT_ROWS;
     const size_t cap = (size_t)tdq_sm_count();
     if (grid > cap) grid = cap;
     if (grid == 0) grid = 1;
-    kern<<<(unsigned)grid, G * 128, AT_SMEM, st>>>(c, y0, k0, out, wt, partials, norm_out, seg_counts, store_always, n_rows);
+    kern<<<(unsigned)grid, AT_THREADS, AT_SMEM, st>>>(c, y0, k0, out, wt, partials, norm_out, seg_counts, store_always, n_rows);
     return 0;
 }
 
 template <int S, unsigned long long RM, unsigned EM>
 int launch_attempt(TdqCtrl *c, const float *y0, const float *k0, const AttOut &out, const uint32_t *wt, double *partials,
                    double *norm_out, const int64_t *seg_counts, int store_always, size_t n_rows, cudaStream_t st) {
-    constexpr int G = AT_GROUPS;
-    return seg_counts ? launch_attempt_g<S, RM, EM, G, true>(c, y0, k0, out, wt, partials, norm_out, seg_counts, store_always, n_rows, st)
-                      : launch_attempt_g<S, RM, EM, G, false>(c, y0, k0, out, wt, partials, norm_out, seg_counts, store_always, n_rows, st);
+    return seg_counts ? launch_attempt_c<S, RM, EM, true>(c, y0, k0, out, wt, partials, norm_out, seg_counts, store_always, n_rows, st)
+                      : launch_attempt_c<S, RM, EM, false>(c, y0, k0, out, wt, partials, norm_out, seg_counts, store_always, n_rows, st);
 }
 
 // row / error masks of a tableau, or false if it is not FSAL with 2..AT_MAX_S stages and an error weight on k_S

@@ -132,10 +132,10 @@ k_linear_stage(const TdqCtrl *__restrict__ c, int row, const float *y0, LinK kp,
         }
         // the previous tile's product has been read by every warp of the group (its wgmma_wait is behind each of them)
         asm volatile("bar.sync %0, 128;" :: "r"(g + 1) : "memory");
-        store_planes(stage, y, w, lane);
+        store_planes(stage, y, 0, w, lane);
         fence_async_smem();
         asm volatile("bar.sync %0, 128;" :: "r"(g + 1) : "memory");
-        TileAcc acc;
+        TileAcc<TILE_ROWS> acc;
         float kr[16];
         tile_product(wsm, stage, acc);
         wgmma_wait();

@@ -1,10 +1,12 @@
 // tdq_tc.cuh -- the float32 -> 3 x bfloat16 split and the warpgroup MMA (wgmma) tile product shared by the tensor-core
 // kernels of libtdq (tdq_linear.cu: one stage per launch; tdq_attempt.cu: a whole attempt per launch).  sm_90a.
 //
-// The product of one tile: K^T = W Y^T for 16 state rows, with M = 128 output features (two m64 halves, "chains"), N = 16
-// state rows, K = 128 input features.  A = the weight planes (K-major), B = the stage-value planes (MN-major), both in shared
-// memory without swizzle; the accumulators are registers.  Every kernel issues exactly this instruction sequence, so a row's
-// result does not depend on which kernel computed it or where the row sits in the tiling.
+// The product of one tile: K^T = W Y^T for N state rows (N = 16 in the stage kernels, 32 in the attempt kernel) and K = 128
+// input features, issued by one warpgroup over C = 32 / N m64 halves of the output features ("chains"; with N = 32 the two
+// warpgroups of a CTA take one half each).  A = the weight planes (K-major), B = the stage-value planes (MN-major), both in
+// shared memory without swizzle; the accumulators are registers, 16 per thread for either N.  Every kernel issues the same
+// sequence of products into each accumulator, so a row's result does not depend on which kernel computed it or where the
+// row sits in the tiling (tests/test_gpu_linear.py compares the attempt kernel with the stage kernel bitwise).
 #pragma once
 
 #include <cstdint>
@@ -14,24 +16,30 @@
 namespace tdq_tc {
 
 constexpr int LD = 128;                       // state width = output features = GEMM K and M
-constexpr int TILE_ROWS = 16;                 // state rows per tile = MMA N
+constexpr int TILE_ROWS = 16;                 // state rows per tile of the stage kernels = MMA N
 // Weights, one plane: element (feature f, input k) at (f >> 3) * 2048 + (k >> 3) * 128 + (f & 7) * 16 + (k & 7) * 2
 // (core matrices of 8 x 8 bf16 = 128 contiguous bytes, K-major).  The global image written by tdq_linear_prepare is exactly
 // the shared-memory image: 3 planes (hi, mid, lo).
 constexpr int W_PLANE = LD * LD * 2;
 constexpr int W_BYTES = 3 * W_PLANE;
-// Stage values of a tile, one plane: element (row n, feature k) at (n >> 3) * 2048 + (k >> 3) * 128 + (k & 7) * 16 + (n & 7) * 2
-// (core matrices of 8 rows x 8 features, MN-major: 8 consecutive rows of one feature are 16 contiguous bytes).
-constexpr int Y_PLANE = TILE_ROWS * LD * 2;
+// Stage values of an N-row tile, one plane: element (row n, feature k) at (n >> 3) * 2048 + (k >> 3) * 128 + (k & 7) * 16 +
+// (n & 7) * 2 (core matrices of 8 rows x 8 features, MN-major: 8 consecutive rows of one feature are 16 contiguous bytes).
+template <int N> __host__ __device__ constexpr int y_plane() { return N * LD * 2; }
+constexpr int Y_PLANE = y_plane<TILE_ROWS>();
 constexpr int Y_STAGE = 3 * Y_PLANE;
 // no swizzle: leading byte offset = next core matrix along K, stride byte offset = next core matrix along M / N (both operands)
 constexpr uint32_t LBO = 128, SBO = 2048;
 
-// Register layout of a thread's 16 elements of a tile (the m64n16 accumulator layout, twice): element e = 8 c + 4 j + 2 i + b
-// is feature 64 c + 16 w + (lane >> 2) + 8 i of row 8 j + 2 (lane & 3) + b, w = warp index inside the warpgroup.
-// Element e of a tile sits at row0 * LD + thread_offset(w, lane) + elem_offset(e) in the [rows][LD] state.
-__device__ __forceinline__ int elem_row(int e, int lane) { return 8 * ((e >> 2) & 1) + 2 * (lane & 3) + (e & 1); }
-__host__ __device__ constexpr int elem_offset(int e) { return (8 * ((e >> 2) & 1) + (e & 1)) * LD + 64 * (e >> 3) + 8 * ((e >> 1) & 1); }
+// Register layout of a thread's 16 elements of an N-row tile (the m64nN accumulator layout, C = 32 / N times): element
+// e = 4 (N / 8) c + 4 j + 2 i + b is feature 64 (c0 + c) + 16 w + (lane >> 2) + 8 i of row 8 j + 2 (lane & 3) + b, w = warp
+// index inside the warpgroup, c0 = the warpgroup's first chain (0 when it issues both).
+// Element e of a tile sits at row0 * LD + thread_offset(w, lane) + 64 c0 + elem_offset<N>(e) in the [rows][LD] state.
+template <int N = TILE_ROWS> __device__ __forceinline__ int elem_row(int e, int lane) {
+    return 8 * ((e >> 2) % (N / 8)) + 2 * (lane & 3) + (e & 1);
+}
+template <int N = TILE_ROWS> __host__ __device__ constexpr int elem_offset(int e) {
+    return (8 * ((e >> 2) % (N / 8)) + (e & 1)) * LD + 64 * ((e >> 2) / (N / 8)) + 8 * ((e >> 1) & 1);
+}
 __device__ __forceinline__ int thread_offset(int w, int lane) { return 2 * (lane & 3) * LD + 16 * w + (lane >> 2); }
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -47,19 +55,22 @@ __device__ __forceinline__ void split2(float a, float b, uint32_t &h, uint32_t &
 
 __device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" :: "r"(addr), "r"(v) : "memory"); }
 
-// Split a thread's 16 stage values and store them into the three planes of a tile (stage = shared address of plane 0).  Each
-// pair (b = 0, 1) is two consecutive rows of one feature: one 32-bit store per plane; a warp's store is 128 contiguous bytes.
-__device__ __forceinline__ void store_planes(uint32_t stage, const float (&y)[16], int w, int lane) {
-    // feature 64 c + 16 w + (lane >> 2) + 8 i = 8 (8 c + 2 w + i) + (lane >> 2); rows 8 j + 2 (lane & 3) + {0, 1}
-    stage += (uint32_t)(2 * w * LBO + (lane >> 2) * 16 + (lane & 3) * 4);
+// Split a thread's 16 stage values and store them into the three planes of an N-row tile (stage = shared address of plane 0;
+// c0 as above).  Each pair (b = 0, 1) is two consecutive rows of one feature: one 32-bit store per plane; a warp's store is
+// 128 contiguous bytes.
+template <int N = TILE_ROWS>
+__device__ __forceinline__ void store_planes(uint32_t stage, const float (&y)[16], int c0, int w, int lane) {
+    // feature 64 (c0 + c) + 16 w + (lane >> 2) + 8 i = 8 (8 (c0 + c) + 2 w + i) + (lane >> 2); rows 8 j + 2 (lane & 3) + {0, 1}
+    stage += (uint32_t)((8 * c0 + 2 * w) * LBO + (lane >> 2) * 16 + (lane & 3) * 4);
 #pragma unroll
     for (int e = 0; e < 16; e += 2) {
-        const uint32_t off = ((e >> 2) & 1) * SBO + (8 * (e >> 3) + ((e >> 1) & 1)) * LBO;
+        const int j = (e >> 2) % (N / 8), c = (e >> 2) / (N / 8);
+        const uint32_t off = j * SBO + (8 * c + ((e >> 1) & 1)) * LBO;
         uint32_t h, m, l;
         split2(y[e], y[e + 1], h, m, l);
         sts_u32(stage + off, h);
-        sts_u32(stage + Y_PLANE + off, m);
-        sts_u32(stage + 2 * Y_PLANE + off, l);
+        sts_u32(stage + y_plane<N>() + off, m);
+        sts_u32(stage + 2 * y_plane<N>() + off, l);
     }
 }
 
@@ -68,16 +79,28 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
     return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(LBO >> 4) << 16) | ((uint64_t)(SBO >> 4) << 32);
 }
 
-// D (+)= A B, m64n16k16, bf16 x bf16 -> f32; A K-major, B MN-major (transposed)
-__device__ __forceinline__ void wgmma_16(float (&d)[8], uint64_t da, uint64_t db, uint32_t accumulate) {
+// D (+)= A B, m64nNk16 (N = 16 or 32), bf16 x bf16 -> f32; A K-major, B MN-major (transposed)
+template <int N> __device__ __forceinline__ void wgmma_n(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate);
+template <> __device__ __forceinline__ void wgmma_n<16>(float (&d)[8], uint64_t da, uint64_t db, uint32_t accumulate) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
                  "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 1;\n\t}\n"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
                  : "l"(da), "l"(db), "r"(accumulate));
 }
+template <> __device__ __forceinline__ void wgmma_n<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 1;\n\t}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "l"(da), "l"(db), "r"(accumulate));
+}
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// wait until at most `pending` committed groups are still in flight
+template <int pending = 0> __device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(pending) : "memory");
+}
 // keeps the compiler from moving accesses of v across the asm statements around it (accumulators of an MMA in flight)
 template <int N> __device__ __forceinline__ void reg_fence(float (&v)[N]) {
 #pragma unroll
@@ -86,73 +109,97 @@ template <int N> __device__ __forceinline__ void reg_fence(float (&v)[N]) {
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 
-// Accumulators of one tile product (registers): chain c = output features [64 c, 64 c + 64).
-struct TileAcc {
-    float small[2][8], big[2][8], part[2][8];
+// Accumulators of one N-row tile product (registers): chain c = output features [64 (c0 + c), 64 (c0 + c) + 64).
+template <int N> struct TileAcc {
+    static constexpr int C = 32 / N;
+    float small[C][N / 2], big[C][N / 2], part[C][N / 2];
 };
-__device__ __forceinline__ void acc_fence(TileAcc &a) {
-    reg_fence(a.small[0]); reg_fence(a.small[1]); reg_fence(a.big[0]); reg_fence(a.big[1]);
-    reg_fence(a.part[0]); reg_fence(a.part[1]);
+template <int N> __device__ __forceinline__ void fence_hi(TileAcc<N> &a) {
+#pragma unroll
+    for (int c = 0; c < TileAcc<N>::C; ++c) {
+        reg_fence(a.big[c]);
+        reg_fence(a.part[c]);
+    }
+}
+template <int N> __device__ __forceinline__ void acc_fence(TileAcc<N> &a) {
+#pragma unroll
+    for (int c = 0; c < TileAcc<N>::C; ++c) reg_fence(a.small[c]);
+    fence_hi(a);
 }
 
-// weight plane PW x stage plane PY over k-steps [k0, k1) into d (d is overwritten at k0 when `fresh`)
+// weight plane PW x stage plane PY over k-steps [k0, k1) into d (d is overwritten at k0 when `fresh`); wsm = the weights of
+// the warpgroup's first chain
+template <int N>
 __device__ __forceinline__ void plane_product(uint32_t wsm, uint32_t stage, int pw, int py, int k0, int k1, bool fresh,
-                                              float (&d)[2][8]) {
+                                              float (&d)[32 / N][N / 2]) {
 #pragma unroll
     for (int ks = k0; ks < k1; ++ks) {
 #pragma unroll
-        for (int c = 0; c < 2; ++c)
-            wgmma_16(d[c], make_desc(wsm + pw * W_PLANE + c * 8 * SBO + ks * 2 * LBO), make_desc(stage + py * Y_PLANE + ks * 2 * LBO),
-                     fresh && ks == k0 ? 0u : 1u);
+        for (int c = 0; c < 32 / N; ++c)
+            wgmma_n<N>(d[c], make_desc(wsm + pw * W_PLANE + c * 8 * SBO + ks * 2 * LBO),
+                       make_desc(stage + py * y_plane<N>() + ks * 2 * LBO), fresh && ks == k0 ? 0u : 1u);
     }
 }
-__device__ __forceinline__ void add_part(TileAcc &a) {
+template <int N> __device__ __forceinline__ void add_part(TileAcc<N> &a) {
 #pragma unroll
-    for (int c = 0; c < 2; ++c) {
+    for (int c = 0; c < TileAcc<N>::C; ++c) {
 #pragma unroll
-        for (int r = 0; r < 8; ++r) a.big[c][r] = a.big[c][r] + a.part[c][r];
+        for (int r = 0; r < N / 2; ++r) a.big[c][r] = a.big[c][r] + a.part[c][r];
     }
 }
 
-// Issue the product of one tile (stage planes at shared address `stage`, weight planes at `wsm`); the caller waits
-// (wgmma_wait) and then calls tile_result.  Weight plane PW x stage plane PY: mid.mid, lo.hi, hi.lo, mid.hi, hi.mid -- the
-// five cross terms >= 2^-16, ascending in magnitude -- into the small accumulator; hi.hi into the big one; k = small + big.
-// The three remaining cross terms (lo.lo, lo.mid, mid.lo) are below 2^-24 of a product, the rounding of a float32 product
-// itself, and are not computed.
+// cross term p of the list below into `small`
+template <int N> __device__ __forceinline__ void cross_term(uint32_t wsm, uint32_t stage, int p, TileAcc<N> &a) {
+    constexpr int PW[5] = {1, 2, 0, 1, 0}, PY[5] = {1, 0, 2, 0, 1};
+    plane_product<N>(wsm, stage, PW[p], PY[p], 0, LD / 16, p == 0, a.small);
+}
+// partial q (k-steps 2q, 2q + 1) of hi.hi into `part`, once the previous partial has been added to `big`
+template <int N> __device__ __forceinline__ void next_partial(uint32_t wsm, uint32_t stage, int q, TileAcc<N> &a) {
+    wgmma_wait<1>();                                      // the group holding partial q - 1 (only newer cross terms may run)
+    fence_hi(a);
+    add_part(a);
+    fence_hi(a);
+    wgmma_fence();
+    plane_product<N>(wsm, stage, 0, 0, 2 * q, 2 * q + 2, true, a.part);
+    wgmma_commit();
+}
+// Issue the product of one tile (stage planes at shared address `stage`, weight planes of the first chain at `wsm`); the
+// caller waits (wgmma_wait) and then calls tile_result.  Weight plane PW x stage plane PY: mid.mid, lo.hi, hi.lo, mid.hi,
+// hi.mid -- the five cross terms >= 2^-16, ascending in magnitude -- into the small accumulator; hi.hi into the big one;
+// k = small + big.  The three remaining cross terms (lo.lo, lo.mid, mid.lo) are below 2^-24 of a product, the rounding of a
+// float32 product itself, and are not computed.
 // The tensor cores round a float32 accumulation toward zero, which over the eight k-steps of hi.hi shrinks every k by about
 // one unit in the last place (measured on H100: -9e-8 relative, where a float32 SGEMM is unbiased).  So hi.hi is taken as
 // four partial sums of two k-steps each, added here in float32 with round-to-nearest: the truncation of a partial then has
-// no preferred sign with respect to k.  Issued by the whole warpgroup.
-__device__ __forceinline__ void tile_product(uint32_t wsm, uint32_t stage, TileAcc &a) {
+// no preferred sign with respect to k.
+// Issue order: each wait for a hi.hi partial (which is needed on the CUDA cores before the next one can be issued into the
+// same accumulator) has a batch of cross terms queued behind it, so the tensor pipe does not drain while `big += part` runs.
+// Each accumulator still sees the same products and float32 additions in the same order.  Issued by the whole warpgroup.
+template <int N> __device__ __forceinline__ void tile_product(uint32_t wsm, uint32_t stage, TileAcc<N> &a) {
     acc_fence(a);
     wgmma_fence();
-    plane_product(wsm, stage, 0, 0, 0, 2, true, a.big);
-    plane_product(wsm, stage, 0, 0, 2, 4, true, a.part);
+    plane_product<N>(wsm, stage, 0, 0, 0, 2, true, a.big);
+    plane_product<N>(wsm, stage, 0, 0, 2, 4, true, a.part);
     wgmma_commit();
-#pragma unroll
-    for (int q = 2; q < 4; ++q) {
-        wgmma_wait();
-        acc_fence(a);
-        add_part(a);
-        acc_fence(a);
-        wgmma_fence();
-        plane_product(wsm, stage, 0, 0, 2 * q, 2 * q + 2, true, a.part);
-        wgmma_commit();
-    }
-    constexpr int NSMALL = 5;
-    constexpr int PW[NSMALL] = {1, 2, 0, 1, 0}, PY[NSMALL] = {1, 0, 2, 0, 1};
-#pragma unroll
-    for (int p = 0; p < NSMALL; ++p) plane_product(wsm, stage, PW[p], PY[p], 0, LD / 16, p == 0, a.small);
+    cross_term(wsm, stage, 0, a);
+    cross_term(wsm, stage, 1, a);
+    wgmma_commit();
+    next_partial(wsm, stage, 2, a);
+    cross_term(wsm, stage, 2, a);
+    cross_term(wsm, stage, 3, a);
+    wgmma_commit();
+    next_partial(wsm, stage, 3, a);
+    cross_term(wsm, stage, 4, a);
     wgmma_commit();
     acc_fence(a);
 }
 
 // after wgmma_wait: k of the thread's 16 elements, in the element order above
-__device__ __forceinline__ void tile_result(TileAcc &a, float (&k)[16]) {
+template <int N> __device__ __forceinline__ void tile_result(TileAcc<N> &a, float (&k)[16]) {
     acc_fence(a);
     add_part(a);
 #pragma unroll
-    for (int e = 0; e < 16; ++e) k[e] = a.small[e >> 3][e & 7] + a.big[e >> 3][e & 7];
+    for (int e = 0; e < 16; ++e) k[e] = a.small[e / (N / 2)][e % (N / 2)] + a.big[e / (N / 2)][e % (N / 2)];
 }
 
 // the weight image (W_BYTES, 16-byte aligned) -> shared memory, by all `threads` threads of the block; the caller then
