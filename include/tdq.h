@@ -327,7 +327,7 @@ int tdq_linear_stage(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, int3
                      void *stream);
 
 /* ---- A WHOLE attempt of a linear vector field in one launch (tdq_attempt.cu) ---------------------------------------------
- * For f(t, y) = y W^T an attempt is row-local, so one kernel takes every tile of 16 state rows through all S stages on chip:
+ * For f(t, y) = y W^T an attempt is row-local, so one kernel takes every tile of 32 state rows through all S stages on chip:
  * rk_common.py:43-90 (_runge_kutta_step: every y_i, every k_i, y1, the error estimate), the squared error ratio of
  * misc.py:80-82 and the candidate commit of rk_common.py:341/:352 -- what S x tdq_linear_stage + tdq_error_norm_commit do
  * in S + 1 launches.  HBM traffic: 2 reads + 2 writes per element.  Same arithmetic, operation for operation: k_i, y1 and the
@@ -339,9 +339,8 @@ int tdq_linear_stage(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, int3
  * partials / norm_out (both or neither): norm_out[0] = sum over the state of ((err_pre + k_S e_S) / (atol + rtol max(|y0|,|y1|)))^2,
  * norm_out[1] = number of non-finite y1 elements (what tdq_error_norm_commit writes for one segment), and y1 -> ybuf[par^1],
  * k_S -> kbuf[par^1]; partials needs tdq_norm_partials_len doubles, zeroed once.  Scalar tolerances only.  No-op after halt.
- * seg_counts_dev != NULL (needs partials / norm_out): the last block to finish also performs the controller step, exactly
- * what tdq_controller(ctrl, dtype, norm_out, seg_counts_dev, 1, NULL) would do next (rk_common.py:323-361, misc.py:85-95,
- * the peer exchange of a sharded solve included) -- the caller then skips that launch. */
+ * The controller step is the caller's next launch: tdq_controller(ctrl, dtype, norm_out, <element count>, 1, NULL).
+ * seg_counts_dev is reserved and must be NULL; any other value is refused before the device is touched. */
 int tdq_linear_attempt_supported(const tdq_tableau *tab, int32_t dtype, int32_t width);
 int tdq_linear_attempt(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, void *const *k_out, void *y1_out, void *err_out,
                        const void *y0, const void *k0, const void *planes, int32_t width, size_t n, double *partials,

@@ -78,12 +78,13 @@ def test_linear_attempt_host_side_contract():
     bad = C.c_void_p(16)                                                             # never dereferenced: the checks come first
     kp = _lib.ptr_array([None] + [16] * 6)
     # null control block / float64 / state not a whole number of rows / norm outputs that do not go together /
-    # the controller step without the folded norm
+    # the reserved seg_counts_dev not NULL, without and with the folded norm
     assert lib.tdq_linear_attempt(None, C.byref(tab), 0, kp, bad, bad, None, None, bad, 128, 1280, None, None, None, 1, None) != 0
     assert lib.tdq_linear_attempt(bad, C.byref(tab), 1, kp, bad, bad, None, None, bad, 128, 1280, None, None, None, 1, None) != 0
     assert lib.tdq_linear_attempt(bad, C.byref(tab), 0, kp, bad, bad, None, None, bad, 128, 1281, None, None, None, 1, None) != 0
     assert lib.tdq_linear_attempt(bad, C.byref(tab), 0, kp, bad, bad, None, None, bad, 128, 1280, bad, None, None, 1, None) != 0
     assert lib.tdq_linear_attempt(bad, C.byref(tab), 0, kp, bad, bad, None, None, bad, 128, 1280, None, None, bad, 1, None) != 0
+    assert lib.tdq_linear_attempt(bad, C.byref(tab), 0, kp, bad, bad, None, None, bad, 128, 1280, bad, bad, bad, 1, None) != 0
     # a tableau the kernel does not take is refused as well
     t8 = _lib.tableau("dopri8")
     k8 = _lib.ptr_array([None] + [16] * 13)

@@ -6,7 +6,7 @@ tdq_linear_stage == tdq_linear_apply(tdq_stage_combine(...)) BITWISE, and the FS
 bitwise.  Solve level: the fused solve against the generic one (func as a torch call), against the oracle, and against the golden
 vectors of the unmodified reference for the configs[1]-shaped problem (rtol 1e-4 / atol 1e-6, the tolerance north_star states).
 The whole-attempt kernel (csrc/tdq_attempt.cu, the default for dopri5 / bosh3, so every solve-level test above runs through it):
-tdq_linear_attempt == S x tdq_linear_stage + tdq_error_norm_commit (+ tdq_controller) BITWISE at the kernel level, and the solves
+tdq_linear_attempt == S x tdq_linear_stage + tdq_error_norm_commit BITWISE at the kernel level, and the solves
 it drives against the per-stage path in every execution mode."""
 import ctypes as C
 import os
@@ -414,9 +414,11 @@ def test_linear_attempt_argument_checks():
     assert not ok(lib.tdq_linear_attempt(ctrl, tabp, 0, kp, y1, er, None, None, planes.data_ptr(), 128, 1281, None, None, None, 1, _stream()))
     assert not ok(lib.tdq_linear_attempt(ctrl, tabp, 0, kp, y1, er, None, None, planes.data_ptr(), 128, 1280,
                                          eng.partials.data_ptr(), None, None, 1, _stream()))
-    # the controller step needs the folded norm
+    # seg_counts_dev is reserved: refused without and with the folded norm
     assert not ok(lib.tdq_linear_attempt(ctrl, tabp, 0, kp, y1, er, None, None, planes.data_ptr(), 128, 1280,
                                          None, None, eng.seg_counts.data_ptr(), 1, _stream()))
+    assert not ok(lib.tdq_linear_attempt(ctrl, tabp, 0, kp, y1, er, None, None, planes.data_ptr(), 128, 1280,
+                                         eng.partials.data_ptr(), eng.norm_out.data_ptr(), eng.seg_counts.data_ptr(), 1, _stream()))
     for m, want in (("dopri5", 1), ("bosh3", 1), ("tsit5", 0), ("dopri8", 0), ("fehlberg2", 0), ("adaptive_heun", 0)):
         e2, _, _ = _engine(m, torch.float32, 1280, 0.01)
         assert lib.tdq_linear_attempt_supported(C.byref(e2.tab), 0, 128) == want, m
@@ -446,12 +448,10 @@ def test_whole_attempt_solve_matches_stage_path(method, batch):
     if (sa["n_accept"], sa["n_reject"]) == (ss["n_accept"], ss["n_reject"]):
         assert torch.equal(ya, ys)
     assert torch.allclose(ya, ys, rtol=1e-4, atol=2e-5), float((ya - ys).abs().max())
-    # lock step, run-ahead, graph + device loop: the same bits; the controller step inside the attempt launch too
+    # lock step, run-ahead, graph + device loop: the same bits
     b, _ = _solve(f, y0, t, method, graph=False, run_ahead=0)
     c, _ = _solve(f, y0, t, method, graph=True)
-    d, sd = _solve(f, y0, t, method, fused_controller=True)
-    assert torch.equal(ya, b) and torch.equal(ya, c) and torch.equal(ya, d)
-    assert (sd["n_accept"], sd["n_reject"]) == (sa["n_accept"], sa["n_reject"])
+    assert torch.equal(ya, b) and torch.equal(ya, c)
 
 
 def test_whole_attempt_dense_and_events():
@@ -466,38 +466,3 @@ def test_whole_attempt_dense_and_events():
         for tq in (0.1, 0.77, 1.5):
             tt = torch.tensor(tq, device=DEV)
             assert torch.allclose(da(tt), ds(tt), rtol=1e-5, atol=1e-6)
-
-
-@pytest.mark.parametrize("method,dt,accepted", [("dopri5", 1e-7, 1), ("dopri5", 0.0371, 0), ("bosh3", 1e-7, 1)])
-def test_linear_attempt_with_controller_step(method, dt, accepted):
-    """seg_counts given: the last block of tdq_linear_attempt runs the controller step.  The control block afterwards is
-    bit for bit what tdq_linear_attempt + tdq_controller leave behind (accepted and rejected attempts)."""
-    rows = 777
-    n = rows * 128
-    eng, _lib, _stream = _engine(method, torch.float32, n, dt, 0.5, 1.0)
-    lib = eng.lib
-    S = O.tableau(method)["n_stages"]
-    planes = _planes(lib, _lib, _weight(seed=11), _stream)
-    y0 = _rand(n, torch.float32, 1).to(DEV)
-    k0 = _rand(n, torch.float32, 2).to(DEV)
-    outs = [None] + [torch.zeros(n, device=DEV) for _ in range(S)]
-    y1a, era = torch.zeros(n, device=DEV), torch.zeros(n, device=DEV)
-    kp = _lib.ptr_array([None] + [o.data_ptr() for o in outs[1:]])
-    ctrl0 = eng.ctrl.clone()
-
-    def run(with_ctrl):
-        eng.ctrl.copy_(ctrl0)
-        eng.norm_out.zero_()
-        _lib.check(lib.tdq_linear_attempt(eng.ctrl.data_ptr(), C.byref(eng.tab), 0, kp, y1a.data_ptr(), era.data_ptr(), y0.data_ptr(),
-                                          k0.data_ptr(), planes.data_ptr(), 128, n, eng.partials.data_ptr(), eng.norm_out.data_ptr(),
-                                          eng.seg_counts.data_ptr() if with_ctrl else None, 0, _stream()))
-        if not with_ctrl:
-            _lib.check(lib.tdq_controller(eng.ctrl.data_ptr(), 0, eng.norm_out.data_ptr(), eng.seg_counts.data_ptr(), 1, None, _stream()))
-        torch.cuda.synchronize()
-        return eng.ctrl.clone(), eng.mbox_host.contents.accept, eng.mbox_host.contents.seq
-
-    a, acc_a, _ = run(False)
-    b, acc_b, _ = run(True)
-    assert torch.equal(a, b)
-    assert acc_a == acc_b == accepted          # random slopes: only a tiny step passes the error test
-    assert not torch.equal(a, ctrl0)

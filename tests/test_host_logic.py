@@ -216,10 +216,10 @@ def test_fused_linear_options_and_eligibility():
 
     with warnings.catch_warnings(record=True) as w:
         warnings.simplefilter("always")
-        O_._warn_unused("dopri5", {"fused_linear": False, "fused_attempt": False, "fused_controller": False, "run_ahead": 0}, set())
+        O_._warn_unused("dopri5", {"fused_linear": False, "fused_attempt": False, "run_ahead": 0}, set())
         assert not w
-        O_._warn_unused("dopri5", {"not_an_option": 1}, set())
-        assert len(w) == 1 and "not_an_option" in str(w[0].message)
+        O_._warn_unused("dopri5", {"not_an_option": 1, "fused_controller": True}, set())
+        assert len(w) == 1 and "not_an_option" in str(w[0].message) and "fused_controller" in str(w[0].message)
 
     lib = _lib.load()
     cpu = torch.device("cpu")

@@ -323,14 +323,11 @@ class AdaptiveEngine:
             self.post_fn(buf)
         return buf
 
-    def set_linear(self, weight, whole_attempt=True, fused_controller=False):
+    def set_linear(self, weight, whole_attempt=True):
         """Fuse the stage combination with func = y @ weight^T (torchdiffeq_b200.LinearField): tdq_linear_stage replaces
         tdq_stage_combine + the torch call for every row (rk_common.py:79-81 in one launch; csrc/tdq_linear.cu).
         For dopri5 / bosh3 the whole attempt -- every stage, the error norm, the candidate commit -- is ONE launch
-        (tdq_linear_attempt, csrc/tdq_attempt.cu) unless whole_attempt=False.  fused_controller=True runs the controller
-        step in the last block of that launch instead of a launch of its own: one launch less per attempt, but the device-
-        runtime call it contains makes ptxas serialise the kernel's wgmma pipeline (H100: 43.7 instead of 34.2 ms per solve
-        of configs[1]), so it is off by default.
+        (tdq_linear_attempt, csrc/tdq_attempt.cu) unless whole_attempt=False.
         Returns False (and changes nothing) if a row of the tableau has more terms than the fused kernel takes."""
         width, S = int(weight.shape[0]), self.S
         if self.pieces is not None or self.post_fn is not None or self.n % width:
@@ -347,7 +344,7 @@ class AdaptiveEngine:
         # at most 7 stages); the squared norm is folded in when it is the plain one (one segment, scalar tolerances)
         whole = bool(whole_attempt) and bool(self.lib.tdq_linear_attempt_supported(C.byref(self.tab), self.dt_code, width))
         fold = (whole and self.norm_table is None and self.n_seg == 1 and self.rtol_vec is None and self.norm_fn is None)
-        self.linear = dict(weight=weight, width=width, planes=planes, whole=whole, fold=fold, ctrl=bool(fused_controller),
+        self.linear = dict(weight=weight, width=width, planes=planes, whole=whole, fold=fold,
                            k=[torch.zeros(self.n, dtype=self.dtype, device=self.device) for _ in range(S)])
         self._drop_graph()
         return True
@@ -432,18 +429,12 @@ class AdaptiveEngine:
             for i in range(S):
                 k[i + 1] = L["k"][i].data_ptr()
             folded = L["fold"]
-            # ... and, if asked for (fused_controller), the controller step too (the last block to finish runs it), unless a
-            # host-launched collective has to reduce the norm sums between the two (NCCL / gloo exchange)
-            with_ctrl = folded and L["ctrl"] and (self.reduce_fn is None or self.exchange is not None)
             self._launch(lib.tdq_linear_attempt(ctrl, tab, dc, _lib.ptr_array(k), self.y1.data_ptr(), self.errp.data_ptr(),
                                                 None, None, L["planes"].data_ptr(), L["width"], self.n,
                                                 self.partials.data_ptr() if folded else None,
                                                 self.norm_out.data_ptr() if folded else None,
-                                                self.seg_counts.data_ptr() if with_ctrl else None,
-                                                0 if folded else 1, st))
+                                                None, 0 if folded else 1, st))
             self.nfe += S
-            if with_ctrl:
-                return k, _lib.ptr_array(k), keep
         elif self.linear is not None:
             # combination + evaluation of every row in one wgmma launch (csrc/tdq_linear.cu); the FSAL row also writes
             # y1 and the error-sum prefix exactly as tdq_stage_combine_final does

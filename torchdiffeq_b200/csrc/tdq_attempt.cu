@@ -23,14 +23,13 @@
 // folded into.  Per stage: newest term + split + st.shared of the warpgroup's feature half of the B planes,
 // fence.proxy.async, bar.sync (all 256 threads: the product needs both halves), 48 wgmma + commits per warpgroup; while they
 // run, the prefix of the next row's sum; then wgmma.wait and k_{i+1} = small + big.  The chain of a tile is serial by nature
-// (stage i+1 needs k_i).  The last block to finish adds the per-block partials of the squared error norm and runs the
-// controller step (tdq_ctrl_dev.cuh).
+// (stage i+1 needs k_i).  The last block to finish adds the per-block partials of the squared error norm; the controller
+// step is the next launch (tdq_controller, tdq_ctrl.cu).
 //
 // Stage derivatives, y1 and the error prefix are written to HBM only for attempts that can contain an output time (the
 // lazy interpolant fit needs them, tdq_interp.cu) or when the caller keeps every step (dense output, events).
 #include "tdq_shape.cuh"
 #include "tdq_tc.cuh"
-#include "tdq_ctrl_dev.cuh"
 
 #include <type_traits>
 
@@ -68,18 +67,11 @@ __host__ __device__ constexpr int popc_below(unsigned mask, int j) {
 
 // S: stages of an FSAL tableau (rows 0..S-1, the last one is c_sol and yields y1).  RM: 8 bits per row, bit j set <=> slot j has
 // a non-zero coefficient in that row.  EM: the same for the error weights of slots 0..S-1 (k_S always carries the last one).
-// CTRL: the last block to finish also runs the controller step (tdq_ctrl_dev.cuh: accept / reject, next step size, the next
-// attempt's tables, the device-side loop's condition) -- one launch per attempt instead of two.
-template <int S, unsigned long long RM, unsigned EM, bool CTRL>
+template <int S, unsigned long long RM, unsigned EM>
 __global__ void __launch_bounds__(AT_THREADS, 1)
 k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const uint32_t *__restrict__ wt,
-                 double *partials, double *norm_out, const int64_t *seg_counts, int store_always, size_t n_rows_sz) {
-    if (c->halt) {
-        // An attempt issued after the end of the solve is a no-op -- but its controller step still has to tick the mailbox:
-        // a host that runs ahead (eager run_ahead, graph replay) accounts for every attempt it queued (tdq_ctrl_dev.cuh).
-        if (CTRL && blockIdx.x == 0) tdq_ctrl_dev::controller_block<float, AT_THREADS>(c, norm_out, seg_counts, 1, nullptr);
-        return;
-    }
+                 double *partials, double *norm_out, int store_always, size_t n_rows_sz) {
+    if (c->halt) return;                                  // an attempt issued after the end of the solve is a no-op
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
     uint8_t *aux = smem + W_BYTES + AT_STAGE + AT_Y0;
@@ -386,11 +378,6 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
             *ticket = 0;                                                  // self-reset for the next launch
         }
     }
-    if (CTRL) {
-        __threadfence();
-        __syncthreads();
-        tdq_ctrl_dev::controller_block<float, AT_THREADS>(c, norm_out, seg_counts, 1, nullptr);
-    }
 }
 
 // the sparsity of the supported FSAL tableaus (row masks 8 bits per row, error-prefix mask); tsit5 as the reference
@@ -398,24 +385,17 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
 constexpr unsigned long long RM_DOPRI5 = 0x01ull | (0x03ull << 8) | (0x07ull << 16) | (0x0full << 24) | (0x1full << 32) | (0x3dull << 40);
 constexpr unsigned long long RM_BOSH3 = 0x01ull | (0x02ull << 8) | (0x07ull << 16);
 
-template <int S, unsigned long long RM, unsigned EM, bool CTRL>
-int launch_attempt_c(TdqCtrl *c, const float *y0, const float *k0, const AttOut &out, const uint32_t *wt, double *partials,
-                     double *norm_out, const int64_t *seg_counts, int store_always, size_t n_rows, cudaStream_t st) {
-    auto kern = k_linear_attempt<S, RM, EM, CTRL>;
+template <int S, unsigned long long RM, unsigned EM>
+int launch_attempt(TdqCtrl *c, const float *y0, const float *k0, const AttOut &out, const uint32_t *wt, double *partials,
+                   double *norm_out, int store_always, size_t n_rows, cudaStream_t st) {
+    auto kern = k_linear_attempt<S, RM, EM>;
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM) != cudaSuccess) return -2;
     size_t grid = (n_rows + AT_ROWS - 1) / AT_ROWS;
     const size_t cap = (size_t)tdq_sm_count();
     if (grid > cap) grid = cap;
     if (grid == 0) grid = 1;
-    kern<<<(unsigned)grid, AT_THREADS, AT_SMEM, st>>>(c, y0, k0, out, wt, partials, norm_out, seg_counts, store_always, n_rows);
+    kern<<<(unsigned)grid, AT_THREADS, AT_SMEM, st>>>(c, y0, k0, out, wt, partials, norm_out, store_always, n_rows);
     return 0;
-}
-
-template <int S, unsigned long long RM, unsigned EM>
-int launch_attempt(TdqCtrl *c, const float *y0, const float *k0, const AttOut &out, const uint32_t *wt, double *partials,
-                   double *norm_out, const int64_t *seg_counts, int store_always, size_t n_rows, cudaStream_t st) {
-    return seg_counts ? launch_attempt_c<S, RM, EM, true>(c, y0, k0, out, wt, partials, norm_out, seg_counts, store_always, n_rows, st)
-                      : launch_attempt_c<S, RM, EM, false>(c, y0, k0, out, wt, partials, norm_out, seg_counts, store_always, n_rows, st);
 }
 
 // row / error masks of a tableau, or false if it is not FSAL with 2..AT_MAX_S stages and an error weight on k_S
@@ -463,7 +443,7 @@ int tdq_linear_attempt(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, vo
     TDQ_REQUIRE(dtype == TDQ_F32 && width == LD, "the fused linear field is float32, width 128");
     TDQ_REQUIRE(n % (size_t)width == 0, "state size is not a multiple of the field width");
     TDQ_REQUIRE((partials == nullptr) == (norm_out == nullptr), "partials and norm_out go together");
-    TDQ_REQUIRE(seg_counts_dev == nullptr || partials != nullptr, "the controller step needs the folded error norm");
+    TDQ_REQUIRE(seg_counts_dev == nullptr, "seg_counts_dev is reserved and must be NULL");
     const size_t n_rows = n / (size_t)width;
     TDQ_REQUIRE(n_rows < ((size_t)1 << 31) - 64, "too many rows");
     TdqHostShape hs;
@@ -486,9 +466,9 @@ int tdq_linear_attempt(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, vo
     cudaStream_t st = (cudaStream_t)stream;
     int rc = -1;
     if (S == 6 && rm == RM_DOPRI5 && em == 0x3du)
-        rc = launch_attempt<6, RM_DOPRI5, 0x3du>(c, (const float *)y0, (const float *)k0, out, wt, partials, norm_out, seg_counts_dev, store_always, n_rows, st);
+        rc = launch_attempt<6, RM_DOPRI5, 0x3du>(c, (const float *)y0, (const float *)k0, out, wt, partials, norm_out, store_always, n_rows, st);
     else if (S == 3 && rm == RM_BOSH3 && em == 0x07u)
-        rc = launch_attempt<3, RM_BOSH3, 0x07u>(c, (const float *)y0, (const float *)k0, out, wt, partials, norm_out, seg_counts_dev, store_always, n_rows, st);
+        rc = launch_attempt<3, RM_BOSH3, 0x07u>(c, (const float *)y0, (const float *)k0, out, wt, partials, norm_out, store_always, n_rows, st);
     TDQ_REQUIRE(rc != -1, "no whole-attempt kernel for this tableau (tdq_linear_attempt_supported)");
     TDQ_REQUIRE(rc == 0, "launch configuration failed");
     TDQ_CHECK_CUDA(cudaGetLastError());

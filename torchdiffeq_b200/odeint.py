@@ -32,7 +32,7 @@ _ADAPTIVE_OPTIONS = {"min_step", "max_step", "first_step", "step_t", "jump_t", "
                      "max_num_steps", "dtype", "norm"}
 _FIXED_OPTIONS = {"step_size", "grid_constructor", "interp", "perturb", "norm"}
 _ADAMS_OPTIONS = _FIXED_OPTIONS | {"max_iters", "max_order"}
-_OUR_OPTIONS = {"graph", "run_ahead", "process_group", "cache", "exchange", "device_loop", "fused_linear", "fused_attempt", "fused_controller"}
+_OUR_OPTIONS = {"graph", "run_ahead", "process_group", "cache", "exchange", "device_loop", "fused_linear", "fused_attempt"}
 
 
 def _rms_norm(tensor):
@@ -298,7 +298,7 @@ def _make_adaptive_engine(p, method, rtol, atol, rtol_vec, atol_vec, options, fn
         from .fields import fusable
         w = fusable(getattr(p, "original_func", None), tuple(p.shape), p.dtype, p.device, eng.lib)
         if w is not None:
-            eng.set_linear(w, whole_attempt=o.get("fused_attempt", True), fused_controller=o.get("fused_controller", False))
+            eng.set_linear(w, whole_attempt=o.get("fused_attempt", True))
     return eng
 
 
