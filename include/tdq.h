@@ -309,7 +309,9 @@ int tdq_lincomb(int32_t dtype, void *out, const void *base, const void *const *x
  * What rk_common.py:79-81 does with two kernels and a round trip of y_i through memory -- y_i = y0 + sum_j coef_ij k_j, then
  * k_i = func(t_i, y_i) -- in one launch when func is `torchdiffeq_b200.LinearField` (float32 states [..., 128], W 128 x 128):
  * y_i is formed in registers (same products, same order as tdq_stage_combine), split into three bfloat16 planes and multiplied
- * on the tensor cores (wgmma) with float32 register accumulators (three bf16 planes per operand, six products: float32-grade, rel. rms error 1e-7 against float64).
+ * on the tensor cores (wgmma) with float32 register accumulators (three bf16 planes per operand, six products): every element
+ * satisfies |k - y.w| <= 12 u S + 2 FLT_MIN against float64, u = 2^-24, S = sum |y||w|, for finite operands up to FLT_MAX
+ * where S < 2^127; non-finite operands stay in their row (tests/test_gpu_linear_numerics.py, DESIGN.md section 3b).
  * tdq_linear_supported: 1 if (dtype, width) has a fused kernel.  tdq_linear_weights_bytes: size of the split weights.
  * tdq_linear_prepare: W (row-major [width][width], W[n][k] = d k_n / d y_k, i.e. func = y @ W^T) -> split planes (once per solve).
  * tdq_linear_apply: k_out = y W^T for n_rows rows, no control block (f0, tests).

@@ -44,9 +44,11 @@ __device__ __forceinline__ int thread_offset(int w, int lane) { return 2 * (lane
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// two float32 -> packed bf16 pairs of the three planes (element 0 in the low half); the remainders are exact
+// two float32 -> packed bf16 pairs of the three planes (element 0 in the low half); the remainders are exact.  The hi plane
+// saturates (.satfinite): a finite |x| >= 0x7F7F8000 would round to bf16 infinity, and the remainder x - inf would make the
+// lower planes NaN; saturated to +-0x7F7F the three planes still sum to x.  Non-finite x still gives non-finite planes.
 __device__ __forceinline__ void split2(float a, float b, uint32_t &h, uint32_t &m, uint32_t &l) {
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(h) : "f"(b), "f"(a));
+    asm("cvt.rn.satfinite.bf16x2.f32 %0, %1, %2;" : "=r"(h) : "f"(b), "f"(a));
     const float ra = a - __uint_as_float(h << 16), rb = b - __uint_as_float(h & 0xffff0000u);
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(m) : "f"(rb), "f"(ra));
     const float sa = ra - __uint_as_float(m << 16), sb = rb - __uint_as_float(m & 0xffff0000u);
@@ -170,8 +172,9 @@ template <int N> __device__ __forceinline__ void next_partial(uint32_t wsm, uint
 // float32 product itself, and are not computed.
 // The tensor cores round a float32 accumulation toward zero, which over the eight k-steps of hi.hi shrinks every k by about
 // one unit in the last place (measured on H100: -9e-8 relative, where a float32 SGEMM is unbiased).  So hi.hi is taken as
-// four partial sums of two k-steps each, added here in float32 with round-to-nearest: the truncation of a partial then has
-// no preferred sign with respect to k.
+// four partial sums of two k-steps each, added here in float32 with round-to-nearest.  A partial is still correlated with
+// k, so some bias remains: mean(sign(k) (k - exact) / (2^-24 sum |y||w|)) is -0.045 against -0.165 for one accumulator and
+// +-0.0002 for cuBLAS' SGEMM (H100; tests/test_gpu_linear_numerics.py pins it).
 // Issue order: each wait for a hi.hi partial (which is needed on the CUDA cores before the next one can be issued into the
 // same accumulator) has a batch of cross terms queued behind it, so the tensor pipe does not drain while `big += part` runs.
 // Each accumulator still sees the same products and float32 additions in the same order.  Issued by the whole warpgroup.
