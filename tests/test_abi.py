@@ -91,3 +91,145 @@ def test_linear_attempt_host_side_contract():
     assert lib.tdq_linear_attempt(bad, C.byref(t8), 0, k8, bad, bad, None, None, bad, 128, 1280, None, None, None, 1, None) != 0
     # an empty state is a no-op that succeeds without a launch
     assert lib.tdq_linear_attempt(bad, C.byref(tab), 0, kp, bad, bad, None, None, bad, 128, 0, None, None, None, 1, None) == 0
+
+
+def test_stage_launchers_host_side_contract(lib):
+    """The stage launchers refuse bad arguments before they touch the device, with a message naming the entry point, and
+    an empty state (n == 0) succeeds without a launch.  Every pointer is fake: none of these calls may dereference one."""
+    import ctypes as C
+    L = lib.load()
+    P, MIS = 16, 8                                               # a fake device pointer, and a misaligned one
+    tab = lambda name: C.byref(lib.tableau(name))
+
+    def refused(rc, fn, msg):
+        assert rc != 0 and L.tdq_last_error().decode() == "%s: %s" % (fn, msg)
+
+    def ks(S, missing=()):                                       # slots k_0..k_S, NULL where listed
+        return lib.ptr_array([None if j in missing else P for j in range(S + 1)])
+
+    def emptied(name, row, err=False, mid=False):                # a tableau with one row (and the weights) cleared
+        t = lib.tableau(name)
+        for j in range(17):
+            if row is not None:
+                if row < t.n_stages:
+                    t.beta[row][j] = 0.0
+                else:
+                    t.c_sol[j] = 0.0
+            if err and j < t.n_stages:
+                t.c_err[j] = 0.0
+            if mid:
+                t.c_mid[j] = 0.0
+        return C.byref(t)
+
+    # tdq_stage_combine(ctrl, tab, dtype, row, y_out, y0, k, n, stream)
+    sc, fn = L.tdq_stage_combine, "tdq_stage_combine"
+    refused(sc(None, tab("dopri5"), 0, 2, P, P, ks(6), 4096, None), fn, "null argument")
+    refused(sc(P, None, 0, 2, P, P, ks(6), 4096, None), fn, "null argument")
+    refused(sc(P, tab("dopri5"), 0, 2, P, P, None, 4096, None), fn, "null argument")
+    for row in (-1, 7):
+        refused(sc(P, tab("dopri5"), 0, row, P, P, ks(6), 4096, None), fn, "row out of range")
+    refused(sc(P, emptied("dopri5", 1), 0, 1, P, P, ks(6), 4096, None), fn, "empty tableau row")
+    refused(sc(P, tab("dopri5"), 0, 2, P, P, ks(6, {1}), 4096, None), fn, "missing stage slot for a non-zero tableau entry")
+    refused(sc(P, tab("dopri5"), 0, 2, P, P, ks(6, {1}), 0, None), fn, "missing stage slot for a non-zero tableau entry")
+    for name, S in (("dopri5", 6), ("dopri8", 13), ("tsit5", 6)):
+        for row in range(S + 1):
+            assert sc(P, tab(name), 0, row, P, P, ks(S), 0, None) == 0
+    assert sc(P, tab("dopri5"), 1, 3, MIS, None, ks(6, {0}), 0, None) == 0     # k_0 may come from the control block
+
+    # tdq_stage_combine_final(ctrl, tab, dtype, y1_out, err_out, y0, k, n, stream)
+    sf, fn = L.tdq_stage_combine_final, "tdq_stage_combine_final"
+    refused(sf(None, tab("dopri5"), 0, P, P, P, ks(6), 4096, None), fn, "null argument")
+    refused(sf(P, tab("dopri5"), 0, P, None, P, ks(6), 4096, None), fn, "null argument")
+    refused(sf(P, tab("dopri5"), 0, P, P, P, ks(6, {3}), 4096, None), fn, "missing stage slot for a non-zero tableau entry")
+    refused(sf(P, tab("tsit5"), 0, P, P, P, ks(6, {6}), 4096, None), fn, "missing stage slot for a non-zero tableau entry")
+    refused(sf(P, emptied("bosh3", 2, err=True), 0, P, P, P, ks(3), 4096, None), fn, "empty tableau row")
+    assert sf(P, tab("dopri5"), 0, P, P, P, ks(6, {6}), 0, None) == 0          # FSAL: k_S is not read
+    for name, S in (("dopri8", 13), ("tsit5", 6), ("bosh3", 3), ("fehlberg2", 2), ("adaptive_heun", 1)):
+        assert sf(P, tab(name), 1, P, P, P, ks(S), 0, None) == 0
+
+    # tdq_linear_stage(ctrl, tab, dtype, row, k_out, y1_out, err_out, y0, k, planes, width, n, stream)
+    ls, fn = L.tdq_linear_stage, "tdq_linear_stage"
+    shape, fused = "the fused linear field is float32, width 128", "unsupported number of stage terms for the fused row"
+    y1msg = "y1_out / err_out are given for, and only for, the row that yields y1 of an FSAL tableau"
+    missing = "missing stage slot for a non-zero tableau entry"
+    refused(ls(None, tab("dopri5"), 0, 2, P, None, None, P, ks(6), P, 128, 1280, None), fn, "null argument")
+    refused(ls(P, tab("dopri5"), 0, 2, P, None, None, P, ks(6), None, 128, 1280, None), fn, "null argument")
+    refused(ls(P, tab("dopri5"), 1, 2, P, None, None, P, ks(6), P, 128, 1280, None), fn, shape)
+    refused(ls(P, tab("dopri5"), 0, 2, P, None, None, P, ks(6), P, 64, 1280, None), fn, shape)
+    refused(ls(P, tab("dopri5"), 0, 2, P, None, None, P, ks(6), P, 128, 1281, None), fn,
+            "state size is not a multiple of the field width")
+    for row in (-1, 6):
+        refused(ls(P, tab("dopri5"), 0, row, P, None, None, P, ks(6), P, 128, 1280, None), fn, "row out of range")
+    refused(ls(P, tab("dopri5"), 0, 2, P, P, P, P, ks(6), P, 128, 1280, None), fn, y1msg)
+    refused(ls(P, tab("dopri5"), 0, 5, P, None, None, P, ks(6), P, 128, 1280, None), fn, y1msg)
+    refused(ls(P, tab("tsit5"), 0, 5, P, P, P, P, ks(6), P, 128, 1280, None), fn, y1msg)   # not FSAL: no such row
+    refused(ls(P, tab("dopri8"), 0, 11, P, None, None, P, ks(13), P, 128, 1280, None), fn, fused)
+    refused(ls(P, tab("dopri8"), 0, 12, P, P, P, P, ks(13), P, 128, 1280, None), fn, fused)
+    # the union of dopri8's last row is k_0, k_5..k_12: a missing slot among the first eight is reported as such, the
+    # ninth term is refused for its count first
+    refused(ls(P, tab("dopri8"), 0, 12, P, P, P, P, ks(13, {5}), P, 128, 1280, None), fn, missing)
+    refused(ls(P, tab("dopri8"), 0, 12, P, P, P, P, ks(13, {12}), P, 128, 1280, None), fn, fused)
+    refused(ls(P, tab("dopri8"), 0, 4, P, None, None, P, ks(13, {3}), P, 128, 1280, None), fn, missing)
+    refused(ls(P, tab("dopri5"), 0, 2, P, None, None, P, ks(6, {1}), P, 128, 1280, None), fn, missing)
+    refused(ls(P, tab("dopri5"), 0, 5, P, P, P, P, ks(6, {2}), P, 128, 1280, None), fn, missing)
+    refused(ls(P, emptied("bosh3", 1), 0, 1, P, None, None, P, ks(3), P, 128, 1280, None), fn, fused)
+    refused(ls(P, emptied("bosh3", 2, err=True), 0, 2, P, P, P, P, ks(3), P, 128, 1280, None), fn, "empty tableau row")
+    refused(ls(P, tab("dopri5"), 0, 2, MIS, None, None, P, ks(6), P, 128, 1280, None), fn, "operands must be 16-byte aligned")
+    refused(ls(P, tab("dopri5"), 0, 2, P, None, None, P, lib.ptr_array([P, P, MIS] + [P] * 4), P, 128, 1280, None), fn,
+            "operands must be 16-byte aligned")
+    for row in range(5):
+        assert ls(P, tab("dopri5"), 0, row, P, None, None, None, ks(6, {0}), P, 128, 0, None) == 0
+    assert ls(P, tab("dopri5"), 0, 5, P, P, P, P, ks(6), P, 128, 0, None) == 0
+    assert ls(P, tab("bosh3"), 0, 2, P, P, P, P, ks(3), P, 128, 0, None) == 0
+
+    # tdq_interp_fit_eval(ctrl, tab, dtype, y1, k, coeff, solution, n, stream)
+    fe, fn = L.tdq_interp_fit_eval, "tdq_interp_fit_eval"
+    co = lib.ptr_array([P] * 5)
+    refused(fe(None, tab("dopri5"), 0, P, ks(6), co, P, 4096, None), fn, "null argument")
+    refused(fe(P, tab("dopri5"), 0, P, ks(6), co, None, 4096, None), fn, "null argument")
+    refused(fe(P, emptied("dopri5", None, mid=True), 0, P, ks(6), co, P, 4096, None), fn, "tableau has no mid-point weights")
+    refused(fe(P, tab("dopri5"), 0, P, ks(6, {6}), co, P, 4096, None), fn, "k_S is required")
+    refused(fe(P, tab("dopri5"), 0, P, ks(6, {2}), co, P, 4096, None), fn, "missing stage slot for a non-zero mid-point weight")
+    refused(fe(P, tab("dopri5"), 0, P, ks(6, {1}), lib.ptr_array([P, P, None, P, P]), P, 4096, None), fn,
+            "five coefficient buffers are required")
+    for name, S in (("dopri5", 6), ("dopri8", 13), ("tsit5", 6), ("bosh3", 3)):
+        assert fe(P, tab(name), 1, P, ks(S, {0}), co, P, 0, None) == 0
+        assert fe(P, tab(name), 0, P, ks(S), None, P, 0, None) == 0
+
+    # tdq_rk4_stage(dtype, which, y_out, y0, k1, k2, k3, k4, dt, step, n, stream)
+    rk, fn = L.tdq_rk4_stage, "tdq_rk4_stage"
+    refused(rk(0, 1, None, P, P, P, P, P, P, None, 4096, None), fn, "null argument")
+    refused(rk(0, 1, P, P, P, P, P, P, None, None, 4096, None), fn, "null argument")
+    for which in (0, 10):
+        refused(rk(0, which, P, P, P, P, P, P, P, None, 4096, None), fn, "which must be 1..9")
+    refused(rk(0, 1, P, P, None, P, P, P, P, None, 4096, None), fn, "k1 required")
+    refused(rk(0, 2, P, P, P, None, P, P, P, None, 4096, None), fn, "k2 required")
+    refused(rk(0, 9, P, P, P, P, None, P, P, None, 4096, None), fn, "k3 required")
+    refused(rk(0, 4, P, P, P, P, P, None, P, None, 4096, None), fn, "k4 required")
+    for which in range(1, 10):
+        assert rk(which % 2, which, P, P, P, P, P, P, P, None, 0, None) == 0
+
+    # tdq_fixed_final_emit(dtype, which, y0, k1..k4, dt, solution, rec_begin, out_idx, mode, slope, step, tstage_all,
+    # tstage_cur, n_steps, n, stream): it launches even for n == 0 (its last block advances the step counter), so only
+    # the refusals are checked here
+    ff, fn = L.tdq_fixed_final_emit, "tdq_fixed_final_emit"
+    tail = (P, P, P, P, P, P, P, P, 4)
+    refused(ff(0, 4, None, P, P, P, P, P, *tail, 4096, None), fn, "null argument")
+    refused(ff(0, 4, P, P, P, P, P, P, P, P, P, P, P, P, P, None, 4, 4096, None), fn, "null argument")
+    for which in (1, 6, 8, 10):
+        refused(ff(0, which, P, P, P, P, P, P, *tail, 4096, None), fn, "which must be a final expression (4, 5, 7, 9)")
+    refused(ff(0, 5, P, None, P, P, P, P, *tail, 4096, None), fn, "missing stage slot")
+    refused(ff(0, 7, P, P, None, P, P, P, *tail, 4096, None), fn, "missing stage slot")
+    refused(ff(0, 9, P, P, P, None, P, P, *tail, 4096, None), fn, "missing stage slot")
+    refused(ff(0, 4, P, P, P, P, None, P, *tail, 4096, None), fn, "missing stage slot")
+
+    # tdq_lincomb(dtype, out, base, x, coefs, n_terms, n, stream)
+    lc, fn = L.tdq_lincomb, "tdq_lincomb"
+    cf = (C.c_double * 17)()
+    refused(lc(0, None, None, lib.ptr_array([P] * 17), cf, 3, 4096, None), fn, "null argument")
+    refused(lc(0, P, None, lib.ptr_array([P] * 17), None, 3, 4096, None), fn, "null argument")
+    for nt in (0, 18):
+        refused(lc(0, P, None, lib.ptr_array([P] * 18), cf, nt, 4096, None), fn, "n_terms out of range")
+    refused(lc(0, P, P, lib.ptr_array([P, None, P]), cf, 3, 4096, None), fn, "null term")
+    for nt in (1, 17):
+        assert lc(nt % 2, P, None, lib.ptr_array([P] * 17), cf, nt, 0, None) == 0

@@ -1,8 +1,10 @@
-// tdq_api.cu -- library-level entry points of the C ABI: errors, device query, mailbox, tableaus.
+// tdq_api.cu -- library-level entry points of the C ABI: errors, device query, mailbox, tableaus; and the host helpers
+// every launcher shares (tdq_shape.cuh).
 #include <stdarg.h>
 #include <stdio.h>
 
 #include "tdq_common.cuh"
+#include "tdq_shape.cuh"
 
 static thread_local char g_err[512] = "";
 
@@ -11,6 +13,43 @@ void tdq_set_error(const char *fmt, ...) {
     va_start(ap, fmt);
     vsnprintf(g_err, sizeof(g_err), fmt, ap);
     va_end(ap);
+}
+
+int tdq_sm_count() {
+    static int sms = 0;
+    if (sms == 0) {
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess ||
+            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
+            sms = 132;
+    }
+    return sms;
+}
+
+void tdq_shape_from_tableau(const tdq_tableau *tab, TdqHostShape *h) {
+    memset(h, 0, sizeof(*h));
+    const int S = tab->n_stages;
+    h->n_stages = S;
+    h->fsal = tab->fsal;
+    for (int i = 0; i < S; ++i) {
+        int m = 0;
+        for (int j = 0; j <= i; ++j)
+            if (tab->beta[i][j] != 0.0) h->row_idx[i][m++] = j;
+        h->row_nnz[i] = m;
+    }
+    int m = 0;
+    for (int j = 0; j <= S; ++j)
+        if (tab->c_sol[j] != 0.0) h->row_idx[S][m++] = j;
+    h->row_nnz[S] = m;
+    m = 0;
+    for (int j = 0; j <= S; ++j)
+        if (tab->c_err[j] != 0.0) h->err_idx[m++] = j;
+    h->err_nnz = m;
+    m = 0;
+    for (int j = 0; j <= S; ++j)
+        if (tab->c_mid[j] != 0.0) h->mid_idx[m++] = j;
+    h->mid_nnz = m;
+    h->valid = 1;
 }
 
 // ------------------------------------------------------------------------------------------------

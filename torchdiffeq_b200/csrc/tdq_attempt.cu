@@ -390,11 +390,7 @@ int launch_attempt(TdqCtrl *c, const float *y0, const float *k0, const AttOut &o
                    double *norm_out, int store_always, size_t n_rows, cudaStream_t st) {
     auto kern = k_linear_attempt<S, RM, EM>;
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM) != cudaSuccess) return -2;
-    size_t grid = (n_rows + AT_ROWS - 1) / AT_ROWS;
-    const size_t cap = (size_t)tdq_sm_count();
-    if (grid > cap) grid = cap;
-    if (grid == 0) grid = 1;
-    kern<<<(unsigned)grid, AT_THREADS, AT_SMEM, st>>>(c, y0, k0, out, wt, partials, norm_out, store_always, n_rows);
+    kern<<<tdq_grid(n_rows, AT_ROWS, 1), AT_THREADS, AT_SMEM, st>>>(c, y0, k0, out, wt, partials, norm_out, store_always, n_rows);
     return 0;
 }
 

@@ -492,27 +492,22 @@ int tdq_ctrl_init(void *ctrl_dev, const tdq_tableau *tab, const tdq_options *opt
     h.fsal = tab->fsal ? 1 : 0;
     h.ratio_f64 = (opt->ratio_f64 || !f32) ? 1 : 0;
     h.n_out = n_out;
-    for (int i = 0; i < S; ++i) {
-        h.alpha[i] = rT(tab->alpha[i]);
-        int m = 0;
-        for (int j = 0; j <= i; ++j)
-            if (tab->beta[i][j] != 0.0) { h.row_idx[i][m] = j; h.beta[i][m] = rT(tab->beta[i][j]); ++m; }
-        h.row_nnz[i] = m;
+    TdqHostShape hs;
+    tdq_shape_from_tableau(tab, &hs);
+    static_assert(sizeof(h.row_idx) == sizeof(hs.row_idx) && sizeof(h.err_idx) == sizeof(hs.err_idx), "index layouts");
+    memcpy(h.row_nnz, hs.row_nnz, sizeof(h.row_nnz));
+    memcpy(h.row_idx, hs.row_idx, sizeof(h.row_idx));
+    memcpy(h.err_idx, hs.err_idx, sizeof(h.err_idx));
+    memcpy(h.mid_idx, hs.mid_idx, sizeof(h.mid_idx));
+    h.err_nnz = hs.err_nnz;
+    h.mid_nnz = hs.mid_nnz;
+    for (int i = 0; i < S; ++i) h.alpha[i] = rT(tab->alpha[i]);
+    for (int i = 0; i <= S; ++i) {
+        const double *w = i < S ? tab->beta[i] : tab->c_sol;           // row S is the c_sol row
+        for (int m = 0; m < hs.row_nnz[i]; ++m) h.beta[i][m] = rT(w[hs.row_idx[i][m]]);
     }
-    {
-        int m = 0;
-        for (int j = 0; j <= S; ++j)
-            if (tab->c_sol[j] != 0.0) { h.row_idx[S][m] = j; h.beta[S][m] = rT(tab->c_sol[j]); ++m; }
-        h.row_nnz[S] = m;
-        m = 0;
-        for (int j = 0; j <= S; ++j)
-            if (tab->c_err[j] != 0.0) { h.err_idx[m] = j; h.c_err[m] = rT(tab->c_err[j]); ++m; }
-        h.err_nnz = m;
-        m = 0;
-        for (int j = 0; j <= S; ++j)
-            if (tab->c_mid[j] != 0.0) { h.mid_idx[m] = j; h.c_mid[m] = rT(tab->c_mid[j]); ++m; }
-        h.mid_nnz = m;
-    }
+    for (int m = 0; m < hs.err_nnz; ++m) h.c_err[m] = rT(tab->c_err[hs.err_idx[m]]);
+    for (int m = 0; m < hs.mid_nnz; ++m) h.c_mid[m] = rT(tab->c_mid[hs.mid_idx[m]]);
     h.rtol = opt->rtol;
     h.atol = opt->atol;
     h.min_step = opt->min_step;

@@ -80,20 +80,12 @@ k_rk4(T *__restrict__ out, const T *__restrict__ y0, const T *__restrict__ k1, c
 template <typename T, int WHICH>
 void launch_rk4(void *out, const void *y0, const void *k1, const void *k2, const void *k3, const void *k4,
                 const void *dt, const int64_t *step, size_t n, bool vec, cudaStream_t st) {
-    if (vec) {
-        const size_t nvec = n / Vec<T>::N;
-        size_t blocks = (nvec + kThreads - 1) / kThreads;
-        if (blocks == 0) blocks = 1;
-        k_rk4<T, WHICH, true><<<(unsigned)blocks, kThreads, 0, st>>>((T *)out, (const T *)y0, (const T *)k1,
-                                                                      (const T *)k2, (const T *)k3, (const T *)k4,
-                                                                      (const T *)dt, step, n);
+    if (vec) {   // one vector per thread, not grid-stride: no cap
+        k_rk4<T, WHICH, true><<<tdq_grid(n / Vec<T>::N, kThreads, 0), kThreads, 0, st>>>(
+            (T *)out, (const T *)y0, (const T *)k1, (const T *)k2, (const T *)k3, (const T *)k4, (const T *)dt, step, n);
     } else {
-        size_t blocks = (n + kThreads - 1) / kThreads;
-        if (blocks == 0) blocks = 1;
-        if (blocks > 132 * 16) blocks = 132 * 16;
-        k_rk4<T, WHICH, false><<<(unsigned)blocks, kThreads, 0, st>>>((T *)out, (const T *)y0, (const T *)k1,
-                                                                       (const T *)k2, (const T *)k3, (const T *)k4,
-                                                                       (const T *)dt, step, n);
+        k_rk4<T, WHICH, false><<<tdq_grid(n, kThreads, 16), kThreads, 0, st>>>(
+            (T *)out, (const T *)y0, (const T *)k1, (const T *)k2, (const T *)k3, (const T *)k4, (const T *)dt, step, n);
     }
 }
 
@@ -256,17 +248,10 @@ int tdq_rk4_stage(int32_t dtype, int32_t which, void *y_out, const void *y0, con
     bool vec = tdq_aligned16(y_out) && tdq_aligned16(y0) && (!nA || tdq_aligned16(k1)) && (!nB || tdq_aligned16(k2)) &&
                (!nC || tdq_aligned16(k3)) && (!nD || tdq_aligned16(k4));
     cudaStream_t st = (cudaStream_t)stream;
-    switch (which) {
-        case 1: TDQ_DISPATCH_T(dtype, (launch_rk4<T, 1>(y_out, y0, k1, k2, k3, k4, dt_dev, step_dev, n, vec, st))); break;
-        case 2: TDQ_DISPATCH_T(dtype, (launch_rk4<T, 2>(y_out, y0, k1, k2, k3, k4, dt_dev, step_dev, n, vec, st))); break;
-        case 3: TDQ_DISPATCH_T(dtype, (launch_rk4<T, 3>(y_out, y0, k1, k2, k3, k4, dt_dev, step_dev, n, vec, st))); break;
-        case 4: TDQ_DISPATCH_T(dtype, (launch_rk4<T, 4>(y_out, y0, k1, k2, k3, k4, dt_dev, step_dev, n, vec, st))); break;
-        case 5: TDQ_DISPATCH_T(dtype, (launch_rk4<T, 5>(y_out, y0, k1, k2, k3, k4, dt_dev, step_dev, n, vec, st))); break;
-        case 6: TDQ_DISPATCH_T(dtype, (launch_rk4<T, 6>(y_out, y0, k1, k2, k3, k4, dt_dev, step_dev, n, vec, st))); break;
-        case 7: TDQ_DISPATCH_T(dtype, (launch_rk4<T, 7>(y_out, y0, k1, k2, k3, k4, dt_dev, step_dev, n, vec, st))); break;
-        case 8: TDQ_DISPATCH_T(dtype, (launch_rk4<T, 8>(y_out, y0, k1, k2, k3, k4, dt_dev, step_dev, n, vec, st))); break;
-        default: TDQ_DISPATCH_T(dtype, (launch_rk4<T, 9>(y_out, y0, k1, k2, k3, k4, dt_dev, step_dev, n, vec, st))); break;
-    }
+    TDQ_DISPATCH_T(dtype, tdq_dispatch(TdqRange<1, 9>{}, which, [&](auto W) {
+                       launch_rk4<T, W>(y_out, y0, k1, k2, k3, k4, dt_dev, step_dev, n, vec, st);
+                       return 0;
+                   }));
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
 }
@@ -278,10 +263,7 @@ int tdq_fixed_emit(int32_t dtype, void *y0, const void *y1, void *solution, cons
                     tstage_all_dev && tstage_cur_dev,
                 "null argument");
     cudaStream_t st = (cudaStream_t)stream;
-    size_t blocks = (n + kThreads - 1) / kThreads;
-    if (blocks == 0) blocks = 1;
-    if (blocks > 132 * 8) blocks = 132 * 8;
-    TDQ_DISPATCH_T(dtype, (k_fixed_emit<T><<<(unsigned)blocks, kThreads, 0, st>>>(
+    TDQ_DISPATCH_T(dtype, (k_fixed_emit<T><<<tdq_grid(n, kThreads, 8), kThreads, 0, st>>>(
                                (T *)y0, (const T *)y1, (T *)solution, rec_begin_dev, out_idx_dev, mode_dev,
                                (const T *)slope_dev, step_dev, (const unsigned char *)tstage_all_dev,
                                (unsigned char *)tstage_cur_dev, n_steps, n)));
@@ -300,18 +282,13 @@ int tdq_fixed_final_emit(int32_t dtype, int32_t which, void *y0, const void *k1,
     TDQ_REQUIRE(k1 && (which == 5 || which == 9 || k2) && (which != 4 && which != 9 || k3) && (which != 4 || k4),
                 "missing stage slot");
     cudaStream_t st = (cudaStream_t)stream;
-    size_t blocks = (n + kThreads - 1) / kThreads;
-    if (blocks == 0) blocks = 1;
-    if (blocks > 132 * 8) blocks = 132 * 8;
-#define TDQ_FE(W) TDQ_DISPATCH_T(dtype, (k_final_emit<T, W><<<(unsigned)blocks, kThreads, 0, st>>>(                    \
-        (T *)y0, (const T *)k1, (const T *)k2, (const T *)k3, (const T *)k4, (const T *)dt_dev, (T *)solution,              \
-        rec_begin_dev, out_idx_dev, mode_dev, (const T *)slope_dev, step_dev, (const unsigned char *)tstage_all_dev,        \
-        (unsigned char *)tstage_cur_dev, n_steps, n)))
-    if (which == 4) TDQ_FE(4);
-    else if (which == 5) TDQ_FE(5);
-    else if (which == 7) TDQ_FE(7);
-    else TDQ_FE(9);
-#undef TDQ_FE
+    TDQ_DISPATCH_T(dtype, tdq_dispatch(std::integer_sequence<int, 4, 5, 7, 9>{}, which, [&](auto W) {
+                       k_final_emit<T, W><<<tdq_grid(n, kThreads, 8), kThreads, 0, st>>>(
+                           (T *)y0, (const T *)k1, (const T *)k2, (const T *)k3, (const T *)k4, (const T *)dt_dev,
+                           (T *)solution, rec_begin_dev, out_idx_dev, mode_dev, (const T *)slope_dev, step_dev,
+                           (const unsigned char *)tstage_all_dev, (unsigned char *)tstage_cur_dev, n_steps, n);
+                       return 0;
+                   }));
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
 }
@@ -328,9 +305,7 @@ int tdq_lincomb(int32_t dtype, void *out, const void *base, const void *const *x
         a.c[m] = coefs[m];
     }
     if (n == 0) return TDQ_OK;
-    size_t blocks = (n + kThreads - 1) / kThreads;
-    if (blocks > 132 * 8) blocks = 132 * 8;
-    TDQ_DISPATCH_T(dtype, (k_lincomb<T><<<(unsigned)blocks, kThreads, 0, (cudaStream_t)stream>>>(
+    TDQ_DISPATCH_T(dtype, (k_lincomb<T><<<tdq_grid(n, kThreads, 8), kThreads, 0, (cudaStream_t)stream>>>(
                                (T *)out, (const T *)base, a, n_terms, n)));
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
@@ -342,9 +317,7 @@ int tdq_fixed_emit_cubic(int32_t dtype, const void *y0, const void *y1, const vo
     TDQ_REQUIRE(y0 && y1 && f0 && f1 && solution && out_idx_dev && coef_dev, "null argument");
     TDQ_REQUIRE(rec_lo >= 0 && rec_hi >= rec_lo, "bad record range");
     if (n == 0 || rec_hi == rec_lo) return TDQ_OK;
-    size_t blocks = (n + kThreads - 1) / kThreads;
-    if (blocks > 132 * 8) blocks = 132 * 8;
-    TDQ_DISPATCH_T(dtype, (k_fixed_emit_cubic<T><<<(unsigned)blocks, kThreads, 0, (cudaStream_t)stream>>>(
+    TDQ_DISPATCH_T(dtype, (k_fixed_emit_cubic<T><<<tdq_grid(n, kThreads, 8), kThreads, 0, (cudaStream_t)stream>>>(
                                (const T *)y0, (const T *)y1, (const T *)f0, (const T *)f1, (T *)solution, out_idx_dev,
                                (const T *)coef_dev, rec_lo, rec_hi, n)));
     TDQ_CHECK_CUDA(cudaGetLastError());
@@ -367,10 +340,7 @@ int tdq_pack_segments(int32_t dtype, void *dst, const void *const *src, const in
         if (lens[i] > max_len) max_len = lens[i];
     }
     if (max_len == 0) return TDQ_OK;
-    size_t bx = (size_t)((max_len + kThreads * 4 - 1) / (kThreads * 4));
-    if (bx == 0) bx = 1;
-    if (bx > 132 * 8) bx = 132 * 8;
-    dim3 grid((unsigned)bx, (unsigned)n_src);
+    dim3 grid(tdq_grid((size_t)max_len, kThreads * 4, 8), (unsigned)n_src);
     TDQ_DISPATCH_T(dtype, (k_pack<T><<<grid, kThreads, 0, (cudaStream_t)stream>>>((T *)dst, a, n_src)));
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;

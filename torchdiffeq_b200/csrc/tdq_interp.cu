@@ -129,33 +129,18 @@ k_fit_eval(const TdqCtrl *__restrict__ c, const T *__restrict__ y1p, const T *__
 template <typename T, int NK>
 int launch_fit(const TdqCtrl *c, const void *y1, const void *kS, const KPtrs &kmid, void *const *coeff, void *solution,
                size_t n, bool vec, cudaStream_t st) {
-    size_t blocks = ((vec ? n / Vec<T>::N : n) + kThreads - 1) / kThreads;
     // persistent, two blocks per SM: 64 KB of loads in flight per SM saturate HBM when the fit runs, and the usual no-op
     // launch (73 of 74 attempts of configs[1]) costs a few hundred blocks' worth of scheduling less
-    const size_t cap = (size_t)tdq_sm_count() * 2;
-    if (blocks > cap) blocks = cap;
-    if (blocks == 0) blocks = 1;
+    const unsigned blocks = tdq_grid(vec ? n / Vec<T>::N : n, kThreads, 2);
     T *co[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
     if (coeff) for (int i = 0; i < 5; ++i) co[i] = (T *)coeff[i];
-#define TDQ_L(V_, S_) k_fit_eval<T, NK, V_, S_><<<(unsigned)blocks, kThreads, 0, st>>>( \
-        c, (const T *)y1, (const T *)kS, kmid, co[0], co[1], co[2], co[3], co[4], (T *)solution, n)
-    if (vec) { if (coeff) TDQ_L(true, true); else TDQ_L(true, false); }
-    else     { if (coeff) TDQ_L(false, true); else TDQ_L(false, false); }
-#undef TDQ_L
-    return 0;
-}
-
-template <typename T>
-int dispatch_fit(int nk, const TdqCtrl *c, const void *y1, const void *kS, const KPtrs &kmid, void *const *coeff,
-                 void *solution, size_t n, bool vec, cudaStream_t st) {
-    switch (nk) {
-#define TDQ_CASE(N) case N: return launch_fit<T, N>(c, y1, kS, kmid, coeff, solution, n, vec, st);
-        TDQ_CASE(1) TDQ_CASE(2) TDQ_CASE(3) TDQ_CASE(4) TDQ_CASE(5) TDQ_CASE(6) TDQ_CASE(7) TDQ_CASE(8)
-        TDQ_CASE(9) TDQ_CASE(10) TDQ_CASE(11) TDQ_CASE(12) TDQ_CASE(13) TDQ_CASE(14) TDQ_CASE(15)
-        TDQ_CASE(16) TDQ_CASE(17)
-#undef TDQ_CASE
-    }
-    return -1;
+    return tdq_dispatch(TdqBool{}, vec, [&](auto V) {
+        return tdq_dispatch(TdqBool{}, coeff != nullptr, [&](auto S) {
+            k_fit_eval<T, NK, V, S><<<blocks, kThreads, 0, st>>>(c, (const T *)y1, (const T *)kS, kmid, co[0], co[1], co[2],
+                                                                 co[3], co[4], (T *)solution, n);
+            return 0;
+        });
+    });
 }
 
 // p(x) for a caller-supplied abscissa x (float64, cast to T like interp.py:39-40); used by dense-output
@@ -201,9 +186,8 @@ int tdq_initial_step_probe(void *ctrl_dev, int32_t dtype, void *y_probe, const v
                            void *stream) {
     TDQ_REQUIRE(ctrl_dev && y_probe, "null argument");
     if (n == 0) return TDQ_OK;
-    size_t blocks = (n + kThreads - 1) / kThreads;
-    if (blocks > (size_t)tdq_sm_count() * 16) blocks = (size_t)tdq_sm_count() * 16;
-    TDQ_DISPATCH_T(dtype, (k_probe<T><<<(unsigned)blocks, kThreads, 0, (cudaStream_t)stream>>>(
+    const unsigned blocks = tdq_grid(n, kThreads, 16);
+    TDQ_DISPATCH_T(dtype, (k_probe<T><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(
                                (const TdqCtrl *)ctrl_dev, (T *)y_probe, (const T *)y0, (const T *)f0, n)));
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
@@ -219,15 +203,10 @@ int tdq_interp_fit_eval(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, c
     TDQ_REQUIRE(nk >= 1, "tableau has no mid-point weights");
     TDQ_REQUIRE(k[S] != nullptr, "k_S is required");
     KPtrs kmid;
-    memset(&kmid, 0, sizeof(kmid));
     bool vec = tdq_aligned16(y1) && tdq_aligned16(k[S]) && tdq_aligned16(solution) &&
                ((n * (dtype == TDQ_F32 ? 4 : 8)) % 16 == 0);
-    for (int m = 0; m < nk; ++m) {
-        const int j = hs.mid_idx[m];
-        kmid.p[m] = k[j];
-        TDQ_REQUIRE(kmid.p[m] != nullptr || j == 0, "missing stage slot for a non-zero mid-point weight");
-        vec = vec && tdq_aligned16(kmid.p[m]);
-    }
+    TDQ_REQUIRE(tdq_plan_terms(hs.mid_idx, nk, k, kmid.p, vec) == TDQ_PLAN_OK,
+                "missing stage slot for a non-zero mid-point weight");
     if (coeff)
         for (int i = 0; i < 5; ++i) {
             TDQ_REQUIRE(coeff[i] != nullptr, "five coefficient buffers are required");
@@ -235,8 +214,10 @@ int tdq_interp_fit_eval(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, c
         }
     if (n == 0) return TDQ_OK;
     int rc = -1;
-    TDQ_DISPATCH_T(dtype, rc = dispatch_fit<T>(nk, (const TdqCtrl *)ctrl_dev, y1, k[S], kmid, coeff, solution, n, vec,
-                                               (cudaStream_t)stream));
+    TDQ_DISPATCH_T(dtype, rc = tdq_dispatch(TdqRange<1, TDQ_MAX_K>{}, nk, [&](auto NK) {
+                       return launch_fit<T, NK>((const TdqCtrl *)ctrl_dev, y1, k[S], kmid, coeff, solution, n, vec,
+                                                (cudaStream_t)stream);
+                   }));
     TDQ_REQUIRE(rc == 0, "unsupported number of mid-point terms");
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
@@ -246,9 +227,8 @@ int tdq_poly_eval(int32_t dtype, const void *const *coeff, double x, void *out, 
     TDQ_REQUIRE(coeff && out, "null argument");
     for (int i = 0; i < 5; ++i) TDQ_REQUIRE(coeff[i] != nullptr, "five coefficient buffers are required");
     if (n == 0) return TDQ_OK;
-    size_t blocks = (n + kThreads - 1) / kThreads;
-    if (blocks > (size_t)tdq_sm_count() * 8) blocks = (size_t)tdq_sm_count() * 8;
-    TDQ_DISPATCH_T(dtype, (k_poly_eval<T><<<(unsigned)blocks, kThreads, 0, (cudaStream_t)stream>>>(
+    const unsigned blocks = tdq_grid(n, kThreads, 8);
+    TDQ_DISPATCH_T(dtype, (k_poly_eval<T><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(
                                (const T *)coeff[0], (const T *)coeff[1], (const T *)coeff[2], (const T *)coeff[3],
                                (const T *)coeff[4], (T *)out, x, n)));
     TDQ_CHECK_CUDA(cudaGetLastError());
@@ -260,9 +240,8 @@ int tdq_interp_eval_at(void *ctrl_dev, int32_t dtype, const void *const *coeff, 
     TDQ_REQUIRE(ctrl_dev && coeff && out && t_dev, "null argument");
     for (int i = 0; i < 5; ++i) TDQ_REQUIRE(coeff[i] != nullptr, "five coefficient buffers are required");
     if (n == 0) return TDQ_OK;
-    size_t blocks = (n + kThreads - 1) / kThreads;
-    if (blocks > (size_t)tdq_sm_count() * 8) blocks = (size_t)tdq_sm_count() * 8;
-    TDQ_DISPATCH_T(dtype, (k_interp_eval_at<T><<<(unsigned)blocks, kThreads, 0, (cudaStream_t)stream>>>(
+    const unsigned blocks = tdq_grid(n, kThreads, 8);
+    TDQ_DISPATCH_T(dtype, (k_interp_eval_at<T><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(
                                (const TdqCtrl *)ctrl_dev, (const T *)coeff[0], (const T *)coeff[1], (const T *)coeff[2],
                                (const T *)coeff[3], (const T *)coeff[4], (T *)out, t_dev, n)));
     TDQ_CHECK_CUDA(cudaGetLastError());

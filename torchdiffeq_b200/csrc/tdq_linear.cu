@@ -152,24 +152,9 @@ int launch_linear(const TdqCtrl *c, int row, const float *y0, const LinK &kp, co
     auto kern = k_linear_stage<NU, MODE>;
     // per function AND per device; idempotent and cheap, so set on every launch (legal during stream capture)
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L_SMEM) != cudaSuccess) return -2;
-    const size_t tiles = (n_rows + TILE_ROWS - 1) / TILE_ROWS;
-    size_t grid = (tiles + L_GROUPS - 1) / L_GROUPS;
-    const size_t cap = (size_t)tdq_sm_count();
-    if (grid > cap) grid = cap;
-    if (grid == 0) grid = 1;
-    kern<<<(unsigned)grid, L_THREADS, L_SMEM, st>>>(c, row, y0, kp, fm, wt, kout, yout, eout, (int)n_rows);
+    const unsigned grid = tdq_grid((n_rows + TILE_ROWS - 1) / TILE_ROWS, L_GROUPS, 1);
+    kern<<<grid, L_THREADS, L_SMEM, st>>>(c, row, y0, kp, fm, wt, kout, yout, eout, (int)n_rows);
     return 0;
-}
-
-template <int MODE>
-int dispatch_linear(int nu, const TdqCtrl *c, int row, const float *y0, const LinK &kp, const LinMap &fm, const uint32_t *wt,
-                    float *kout, float *yout, float *eout, size_t n_rows, cudaStream_t st) {
-    switch (nu) {
-#define TDQ_CASE(N) case N: return launch_linear<N, MODE>(c, row, y0, kp, fm, wt, kout, yout, eout, n_rows, st);
-        TDQ_CASE(1) TDQ_CASE(2) TDQ_CASE(3) TDQ_CASE(4) TDQ_CASE(5) TDQ_CASE(6) TDQ_CASE(7) TDQ_CASE(8)
-#undef TDQ_CASE
-    }
-    return -1;
 }
 
 bool linear_shape_ok(int32_t dtype, int32_t width) { return dtype == TDQ_F32 && width == LD; }
@@ -225,47 +210,29 @@ int tdq_linear_stage(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, int3
                 "y1_out / err_out are given for, and only for, the row that yields y1 of an FSAL tableau");
     LinK kp;
     LinMap fm;
-    memset(&kp, 0, sizeof(kp));
-    memset(&fm, 0xff, sizeof(fm));
+    memset(&fm, 0xff, sizeof(fm));                // the union fills it; a middle row passes it unread
     bool aligned = tdq_aligned16(k_out) && tdq_aligned16(y0) && tdq_aligned16(planes) && tdq_aligned16(y1_out) &&
                    tdq_aligned16(err_out);
-    int nu = 0;
+    int nu = hs.row_nnz[row];
+    TdqPlanStatus plan;
     if (!final_row) {
-        nu = hs.row_nnz[row];
         TDQ_REQUIRE(nu >= 1 && nu <= MAX_TERMS, "unsupported number of stage terms for the fused row");
-        for (int m = 0; m < nu; ++m) {
-            const int j = hs.row_idx[row][m];
-            kp.p[m] = (const float *)k[j];
-            TDQ_REQUIRE(kp.p[m] != nullptr || j == 0, "missing stage slot for a non-zero tableau entry");
-            aligned = aligned && tdq_aligned16(kp.p[m]);
-        }
+        plan = tdq_plan_terms(hs.row_idx[row], nu, k, kp.p, aligned);
     } else {
-        // union of the row's and the error weights' slots, ascending (tdq_stage_combine_final)
-        int used_r[TDQ_MAX_K], used_e[TDQ_MAX_K];
-        for (int j = 0; j < TDQ_MAX_K; ++j) used_r[j] = used_e[j] = -1;
-        for (int m = 0; m < hs.row_nnz[row]; ++m) used_r[hs.row_idx[row][m]] = m;
-        for (int m = 0; m < hs.err_nnz; ++m)
-            if (hs.err_idx[m] <= S - 1) used_e[hs.err_idx[m]] = m;
-        for (int j = 0; j <= S - 1; ++j) {
-            if (used_r[j] < 0 && used_e[j] < 0) continue;
-            TDQ_REQUIRE(nu < MAX_TERMS, "unsupported number of stage terms for the fused row");
-            kp.p[nu] = (const float *)k[j];
-            TDQ_REQUIRE(kp.p[nu] != nullptr || j == 0, "missing stage slot for a non-zero tableau entry");
-            aligned = aligned && tdq_aligned16(kp.p[nu]);
-            fm.rpos[nu] = (signed char)used_r[j];
-            fm.epos[nu] = (signed char)used_e[j];
-            ++nu;
-        }
-        TDQ_REQUIRE(nu >= 1, "empty tableau row");
+        plan = tdq_plan_union(hs, row, S - 1, k, kp.p, fm, nu, aligned);
     }
+    TDQ_REQUIRE(plan != TDQ_PLAN_TOO_MANY, "unsupported number of stage terms for the fused row");
+    TDQ_REQUIRE(plan != TDQ_PLAN_MISSING_SLOT, "missing stage slot for a non-zero tableau entry");
+    TDQ_REQUIRE(nu >= 1, "empty tableau row");
     TDQ_REQUIRE(aligned, "operands must be 16-byte aligned");
     if (n_rows == 0) return TDQ_OK;
-    const int rc = final_row ? dispatch_linear<2>(nu, (const TdqCtrl *)ctrl_dev, row, (const float *)y0, kp, fm,
-                                                  (const uint32_t *)planes, (float *)k_out, (float *)y1_out, (float *)err_out,
-                                                  n_rows, (cudaStream_t)stream)
-                             : dispatch_linear<1>(nu, (const TdqCtrl *)ctrl_dev, row, (const float *)y0, kp, fm,
-                                                  (const uint32_t *)planes, (float *)k_out, nullptr, nullptr, n_rows,
-                                                  (cudaStream_t)stream);
+    const TdqCtrl *c = (const TdqCtrl *)ctrl_dev;
+    const int rc = tdq_dispatch(TdqRange<1, MAX_TERMS>{}, nu, [&](auto NU) {
+        return final_row ? launch_linear<NU, 2>(c, row, (const float *)y0, kp, fm, (const uint32_t *)planes, (float *)k_out,
+                                                (float *)y1_out, (float *)err_out, n_rows, (cudaStream_t)stream)
+                         : launch_linear<NU, 1>(c, row, (const float *)y0, kp, fm, (const uint32_t *)planes, (float *)k_out,
+                                                nullptr, nullptr, n_rows, (cudaStream_t)stream);
+    });
     TDQ_REQUIRE(rc == 0, "launch configuration failed");
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;

@@ -284,34 +284,26 @@ int launch_norm(const TdqCtrl *c, NormArgs &a, bool vec, cudaStream_t st) {
     const bool vtol = a.rtol_v != nullptr;
     const bool multi = a.table != nullptr;
     const bool wq = a.q_out != nullptr;
-    unsigned grid;
-    if (multi) {
-        grid = (unsigned)a.n_parts;
-        const unsigned cap = (unsigned)tdq_sm_count() * 8;
-        if (grid > cap) grid = cap;
-    } else {
-        grid = (unsigned)a.n_parts;
-    }
-    if (grid == 0) grid = 1;
-#define TDQ_L(V_, VT_, M_, WQ_) k_norm<T, MODE, V_, VT_, M_, WQ_><<<grid, kThreads, 0, st>>>(c, a)
-#define TDQ_L3(V_, VT_, M_) do { if (wq && MODE == 0) TDQ_L(V_, VT_, M_, (MODE == 0)); else TDQ_L(V_, VT_, M_, false); } while (0)
-#define TDQ_L2(V_, VT_) do { if (multi) TDQ_L3(V_, VT_, true); else TDQ_L3(V_, VT_, false); } while (0)
-    if (vec) { if (vtol) TDQ_L2(true, true); else TDQ_L2(true, false); }
-    else     { if (vtol) TDQ_L2(false, true); else TDQ_L2(false, false); }
-#undef TDQ_L2
-#undef TDQ_L3
-#undef TDQ_L
-    return 0;
+    // the single-segment grid is its partial count, which single_parts already bounds by kMaxGrid
+    const unsigned grid = multi ? tdq_grid((size_t)a.n_parts, 1, 8) : (unsigned)a.n_parts;
+    return tdq_dispatch(TdqBool{}, vec, [&](auto V) {
+        return tdq_dispatch(TdqBool{}, vtol, [&](auto VT) {
+            return tdq_dispatch(TdqBool{}, multi, [&](auto M) {
+                return tdq_dispatch(TdqBool{}, wq, [&](auto WQ) {       // only the error norm (MODE 0) writes err/tol
+                    k_norm<T, MODE, V, VT, M, WQ && MODE == 0><<<grid, kThreads, 0, st>>>(c, a);
+                    return 0;
+                });
+            });
+        });
+    });
 }
 
 // number of partials (= blocks) of the single-segment path for n elements
 inline int single_parts(size_t n, bool vec, int vn) {
     const size_t units = vec ? n / vn : n;                              // vectors or scalars to distribute
     const size_t per_block = vec ? (size_t)kThreads * 2 : (size_t)kThreads;
-    size_t blocks = (units + per_block - 1) / per_block;
-    if (blocks > (size_t)kMaxGrid) blocks = kMaxGrid;
-    if (blocks < 1) blocks = 1;
-    return (int)blocks;
+    const unsigned blocks = tdq_grid(units, per_block, 0);
+    return blocks > (unsigned)kMaxGrid ? kMaxGrid : (int)blocks;
 }
 
 }  // namespace
@@ -453,10 +445,8 @@ int tdq_scaled_sumsq(void *ctrl_dev, int32_t dtype, const void *x, const void *x
 int tdq_commit_candidates(void *ctrl_dev, int32_t dtype, const void *y1, const void *k_last, size_t n, void *stream) {
     TDQ_REQUIRE(ctrl_dev && y1 && k_last, "null argument");
     if (n == 0) return TDQ_OK;
-    size_t blocks = (n + kThreads - 1) / kThreads;
-    const size_t cap = (size_t)tdq_sm_count() * 8;
-    if (blocks > cap) blocks = cap;
-    TDQ_DISPATCH_T(dtype, (k_commit<T><<<(unsigned)blocks, kThreads, 0, (cudaStream_t)stream>>>(
+    const unsigned blocks = tdq_grid(n, kThreads, 8);
+    TDQ_DISPATCH_T(dtype, (k_commit<T><<<blocks, kThreads, 0, (cudaStream_t)stream>>>(
                                (const TdqCtrl *)ctrl_dev, (const T *)y1, (const T *)k_last, n)));
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;

@@ -102,34 +102,13 @@ int launch_combine(const TdqCtrl *c, int row, void *out, const void *y0, const K
     constexpr int U = kFew ? 4 : 2;
     constexpr int PER_SM = kFew ? 2 : 8;
     if (vec) {
-        using V = Vec<T>;
-        const size_t nvec = n / V::N;
-        size_t blocks = (nvec + (size_t)THREADS * U - 1) / ((size_t)THREADS * U);
-        const size_t cap = (size_t)tdq_sm_count() * PER_SM;       // one resident wave; the loop covers the rest
-        if (blocks > cap) blocks = cap;
-        if (blocks == 0) blocks = 1;
-        k_combine<T, NK, THREADS, U, true><<<(unsigned)blocks, THREADS, 0, st>>>(c, row, (T *)out, (const T *)y0, kp, n);
+        const unsigned blocks = tdq_grid(n / Vec<T>::N, THREADS * U, PER_SM);
+        k_combine<T, NK, THREADS, U, true><<<blocks, THREADS, 0, st>>>(c, row, (T *)out, (const T *)y0, kp, n);
     } else {
-        size_t blocks = (n + THREADS - 1) / THREADS;
-        const size_t cap = (size_t)tdq_sm_count() * PER_SM * 2;
-        if (blocks > cap) blocks = cap;
-        if (blocks == 0) blocks = 1;
-        k_combine<T, NK, THREADS, U, false><<<(unsigned)blocks, THREADS, 0, st>>>(c, row, (T *)out, (const T *)y0, kp, n);
+        const unsigned blocks = tdq_grid(n, THREADS, PER_SM * 2);
+        k_combine<T, NK, THREADS, U, false><<<blocks, THREADS, 0, st>>>(c, row, (T *)out, (const T *)y0, kp, n);
     }
     return 0;
-}
-
-template <typename T>
-int dispatch_combine(int nk, const TdqCtrl *c, int row, void *out, const void *y0, const KPtrs &kp, size_t n,
-                     bool vec, cudaStream_t st) {
-    switch (nk) {
-#define TDQ_CASE(N) case N: return launch_combine<T, N>(c, row, out, y0, kp, n, vec, st);
-        TDQ_CASE(1) TDQ_CASE(2) TDQ_CASE(3) TDQ_CASE(4) TDQ_CASE(5) TDQ_CASE(6) TDQ_CASE(7) TDQ_CASE(8)
-        TDQ_CASE(9) TDQ_CASE(10) TDQ_CASE(11) TDQ_CASE(12) TDQ_CASE(13) TDQ_CASE(14) TDQ_CASE(15)
-        TDQ_CASE(16) TDQ_CASE(17)
-#undef TDQ_CASE
-    }
-    return -1;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -246,75 +225,16 @@ int launch_final(const TdqCtrl *c, int row, void *out, void *err_out, const void
                  const FinalMap &fm, size_t n, bool vec, cudaStream_t st) {
     constexpr int THREADS = 256, U = 2;
     if (vec) {
-        const size_t nvec = n / Vec<T>::N;
-        size_t blocks = (nvec + (size_t)THREADS * U - 1) / ((size_t)THREADS * U);
-        const size_t cap = (size_t)tdq_sm_count() * 8;
-        if (blocks > cap) blocks = cap;
-        if (blocks == 0) blocks = 1;
-        k_combine_final<T, NU, true><<<(unsigned)blocks, THREADS, 0, st>>>(c, row, (T *)out, (T *)err_out,
-                                                                            (const T *)y0, kp, fm, n);
+        const unsigned blocks = tdq_grid(n / Vec<T>::N, THREADS * U, 8);
+        k_combine_final<T, NU, true><<<blocks, THREADS, 0, st>>>(c, row, (T *)out, (T *)err_out, (const T *)y0, kp, fm, n);
     } else {
-        size_t blocks = (n + THREADS - 1) / THREADS;
-        const size_t cap = (size_t)tdq_sm_count() * 16;
-        if (blocks > cap) blocks = cap;
-        if (blocks == 0) blocks = 1;
-        k_combine_final<T, NU, false><<<(unsigned)blocks, THREADS, 0, st>>>(c, row, (T *)out, (T *)err_out,
-                                                                             (const T *)y0, kp, fm, n);
+        const unsigned blocks = tdq_grid(n, THREADS, 16);
+        k_combine_final<T, NU, false><<<blocks, THREADS, 0, st>>>(c, row, (T *)out, (T *)err_out, (const T *)y0, kp, fm, n);
     }
     return 0;
 }
 
-template <typename T>
-int dispatch_final(int nu, const TdqCtrl *c, int row, void *out, void *err_out, const void *y0, const KPtrs &kp,
-                   const FinalMap &fm, size_t n, bool vec, cudaStream_t st) {
-    switch (nu) {
-#define TDQ_CASE(N) case N: return launch_final<T, N>(c, row, out, err_out, y0, kp, fm, n, vec, st);
-        TDQ_CASE(1) TDQ_CASE(2) TDQ_CASE(3) TDQ_CASE(4) TDQ_CASE(5) TDQ_CASE(6) TDQ_CASE(7) TDQ_CASE(8)
-        TDQ_CASE(9) TDQ_CASE(10) TDQ_CASE(11) TDQ_CASE(12) TDQ_CASE(13) TDQ_CASE(14) TDQ_CASE(15)
-        TDQ_CASE(16) TDQ_CASE(17)
-#undef TDQ_CASE
-    }
-    return -1;
-}
-
 }  // namespace
-
-int tdq_sm_count() {
-    static int sms = 0;
-    if (sms == 0) {
-        int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess ||
-            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-            sms = 132;
-    }
-    return sms;
-}
-
-void tdq_shape_from_tableau(const tdq_tableau *tab, TdqHostShape *h) {
-    memset(h, 0, sizeof(*h));
-    const int S = tab->n_stages;
-    h->n_stages = S;
-    h->fsal = tab->fsal;
-    for (int i = 0; i < S; ++i) {
-        int m = 0;
-        for (int j = 0; j <= i; ++j)
-            if (tab->beta[i][j] != 0.0) h->row_idx[i][m++] = j;
-        h->row_nnz[i] = m;
-    }
-    int m = 0;
-    for (int j = 0; j <= S; ++j)
-        if (tab->c_sol[j] != 0.0) h->row_idx[S][m++] = j;
-    h->row_nnz[S] = m;
-    m = 0;
-    for (int j = 0; j <= S; ++j)
-        if (tab->c_err[j] != 0.0) h->err_idx[m++] = j;
-    h->err_nnz = m;
-    m = 0;
-    for (int j = 0; j <= S; ++j)
-        if (tab->c_mid[j] != 0.0) h->mid_idx[m++] = j;
-    h->mid_nnz = m;
-    h->valid = 1;
-}
 
 extern "C" {
 
@@ -327,18 +247,15 @@ int tdq_stage_combine(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, int
     const int nk = hs.row_nnz[row];
     TDQ_REQUIRE(nk >= 1, "empty tableau row");
     KPtrs kp;
-    memset(&kp, 0, sizeof(kp));
     bool vec = tdq_aligned16(y_out) && tdq_aligned16(y0);
-    for (int m = 0; m < nk; ++m) {
-        const int j = hs.row_idx[row][m];
-        kp.p[m] = k[j];
-        TDQ_REQUIRE(kp.p[m] != nullptr || j == 0, "missing stage slot for a non-zero tableau entry");
-        vec = vec && tdq_aligned16(kp.p[m]);
-    }
+    TDQ_REQUIRE(tdq_plan_terms(hs.row_idx[row], nk, k, kp.p, vec) == TDQ_PLAN_OK,
+                "missing stage slot for a non-zero tableau entry");
     if (n == 0) return TDQ_OK;
     int rc = -1;
-    TDQ_DISPATCH_T(dtype, rc = dispatch_combine<T>(nk, (const TdqCtrl *)ctrl_dev, row, y_out, y0, kp, n, vec,
-                                                   (cudaStream_t)stream));
+    TDQ_DISPATCH_T(dtype, rc = tdq_dispatch(TdqRange<1, TDQ_MAX_K>{}, nk, [&](auto NK) {
+                       return launch_combine<T, NK>((const TdqCtrl *)ctrl_dev, row, y_out, y0, kp, n, vec,
+                                                    (cudaStream_t)stream);
+                   }));
     TDQ_REQUIRE(rc == 0, "unsupported number of stage terms");
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
@@ -352,32 +269,19 @@ int tdq_stage_combine_final(void *ctrl_dev, const tdq_tableau *tab, int32_t dtyp
     const int S = hs.n_stages;
     const int row = hs.fsal ? S - 1 : S;          // FSAL: y1 is the last stage value (rk_common.py:83-87)
     const int avail = hs.fsal ? S - 1 : S;        // highest stage slot that exists when the row is evaluated
-    // union of the row's and the error weights' slots, ascending
-    int used_r[TDQ_MAX_K], used_e[TDQ_MAX_K];
-    for (int j = 0; j < TDQ_MAX_K; ++j) used_r[j] = used_e[j] = -1;
-    for (int m = 0; m < hs.row_nnz[row]; ++m) used_r[hs.row_idx[row][m]] = m;
-    for (int m = 0; m < hs.err_nnz; ++m)
-        if (hs.err_idx[m] <= avail) used_e[hs.err_idx[m]] = m;
     KPtrs kp;
     FinalMap fm;
-    memset(&kp, 0, sizeof(kp));
-    memset(&fm, 0xff, sizeof(fm));
     int nu = 0;
     bool vec = tdq_aligned16(y1_out) && tdq_aligned16(err_out) && tdq_aligned16(y0);
-    for (int j = 0; j <= avail; ++j) {
-        if (used_r[j] < 0 && used_e[j] < 0) continue;
-        kp.p[nu] = k[j];
-        TDQ_REQUIRE(kp.p[nu] != nullptr || j == 0, "missing stage slot for a non-zero tableau entry");
-        vec = vec && tdq_aligned16(kp.p[nu]);
-        fm.rpos[nu] = (signed char)used_r[j];
-        fm.epos[nu] = (signed char)used_e[j];
-        ++nu;
-    }
+    TDQ_REQUIRE(tdq_plan_union(hs, row, avail, k, kp.p, fm, nu, vec) == TDQ_PLAN_OK,
+                "missing stage slot for a non-zero tableau entry");
     TDQ_REQUIRE(nu >= 1, "empty tableau row");
     if (n == 0) return TDQ_OK;
     int rc = -1;
-    TDQ_DISPATCH_T(dtype, rc = dispatch_final<T>(nu, (const TdqCtrl *)ctrl_dev, row, y1_out, err_out, y0, kp, fm, n,
-                                                 vec, (cudaStream_t)stream));
+    TDQ_DISPATCH_T(dtype, rc = tdq_dispatch(TdqRange<1, TDQ_MAX_K>{}, nu, [&](auto NU) {
+                       return launch_final<T, NU>((const TdqCtrl *)ctrl_dev, row, y1_out, err_out, y0, kp, fm, n, vec,
+                                                  (cudaStream_t)stream);
+                   }));
     TDQ_REQUIRE(rc == 0, "unsupported number of stage terms");
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
