@@ -17,7 +17,9 @@
 //
 // Layout: one CTA of two warpgroups per SM, persistent; the weight planes (96 KB) sit in shared memory once per CTA.  A tile
 // is 32 state rows x 128 features; warpgroup h owns output features [64 h, 64 h + 64) of it and issues m64n32k16 products
-// (tdq_tc.cuh), so every 2 KB weight operand fetched from shared memory serves 32 rows (DESIGN.md section 3c).  A thread
+// (tdq_tc.cuh), so every 2 KB weight operand fetched from shared memory serves 32 rows (DESIGN.md section 3c).  The hi
+// weight plane of the warpgroup's features is in registers instead (32 per thread, loaded once per CTA): it is the A operand
+// of 24 of the 48 products of a stage, which then read only their 1 KB B operand from shared memory.  A thread
 // owns 16 elements of the tile in the accumulator layout of tdq_tc.cuh.  State per thread: k_0..k_3 in registers, y0 in
 // shared memory; once k_0..k_3 are known the remaining rows and the error estimate are running sums that each later k_j is
 // folded into.  Per stage: newest term + split + st.shared of the warpgroup's feature half of the B planes,
@@ -120,6 +122,18 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
     const uint32_t wsm_h = wsm + h * 8 * SBO;                             // the weight rows of features [64 h, 64 h + 64)
     const uint32_t stage = wsm + W_BYTES;
     const uint32_t sy0 = stage + AT_STAGE + tid * 4;                      // element e at sy0 + 1024 e: this thread's only
+    const uint64_t dw = make_desc(wsm_h), dy = make_desc(stage);          // every wgmma descriptor is one of these + offset
+    // the hi weight plane of the warpgroup's features as the register A operand of every hi.* product (k-step ks: ahi[ks])
+    uint32_t ahi[LD / 16][4];
+#pragma unroll
+    for (int ks = 0; ks < LD / 16; ++ks) {
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const int f = 16 * w + (lane >> 2) + 8 * (r & 1), k = 16 * ks + 2 * (lane & 3) + 8 * (r >> 1);
+            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(ahi[ks][r])
+                         : "r"(wsm_h + (f >> 3) * SBO + (k >> 3) * LBO + (f & 7) * 16 + (k & 7) * 2));
+        }
+    }
     const int toff = thread_offset(w, lane) + 64 * h;
 
     const int tiles = (n_rows + AT_ROWS - 1) / AT_ROWS;
@@ -193,7 +207,7 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
             fence_async_smem();
             __syncthreads();                                              // both feature halves of the B planes are stored
             TileAcc<AT_ROWS> tacc;
-            tile_product(wsm_h, stage, tacc);
+            tile_product(dw, dy, tacc, ahi);
             // ---- MMA window ----
             if (i + 1 < KEEP && i + 1 < S) {
                 // prefix of the next row's sum over the slots known so far

@@ -59,6 +59,7 @@ k_linear_stage(const TdqCtrl *__restrict__ c, int row, const float *y0, LinK kp,
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
     const int g = warp >> 2, w = warp & 3;
     const uint32_t wsm = smem_u32(smem), stage = wsm + W_BYTES + g * Y_STAGE;
+    const uint64_t dw = make_desc(wsm), dy = make_desc(stage);            // every wgmma descriptor is one of these + offset
 
     constexpr int NKK = NU > 0 ? NU : 1;
     float cr[NKK], ce[NKK];
@@ -137,7 +138,7 @@ k_linear_stage(const TdqCtrl *__restrict__ c, int row, const float *y0, LinK kp,
         asm volatile("bar.sync %0, 128;" :: "r"(g + 1) : "memory");
         TileAcc<TILE_ROWS> acc;
         float kr[16];
-        tile_product(wsm, stage, acc);
+        tile_product(dw, dy, acc);
         wgmma_wait();
         tile_result(acc, kr);
 #pragma unroll

@@ -4,7 +4,9 @@
 // The product of one tile: K^T = W Y^T for N state rows (N = 16 in the stage kernels, 32 in the attempt kernel) and K = 128
 // input features, issued by one warpgroup over C = 32 / N m64 halves of the output features ("chains"; with N = 32 the two
 // warpgroups of a CTA take one half each).  A = the weight planes (K-major), B = the stage-value planes (MN-major), both in
-// shared memory without swizzle; the accumulators are registers, 16 per thread for either N.  Every kernel issues the same
+// shared memory without swizzle, except that the attempt kernel holds its warpgroup's hi weight plane in registers (the A
+// operand of the 24 hi.* products of a tile, loaded once per CTA: tile_product's `ahi`), so those products fetch only their
+// B operand from shared memory; the accumulators are registers, 16 per thread for either N.  Every kernel issues the same
 // sequence of products into each accumulator, so a row's result does not depend on which kernel computed it or where the
 // row sits in the tiling (tests/test_gpu_linear.py compares the attempt kernel with the stage kernel bitwise).
 #pragma once
@@ -80,6 +82,13 @@ __device__ __forceinline__ void store_planes(uint32_t stage, const float (&y)[16
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
     return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(LBO >> 4) << 16) | ((uint64_t)(SBO >> 4) << 32);
 }
+// the descriptor of the operand `off` bytes (a compile-time constant) past the one of `base`: only the start field of the
+// low word changes.  Exact: shared addresses are below 228 KB, so start >> 4 < 2^14 never carries into the LBO field.
+// Every wgmma descriptor of a tile product is formed this way from the two bases (weights, stage planes): one add instead
+// of the mask / shift / or chain of make_desc per operand.
+__device__ __forceinline__ uint64_t desc_add(uint64_t base, uint32_t off) {
+    return (base & 0xFFFFFFFF00000000ull) | (uint32_t)((uint32_t)base + (off >> 4));
+}
 
 // D (+)= A B, m64nNk16 (N = 16 or 32), bf16 x bf16 -> f32; A K-major, B MN-major (transposed)
 template <int N> __device__ __forceinline__ void wgmma_n(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate);
@@ -96,6 +105,16 @@ template <> __device__ __forceinline__ void wgmma_n<32>(float (&d)[16], uint64_t
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
                    "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
                  : "l"(da), "l"(db), "r"(accumulate));
+}
+// D (+)= A B, m64n32k16, A from registers (the m64k16 fragment of the thread: a[0..3] = rows 16 w + (lane >> 2) + 8 (r & 1),
+// inputs 2 (lane & 3) + 8 (r >> 1) + {0, 1}), B MN-major by descriptor
+__device__ __forceinline__ void wgmma_rs32(float (&d)[16], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 1;\n\t}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -129,17 +148,26 @@ template <int N> __device__ __forceinline__ void acc_fence(TileAcc<N> &a) {
     fence_hi(a);
 }
 
-// weight plane PW x stage plane PY over k-steps [k0, k1) into d (d is overwritten at k0 when `fresh`); wsm = the weights of
-// the warpgroup's first chain
+// weight plane PW x stage plane PY over k-steps [k0, k1) into d (d is overwritten at k0 when `fresh`); dw = the descriptor
+// of the weights of the warpgroup's first chain, dy = the descriptor of stage plane 0; with ahi (N = 32) the hi plane's A
+// operand of k-step ks is the register fragment ahi[ks]
 template <int N>
-__device__ __forceinline__ void plane_product(uint32_t wsm, uint32_t stage, int pw, int py, int k0, int k1, bool fresh,
-                                              float (&d)[32 / N][N / 2]) {
+__device__ __forceinline__ void plane_product(uint64_t dw, uint64_t dy, int pw, int py, int k0, int k1, bool fresh,
+                                              float (&d)[32 / N][N / 2], const uint32_t (*ahi)[4]) {
 #pragma unroll
     for (int ks = k0; ks < k1; ++ks) {
 #pragma unroll
-        for (int c = 0; c < 32 / N; ++c)
-            wgmma_n<N>(d[c], make_desc(wsm + pw * W_PLANE + c * 8 * SBO + ks * 2 * LBO),
-                       make_desc(stage + py * y_plane<N>() + ks * 2 * LBO), fresh && ks == k0 ? 0u : 1u);
+        for (int c = 0; c < 32 / N; ++c) {
+            const uint64_t db = desc_add(dy, py * y_plane<N>() + ks * 2 * LBO);
+            const uint32_t acc = fresh && ks == k0 ? 0u : 1u;
+            if constexpr (N == 32) {
+                if (pw == 0 && ahi != nullptr) {
+                    wgmma_rs32(d[c], ahi[ks], db, acc);
+                    continue;
+                }
+            }
+            wgmma_n<N>(d[c], desc_add(dw, pw * W_PLANE + c * 8 * SBO + ks * 2 * LBO), db, acc);
+        }
     }
 }
 template <int N> __device__ __forceinline__ void add_part(TileAcc<N> &a) {
@@ -151,23 +179,26 @@ template <int N> __device__ __forceinline__ void add_part(TileAcc<N> &a) {
 }
 
 // cross term p of the list below into `small`
-template <int N> __device__ __forceinline__ void cross_term(uint32_t wsm, uint32_t stage, int p, TileAcc<N> &a) {
+template <int N>
+__device__ __forceinline__ void cross_term(uint64_t dw, uint64_t dy, int p, TileAcc<N> &a, const uint32_t (*ahi)[4]) {
     constexpr int PW[5] = {1, 2, 0, 1, 0}, PY[5] = {1, 0, 2, 0, 1};
-    plane_product<N>(wsm, stage, PW[p], PY[p], 0, LD / 16, p == 0, a.small);
+    plane_product<N>(dw, dy, PW[p], PY[p], 0, LD / 16, p == 0, a.small, ahi);
 }
 // partial q (k-steps 2q, 2q + 1) of hi.hi into `part`, once the previous partial has been added to `big`
-template <int N> __device__ __forceinline__ void next_partial(uint32_t wsm, uint32_t stage, int q, TileAcc<N> &a) {
+template <int N>
+__device__ __forceinline__ void next_partial(uint64_t dw, uint64_t dy, int q, TileAcc<N> &a, const uint32_t (*ahi)[4]) {
     wgmma_wait<1>();                                      // the group holding partial q - 1 (only newer cross terms may run)
     fence_hi(a);
     add_part(a);
     fence_hi(a);
     wgmma_fence();
-    plane_product<N>(wsm, stage, 0, 0, 2 * q, 2 * q + 2, true, a.part);
+    plane_product<N>(dw, dy, 0, 0, 2 * q, 2 * q + 2, true, a.part, ahi);
     wgmma_commit();
 }
-// Issue the product of one tile (stage planes at shared address `stage`, weight planes of the first chain at `wsm`); the
-// caller waits (wgmma_wait) and then calls tile_result.  Weight plane PW x stage plane PY: mid.mid, lo.hi, hi.lo, mid.hi,
-// hi.mid -- the five cross terms >= 2^-16, ascending in magnitude -- into the small accumulator; hi.hi into the big one;
+// Issue the product of one tile (dy = make_desc of the stage planes, dw = make_desc of the weight planes of the first chain,
+// both formed once per kernel; ahi = the hi weight plane as register fragments, N = 32 only, or nullptr to read it from
+// shared memory like the other planes); the caller waits (wgmma_wait) and then calls tile_result.  Weight plane PW x stage
+// plane PY: mid.mid, lo.hi, hi.lo, mid.hi, hi.mid -- the five cross terms >= 2^-16, ascending in magnitude -- into the small accumulator; hi.hi into the big one;
 // k = small + big.  The three remaining cross terms (lo.lo, lo.mid, mid.lo) are below 2^-24 of a product, the rounding of a
 // float32 product itself, and are not computed.
 // The tensor cores round a float32 accumulation toward zero, which over the eight k-steps of hi.hi shrinks every k by about
@@ -178,21 +209,22 @@ template <int N> __device__ __forceinline__ void next_partial(uint32_t wsm, uint
 // Issue order: each wait for a hi.hi partial (which is needed on the CUDA cores before the next one can be issued into the
 // same accumulator) has a batch of cross terms queued behind it, so the tensor pipe does not drain while `big += part` runs.
 // Each accumulator still sees the same products and float32 additions in the same order.  Issued by the whole warpgroup.
-template <int N> __device__ __forceinline__ void tile_product(uint32_t wsm, uint32_t stage, TileAcc<N> &a) {
+template <int N> __device__ __forceinline__ void tile_product(uint64_t dw, uint64_t dy, TileAcc<N> &a,
+                                                   const uint32_t (*ahi)[4] = nullptr) {
     acc_fence(a);
     wgmma_fence();
-    plane_product<N>(wsm, stage, 0, 0, 0, 2, true, a.big);
-    plane_product<N>(wsm, stage, 0, 0, 2, 4, true, a.part);
+    plane_product<N>(dw, dy, 0, 0, 0, 2, true, a.big, ahi);
+    plane_product<N>(dw, dy, 0, 0, 2, 4, true, a.part, ahi);
     wgmma_commit();
-    cross_term(wsm, stage, 0, a);
-    cross_term(wsm, stage, 1, a);
+    cross_term(dw, dy, 0, a, ahi);
+    cross_term(dw, dy, 1, a, ahi);
     wgmma_commit();
-    next_partial(wsm, stage, 2, a);
-    cross_term(wsm, stage, 2, a);
-    cross_term(wsm, stage, 3, a);
+    next_partial(dw, dy, 2, a, ahi);
+    cross_term(dw, dy, 2, a, ahi);
+    cross_term(dw, dy, 3, a, ahi);
     wgmma_commit();
-    next_partial(wsm, stage, 3, a);
-    cross_term(wsm, stage, 4, a);
+    next_partial(dw, dy, 3, a, ahi);
+    cross_term(dw, dy, 4, a, ahi);
     wgmma_commit();
     acc_fence(a);
 }
