@@ -273,7 +273,9 @@ int tdq_ctrl_set_loop(void *ctrl_dev, uint64_t loop_handle, void *stream);
 /* which = 1: y0 + (dt*k1)*(1/3);  2: y0 + dt*(k2 - k1*(1/3));  3: y0 + dt*((k1 - k2) + k3);
  * 4: y1 = y0 + ((k1 + 3*(k2 + k3)) + k4)*dt*0.125 (solvers.py:115);
  * 5: y0 + dt*k1 (euler; midpoint and heun2 pass the relevant k as k1);  6: y0 + k1*(0.5*dt) (midpoint stage);
- * 7: y0 + dt*(k1*0.5 + k2*0.5) (heun2);  8: y0 + dt*(k2*(2/3)) (heun3 stage 3);  9: y0 + dt*(k1*0.25 + k3*0.75) (heun3).
+ * 7: y0 + dt*(k1*0.5 + k2*0.5) (heun2);  8: y0 + dt*(k1*0.0 + k2*(2/3)) (heun3 stage 3);
+ * 9: y0 + dt*((k1*0.25 + k2*0.0) + k3*0.75) (heun3).  The zero-weight products are evaluated, as in the reference: a
+ * non-finite k there gives NaN, and a finite one's signed zero can turn a -0.0 sum into +0.0.
  * dt is dt_dev[step_dev[0]] (state dtype array, int64 device step counter; step_dev may be NULL for
  * index 0) so that one captured graph serves every step of the grid. */
 int tdq_rk4_stage(int32_t dtype, int32_t which, void *y_out, const void *y0, const void *k1,

@@ -205,6 +205,9 @@ def test_stage_launchers_host_side_contract(lib):
     refused(rk(0, 1, P, P, None, P, P, P, P, None, 4096, None), fn, "k1 required")
     refused(rk(0, 2, P, P, P, None, P, P, P, None, 4096, None), fn, "k2 required")
     refused(rk(0, 9, P, P, P, P, None, P, P, None, 4096, None), fn, "k3 required")
+    # heun3 evaluates its zero-weight terms: which 8 reads k1, which 9 reads k2
+    refused(rk(0, 8, P, P, None, P, P, P, P, None, 4096, None), fn, "k1 required")
+    refused(rk(0, 9, P, P, P, None, P, P, P, None, 4096, None), fn, "k2 required")
     refused(rk(0, 4, P, P, P, P, P, None, P, None, 4096, None), fn, "k4 required")
     for which in range(1, 10):
         assert rk(which % 2, which, P, P, P, P, P, P, P, None, 0, None) == 0
@@ -221,6 +224,7 @@ def test_stage_launchers_host_side_contract(lib):
     refused(ff(0, 5, P, None, P, P, P, P, *tail, 4096, None), fn, "missing stage slot")
     refused(ff(0, 7, P, P, None, P, P, P, *tail, 4096, None), fn, "missing stage slot")
     refused(ff(0, 9, P, P, P, None, P, P, *tail, 4096, None), fn, "missing stage slot")
+    refused(ff(0, 9, P, P, None, P, P, P, *tail, 4096, None), fn, "missing stage slot")
     refused(ff(0, 4, P, P, P, P, None, P, *tail, 4096, None), fn, "missing stage slot")
 
     # tdq_lincomb(dtype, out, base, x, coefs, n_terms, n, stream)

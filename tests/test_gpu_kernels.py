@@ -27,11 +27,12 @@ def _engine(method, dtype, n, dt, t0=0.5, t_sign=1.0, rtol=1e-5, atol=1e-7, segs
     return eng, _lib, _stream
 
 
-def _norm_commit(eng, _lib, _stream, errp, k_last, y0, y1, n, q_out=None):
-    """tdq_error_norm_commit with the engine's segment table and explicit state pointers."""
+def _norm_commit(eng, _lib, _stream, errp, k_last, y0, y1, n, q_out=None, rtol_vec=None, atol_vec=None):
+    """tdq_error_norm_commit with the engine's segment table and explicit state pointers (and tolerance vectors)."""
+    p = lambda t: t.data_ptr() if t is not None else None
     _lib.check(eng.lib.tdq_error_norm_commit(
         eng.ctrl.data_ptr(), eng.dt_code, errp.data_ptr(), k_last.data_ptr(), y0.data_ptr() if y0 is not None else None,
-        y1.data_ptr(), None, None, eng.norm_table.data_ptr() if eng.norm_table is not None else None, eng.n_chunks,
+        y1.data_ptr(), p(rtol_vec), p(atol_vec), eng.norm_table.data_ptr() if eng.norm_table is not None else None, eng.n_chunks,
         eng.table_aligned, eng.n_seg, n, eng.partials.data_ptr(), eng.norm_out.data_ptr(),
         q_out.data_ptr() if q_out is not None else None, _stream()))
 
@@ -46,6 +47,57 @@ def _final(eng, _lib, _stream, y1_out, err_out, y0, ksd, n):
 def _rand(n, dtype, seed):
     g = torch.Generator().manual_seed(seed)
     return torch.randn(n, generator=g, dtype=torch.float64).to(dtype)
+
+
+def _edge(n, dtype, seed):
+    """_rand with the values elementwise kernels get wrong -- +-0, subnormals, values near the dtype's max, +-inf and
+    NaN -- at seeded positions (for large n mostly in the vector body) and in the last elements (the scalar tail)."""
+    x = _rand(n, dtype, seed)
+    fi = torch.finfo(dtype)
+    special = torch.tensor([0.0, -0.0, fi.tiny / 4, -fi.tiny / 8, fi.max, -fi.max / 3, float("inf"), float("-inf"),
+                            float("nan")], dtype=torch.float64).to(dtype)
+    g = torch.Generator().manual_seed(1000 + seed)
+    perm = torch.randperm(len(special), generator=g)
+    x[torch.randint(0, n, (3 * len(special),), generator=g)] = special[perm].repeat(3)
+    tail = min(n, 3)
+    x[n - tail:] = special[perm[:tail]]
+    return x
+
+
+def _same_bits(got, want):
+    """Bit-for-bit equality, which torch.equal is not (it takes -0.0 == +0.0 and NaN != NaN): NaN at the same
+    positions, whatever the payload, and every other element with the same bit pattern."""
+    got, want = got.cpu(), want.cpu()
+    assert got.dtype == want.dtype and got.shape == want.shape, (got.dtype, want.dtype, got.shape, want.shape)
+    gn, wn = torch.isnan(got), torch.isnan(want)
+    if not torch.equal(gn, wn):
+        return False
+    iv = torch.int32 if got.dtype == torch.float32 else torch.int64
+    return torch.equal(got.view(iv)[~gn], want.view(iv)[~wn])
+
+
+# The expressions of one fixed-grid step as tdq_rk4_stage numbers them: method -> stage expressions and the final one,
+# each (which, indices of the stage slots passed as k1..k4).  Together they cover which = 1..9.
+FIXED_EXPRS = {
+    "rk4": ([(1, [0]), (2, [0, 1]), (3, [0, 1, 2])], (4, [0, 1, 2, 3])),
+    "euler": ([], (5, [0])),
+    "midpoint": ([(6, [0])], (5, [1])),
+    "heun2": ([(5, [0])], (7, [0, 1])),
+    "heun3": ([(1, [0]), (8, [0, 1])], (9, [0, 1, 2])),
+}
+
+
+def _fixed_oracle(method, h, y0, ks):
+    """One step of `method` through O.fixed_increment with a func that hands out `ks` in order: the states func is
+    called with after y0 (the stage expressions of FIXED_EXPRS, in order) and y1 = y0 + dy (the final one)."""
+    seen, it = [], iter(ks)
+
+    def func(t, y):
+        seen.append(y)
+        return next(it)
+    t0 = torch.zeros((), dtype=h.dtype)
+    dy = O.fixed_increment(method, func, t0, h, t0 + h, y0)
+    return seen[1:], y0 + dy
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
@@ -120,28 +172,37 @@ def test_error_norm_commit(method, dtype, layout):
     ks = [_rand(n, dtype, 10 + j) for j in range(S + 1)]
     dtT = torch.tensor(dt, dtype=torch.float64).to(dtype)
     err = O._weighted(ks, dtT * ct["c_err"])
-    tol = torch.tensor(1e-7, dtype=torch.float64) + torch.tensor(1e-5, dtype=torch.float64) * torch.max(y0.abs(), y1.abs())
-    assert tol.dtype == dtype
-    q = err / tol
     seg_list = segs if segs is not None else [(0, n)]
-    want = [float((q[o:o + l].double() ** 2).sum()) if dtype == torch.float64 else
-            float(((q[o:o + l] * q[o:o + l]).double()).sum()) for o, l in seg_list]
     y0d, y1d, ksd = y0.cuda(), y1.cuda(), [k.cuda() for k in ks]
     errp = torch.empty(n, dtype=dtype, device="cuda")
     y1tmp = torch.empty(n, dtype=dtype, device="cuda")
     _final(eng, _lib, _stream, y1tmp, errp, y0d, ksd, n)
-    qd = torch.full((n,), 7.0, dtype=dtype, device="cuda")
-    for q_out in (None, qd):
-        eng.ybuf[1].zero_(); eng.kbuf[1].zero_()
-        _norm_commit(eng, _lib, _stream, errp, ksd[S], y0d, y1d, n, q_out)
-        got = eng.norm_out.cpu().tolist()
-        for g, w in zip(got[:len(want)], want):
-            assert abs(g - w) <= 1e-12 * abs(w)
-        assert got[len(want)] == 0.0
-        # candidate commit: the WHOLE state (segments, gaps and padding) lands in the other pair
-        assert torch.equal(eng.ybuf[1].cpu(), y1) and torch.equal(eng.kbuf[1].cpu(), ks[S])
-    for o, l in seg_list:
-        assert torch.equal(qd.cpu()[o:o + l], q[o:o + l])
+    g = torch.Generator().manual_seed(17)
+    rv = 1e-5 * (1 + torch.rand(n, generator=g, dtype=torch.float64))
+    av = 1e-7 * (1 + torch.rand(n, generator=g, dtype=torch.float64))
+    for vtol in (False, True):
+        if vtol:      # per-element float64 tolerances: tol and err/tol in float64 (misc.py:80-82 with tensor tolerances)
+            q = err.double() / (av + rv * torch.max(y0.abs(), y1.abs()).double())
+            tv = dict(rtol_vec=rv.cuda(), atol_vec=av.cuda())
+        else:
+            tol = torch.tensor(1e-7, dtype=torch.float64) + torch.tensor(1e-5, dtype=torch.float64) * torch.max(
+                y0.abs(), y1.abs())
+            assert tol.dtype == dtype
+            q = err / tol
+            tv = {}
+        want = [float((q[o:o + l] * q[o:o + l]).double().sum()) for o, l in seg_list]
+        qd = torch.full((n,), 7.0, dtype=q.dtype, device="cuda")
+        for q_out in (None, qd):
+            eng.ybuf[1].zero_(); eng.kbuf[1].zero_()
+            _norm_commit(eng, _lib, _stream, errp, ksd[S], y0d, y1d, n, q_out, **tv)
+            got = eng.norm_out.cpu().tolist()
+            for g_, w in zip(got[:len(want)], want):
+                assert abs(g_ - w) <= 1e-12 * abs(w), vtol
+            assert got[len(want)] == 0.0
+            # candidate commit: the WHOLE state (segments, gaps and padding) lands in the other pair
+            assert _same_bits(eng.ybuf[1], y1) and _same_bits(eng.kbuf[1], ks[S]), vtol
+        for o, l in seg_list:
+            assert _same_bits(qd[o:o + l], q[o:o + l]), vtol
     # determinism: the same launch twice gives the identical float64 sums (fixed reduction order, no atomics on data)
     _norm_commit(eng, _lib, _stream, errp, ksd[S], y0d, y1d, n)
     first = eng.norm_out.clone()
@@ -155,12 +216,22 @@ def test_error_norm_commit(method, dtype, layout):
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
-@pytest.mark.parametrize("method,t_sign", [("dopri5", 1.0), ("dopri8", -1.0)])
+@pytest.mark.parametrize("method,t_sign", [("dopri5", 1.0), ("dopri8", -1.0), ("tsit5", 1.0), ("bosh3", -1.0),
+                                           ("fehlberg2", 1.0), ("adaptive_heun", -1.0)])
 def test_controller_fit_eval(method, dtype, t_sign):
     """One full attempt with hand-made stage values: accept decision, dt_next (misc.py:85-95), the
-    quartic fit (bitwise) and the dense output rows (bitwise)."""
-    n, dt, t0 = 2051, 0.0213, 0.5
-    eng, _lib, _stream = _engine(method, dtype, n, dt, t0, t_sign, t_end=t0 + dt * 0.75, keep_interp=True)
+    quartic fit (bitwise) and the dense output rows (bitwise) -- with the coefficients stored and not stored
+    (coeff == NULL), at n = 2051 (the scalar kernel) and at 2^20 (the vector kernel, grid-stride over many blocks)."""
+    for n in (2051, 2 ** 20):
+        for store in (True, False):
+            _controller_fit_eval(method, dtype, t_sign, n, store)
+
+
+def _controller_fit_eval(method, dtype, t_sign, n, store):
+    dt, t0 = 0.0213, 0.5
+    rtol, atol = 1e-3, 1e-5                                # loose enough that every tableau accepts the attempt
+    eng, _lib, _stream = _engine(method, dtype, n, dt, t0, t_sign, rtol=rtol, atol=atol, t_end=t0 + dt * 0.75,
+                                 keep_interp=store)
     # outputs at t0 + {0.25, 0.75} dt
     eng.t_out = torch.tensor([t0, t0 + 0.25 * dt, t0 + 0.75 * dt], dtype=torch.float64, device="cuda")
     eng.solution = torch.zeros(3, n, dtype=dtype, device="cuda")
@@ -176,10 +247,13 @@ def test_controller_fit_eval(method, dtype, t_sign):
     ks = [t_sign * k for k in ks_raw]                      # what the reference would hold
     dt64 = torch.tensor(dt, dtype=torch.float64)
     dtT = dt64.to(dtype)
-    y1 = y0 + O._weighted(ks[:S], ct["beta"][S - 1] * dtT)
+    # y1: the last stage row of an FSAL tableau, the c_sol row otherwise (rk_common.py:83-85)
+    coefs = ct["beta"][S - 1] * dtT if tab["fsal"] else dtT * ct["c_sol"]
+    y1 = y0 + O._weighted(ks[:len(coefs)], coefs)
     err = O._weighted(ks, dtT * ct["c_err"])
-    rtol, atol = torch.tensor(1e-5, dtype=torch.float64), torch.tensor(1e-7, dtype=torch.float64)
-    ratio = O.error_ratio(err, rtol, atol, y0, y1, O.rms)
+    ratio = O.error_ratio(err, torch.tensor(rtol, dtype=torch.float64), torch.tensor(atol, dtype=torch.float64), y0, y1,
+                          O.rms)
+    assert ratio <= 1, (method, float(ratio))              # the attempt must be accepted for the fit to run
     y0d, y1d = y0.cuda(), y1.cuda()
     ksd = [k.cuda() for k in ks_raw]
     # the pointer table's current pair holds (y0, k_0); the stage slots 1..S are the caller's
@@ -199,45 +273,52 @@ def test_controller_fit_eval(method, dtype, t_sign):
     torch.cuda.synchronize()
     mb = eng.mbox_host.contents
     assert mb.seq == 1 and mb.status == 0
-    assert bool(mb.accept) == bool(ratio <= 1)
+    assert mb.accept == 1
     assert abs(mb.ratio - float(ratio)) <= (2e-6 if dtype == torch.float32 else 1e-12) * float(ratio)
-    if mb.accept:
-        want_dt = O.optimal_step(dt64, torch.tensor(mb.ratio, dtype=torch.float64).to(ratio.dtype),
-                                 *[torch.tensor(v, dtype=torch.float64) for v in (0.9, 10.0, 0.2)], tab["order"])
-        assert abs(mb.dt - float(want_dt)) <= 1e-14 * float(want_dt)
-        coeffs = O.interp_fit(y0, y1, ks, dt64, ct)
-        for got, want in zip(eng.coeff, coeffs):
-            assert torch.equal(got.cpu(), want)
-        assert mb.par == 1                                      # committed: the table flipped to the candidate pair
-        assert torch.equal(eng.y0w.cpu(), y1)
-        assert torch.equal(eng.k0.cpu(), ks_raw[S])             # FSAL carry
-        t0_, t1_ = torch.tensor(t0, dtype=torch.float64), torch.tensor(t0, dtype=torch.float64) + dt64
-        for j in (1, 2):
-            want = O.interp_eval(coeffs, t0_, t1_, eng.t_out[j].cpu())
-            assert torch.equal(eng.solution[j].cpu(), want)
-        assert mb.done == 1 and mb.out_cursor == 3
+    want_dt = O.optimal_step(dt64, torch.tensor(mb.ratio, dtype=torch.float64).to(ratio.dtype),
+                             *[torch.tensor(v, dtype=torch.float64) for v in (0.9, 10.0, 0.2)], tab["order"])
+    assert abs(mb.dt - float(want_dt)) <= 1e-14 * float(want_dt)
+    coeffs = O.interp_fit(y0, y1, ks, dt64, ct)
+    assert len(eng.coeff) == (5 if store else 0)
+    for got, want in zip(eng.coeff, coeffs):
+        assert _same_bits(got, want), (method, n)
+    assert mb.par == 1                                      # committed: the table flipped to the candidate pair
+    assert torch.equal(eng.y0w.cpu(), y1)
+    assert torch.equal(eng.k0.cpu(), ks_raw[S])             # FSAL carry
+    t0_, t1_ = torch.tensor(t0, dtype=torch.float64), torch.tensor(t0, dtype=torch.float64) + dt64
+    for j in (1, 2):
+        want = O.interp_eval(coeffs, t0_, t1_, eng.t_out[j].cpu())
+        assert _same_bits(eng.solution[j], want), (method, n, store, j)
+    assert mb.done == 1 and mb.out_cursor == 3
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
 def test_rk4_stages_bitwise(dtype):
     from torchdiffeq_b200 import _lib
     from torchdiffeq_b200._engine import _stream
+    """Every expression (which = 1..9) against O.fixed_increment, with 16-byte aligned operands (the vector kernel) and
+    with every operand a view one element off (the scalar kernel)."""
     lib = _lib.load()
     dc = _lib.TDQ_F32 if dtype == torch.float32 else _lib.TDQ_F64
     n = 3001
     y0, k1, k2, k3, k4 = [_rand(n, dtype, s) for s in range(5)]
     dt = torch.tensor([0.1, 0.037], dtype=dtype)
     step = torch.tensor([1], dtype=torch.int64, device="cuda")
-    d = [x.cuda() for x in (y0, k1, k2, k3, k4)]
-    out = torch.empty(n, dtype=dtype, device="cuda")
     dtd = dt.cuda()
     h = dt[1]
-    wants = [y0 + h * k1 * (1 / 3), y0 + h * (k2 - k1 * (1 / 3)), y0 + h * (k1 - k2 + k3),
-             y0 + (k1 + 3 * (k2 + k3) + k4) * h * 0.125]
-    for which, want in enumerate(wants, 1):
-        _lib.check(lib.tdq_rk4_stage(dc, which, out.data_ptr(), d[0].data_ptr(), d[1].data_ptr(), d[2].data_ptr(),
-                                     d[3].data_ptr(), d[4].data_ptr(), dtd.data_ptr(), step.data_ptr(), n, _stream()))
-        assert torch.equal(out.cpu(), want), which
+    covered = set()
+    for off in (0, 1):
+        d = [torch.cat([x[:off], x]).cuda()[off:] for x in (y0, k1, k2, k3, k4)]
+        out = torch.empty(n + off, dtype=dtype, device="cuda")[off:]
+        for method, (stages, final) in FIXED_EXPRS.items():
+            wants, y1 = _fixed_oracle(method, h, y0, [k1, k2, k3, k4])
+            for (which, idx), want in zip(stages + [final], wants + [y1]):
+                ks = [d[1 + i].data_ptr() for i in idx] + [None] * (4 - len(idx))
+                _lib.check(lib.tdq_rk4_stage(dc, which, out.data_ptr(), d[0].data_ptr(), *ks, dtd.data_ptr(),
+                                             step.data_ptr(), n, _stream()))
+                assert _same_bits(out, want), (method, which, off)
+                covered.add(which)
+    assert covered == set(range(1, 10))
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float64])

@@ -191,9 +191,9 @@ class FixedGridEngine:
         else:                                                  # heun3
             stage(1, ya, k1)                                   # y0 + dt * k1 * (1/3)
             k2 = self._call_fn(self.tcur[1], self.ytmp, None)
-            stage(8, y1, None, k2)                             # y0 + dt * (k1*0 + k2*(2/3))
+            stage(8, y1, k1, k2)                               # y0 + dt * (k1*0 + k2*(2/3))
             k3 = self._call_fn(self.tcur[2], self.y1, None)
-            stage(9, y1, k1, None, k3)                         # y0 + dt * (k1/4 + k2*0 + 3*k3/4)
+            stage(9, y1, k1, k2, k3)                           # y0 + dt * (k1/4 + k2*0 + 3*k3/4)
             keep += [k2, k3]
         return keep
 

@@ -31,9 +31,12 @@ __device__ __forceinline__ T rk_expr(T dt, T y, T a, T b, T c_, T d) {
         if (WHICH == 5) return A::add(y, A::mul(dt, a));                                // euler / midpoint final / heun2 stage: y0 + dt*k
         if (WHICH == 6) return A::add(y, A::mul(a, A::mul((T)0.5, dt)));                // midpoint stage: y0 + f0*half_dt
         if (WHICH == 7) return A::add(y, A::mul(dt, A::add(A::mul(a, (T)0.5), A::mul(b, (T)0.5))));   // heun2: y0 + dt*(k1/2 + k2/2)
-        if (WHICH == 8) return A::add(y, A::mul(dt, A::mul(b, (T)(2.0 / 3.0))));        // heun3 stage 3: y0 + dt*(k1*0 + k2*2/3)
+        // heun3 keeps the tableau's zero weights (rk_common.py:121-139): k*0.0 is NaN for a non-finite k and a signed
+        // zero otherwise, so dropping the term would change both the NaNs and the signed zeros of the result
+        if (WHICH == 8)                                                                 // heun3 stage 3: y0 + dt*(k1*0 + k2*2/3)
+            return A::add(y, A::mul(dt, A::add(A::mul(a, (T)0), A::mul(b, (T)(2.0 / 3.0)))));
         // heun3 final: y0 + dt*(k1*1/4 + k2*0 + k3*3/4)
-        return A::add(y, A::mul(dt, A::add(A::mul(a, (T)0.25), A::mul(c_, (T)0.75))));
+        return A::add(y, A::mul(dt, A::add(A::add(A::mul(a, (T)0.25), A::mul(b, (T)0)), A::mul(c_, (T)0.75))));
     }
 }
 
@@ -43,8 +46,8 @@ k_rk4(T *__restrict__ out, const T *__restrict__ y0, const T *__restrict__ k1, c
       const T *__restrict__ k3, const T *__restrict__ k4, const T *__restrict__ dt_arr,
       const int64_t *__restrict__ step, size_t n) {
     // which operands the expression reads (k1,k2,k3,k4)
-    constexpr bool kA = WHICH != 8;
-    constexpr bool kB = WHICH == 2 || WHICH == 3 || WHICH == 4 || WHICH == 7 || WHICH == 8;
+    constexpr bool kA = true;
+    constexpr bool kB = WHICH == 2 || WHICH == 3 || WHICH == 4 || WHICH == 7 || WHICH == 8 || WHICH == 9;
     constexpr bool kC = WHICH == 3 || WHICH == 4 || WHICH == 9;
     constexpr bool kD = WHICH == 4;
     const T dt = dt_arr[step ? *step : 0];
@@ -135,8 +138,8 @@ k_final_emit(T *__restrict__ y0, const T *__restrict__ k1, const T *__restrict__
              const int32_t *__restrict__ mode, const T *__restrict__ slope, int64_t *step,
              const unsigned char *__restrict__ tst_all, unsigned char *__restrict__ tcur, int64_t n_steps, size_t n) {
     using A = Ar<T>;
-    constexpr bool kA = WHICH != 8;
-    constexpr bool kB = WHICH == 4 || WHICH == 7;
+    constexpr bool kA = true;
+    constexpr bool kB = WHICH == 4 || WHICH == 7 || WHICH == 9;
     constexpr bool kC = WHICH == 4 || WHICH == 9;
     constexpr bool kD = WHICH == 4;
     const int64_t s = step[0];
@@ -238,7 +241,7 @@ int tdq_rk4_stage(int32_t dtype, int32_t which, void *y_out, const void *y0, con
                   void *stream) {
     TDQ_REQUIRE(y_out && y0 && dt_dev, "null argument");
     TDQ_REQUIRE(which >= 1 && which <= 9, "which must be 1..9");
-    const bool nA = which != 8, nB = which == 2 || which == 3 || which == 4 || which == 7 || which == 8,
+    const bool nA = true, nB = which == 2 || which == 3 || which == 4 || which == 7 || which == 8 || which == 9,
                nC = which == 3 || which == 4 || which == 9, nD = which == 4;
     TDQ_REQUIRE(!nA || k1, "k1 required");
     TDQ_REQUIRE(!nB || k2, "k2 required");
@@ -279,7 +282,7 @@ int tdq_fixed_final_emit(int32_t dtype, int32_t which, void *y0, const void *k1,
                     tstage_all_dev && tstage_cur_dev,
                 "null argument");
     TDQ_REQUIRE(which == 4 || which == 5 || which == 7 || which == 9, "which must be a final expression (4, 5, 7, 9)");
-    TDQ_REQUIRE(k1 && (which == 5 || which == 9 || k2) && (which != 4 && which != 9 || k3) && (which != 4 || k4),
+    TDQ_REQUIRE(k1 && (which == 5 || k2) && (which != 4 && which != 9 || k3) && (which != 4 || k4),
                 "missing stage slot");
     cudaStream_t st = (cudaStream_t)stream;
     TDQ_DISPATCH_T(dtype, tdq_dispatch(std::integer_sequence<int, 4, 5, 7, 9>{}, which, [&](auto W) {

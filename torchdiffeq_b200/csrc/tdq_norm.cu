@@ -165,7 +165,7 @@ k_norm(const TdqCtrl *__restrict__ c, NormArgs a) {
             const bool in_seg = (meta >> 32) != 0;
             acc = 0.0;
             bad = 0.0;
-            if (in_seg || MODE == 0) {
+            if (in_seg || MODE != 2) {      // gaps: MODE 0 commits them, MODE 1 counts their non-finite y0
                 if (VECTOR) {
                     const int nvec = len / V::N;
                     V a0[U], a1[U], xa[U], xb[U];
