@@ -359,6 +359,50 @@ int tdq_fixed_emit_cubic(int32_t dtype, const void *y0, const void *y1, const vo
                          const int32_t *out_idx_dev, const void *coef_dev, int32_t rec_lo, int32_t rec_hi, size_t n,
                          void *stream);
 
+/* ---- implicit fixed-grid Runge-Kutta: Broyden's iteration as low-rank streaming passes (tdq_implicit.cu) --------------
+ * rk_common.py:438-459 (FIRK, one solve over every active stage) and :525-547 (DIRK, one solve per stage) keep a dense
+ * M x M Jacobian estimate.  J starts at I and only receives rank-1 updates whose vector is the new residual, so
+ * J_m = I + U D S^T with the residual bank U = [R_1 .. R_m], the step bank S = [s_0 .. s_{m-1}], D = diag(1/(s_j.s_j)),
+ * and J_m s = -R_m is s = -R_m + U w with the m x m system C w = D S^T R_m, C_ij = delta_ij + (s_i.R_{j+1})/(s_i.s_i).
+ * X (the unknown: the active stages' K, stage-major, M = n_stages*n elements) and every bank vector share one layout.
+ * Banks are arrays of M-vectors in chunks: vector j is chunks[j / per_chunk] + (j % per_chunk)*M elements, at most
+ * TDQ_IMPL_MAX_CHUNKS chunks.  Residual-bank slot j holds R_j (slot 0: the residual at the start).  Every dot and norm is
+ * accumulated in float64 and reduced in a fixed order that depends only on n and the vector count (bitwise run to run);
+ * `partials` needs tdq_implicit_partials_len(<vectors>) doubles, zeroed once (its first word is a self-resetting ticket).
+ *
+ * tdq_implicit_residual (rk_common.py:440/:456, :468-483, :556-558; the norm of :444/:531): residual-bank slot `slot` =
+ *   X - F (F = f[a], the func output of active stage a, n elements each), out[0] = sum R^2, out[1+i] = s_i . R for
+ *   i < n_dots (step-bank slots).  s_chunks may be NULL when n_dots == 0.
+ * tdq_implicit_solve (rk_common.py:443-452, :530-539): one CTA, float64.  m = updates made so far.  For m >= 1 it first
+ *   stores upd_out (tdq_implicit_update's out of the previous update: s.s, then s.R_{j+1}) as row m-1 and res_out[1..m]
+ *   as column m-1 of the raw dot matrix in `state`; then *status = TDQ_IMPL_EXHAUSTED when m == max_iters (the
+ *   residual after the last update is not tested), TDQ_IMPL_CONVERGED when sqrt(res_out[0]) < tol (in the state
+ *   dtype), TDQ_IMPL_SINGULAR when LU with partial pivoting of C meets
+ *   an exactly zero pivot, otherwise TDQ_IMPL_CONTINUE with w at state[1 .. 1+m).  state[0] = the residual's L2 norm.
+ *   state: tdq_implicit_state_len(max_iters) doubles, caller-owned, kept for the whole solve (no initialisation needed).
+ * tdq_implicit_update (rk_common.py:450-455, :537-543): m >= 0: s = -R_m + sum_{j<m} w_j R_{j+1} (w_dev = state + 1)
+ *   accumulated in float64 and rounded once to the state dtype, step-bank slot m = s, X += s (state dtype),
+ *   out[0] = s.s, out[1+j] = s.R_{j+1} for j < m.  m < 0 (init, rk_common.py:435/:508): X = f0 in every active stage, no
+ *   banks, no sums.  Both modes then write every active stage value (rk_common.py:439/:526)
+ *       y_out[r*n + e] = (sum_j k_j[e] * T(coefs[r*n_terms + j])) + y0[e]      products and ascending sum in T, no FMA
+ *   k[j] are stage K vectors of n elements; pointers into X see the updated values. */
+#define TDQ_IMPL_MAX_STAGES 4
+#define TDQ_IMPL_MAX_CHUNKS 64
+typedef enum {
+    TDQ_IMPL_CONTINUE = 0, TDQ_IMPL_CONVERGED = 1, TDQ_IMPL_SINGULAR = 2, TDQ_IMPL_EXHAUSTED = 3
+} tdq_impl_status;
+size_t tdq_implicit_partials_len(int32_t max_vectors);
+size_t tdq_implicit_state_len(int32_t max_iters);
+int tdq_implicit_residual(int32_t dtype, const void *x, const void *const *f, int32_t n_stages, size_t n,
+                          const void *const *u_chunks, const void *const *s_chunks, int32_t n_chunks, int64_t per_chunk,
+                          int32_t slot, int32_t n_dots, double *partials, double *out, void *stream);
+int tdq_implicit_solve(int32_t dtype, const double *res_out, const double *upd_out, double *state, int32_t *status,
+                       int32_t m, int32_t max_iters, double tol, void *stream);
+int tdq_implicit_update(int32_t dtype, void *x, int32_t n_stages, size_t n, const void *const *u_chunks,
+                        const void *const *s_chunks, int32_t n_chunks, int64_t per_chunk, int32_t m, const double *w_dev,
+                        const void *f0, void *y_out, const void *y0, const void *const *k, const double *coefs,
+                        int32_t n_terms, double *partials, double *out, void *stream);
+
 /* ---- sharded solves: norm partials exchanged over NVLink peer memory INSIDE tdq_controller ----- */
 /* The reference has no multi-GPU path; its RMS norm is a mean over the whole batch (misc.py:22-23), so
  * batch-sharded ranks must sum their n_seg+1 float64 partials before every accept/reject decision.

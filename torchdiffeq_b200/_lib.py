@@ -117,6 +117,12 @@ _SIGNATURES = {
     "tdq_linear_attempt": (C.c_int, [_vp, _ptab, _i32, _pp, _vp, _vp, _vp, _vp, _vp, _i32, _sz, _vp, _vp, _vp, _i32, _vp]),
     "tdq_fixed_emit_cubic": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _sz, _vp]),
     "tdq_pack_segments": (C.c_int, [_i32, _vp, _pp, _pi64, _pi64, _pdbl, _i32, _vp]),
+    "tdq_implicit_partials_len": (_sz, [_i32]),
+    "tdq_implicit_state_len": (_sz, [_i32]),
+    "tdq_implicit_residual": (C.c_int, [_i32, _vp, _pp, _i32, _sz, _pp, _pp, _i32, _i64, _i32, _i32, _vp, _vp, _vp]),
+    "tdq_implicit_solve": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _i32, _i32, _dbl, _vp]),
+    "tdq_implicit_update": (C.c_int, [_i32, _vp, _i32, _sz, _pp, _pp, _i32, _i64, _i32, _vp, _vp, _vp, _vp, _pp, _pdbl,
+                                      _i32, _vp, _vp, _vp]),
     "tdq_xchg_create": (C.c_int, [_pp, C.POINTER(IpcHandle)]),
     "tdq_xchg_open": (C.c_int, [C.POINTER(IpcHandle), _pp]),
     "tdq_xchg_close": (C.c_int, [_vp]),

@@ -22,6 +22,7 @@ import torch.nn as nn
 from . import _lib
 from ._engine import Layout, on_solver_stream
 from ._fixed import FixedGridEngine
+from ._implicit import IMPLICIT_METHODS
 from .odeint import (ADAPTIVE_METHODS, FIXED_METHODS, _ADJOINT_CALLBACK_NAMES, _CALLBACK_NAMES, _cache_drop, _cache_get,
                      _cache_key, _cache_put, _make_adaptive_engine, _mixed_norm, _rms_norm, _solve, _solve_event, _unflatten,
                      fixed_grid, normalise, Problem)
@@ -159,7 +160,8 @@ class _BackwardSolver:
         bp.t_sign, bp.device, bp.dtype, bp.n, bp.fn = self.bsign, dev, T, lay.n, aug_fn
         bp.original_func = p.original_func          # decides graph='auto' (only nn.Module funcs are captured)
         bp.t_cpu = (p.t_cpu.to(torch.float64) * fwd_sign * self.bsign).flip(0)
-        self.fixed = adjoint_method in FIXED_METHODS
+        self.fixed = adjoint_method in FIXED_METHODS or adjoint_method in IMPLICIT_METHODS
+        self.fixed_method = adjoint_method
         if self.fixed and opts.get("process_group") is not None:
             raise NotImplementedError("sharded adjoint with a fixed-grid adjoint_method is not implemented")
         if self.fixed:
@@ -172,8 +174,15 @@ class _BackwardSolver:
             if set(callbacks) - set(valid):
                 warnings.warn("Solver '{}' does not support callbacks {}".format(adjoint_method, set(callbacks) - set(valid)))
             # never capture inside autograd's backward (see AdaptiveEngine.prime): eager launches
-            self.eng = FixedGridEngine(aug_fn, lay.n, T, dev, method=adjoint_method, t_sign=self.bsign,
-                                       perturb=opts.get("perturb", False), graph=False, callbacks=valid, pieces=pieces)
+            if adjoint_method in IMPLICIT_METHODS:
+                from ._implicit import ImplicitEngine
+                self.eng = ImplicitEngine(aug_fn, lay.n, T, dev, method=adjoint_method,
+                                          max_iters=opts.get("max_iters", 100), t_sign=self.bsign,
+                                          perturb=opts.get("perturb", False), callbacks=valid, pieces=pieces)
+            else:
+                self.eng = FixedGridEngine(aug_fn, lay.n, T, dev, method=adjoint_method, t_sign=self.bsign,
+                                           perturb=opts.get("perturb", False), graph=False, callbacks=valid,
+                                           pieces=pieces)
             return
         # ---- batch-sharded backward solve (SURVEY.md section 8(e)) -------------------------------------------------
         # y and adj_y are this rank's rows; vjp_t and the parameter gradients every evaluation produces are PARTIAL
@@ -255,7 +264,7 @@ class _BackwardSolver:
                 if "grid_constructor" in opts:                       # the user sees the true times (misc.py:283-289)
                     gc, sgn = opts["grid_constructor"], self.bsign
                     opts["grid_constructor"] = lambda f_, y_, t_: sgn * gc(f_, y_, sgn * t_)
-                grid = fixed_grid(eng.method, opts, self.aug_fn, aug, pair)
+                grid = fixed_grid(self.fixed_method, opts, self.aug_fn, aug, pair)
                 sol = eng.solve(aug, grid, pair)
             else:
                 sol = eng.solve(aug, pairs[i - 1], t_start=float(s_cpu[i]))   # ascending for the engine
@@ -404,9 +413,9 @@ def odeint_adjoint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=No
     p = normalise(func, y0, t, rtol, atol, method, options, event_fn)
     if adjoint_method is None:
         adjoint_method = 'dopri5'
-    if adjoint_method not in ADAPTIVE_METHODS + FIXED_METHODS:
+    if adjoint_method not in ADAPTIVE_METHODS + FIXED_METHODS + IMPLICIT_METHODS:
         raise NotImplementedError('adjoint_method "{}" is not implemented on the CUDA path; implemented: {}'
-                                  .format(adjoint_method, ADAPTIVE_METHODS + FIXED_METHODS))
+                                  .format(adjoint_method, ADAPTIVE_METHODS + FIXED_METHODS + IMPLICIT_METHODS))
     if p.is_tuple:
         y0_flat = p.layout.flatten(list(y0))          # differentiable wrt every piece (copy_ into zeros)
     else:

@@ -12,7 +12,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 INCLUDE = os.path.join(ROOT, "include")
-SOURCES = ["tdq_api.cu", "tdq_ctrl.cu", "tdq_stream.cu", "tdq_norm.cu", "tdq_interp.cu", "tdq_fixed.cu", "tdq_graph.cu", "tdq_linear.cu", "tdq_attempt.cu"]
+SOURCES = ["tdq_api.cu", "tdq_ctrl.cu", "tdq_stream.cu", "tdq_norm.cu", "tdq_interp.cu", "tdq_fixed.cu", "tdq_graph.cu", "tdq_linear.cu", "tdq_attempt.cu", "tdq_implicit.cu"]
 HEADERS = [os.path.join(HERE, "tdq_common.cuh"), os.path.join(HERE, "tdq_shape.cuh"), os.path.join(HERE, "tdq_tc.cuh"), os.path.join(HERE, "tdq_tableau_tsit5.inc"), os.path.join(INCLUDE, "tdq.h")]
 LIB = os.path.join(HERE, "libtdq.so")
 STAMP = os.path.join(HERE, "libtdq.stamp")

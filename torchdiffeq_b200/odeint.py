@@ -15,6 +15,7 @@ import torch
 from . import _lib
 from ._engine import AdaptiveEngine, Layout, on_solver_stream
 from ._fixed import FixedGridEngine, grid_from_step_size
+from ._implicit import IMPLICIT_METHODS
 
 ADAPTIVE_METHODS = ("dopri5", "dopri8", "tsit5", "bosh3", "fehlberg2", "adaptive_heun")
 FIXED_METHODS = ("euler", "midpoint", "heun2", "heun3", "rk4")
@@ -32,6 +33,7 @@ _ADAPTIVE_OPTIONS = {"min_step", "max_step", "first_step", "step_t", "jump_t", "
                      "max_num_steps", "dtype", "norm"}
 _FIXED_OPTIONS = {"step_size", "grid_constructor", "interp", "perturb", "norm"}
 _ADAMS_OPTIONS = _FIXED_OPTIONS | {"max_iters", "max_order"}
+_IMPLICIT_OPTIONS = _FIXED_OPTIONS | {"max_iters"}                                  # rk_common.py:382-388
 _OUR_OPTIONS = {"graph", "run_ahead", "process_group", "cache", "exchange", "device_loop", "fused_linear", "fused_attempt"}
 
 
@@ -126,9 +128,9 @@ def normalise(func, y0, t, rtol, atol, method, options, event_fn, adjoint=False)
     if method not in REFERENCE_METHODS:                                               # misc.py:232-234
         raise ValueError('Invalid method "{}". Must be one of {}'.format(
             method, '{"' + '", "'.join(REFERENCE_METHODS) + '"}.'))
-    if method not in ADAPTIVE_METHODS + FIXED_METHODS + tuple(ADAMS_METHODS):
+    if method not in ADAPTIVE_METHODS + FIXED_METHODS + tuple(ADAMS_METHODS) + IMPLICIT_METHODS:
         raise NotImplementedError('method "{}" is not part of the CUDA hot path; implemented: {}'.format(
-            method, ADAPTIVE_METHODS + FIXED_METHODS + tuple(ADAMS_METHODS)))
+            method, ADAPTIVE_METHODS + FIXED_METHODS + tuple(ADAMS_METHODS) + IMPLICIT_METHODS))
     p.method, p.options = method, options
     if p.device.type != "cuda":
         raise _lib.TdqError("torchdiffeq_b200 runs on CUDA devices only (got %s); there is no CPU path" % p.device)
@@ -487,13 +489,31 @@ def fixed_event_solve(eng, y0_flat, t0, step_size, event_fn, atol):
 
 _FIXED_NAMES = {"euler": "Euler", "midpoint": "Midpoint", "heun2": "Heun2", "heun3": "Heun3", "rk4": "RK4",
                 "explicit_adams": "AdamsBashforth", "implicit_adams": "AdamsBashforthMoulton",
-                "fixed_adams": "AdamsBashforthMoulton"}
+                "fixed_adams": "AdamsBashforthMoulton", "implicit_euler": "ImplicitEuler",
+                "implicit_midpoint": "ImplicitMidpoint", "trapezoid": "Trapezoid", "gl4": "GaussLegendre4",
+                "gl6": "GaussLegendre6", "radauIIA3": "RadauIIA3", "radauIIA5": "RadauIIA5", "sdirk2": "SDIRK2",
+                "trbdf2": "TRBDF2"}
+
+
+def _fixed_options(method):
+    """The options a fixed-grid solver class consumes; anything else gets the unused-option warning."""
+    if method in ADAMS_METHODS:
+        return _ADAMS_OPTIONS
+    return _IMPLICIT_OPTIONS if method in IMPLICIT_METHODS else _FIXED_OPTIONS
 
 
 def _fixed_engine(p, graph=None, interp=None):
     """The fixed-grid engine of a normalised problem: explicit RK step kernels, or the Adams multistep driver."""
     o = p.options
     interp = _cubic_or_linear(o.get("interp", "linear")) if interp is None else interp
+    if p.method in IMPLICIT_METHODS:
+        from ._implicit import ImplicitEngine
+        if o.get("process_group") is not None:
+            raise NotImplementedError("the implicit methods do not run on batch-sharded states: every Broyden iteration "
+                                      "would need an all-reduce of its dot products")
+        return ImplicitEngine(p.fn, p.n, p.dtype, p.device, method=p.method, max_iters=o.get("max_iters", 100),
+                              t_sign=p.t_sign, perturb=o.get("perturb", False), callbacks=p.callbacks, pieces=p.pieces,
+                              interp=interp)
     if p.method in ADAMS_METHODS:
         from ._adams import AdamsEngine
         if p.rtol is None or p.atol is None:
@@ -509,7 +529,7 @@ def _fixed_engine(p, graph=None, interp=None):
 def fixed_grid(method, o, func, y0_view, t_cpu, keep_graph=False):
     """Option handling and time grid of FixedGridODESolver (solvers.py:55-79, :85-96, :103-104) for an
     ascending CPU `t_cpu`; the caller has already wrapped a user grid_constructor for reversed time."""
-    _warn_unused(_FIXED_NAMES[method], o, _ADAMS_OPTIONS if method in ADAMS_METHODS else _FIXED_OPTIONS)
+    _warn_unused(_FIXED_NAMES[method], o, _fixed_options(method))
     step_size, gc = o.get("step_size"), o.get("grid_constructor")
     if step_size is None:
         grid_constructor = gc if gc is not None else (lambda f, y0, t: t)
@@ -526,9 +546,9 @@ def fixed_grid(method, o, func, y0_view, t_cpu, keep_graph=False):
 
 def _solve_event(p):
     """odeint.py:97-100 + solvers.py:41-49: integrate until the event; returns (event_t tensor like t, [2, n])."""
-    if p.method in FIXED_METHODS or p.method in ADAMS_METHODS:                         # solvers.py:130-164
+    if p.method in FIXED_METHODS or p.method in ADAMS_METHODS or p.method in IMPLICIT_METHODS:   # solvers.py:130-164
         o = p.options
-        _warn_unused(_FIXED_NAMES[p.method], o, _ADAMS_OPTIONS if p.method in ADAMS_METHODS else _FIXED_OPTIONS)
+        _warn_unused(_FIXED_NAMES[p.method], o, _fixed_options(p.method))
         if o.get("step_size") is None:
             raise AssertionError("Event handling for fixed step solvers currently requires `step_size` to be provided "
                                  "in options.")
@@ -673,6 +693,9 @@ def _odeint_backprop(p, func, y0, t, params, _stats):
         if p.method in ADAMS_METHODS:
             raise NotImplementedError("gradients of the discrete solve are implemented for the explicit Runge-Kutta "
                                       "methods; use odeint_adjoint with the Adams methods")
+        if p.method in IMPLICIT_METHODS:
+            raise NotImplementedError("gradients through the discrete implicit solve (Broyden's iteration) are not "
+                                      "implemented; use odeint_adjoint with the implicit methods")
         if o.get("interp", "linear") != "linear":
             raise NotImplementedError("gradients through interp='cubic' are not implemented (use the default linear "
                                       "interpolation, or odeint_adjoint)")

@@ -34,6 +34,7 @@ import torch
 from . import _lib
 from ._engine import AdaptiveEngine, on_solver_stream
 from ._fixed import FixedGridEngine, grid_from_step_size
+from ._implicit import IMPLICIT_METHODS
 
 ADAPTIVE = ("dopri5", "dopri8", "tsit5", "bosh3", "fehlberg2", "adaptive_heun")
 FIXED = ("euler", "midpoint", "heun2", "heun3", "rk4")
@@ -172,8 +173,10 @@ def make_adaptive(method, **defaults):
 
 def make_fixed(method, **defaults):
     """Class with the interface of FixedGridODESolver (solvers.py:52-128) for one explicit fixed-step method, or of
-    AdamsBashforth / AdamsBashforthMoulton (fixed_adams.py:164-228) for the Adams names."""
+    AdamsBashforth / AdamsBashforthMoulton (fixed_adams.py:164-228) for the Adams names, or of
+    FixedGridFIRKODESolver / FixedGridDIRKODESolver (rk_common.py:378-558) for the implicit names."""
     adams = method in ADAMS
+    implicit = method in IMPLICIT_METHODS
 
     class B200FixedSolver:
         name = method
@@ -185,6 +188,7 @@ def make_fixed(method, **defaults):
             self.atol = unused_kwargs.pop("atol", None)                        # solvers.py:58-61
             self.rtol = unused_kwargs.pop("rtol", None)
             self.adams_kw = {k: unused_kwargs.pop(k) for k in ("max_iters", "max_order") if adams and k in unused_kwargs}
+            self.max_iters = unused_kwargs.pop("max_iters", 100) if implicit else None       # rk_common.py:382
             unused_kwargs.pop("norm", None)
             self.our = {k: unused_kwargs.pop(k) for k in _OUR_KEYS if k in unused_kwargs}
             for k, v in defaults.items():
@@ -209,6 +213,11 @@ def make_fixed(method, **defaults):
         def _make_engine(self, interp, graph):
             shape, base = self.shape, self.base
             fn = lambda t_, yf: base(t_, yf.view(shape))
+            if implicit:
+                from ._implicit import ImplicitEngine
+                return ImplicitEngine(fn, self.y0.numel(), self.y0.dtype, self.y0.device, method=method,
+                                      max_iters=self.max_iters, perturb=self.perturb, callbacks=self.callbacks,
+                                      interp=interp)
             if adams:
                 from ._adams import AdamsEngine
                 return AdamsEngine(fn, self.y0.numel(), self.y0.dtype, self.y0.device, implicit=ADAMS[method],
@@ -267,7 +276,7 @@ class _Dispatch:
         return self.gpu_cls.valid_callbacks()
 
 
-def register(solvers=None, methods=ADAPTIVE + FIXED + tuple(ADAMS), **defaults):
+def register(solvers=None, methods=ADAPTIVE + FIXED + tuple(ADAMS) + IMPLICIT_METHODS, **defaults):
     """Put the libtdq-backed solvers into a SOLVERS dict (default: the reference's, found through
     importlib.import_module('torchdiffeq._impl.odeint') -- the attribute torchdiffeq._impl.odeint is shadowed by the
     function of the same name).  In place, so torchdiffeq._impl.adjoint sees it too.  Returns the dict of replaced
