@@ -44,12 +44,6 @@ def c1():
         ms = timed(lambda: tdq.odeint(f, y0, t, method="rk4"))
     print(json.dumps({"config": "C1 rk4 spiral B=1024 f32, 999 steps", "ms": ms, "traj_per_s": 1024 / ms * 1e3,
                       "steps_per_s": 999 / ms * 1e3, "cpu_reference_build_container": "154 ms (SURVEY 6)"}), flush=True)
-    from torchdiffeq_b200._fixed import FixedGridEngine
-    FixedGridEngine.FUSE_FINAL = False          # same box, same process: the two-launch form (13 graph nodes per step)
-    with torch.no_grad():
-        ms2 = timed(lambda: tdq.odeint(f, y0, t, method="rk4"))
-    FixedGridEngine.FUSE_FINAL = True
-    print(json.dumps({"config": "C1 with the final expression NOT fused into the emit kernel", "ms": ms2}), flush=True)
 
 
 def c3():

@@ -100,7 +100,7 @@ def test_adaptive_reverse_sweep_matches_reference(key):
 
 @pytest.mark.parametrize("key", sorted(k for k in BP if k.startswith("mlp/") and k.split("/")[2] in ("rk4", "midpoint", "euler")
                                        and k.endswith("float64")))
-def test_fixed_reverse_sweep_matches_reference(key):
+def test_fixed_reverse_sweep_on_tabulated_grid_matches_reference(key):
     """Fixed grids: dt = grid[k+1] - grid[k] is differentiated too, and the grid constructor by autograd."""
     case = BP[key]
     _, name, method, dn = key.split("/")
@@ -109,15 +109,14 @@ def test_fixed_reverse_sweep_matches_reference(key):
     t = case["t"]
     p = _problem(f, y0, t)
     p.method = method
-    from torchdiffeq_b200._fixed import FixedGridEngine, grid_from_step_size
+    from torchdiffeq_b200._fixed import _tabulate, grid_from_step_size
     with torch.enable_grad():
         t_req = p.t_cpu.detach().clone().requires_grad_(True)
         gc = grid_from_step_size(case["opts"]["step_size"]) if case["opts"] else (lambda f_, y_, t_: t_)
         grid_req = gc(None, None, t_req)
     grid = grid_req.detach()
-    eng = FixedGridEngine.__new__(FixedGridEngine)
-    eng.dtype, eng.perturb, eng.t_sign, eng.method = torch.float64, False, p.t_sign, method
-    ts, dtT, rec_begin, out_idx, mode, slope, n_steps = eng._tabulate(grid, p.t_cpu)
+    ts, dtT, rec_begin, out_idx, mode, slope, _, _, n_steps = _tabulate(grid, p.t_cpu, method, torch.float64, False,
+                                                                        p.t_sign)
     # forward on the CPU with the sweep's own step formulas
     alpha, beta, wts = B.FIXED_TABLEAUS[method]
     F = lambda s_, y_: (p.fn(s_ * p.t_sign, y_).reshape(-1) * p.t_sign)

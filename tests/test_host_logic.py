@@ -4,7 +4,7 @@ import pytest
 import torch
 
 from torchdiffeq_b200._engine import Layout
-from torchdiffeq_b200._fixed import FixedGridEngine, grid_from_step_size
+from torchdiffeq_b200._fixed import _tabulate, grid_from_step_size
 from torchdiffeq_b200.odeint import _func_signature, _tol_vector
 
 
@@ -58,7 +58,7 @@ def _reference_fixed_loop(grid, t):
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
 @pytest.mark.parametrize("case", ["grid_is_t", "step_size", "coarse_t"])
-def test_fixed_grid_tables(case, dtype):
+def test_tabulate_fixed_grid_tables(case, dtype):
     if case == "grid_is_t":
         t = torch.linspace(0., 25., 50, dtype=dtype)
         grid = t
@@ -68,9 +68,7 @@ def test_fixed_grid_tables(case, dtype):
     else:
         t = torch.tensor([0., 0.3, 0.31, 2.0], dtype=dtype)
         grid = torch.linspace(0., 2., 5, dtype=dtype)
-    eng = FixedGridEngine.__new__(FixedGridEngine)
-    eng.dtype, eng.perturb, eng.t_sign, eng.method = torch.float32, False, 1.0, "rk4"
-    ts, dtT, rec_begin, out_idx, mode, slope, n_steps = eng._tabulate(grid, t)
+    ts, dtT, rec_begin, out_idx, mode, slope, _, _, n_steps = _tabulate(grid, t, "rk4", torch.float32, False, 1.0)
     want = _reference_fixed_loop(grid, t)
     got = []
     for s in range(n_steps):
@@ -82,12 +80,10 @@ def test_fixed_grid_tables(case, dtype):
     assert torch.equal(dtT, (grid[1:] - grid[:-1]).to(torch.float32))
     assert torch.equal(ts[:, 0], grid[:-1].to(torch.float32)) and torch.equal(ts[:, 3], grid[1:].to(torch.float32))
     # perturb: first time moved up one ulp, last time down (misc.py:188-193)
-    eng.perturb = True
-    tsp = eng._tabulate(grid, t)[0]
+    tsp = _tabulate(grid, t, "rk4", torch.float32, True, 1.0).ts
     assert (tsp[:, 0] > ts[:, 0]).all() and (tsp[:, 3] < ts[:, 3]).all()
     # reverse time: sign folded into the func times and into dt
-    eng.perturb, eng.t_sign = False, -1.0
-    tsr, dtr = eng._tabulate(grid, t)[:2]
+    tsr, dtr = _tabulate(grid, t, "rk4", torch.float32, False, -1.0)[:2]
     assert torch.equal(tsr, -ts) and torch.equal(dtr, -dtT)
 
 

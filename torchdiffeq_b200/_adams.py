@@ -25,6 +25,7 @@ from ._engine import _stream
 from ._fixed import FixedGridEngine, _RetryWithCopies
 
 _MIN_ORDER, _MAX_ORDER, _MAX_ITERS = 4, 12, 4            # fixed_adams.py:143-145
+ADAMS_METHODS = {"explicit_adams": False, "implicit_adams": True, "fixed_adams": True}     # name -> implicit (odeint.py:31-42)
 
 
 def _poly_mul(p, q):
@@ -56,23 +57,17 @@ _MOULTON = {k: _adams_weights(k, 1) for k in range(1, _MAX_ORDER + 1)}
 class AdamsEngine(FixedGridEngine):
     """AdamsBashforthMoulton._step_func (fixed_adams.py:193-222) as the step of the fixed-grid engine."""
 
-    def __init__(self, fn, n, dtype, device, *, implicit, rtol, atol, max_iters=_MAX_ITERS, max_order=_MAX_ORDER,
-                 t_sign=1.0, perturb=False, callbacks=None, pieces=None, interp="linear"):
+    def __init__(self, fn, n, dtype, device, *, method, rtol, atol, max_iters, max_order, **kw):
         assert max_order <= _MAX_ORDER, "max_order must be at most {}".format(_MAX_ORDER)          # fixed_adams.py:170
         if max_order < _MIN_ORDER:
             warnings.warn("max_order is below {}, so the solver reduces to `rk4`.".format(_MIN_ORDER))
-        super().__init__(fn, n, dtype, device, method="rk4", t_sign=t_sign, perturb=perturb, graph=False,
-                         callbacks=callbacks, pieces=pieces, interp=interp)
-        self.implicit, self.max_iters, self.max_order = bool(implicit), int(max_iters), int(max_order)
+        super().__init__(fn, n, dtype, device, method=method, **kw)
+        self.implicit, self.max_iters, self.max_order = ADAMS_METHODS[method], int(max_iters), int(max_order)
         # fixed_adams.py:174-175: tolerances of the corrector's stopping test, in the state dtype
         self.rtol = float(torch.as_tensor(rtol, dtype=torch.float64).to(dtype))
         self.atol = float(torch.as_tensor(atol, dtype=torch.float64).to(dtype))
         self.prev_f = collections.deque(maxlen=self.max_order - 1)
         self.prev_t = None
-        self.graph_opt = False
-        self._grid_cpu, self._event_step = None, None
-
-    FUSE_FINAL = False                     # the step is not a single final expression
 
     # ---- history (fixed_adams.py:183-186) ----------------------------------------------------------------------------
     def _update_history(self, t, f):
@@ -87,37 +82,30 @@ class AdamsEngine(FixedGridEngine):
                                         len(terms), self.n, _stream()))
         self.launches += 1
 
-    def _solve_impl(self, y0_flat, grid_cpu, t_cpu):
-        self._grid_cpu, self._step_index, self._event_step = grid_cpu, 0, None
+    def _new_solve(self, y0_flat, n_out):
+        super()._new_solve(y0_flat, n_out)
         self.prev_f.clear()
         self.prev_t = None
-        return super()._solve_impl(y0_flat, grid_cpu, t_cpu)
 
-    def solve_until_event(self, y0_flat, t0, step_size, event_fn, atol, max_itrs=20000):
-        self.prev_f.clear()
-        self.prev_t = None
+    def _step_once(self, rec, emit):
         try:
-            return super().solve_until_event(y0_flat, t0, step_size, event_fn, atol, max_itrs)
-        finally:
-            self._event_step = None
+            keep = self._stages(rec)
+        except _RetryWithCopies:
+            # the history was extended before the retry was requested: undo, then let _step() retry
+            if self.prev_f and self.prev_t is not None:
+                self.prev_f.popleft()
+                self.prev_t = None
+            raise
+        if emit:
+            self._emit_step(rec.k, keep[0])
+        return keep
 
-    def _one_step_tables(self, t0c, dt, t1c):
-        super()._one_step_tables(t0c, dt, t1c)
-        self._event_step = (t0c, dt, t1c)
-
-    def _stages(self, fuse_final=False):
+    def _stages(self, rec):
         """One Adams step: y1 into self.y1; returns [f0] (what _step_func returns besides dy)."""
         T, dev = self.dtype, self.device
-        if getattr(self, "_event_step", None) is not None:                      # event stepping: explicit (t0, dt, t1)
-            t0, dt, t1 = self._event_step
-            dt64 = float(torch.as_tensor(dt, dtype=torch.float64)) if not torch.is_tensor(dt) else float(dt.double())
-            dt_T = float(torch.as_tensor(dt64, dtype=torch.float64).to(T)) if not torch.is_tensor(dt) else float(dt.to(T))
-        else:
-            k = self._step_index
-            t0, t1 = self._grid_cpu[k], self._grid_cpu[k + 1]
-            dtt = t1 - t0                                                        # t's dtype (solvers.py:112)
-            dt64, dt_T = float(dtt.double()), float(dtt.to(T))
-            self._step_index += 1
+        t0 = rec.t0
+        dt = torch.as_tensor(rec.dt, dtype=torch.float64)
+        dt64, dt_T = float(dt), float(dt.to(T))
         sgn = self.t_sign
         # func outputs of earlier steps are kept: a func that reuses one output buffer must be copied
         self._taken = {h.data_ptr() for h in self.prev_f}
@@ -128,23 +116,7 @@ class AdamsEngine(FixedGridEngine):
         self._update_history(t0, f0)
         order = min(len(self.prev_f), self.max_order - 1)
         if order < _MIN_ORDER - 1:                                               # :196-198 RK4 with k1 = prev_f[0]
-            lib, dc, n, st = self.lib, self.dc, self.n, _stream()
-            y0, ya, y1 = self.y0w.data_ptr(), self.ytmp.data_ptr(), self.y1.data_ptr()
-            dtp, stp = self.dt_dev.data_ptr(), self.step_dev.data_ptr()
-            k1 = self.prev_f[0]
-
-            def stage(which, out, *ks):
-                p = [x.data_ptr() if x is not None else None for x in ks] + [None] * (4 - len(ks))
-                _lib.check(lib.tdq_rk4_stage(dc, which, out, y0, p[0], p[1], p[2], p[3], dtp, stp, n, st))
-                self.launches += 1
-            stage(1, ya, k1)
-            k2 = self._call_fn(self.tcur[1], self.ytmp, None)
-            stage(2, y1, k1, k2)
-            k3 = self._call_fn(self.tcur[2], self.y1, None)
-            stage(3, ya, k1, k2, k3)
-            k4 = self._call_fn(self.tcur[3], self.ytmp, None)
-            stage(4, y1, k1, k2, k3, k4)
-            return [f0, k2, k3, k4]
+            return [f0] + self._rk_stages("rk4", self.prev_f[0], False)[1:]
         # Adams-Bashforth predictor (:200-201): dy = sum_m f_{n-m} * T(dt * b_m); the reverse-time sign of the raw
         # func outputs goes into the coefficient (exact)
         hist = list(self.prev_f)[:order]
@@ -179,15 +151,3 @@ class AdamsEngine(FixedGridEngine):
             self._update_history(t0, f)                                          # a no-op: prev_t == t0 (as in the reference)
         self._lincomb(self.y1, self.y0w, [(dy, 1.0)])                            # y1 = y0 + dy (solvers.py:115)
         return [f0]
-
-    def _step_once(self, step=None):
-        try:
-            return super()._step_once(step)
-        except _RetryWithCopies:
-            # the history was extended before the retry was requested: undo, then let _step() retry
-            if self.prev_f and self.prev_t is not None:
-                self.prev_f.popleft()
-                self.prev_t = None
-            if getattr(self, "_event_step", None) is None:
-                self._step_index -= 1
-            raise

@@ -59,16 +59,9 @@ IMPLICIT_METHODS = tuple(TABLEAUS)
 class ImplicitEngine(FixedGridEngine):
     """FixedGridFIRKODESolver / FixedGridDIRKODESolver._step_func (rk_common.py:415-466, :488-554) as the step of the
     fixed-grid engine."""
-    FUSE_FINAL = False
 
-    def __init__(self, fn, n, dtype, device, *, method, max_iters=100, t_sign=1.0, perturb=False, callbacks=None,
-                 pieces=None, interp="linear"):
-        if method not in TABLEAUS:
-            raise ValueError("unknown implicit method %r" % method)
-        super().__init__(fn, n, dtype, device, method="rk4", t_sign=t_sign, perturb=perturb, graph=False,
-                         callbacks=callbacks, pieces=pieces, interp=interp)
-        self.graph_opt = False
-        self.implicit_method = method
+    def __init__(self, fn, n, dtype, device, *, method, max_iters, **kw):
+        super().__init__(fn, n, dtype, device, method=method, **kw)
         dirk, alpha, beta, c_sol = TABLEAUS[method]
         self.dirk = dirk
         T = dtype
@@ -82,7 +75,6 @@ class ImplicitEngine(FixedGridEngine):
         self.tol = 1e-8 if T == torch.float64 else 1e-6                                 # rk_common.py:424-429
         self.iterations = 0              # Broyden updates over the whole solve
         self.n_warnings = 0
-        self._grid_cpu, self._event_step = None, None
         self._bufs = None
         S = len(alpha)
         rows = 1 if dirk else S - sum(self.skipped)
@@ -122,34 +114,9 @@ class ImplicitEngine(FixedGridEngine):
         return (_lib.ptr_array([c.data_ptr() for c in self._u_chunks]),
                 _lib.ptr_array([c.data_ptr() for c in self._s_chunks]), len(self._u_chunks))
 
-    # ---- grid / event bookkeeping (as AdamsEngine) ----------------------------------------------------------------
-    def _solve_impl(self, y0_flat, grid_cpu, t_cpu):
-        self._grid_cpu, self._step_index, self._event_step = grid_cpu, 0, None
+    def _new_solve(self, y0_flat, n_out):
+        super()._new_solve(y0_flat, n_out)
         self._bufs = None
-        return super()._solve_impl(y0_flat, grid_cpu, t_cpu)
-
-    def solve_until_event(self, y0_flat, t0, step_size, event_fn, atol, max_itrs=20000):
-        self._bufs = None
-        try:
-            return super().solve_until_event(y0_flat, t0, step_size, event_fn, atol, max_itrs)
-        finally:
-            self._event_step = None
-
-    def _one_step_tables(self, t0c, dt, t1c):
-        super()._one_step_tables(t0c, dt, t1c)
-        self._event_step = (t0c, dt, t1c)
-
-    def _step_scalars(self):
-        """(t0, dt, t1) of this step as 0-dim CPU tensors of the state dtype (rk_common.py:416-433)."""
-        T = self.dtype
-        if self._event_step is not None:                         # solvers.py:143: dt = step_size, t1 = t0 + dt
-            t0, dt, t1 = self._event_step
-            t0, dt, t1 = (x if torch.is_tensor(x) else torch.tensor(x) for x in (t0, dt, t1))
-        else:
-            k = self._step_index
-            t0, t1 = self._grid_cpu[k], self._grid_cpu[k + 1]
-            dt = t1 - t0                                          # solvers.py:112, t's dtype
-        return t0.to(T), dt.to(T), t1.to(T)
 
     def _stage_time(self, i, t0, dt, t1):
         a = self.alpha_T[i]
@@ -160,11 +127,13 @@ class ImplicitEngine(FixedGridEngine):
         return t0 + a * dt
 
     # ---- one step ---------------------------------------------------------------------------------------------------
-    def _stages(self, fuse_final=False):
-        """One implicit step: y1 into self.y1; returns [f0]."""
+    def _step_once(self, rec, emit):
+        """One implicit step: y1 into self.y1, then the emit; returns [f0]."""
         b = self._alloc()
         T, dev, n, sgn = self.dtype, self.device, self.n, self.t_sign
-        t0, dt, t1 = self._step_scalars()
+        # (t0, dt, t1) as 0-dim tensors of the state dtype (rk_common.py:416-433)
+        t0, dt, t1 = (x if torch.is_tensor(x) else torch.tensor(x) for x in rec[1:])
+        t0, dt, t1 = t0.to(T), dt.to(T), t1.to(T)
         S = len(self.alpha_T)
         self._taken = set()
         f0 = self._call_fn(self.tcur[0], self.y0w, None)          # Perturb.NEXT when perturb (in tcur)
@@ -189,9 +158,9 @@ class ImplicitEngine(FixedGridEngine):
         _lib.check(self.lib.tdq_lincomb(self.dc, self.y1.data_ptr(), self.y0w.data_ptr(), _lib.ptr_array(Kp),
                                         _lib.dbl_array(cs), S, n, _stream()))
         self.launches += 1
-        if self._event_step is None:
-            self._step_index += 1
         self._taken = {f0.data_ptr()}
+        if emit:
+            self._emit_step(rec.k, f0)
         return [f0]
 
     def _broyden(self, b, f0, times, X, Kp, coefs):

@@ -21,9 +21,9 @@ import torch.nn as nn
 
 from . import _lib
 from ._engine import Layout, on_solver_stream
-from ._fixed import FixedGridEngine
+from ._fixed import FIXED_METHODS, make_engine
 from ._implicit import IMPLICIT_METHODS
-from .odeint import (ADAPTIVE_METHODS, FIXED_METHODS, _ADJOINT_CALLBACK_NAMES, _CALLBACK_NAMES, _cache_drop, _cache_get,
+from .odeint import (ADAPTIVE_METHODS, _ADJOINT_CALLBACK_NAMES, _CALLBACK_NAMES, _cache_drop, _cache_get,
                      _cache_key, _cache_put, _make_adaptive_engine, _mixed_norm, _rms_norm, _solve, _solve_event, _unflatten,
                      fixed_grid, normalise, Problem)
 
@@ -174,15 +174,9 @@ class _BackwardSolver:
             if set(callbacks) - set(valid):
                 warnings.warn("Solver '{}' does not support callbacks {}".format(adjoint_method, set(callbacks) - set(valid)))
             # never capture inside autograd's backward (see AdaptiveEngine.prime): eager launches
-            if adjoint_method in IMPLICIT_METHODS:
-                from ._implicit import ImplicitEngine
-                self.eng = ImplicitEngine(aug_fn, lay.n, T, dev, method=adjoint_method,
-                                          max_iters=opts.get("max_iters", 100), t_sign=self.bsign,
-                                          perturb=opts.get("perturb", False), callbacks=valid, pieces=pieces)
-            else:
-                self.eng = FixedGridEngine(aug_fn, lay.n, T, dev, method=adjoint_method, t_sign=self.bsign,
-                                           perturb=opts.get("perturb", False), graph=False, callbacks=valid,
-                                           pieces=pieces)
+            self.eng = make_engine(adjoint_method, aug_fn, lay.n, T, dev, t_sign=self.bsign,
+                                   perturb=opts.get("perturb", False), graph=False, callbacks=valid, pieces=pieces,
+                                   max_iters=opts.get("max_iters"))
             return
         # ---- batch-sharded backward solve (SURVEY.md section 8(e)) -------------------------------------------------
         # y and adj_y are this rank's rows; vjp_t and the parameter gradients every evaluation produces are PARTIAL

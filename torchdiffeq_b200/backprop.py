@@ -27,6 +27,7 @@ import torch
 
 from . import _lib
 from ._engine import on_solver_stream
+from ._fixed import stage_times
 
 
 def discover_params(func):
@@ -305,17 +306,11 @@ def fixed_backward(p, method, tape, grid, t_cpu, grad_sol, params, need_t):
         k = st["k"]
         g0, g1 = grid[k], grid[k + 1]
         dt = g1 - g0                                                   # t's dtype, like the reference (solvers.py:112)
-        dtT, t0T = dt.to(T), g0.to(T)
-        dtf = float(dtT)
+        dtf = float(dt.to(T))
         y0 = st["y0"]
-        # stage times by the reference's dtype rules: t0 + dt*alpha in t's dtype, cast to the state dtype by _PerturbFunc
-        tc = [((g0 + dt * a) if a != 1.0 else (g0 + dt * 1.0 if method == "heun2" else g1)).to(T) for a in alpha]
-        t0_eval = t0T
-        if st["perturb"]:
-            t0_eval = _next(t0T)
-            tc = [(_prev(tt) if a == 1.0 else tt) for tt, a in zip(tc, alpha)]
-        times = [_dev(tt, dev) for tt in tc]
-        t0_dev = _dev(t0_eval, dev)
+        ts = stage_times(method, g0, dt, g1, st["perturb"], T)        # the forward step's func times
+        times = [_dev(tt, dev) for tt in ts[1:1 + len(alpha)]]
+        t0_dev = _dev(ts[0], dev)
         with torch.no_grad():
             k1 = F(t0_dev, y0)
         coefs = [[b * dtf for b in row] for row in beta]

@@ -14,12 +14,11 @@ import torch
 
 from . import _lib
 from ._engine import AdaptiveEngine, Layout, on_solver_stream
-from ._fixed import FixedGridEngine, grid_from_step_size
+from ._adams import ADAMS_METHODS
+from ._fixed import FIXED_METHODS, grid_from_step_size, make_engine
 from ._implicit import IMPLICIT_METHODS
 
 ADAPTIVE_METHODS = ("dopri5", "dopri8", "tsit5", "bosh3", "fehlberg2", "adaptive_heun")
-FIXED_METHODS = ("euler", "midpoint", "heun2", "heun3", "rk4")
-ADAMS_METHODS = {"explicit_adams": False, "implicit_adams": True, "fixed_adams": True}     # name -> implicit (odeint.py:31-42)
 # Every name the reference registers (odeint.py:19-46); the ones outside SURVEY.md section 8 are
 # recognised and rejected explicitly rather than reported as "invalid".
 REFERENCE_METHODS = (
@@ -482,11 +481,6 @@ def _cubic_or_linear(interp):
     return interp
 
 
-def fixed_event_solve(eng, y0_flat, t0, step_size, event_fn, atol):
-    """solvers.py:130-164 on a FixedGridEngine: (event_t, y(event_t))."""
-    return eng.solve_until_event(y0_flat, t0, step_size, event_fn, atol)
-
-
 _FIXED_NAMES = {"euler": "Euler", "midpoint": "Midpoint", "heun2": "Heun2", "heun3": "Heun3", "rk4": "RK4",
                 "explicit_adams": "AdamsBashforth", "implicit_adams": "AdamsBashforthMoulton",
                 "fixed_adams": "AdamsBashforthMoulton", "implicit_euler": "ImplicitEuler",
@@ -502,28 +496,15 @@ def _fixed_options(method):
     return _IMPLICIT_OPTIONS if method in IMPLICIT_METHODS else _FIXED_OPTIONS
 
 
-def _fixed_engine(p, graph=None, interp=None):
-    """The fixed-grid engine of a normalised problem: explicit RK step kernels, or the Adams multistep driver."""
+def _fixed_engine(p, graph=None):
+    """The fixed-grid engine of a normalised problem: explicit Runge-Kutta, Adams or implicit Runge-Kutta."""
     o = p.options
-    interp = _cubic_or_linear(o.get("interp", "linear")) if interp is None else interp
-    if p.method in IMPLICIT_METHODS:
-        from ._implicit import ImplicitEngine
-        if o.get("process_group") is not None:
-            raise NotImplementedError("the implicit methods do not run on batch-sharded states: every Broyden iteration "
-                                      "would need an all-reduce of its dot products")
-        return ImplicitEngine(p.fn, p.n, p.dtype, p.device, method=p.method, max_iters=o.get("max_iters", 100),
-                              t_sign=p.t_sign, perturb=o.get("perturb", False), callbacks=p.callbacks, pieces=p.pieces,
-                              interp=interp)
-    if p.method in ADAMS_METHODS:
-        from ._adams import AdamsEngine
-        if p.rtol is None or p.atol is None:
-            raise NotImplementedError("per-element tolerances are not implemented for the Adams methods")
-        return AdamsEngine(p.fn, p.n, p.dtype, p.device, implicit=ADAMS_METHODS[p.method], rtol=p.rtol, atol=p.atol,
-                           max_iters=o.get("max_iters", 4), max_order=o.get("max_order", 12), t_sign=p.t_sign,
-                           perturb=o.get("perturb", False), callbacks=p.callbacks, pieces=p.pieces, interp=interp)
-    g = _resolve_graph(o.get("graph", "auto"), p.original_func) if graph is None else graph
-    return FixedGridEngine(p.fn, p.n, p.dtype, p.device, method=p.method, t_sign=p.t_sign,
-                           perturb=o.get("perturb", False), graph=g, callbacks=p.callbacks, pieces=p.pieces, interp=interp)
+    if graph is None:
+        graph = _resolve_graph(o.get("graph", "auto"), p.original_func)
+    return make_engine(p.method, p.fn, p.n, p.dtype, p.device, t_sign=p.t_sign, perturb=o.get("perturb", False),
+                       callbacks=p.callbacks, pieces=p.pieces, interp=_cubic_or_linear(o.get("interp", "linear")),
+                       graph=graph, rtol=p.rtol, atol=p.atol, max_iters=o.get("max_iters"), max_order=o.get("max_order"),
+                       sharded=o.get("process_group") is not None)
 
 
 def fixed_grid(method, o, func, y0_view, t_cpu, keep_graph=False):
@@ -556,7 +537,7 @@ def _solve_event(p):
             raise ValueError("step_size and grid_constructor are mutually exclusive arguments.")
         eng = _fixed_engine(p, graph=False)
         tol = p.atol if p.atol is not None else float(p.atol_vec.min())
-        event_t, y_event = fixed_event_solve(eng, p.y0_flat, p.t_cpu[0], o["step_size"], p.event_fn, tol)
+        event_t, y_event = eng.solve_until_event(p.y0_flat, p.t_cpu[0], o["step_size"], p.event_fn, tol)
         sol = torch.stack([p.y0_flat.to(p.dtype), y_event], dim=0)
         return float(event_t) * p.t_sign, sol, eng
     eng = _make_adaptive_engine(p, p.method, p.rtol, p.atol, p.rtol_vec, p.atol_vec,
@@ -704,8 +685,8 @@ def _odeint_backprop(p, func, y0, t, params, _stats):
             t_req = p.t_cpu.detach().clone().requires_grad_(True)
             grid_req = fixed_grid(p.method, o, p.original_func, y0_view, t_req, keep_graph=True)
         grid = grid_req.detach()
-        eng = FixedGridEngine(p.fn, p.n, p.dtype, p.device, method=p.method, t_sign=p.t_sign,
-                              perturb=o.get("perturb", False), graph=False, callbacks=p.callbacks, pieces=p.pieces)
+        eng = make_engine(p.method, p.fn, p.n, p.dtype, p.device, t_sign=p.t_sign, perturb=o.get("perturb", False),
+                          graph=False, callbacks=p.callbacks, pieces=p.pieces)
         sol, tape = eng.solve_taped(p.y0_flat, grid, p.t_cpu)
         holder["eng"] = eng
         return sol, {"kind": "fixed", "tape": tape, "grid": grid, "grid_req": grid_req, "t_req": t_req}

@@ -33,12 +33,11 @@ import torch
 
 from . import _lib
 from ._engine import AdaptiveEngine, on_solver_stream
-from ._fixed import FixedGridEngine, grid_from_step_size
+from ._adams import ADAMS_METHODS
+from ._fixed import FIXED_METHODS, grid_from_step_size, make_engine
 from ._implicit import IMPLICIT_METHODS
 
 ADAPTIVE = ("dopri5", "dopri8", "tsit5", "bosh3", "fehlberg2", "adaptive_heun")
-FIXED = ("euler", "midpoint", "heun2", "heun3", "rk4")
-ADAMS = {"explicit_adams": False, "implicit_adams": True, "fixed_adams": True}
 _CB = ("callback_step", "callback_accept_step", "callback_reject_step")
 _ADAPTIVE_KEYS = ("min_step", "max_step", "first_step", "step_t", "jump_t", "safety", "ifactor", "dfactor", "max_num_steps")
 _OUR_KEYS = ("graph", "run_ahead", "device_loop")
@@ -175,8 +174,9 @@ def make_fixed(method, **defaults):
     """Class with the interface of FixedGridODESolver (solvers.py:52-128) for one explicit fixed-step method, or of
     AdamsBashforth / AdamsBashforthMoulton (fixed_adams.py:164-228) for the Adams names, or of
     FixedGridFIRKODESolver / FixedGridDIRKODESolver (rk_common.py:378-558) for the implicit names."""
-    adams = method in ADAMS
-    implicit = method in IMPLICIT_METHODS
+    # what the iterating methods consume of the seam's options (fixed_adams.py:164-175, rk_common.py:382)
+    iter_keys = ("max_iters", "max_order") if method in ADAMS_METHODS else ("max_iters",) if method in IMPLICIT_METHODS \
+        else ()
 
     class B200FixedSolver:
         name = method
@@ -187,8 +187,7 @@ def make_fixed(method, **defaults):
                 raise _lib.TdqError("torchdiffeq_b200.plugin solvers take CUDA tensors (got %s)" % y0.device)
             self.atol = unused_kwargs.pop("atol", None)                        # solvers.py:58-61
             self.rtol = unused_kwargs.pop("rtol", None)
-            self.adams_kw = {k: unused_kwargs.pop(k) for k in ("max_iters", "max_order") if adams and k in unused_kwargs}
-            self.max_iters = unused_kwargs.pop("max_iters", 100) if implicit else None       # rk_common.py:382
+            self.iter_kw = {k: unused_kwargs.pop(k) for k in iter_keys if k in unused_kwargs}
             unused_kwargs.pop("norm", None)
             self.our = {k: unused_kwargs.pop(k) for k in _OUR_KEYS if k in unused_kwargs}
             for k, v in defaults.items():
@@ -213,19 +212,10 @@ def make_fixed(method, **defaults):
         def _make_engine(self, interp, graph):
             shape, base = self.shape, self.base
             fn = lambda t_, yf: base(t_, yf.view(shape))
-            if implicit:
-                from ._implicit import ImplicitEngine
-                return ImplicitEngine(fn, self.y0.numel(), self.y0.dtype, self.y0.device, method=method,
-                                      max_iters=self.max_iters, perturb=self.perturb, callbacks=self.callbacks,
-                                      interp=interp)
-            if adams:
-                from ._adams import AdamsEngine
-                return AdamsEngine(fn, self.y0.numel(), self.y0.dtype, self.y0.device, implicit=ADAMS[method],
-                                   rtol=self.rtol if self.rtol is not None else 1e-3,
-                                   atol=self.atol if self.atol is not None else 1e-4, perturb=self.perturb,
-                                   callbacks=self.callbacks, interp=interp, **self.adams_kw)
-            return FixedGridEngine(fn, self.y0.numel(), self.y0.dtype, self.y0.device, method=method, perturb=self.perturb,
-                                   graph=graph, callbacks=self.callbacks, interp=interp)
+            return make_engine(method, fn, self.y0.numel(), self.y0.dtype, self.y0.device, perturb=self.perturb,
+                               graph=graph, callbacks=self.callbacks, interp=interp,
+                               rtol=self.rtol if self.rtol is not None else 1e-3,
+                               atol=self.atol if self.atol is not None else 1e-4, **self.iter_kw)
 
         def integrate(self, t):                                                # solvers.py:102-128
             from .odeint import _cubic_or_linear
@@ -242,14 +232,14 @@ def make_fixed(method, **defaults):
             return sol
 
         def integrate_until_event(self, t0, event_fn):                         # solvers.py:130-164
-            from .odeint import _cubic_or_linear, fixed_event_solve
+            from .odeint import _cubic_or_linear
             assert self.step_size is not None, ("Event handling for fixed step solvers currently requires `step_size` "
                                                 "to be provided in options.")
             shape = self.shape
             with torch.no_grad(), on_solver_stream(self.y0.device) as ss:
                 eng = self._make_engine(_cubic_or_linear(self.interp), False)
                 ev = lambda t_, yf: event_fn(t_, yf.view(shape))
-                event_t, y1 = fixed_event_solve(eng, self.y0.detach().reshape(-1), t0, self.step_size, ev, float(self.atol))
+                event_t, y1 = eng.solve_until_event(self.y0.detach().reshape(-1), t0, self.step_size, ev, float(self.atol))
                 sol = torch.stack([self.y0.detach(), y1.view(shape)], dim=0)
                 ss.publish(sol)
             return event_t, sol
@@ -276,7 +266,7 @@ class _Dispatch:
         return self.gpu_cls.valid_callbacks()
 
 
-def register(solvers=None, methods=ADAPTIVE + FIXED + tuple(ADAMS) + IMPLICIT_METHODS, **defaults):
+def register(solvers=None, methods=ADAPTIVE + FIXED_METHODS + tuple(ADAMS_METHODS) + IMPLICIT_METHODS, **defaults):
     """Put the libtdq-backed solvers into a SOLVERS dict (default: the reference's, found through
     importlib.import_module('torchdiffeq._impl.odeint') -- the attribute torchdiffeq._impl.odeint is shadowed by the
     function of the same name).  In place, so torchdiffeq._impl.adjoint sees it too.  Returns the dict of replaced
