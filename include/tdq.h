@@ -421,6 +421,74 @@ int tdq_xchg_destroy(void *dev_ptr);
 int tdq_ctrl_set_exchange(void *ctrl_dev, const void *const *peer_ptrs, int32_t rank, int32_t world,
                           uint64_t epoch, void *stream);
 
+/* ---- independent step-size control per batch row (tdq_rows.cu) ----------------------------------------------------------
+ * A state of B rows x D contiguous elements where row r is solved as the reference solves odeint(func, y0[r:r+1], t) for a
+ * row-wise func: its own error ratio (RMS over its D elements), _select_initial_step, accept/reject and I-controller
+ * (misc.py:36-95, rk_common.py:266-361), max_num_steps per output interval, stage times and interpolant.  The shared
+ * control block (tdq_ctrl_init, with the ybuf/kbuf pointer table, which this mode requires) keeps what the rows share: the
+ * tableau cast to T, the options, the output times, the loop handle and the mailbox; its halt/status/done say whether the
+ * whole solve has ended.  Per-row state lives in one caller-owned device buffer of tdq_rows_size(B) bytes whose fields
+ * (B entries each) start at tdq_rows_offset(field, B): row r's accepted (y0, k_0) is ybuf[par_r] / kbuf[par_r] at
+ * elements [r*D, (r+1)*D), and accepting row r flips par_r.  A row whose output cursor has passed t[-1] is done: its stage
+ * values are copies of its y0, it enters no norm, its outputs never change.  Every reduction over a row adds in an order
+ * that depends on D only (not on B or the row's position), so a row's results do not depend on the rest of the batch.
+ * TDQ_ROWS_T_FIRST / _T_PROBE / _T_STAGE + i hold, in the state dtype, the time func sees for f0, the initial-step probe
+ * and stage i of the attempt in flight (t_sign applied): what func's time argument aliases.
+ * tdq_rows_init:            per-row state at t_start (rk_common.py:213-221).  Not needed again until the next solve.
+ * tdq_rows_sumsq:           out[r] = sum over row r of (x/scale)^2, or ((x - x2)/scale)^2 with x2; scale = atol + |y0|*rtol;
+ *                           without x2 out[B + r] = number of non-finite y0 elements of row r (misc.py:55-58, :69).
+ * tdq_rows_initial_h0 / _probe / _finish: misc.py:60-77 per row from tdq_rows_sumsq's sums; _set_first_step: options
+ *                           ['first_step'] for every row (rk_common.py:218-219).
+ * tdq_rows_prepare:         start of the first attempt for every row (rk_common.py:246-247, :269-287); y0_nonfinite_dev:
+ *                           tdq_rows_sumsq's out for x = y0 (a positive out[B + r] fails row r at :287).
+ * tdq_rows_combine / _combine_final: tdq_stage_combine / tdq_stage_combine_final with every coefficient fl_T(beta_ij *
+ *                           T(dt_r)) formed from the row's own step; done rows copy y0 (y_out) and write 0 (err_out).
+ * tdq_rows_error_norm_commit: out[r] = sum over row r of (err/tol)^2, out[B + r] = number of non-finite y1 elements of row
+ *                           r, and row r's (y1, k_last) -> ybuf/kbuf[par_r ^ 1] (rk_common.py:89, :338-352; misc.py:80-82).
+ * tdq_rows_controller:      one thread per row: accept/reject, I-controller, output cursor, fit flag, done, status, the row's
+ *                           next attempt (rk_common.py:246-247, :269-361; misc.py:85-95); then "every row done" or the
+ *                           smallest failing row ends the solve (mailbox, device-side loop condition).
+ * tdq_rows_fit_eval:        for rows whose accepted step contains output times: y_mid, the quartic, solution[j, r, :]
+ *                           (rk_common.py:363-369, interp.py:1-48).
+ * partials: tdq_rows_partials_len(B, D) doubles, zeroed once.  Row fields not listed below are private to the library. */
+typedef enum {
+    TDQ_ROWS_T0 = 0, TDQ_ROWS_T1, TDQ_ROWS_DT, TDQ_ROWS_RATIO,             /* float64: accepted interval, next dt, ratio */
+    TDQ_ROWS_ATT_T0, TDQ_ROWS_ATT_DT, TDQ_ROWS_ATT_T1, TDQ_ROWS_FIT_DT,    /* float64: attempt in flight, accepted dt    */
+    TDQ_ROWS_H0, TDQ_ROWS_D1,                                              /* float64: initial-step scratch              */
+    TDQ_ROWS_PAR, TDQ_ROWS_ACCEPT, TDQ_ROWS_FIT, TDQ_ROWS_DONE,            /* int32                                      */
+    TDQ_ROWS_STATUS, TDQ_ROWS_CURSOR, TDQ_ROWS_EMIT_LO, TDQ_ROWS_EMIT_HI,  /* int32 (status: tdq_run_status)             */
+    TDQ_ROWS_N_STEPS, TDQ_ROWS_N_ACCEPT, TDQ_ROWS_N_REJECT,                /* int64 (N_STEPS: attempts in this interval) */
+    TDQ_ROWS_T_FIRST, TDQ_ROWS_T_PROBE, TDQ_ROWS_T_STAGE,                  /* state dtype; T_STAGE + i for stage i       */
+    TDQ_ROWS_N_FIELDS = TDQ_ROWS_T_STAGE + TDQ_MAX_STAGES,
+    TDQ_ROWS_HEADER = 255       /* int32 words: [3] = the smallest failing row of the attempt that ended the solve, or -1 */
+} tdq_rows_field;
+size_t tdq_rows_size(size_t n_rows);
+size_t tdq_rows_offset(int32_t field, size_t n_rows);                     /* (size_t)-1 for an unknown field             */
+size_t tdq_rows_partials_len(size_t n_rows, size_t row_len);
+int tdq_rows_init(void *ctrl_dev, void *rows_dev, int32_t dtype, size_t n_rows, double t_start, void *stream);
+int tdq_rows_sumsq(void *ctrl_dev, void *rows_dev, int32_t dtype, const void *x, const void *x2, const double *rtol_vec,
+                   const double *atol_vec, size_t n_rows, size_t row_len, double *partials, double *out, void *stream);
+int tdq_rows_initial_h0(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *d0_sumsq, const double *d1_sumsq,
+                        size_t n_rows, size_t row_len, void *stream);
+int tdq_rows_initial_probe(void *ctrl_dev, void *rows_dev, int32_t dtype, void *y_probe, size_t n_rows, size_t row_len,
+                           void *stream);
+int tdq_rows_initial_finish(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *d2_sumsq, size_t n_rows,
+                            size_t row_len, void *stream);
+int tdq_rows_set_first_step(void *rows_dev, size_t n_rows, double first_step, void *stream);
+int tdq_rows_prepare(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *y0_nonfinite_dev, size_t n_rows,
+                     void *stream);
+int tdq_rows_combine(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, int32_t row, void *y_out,
+                     const void *const *k, size_t n_rows, size_t row_len, void *stream);
+int tdq_rows_combine_final(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, void *y1_out,
+                           void *err_out, const void *const *k, size_t n_rows, size_t row_len, void *stream);
+int tdq_rows_error_norm_commit(void *ctrl_dev, void *rows_dev, int32_t dtype, const void *err_pre, const void *k_last,
+                               const void *y1, const double *rtol_vec, const double *atol_vec, size_t n_rows,
+                               size_t row_len, double *partials, double *out, void *stream);
+int tdq_rows_controller(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in, size_t n_rows,
+                        size_t row_len, void *stream);
+int tdq_rows_fit_eval(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, const void *y1,
+                      const void *const *k, void *solution, size_t n_rows, size_t row_len, void *stream);
+
 /* ---- adjoint augmented state (adjoint.py:72-105, misc.py:137-165) ------------------------- */
 /* dst[offset_i .. offset_i + len_i) = scale_i * src_i for i < n_src, one launch
  * (the torch.cat of _TupleFunc, the unary minus on adj_y and the *(-1) of _ReverseFunc).

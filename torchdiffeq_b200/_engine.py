@@ -918,3 +918,153 @@ class AdaptiveEngine:
         h1 = h1.abs()
         dt = float(torch.min(100 * h0, h1).to(torch.float64))
         self._launch(self.lib.tdq_set_first_step(self.ctrl.data_ptr(), dt, _stream()))
+
+
+class RowsEngine(AdaptiveEngine):
+    """Independent step-size control per batch row (odeint's options={'independent_rows': True}).
+
+    The state is B rows of D contiguous elements, and row r is solved as the reference solves y0[r:r+1] on its own for a
+    row-wise func: its own initial step, error ratio, accept/reject, step size, max_num_steps count and interpolant
+    (csrc/tdq_rows.cu).  func is still called on the whole batch, with t a tensor of shape [B, 1, ...] holding each row's
+    time; finished rows see copies of their last state.  Stage slots, capture, the device-side loop and the run-ahead and
+    lock-step drivers are AdaptiveEngine's; only the launches differ."""
+
+    def __init__(self, fn, shape, dtype, device, method, **kw):
+        shape = torch.Size(shape)
+        self.B = int(shape[0])
+        self.D = int(shape[1:].numel())
+        self.row_shape = shape[1:]
+        super().__init__(fn, self.B * self.D, dtype, device, method, **kw)
+        lib, B = self.lib, self.B
+        self.rows = torch.zeros(lib.tdq_rows_size(B), dtype=torch.uint8, device=device)
+        es = torch.empty((), dtype=dtype).element_size()
+        tshape = (B,) + (1,) * (len(shape) - 1)
+
+        def field(which, dt, size):
+            o = lib.tdq_rows_offset(which, B)
+            return self.rows[o:o + B * size].view(dt)
+        self._field = field
+        self.t_first = field(_lib.ROWS_T_FIRST, dtype, es).view(tshape)     # what func's time argument aliases
+        self.t_probe = field(_lib.ROWS_T_PROBE, dtype, es).view(tshape)
+        self.t_stage = [field(_lib.ROWS_T_STAGE + i, dtype, es).view(tshape) for i in range(self.S)]
+        f64 = dict(dtype=torch.float64, device=device)
+        self.row_partials = torch.zeros(lib.tdq_rows_partials_len(B, self.D), **f64)
+        self.row_norm = torch.zeros(2 * B, **f64)                   # sums of squares, then non-finite counts
+        self.row_dsum = [torch.zeros(2 * B, **f64) for _ in range(3)]
+        self.row_n_accept = self.row_n_reject = None
+
+    def _rows_sumsq(self, x, x2, out):
+        self._launch(self.lib.tdq_rows_sumsq(
+            self.ctrl.data_ptr(), self.rows.data_ptr(), self.dt_code, x.data_ptr(),
+            x2.data_ptr() if x2 is not None else None,
+            self.rtol_vec.data_ptr() if self.rtol_vec is not None else None,
+            self.atol_vec.data_ptr() if self.atol_vec is not None else None,
+            self.B, self.D, self.row_partials.data_ptr(), out.data_ptr(), _stream()))
+
+    def _attempt_front_once(self):
+        lib, ctrl, rows, tab, dc, st = (self.lib, self.ctrl.data_ptr(), self.rows.data_ptr(), C.byref(self.tab),
+                                        self.dt_code, _stream())
+        S, B, D = self.S, self.B, self.D
+        k = [None] * (S + 1)             # k[0] = NULL: each row's k_0 (and y0) comes from its half of the pointer table
+        keep = []
+        for i in range(S):
+            if i == S - 1 and self.fsal:
+                out = self.y1
+                self._launch(lib.tdq_rows_combine_final(ctrl, rows, tab, dc, out.data_ptr(), self.errp.data_ptr(),
+                                                        _lib.ptr_array(k), B, D, st))
+            else:
+                out = self.ytmp
+                self._launch(lib.tdq_rows_combine(ctrl, rows, tab, dc, i, out.data_ptr(), _lib.ptr_array(k), B, D, st))
+            f = self._call_fn(self.t_stage[i], out, i + 1, taken=k)
+            keep.append(f)
+            k[i + 1] = f.data_ptr()
+        if not self.fsal:
+            self._launch(lib.tdq_rows_combine_final(ctrl, rows, tab, dc, self.y1.data_ptr(), self.errp.data_ptr(),
+                                                    _lib.ptr_array(k), B, D, st))
+        kp = _lib.ptr_array(k)
+        self._launch(lib.tdq_rows_error_norm_commit(
+            ctrl, rows, dc, self.errp.data_ptr(), k[S], self.y1.data_ptr(),
+            self.rtol_vec.data_ptr() if self.rtol_vec is not None else None,
+            self.atol_vec.data_ptr() if self.atol_vec is not None else None,
+            B, D, self.row_partials.data_ptr(), self.row_norm.data_ptr(), st))
+        self._launch(lib.tdq_rows_controller(ctrl, rows, dc, self.row_norm.data_ptr(), B, D, st))
+        return k, kp, keep
+
+    def _attempt_back(self, kp):
+        self._launch(self.lib.tdq_rows_fit_eval(self.ctrl.data_ptr(), self.rows.data_ptr(), C.byref(self.tab),
+                                                self.dt_code, self.y1.data_ptr(), kp, self.solution.data_ptr(),
+                                                self.B, self.D, _stream()))
+
+    def _begin(self, y0_flat, t64, t_start=None, loop=False):
+        """rk_common.py:166-241 for every row: f0 on the whole batch, then each row's initial step."""
+        lib = self.lib
+        self.nfe_total += self.nfe
+        self.nfe, self.launches = 0, 0
+        n_out = int(t64.numel())
+        self.t_out = t64.contiguous()
+        if getattr(self, "solution", None) is None or self.solution.shape[0] != n_out:
+            self.solution = torch.empty(n_out, self.n, dtype=self.dtype, device=self.device)
+            self._drop_graph()
+            self._own_ptrs = None
+            loop = False
+        self.solution[0].copy_(y0_flat)
+        self.ybuf[0].copy_(y0_flat)
+        st = _stream()
+        mb = self.mbox_host.contents
+        mb.seq, mb.status, mb.done, mb.par, mb.accept = 0, 0, 0, 0, 0
+        mb.n_accept, mb.n_reject = 0, 0
+        if t_start is None:
+            t_start = float(t64[0])
+        self.opt.loop_handle = self._loop_handle if loop else 0
+        ctrl, rows, dc, B, D = self.ctrl.data_ptr(), self.rows.data_ptr(), self.dt_code, self.B, self.D
+        _lib.check(lib.tdq_ctrl_init(ctrl, C.byref(self.tab), C.byref(self.opt), self.t_out.data_ptr(), float(t_start),
+                                     n_out, self.mbox_dev, st))
+        self._launch(lib.tdq_rows_init(ctrl, rows, dc, B, float(t_start), st))
+        f0 = self._call_fn(self.t_first, self.ybuf[0], 0, dst=self.kbuf[0])
+        if f0.data_ptr() != self.kbuf[0].data_ptr():
+            self.kbuf[0].copy_(f0)
+        del f0
+        d = self.row_dsum
+        self._rows_sumsq(self.ybuf[0], None, d[0])                 # also counts each row's non-finite y0 elements
+        if self.first_step is None:                                 # misc.py:36-77, row by row
+            self._rows_sumsq(self.kbuf[0], None, d[1])
+            self._launch(lib.tdq_rows_initial_h0(ctrl, rows, dc, d[0].data_ptr(), d[1].data_ptr(), B, D, st))
+            self._launch(lib.tdq_rows_initial_probe(ctrl, rows, dc, self.ytmp.data_ptr(), B, D, st))
+            f1 = self._call_fn(self.t_probe, self.ytmp, 1)
+            self._rows_sumsq(f1, self.kbuf[0], d[2])
+            del f1
+            self._launch(lib.tdq_rows_initial_finish(ctrl, rows, dc, d[2].data_ptr(), B, D, st))
+        else:
+            self._launch(lib.tdq_rows_set_first_step(rows, B, float(self.first_step), st))
+        self._launch(lib.tdq_rows_prepare(ctrl, rows, dc, d[0].data_ptr() if n_out > 1 else None, B, st))
+        return n_out
+
+    def row_field(self, which, dtype):
+        return self._field(which, dtype, torch.empty((), dtype=dtype).element_size())
+
+    def _raise_if_failed(self, mb):
+        s = mb.status
+        if s == _lib.RUN_OK:
+            return
+        torch.cuda.current_stream().synchronize()
+        r = int(self.rows[:16].view(torch.int32)[3])               # the smallest failing row
+        where = " (row %d)" % r
+        if s == _lib.RUN_DT_UNDERFLOW:
+            raise SolverFailure("underflow in dt {}".format(float(self.row_field(_lib.ROWS_ATT_DT, torch.float64)[r]))
+                                + where)
+        if s == _lib.RUN_NONFINITE:
+            par = int(self.row_field(_lib.ROWS_PAR, torch.int32)[r])
+            y = self.ybuf[par][r * self.D:(r + 1) * self.D].view(1, *self.row_shape)      # y0[r:r+1]
+            raise SolverFailure("non-finite values in state `y`: {}".format(y) + where)
+        if s == _lib.RUN_MAX_STEPS:
+            m = self.opt.max_num_steps
+            raise SolverFailure("max_num_steps exceeded ({}>={})".format(m, m) + where)
+        raise SolverFailure("solver failed with status %d" % s + where)
+
+    def solve(self, y0_flat, t64, t_start=None):
+        sol = super().solve(y0_flat, t64, t_start)
+        self.row_n_accept = self.row_field(_lib.ROWS_N_ACCEPT, torch.int64).cpu()
+        self.row_n_reject = self.row_field(_lib.ROWS_N_REJECT, torch.int64).cpu()
+        self.n_accept, self.n_reject = int(self.row_n_accept.sum()), int(self.row_n_reject.sum())
+        self.n_attempts = int((self.row_n_accept + self.row_n_reject).max())   # loop iterations that did work
+        return sol

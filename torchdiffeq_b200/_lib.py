@@ -12,6 +12,11 @@ TDQ_MAX_SEGS = 64
 TDQ_F32, TDQ_F64 = 0, 1
 RUN_OK, RUN_DT_UNDERFLOW, RUN_NONFINITE, RUN_MAX_STEPS, RUN_EXCHANGE_TIMEOUT = 0, 1, 2, 3, 4
 TDQ_MAX_RANKS = 16
+# tdq_rows_field (include/tdq.h)
+(ROWS_T0, ROWS_T1, ROWS_DT, ROWS_RATIO, ROWS_ATT_T0, ROWS_ATT_DT, ROWS_ATT_T1, ROWS_FIT_DT, ROWS_H0, ROWS_D1, ROWS_PAR,
+ ROWS_ACCEPT, ROWS_FIT, ROWS_DONE, ROWS_STATUS, ROWS_CURSOR, ROWS_EMIT_LO, ROWS_EMIT_HI, ROWS_N_STEPS, ROWS_N_ACCEPT,
+ ROWS_N_REJECT, ROWS_T_FIRST, ROWS_T_PROBE, ROWS_T_STAGE) = range(24)
+ROWS_HEADER = 255
 ABI_VERSION = 2
 
 
@@ -123,6 +128,21 @@ _SIGNATURES = {
     "tdq_implicit_solve": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _i32, _i32, _dbl, _vp]),
     "tdq_implicit_update": (C.c_int, [_i32, _vp, _i32, _sz, _pp, _pp, _i32, _i64, _i32, _vp, _vp, _vp, _vp, _pp, _pdbl,
                                       _i32, _vp, _vp, _vp]),
+    "tdq_rows_size": (_sz, [_sz]),
+    "tdq_rows_offset": (_sz, [_i32, _sz]),
+    "tdq_rows_partials_len": (_sz, [_sz, _sz]),
+    "tdq_rows_init": (C.c_int, [_vp, _vp, _i32, _sz, _dbl, _vp]),
+    "tdq_rows_sumsq": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _sz, _sz, _vp, _vp, _vp]),
+    "tdq_rows_initial_h0": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _sz, _sz, _vp]),
+    "tdq_rows_initial_probe": (C.c_int, [_vp, _vp, _i32, _vp, _sz, _sz, _vp]),
+    "tdq_rows_initial_finish": (C.c_int, [_vp, _vp, _i32, _vp, _sz, _sz, _vp]),
+    "tdq_rows_set_first_step": (C.c_int, [_vp, _sz, _dbl, _vp]),
+    "tdq_rows_prepare": (C.c_int, [_vp, _vp, _i32, _vp, _sz, _vp]),
+    "tdq_rows_combine": (C.c_int, [_vp, _vp, _ptab, _i32, _i32, _vp, _pp, _sz, _sz, _vp]),
+    "tdq_rows_combine_final": (C.c_int, [_vp, _vp, _ptab, _i32, _vp, _vp, _pp, _sz, _sz, _vp]),
+    "tdq_rows_error_norm_commit": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _vp, _vp, _vp]),
+    "tdq_rows_controller": (C.c_int, [_vp, _vp, _i32, _vp, _sz, _sz, _vp]),
+    "tdq_rows_fit_eval": (C.c_int, [_vp, _vp, _ptab, _i32, _vp, _pp, _vp, _sz, _sz, _vp]),
     "tdq_xchg_create": (C.c_int, [_pp, C.POINTER(IpcHandle)]),
     "tdq_xchg_open": (C.c_int, [C.POINTER(IpcHandle), _pp]),
     "tdq_xchg_close": (C.c_int, [_vp]),

@@ -376,6 +376,8 @@ def odeint_adjoint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=No
                    adjoint_rtol=None, adjoint_atol=None, adjoint_method=None, adjoint_options=None,
                    adjoint_params=None):
     """adjoint.py:156-223, same signature and defaults."""
+    if options and options.get("independent_rows"):
+        raise NotImplementedError("options['independent_rows'] does not support odeint_adjoint")
     if adjoint_params is None and not isinstance(func, nn.Module):                     # adjoint.py:161-164
         raise ValueError('func must be an instance of nn.Module to specify the adjoint parameters; alternatively they '
                          'can be specified explicitly via the `adjoint_params` argument. If there are no parameters '

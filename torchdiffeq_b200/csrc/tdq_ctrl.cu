@@ -6,16 +6,9 @@
 // host, so a whole attempt can sit inside a CUDA graph.
 #include "tdq_common.cuh"
 #include "tdq_shape.cuh"
+#include "tdq_step.cuh"
 
 namespace {
-
-template <typename T> __device__ __forceinline__ T prev_repr(T t);   // misc.py:358-364, Perturb.PREV
-template <> __device__ __forceinline__ float prev_repr<float>(float t) { return nextafterf(t, __fsub_rn(t, 1.0f)); }
-template <> __device__ __forceinline__ double prev_repr<double>(double t) { return nextafter(t, __dsub_rn(t, 1.0)); }
-
-template <typename T> __device__ __forceinline__ T next_repr(T t);   // Perturb.NEXT
-template <> __device__ __forceinline__ float next_repr<float>(float t) { return nextafterf(t, __fadd_rn(t, 1.0f)); }
-template <> __device__ __forceinline__ double next_repr<double>(double t) { return nextafter(t, __dadd_rn(t, 1.0)); }
 
 template <typename T> __device__ __forceinline__ void store_T(unsigned char *raw, int i, T v) {
     reinterpret_cast<T *>(raw)[i] = v;
@@ -232,19 +225,7 @@ __device__ void controller(TdqCtrl &c, const double *norm_in, int n_seg, const v
         c.n_reject += 1;
     }
 
-    // misc.py:85-95 _optimal_step_size (float64), then the clamp of rk_common.py:359
-    double dt_next;
-    if (ratio == 0.0) {
-        dt_next = dt * c.ifactor;
-    } else {
-        const double dfac = (ratio < 1.0) ? 1.0 : c.dfactor;
-        const double expo = 1.0 / (double)c.order;
-        const double cand = c.safety / pow(ratio, expo);
-        double inner = (cand != cand || dfac != dfac) ? CUDART_NAN : fmax(cand, dfac);   // torch.max
-        double factor = (inner != inner) ? CUDART_NAN : fmin(c.ifactor, inner);          // torch.min
-        dt_next = dt * factor;
-    }
-    if (dt_next == dt_next) dt_next = fmin(fmax(dt_next, c.min_step), c.max_step);
+    const double dt_next = tdq_next_dt(ratio, dt, c.safety, c.ifactor, c.dfactor, c.order, c.min_step, c.max_step);
     c.dt = dt_next;
 
     // Output cursor: solvers.py:33-34 asks for t[i] one at a time; every t[i] <= t1 is now covered
@@ -357,16 +338,7 @@ k_controller(TdqCtrl *c, const double *norm_in, const int64_t *cnt, int n_seg, c
 template <typename T>
 __device__ void initial_h0(TdqCtrl &c, double d0d, double d1d) {
     using A = Ar<T>;
-    double h0;
-    if (c.ratio_f64) {
-        h0 = (d0d < 1e-5 || d1d < 1e-5) ? (double)(T)1e-6 : fabs(0.01 * d0d / d1d);
-    } else {
-        const T d0 = (T)d0d, d1 = (T)d1d;
-        T h;
-        if (d0 < (T)1e-5 || d1 < (T)1e-5) h = (T)1e-6;                 // :60-61 (compare after promoting 1e-5)
-        else h = A::div(A::mul((T)0.01, d0), d1);                      // :63
-        h0 = (double)A::abs(h);
-    }
+    const double h0 = tdq_initial_h0<T>(c.ratio_f64 != 0, d0d, d1d);
     c.h0 = h0;
     c.ratio = d1d;                                                     // stash d1 for the finish kernel
     // probe time: t0 (f64) + h0 -> f64, cast to T by _PerturbFunc (misc.py:66-67, :187)
@@ -377,35 +349,7 @@ __device__ void initial_h0(TdqCtrl &c, double d0d, double d1d) {
 // misc.py:69-77
 template <typename T>
 __device__ void initial_finish(TdqCtrl &c, double nd) {
-    using A = Ar<T>;
-    double dt;
-    const double order_p1 = (double)c.order;                           // called with order-1 (rk_common.py:217)
-    if (c.ratio_f64) {
-        const double d1 = c.ratio, h0 = c.h0;
-        const double d2 = fabs(nd / h0);
-        double h1;
-        if (d1 <= 1e-15 && d2 <= 1e-15) h1 = fmax((double)(T)1e-6, h0 * 1e-3);
-        else h1 = pow(0.01 / ((d2 > d1) ? d2 : d1), 1.0 / order_p1);
-        h1 = fabs(h1);
-        dt = fmin(100.0 * h0, h1);
-    } else {
-        const T d1 = (T)c.ratio, h0 = (T)c.h0;
-        const T d2 = A::abs(A::div((T)nd, h0));
-        T h1;
-        if (d1 <= (T)1e-15 && d2 <= (T)1e-15) {
-            const T a = (T)1e-6, b = A::mul(h0, (T)1e-3);
-            h1 = (a != a || b != b) ? (T)CUDART_NAN : (a > b ? a : b);
-        } else {
-            const T m = (d2 > d1) ? d2 : d1;                           // Python max(d1, d2)
-            const T base = A::div((T)0.01, m);
-            const T ex = (T)(1.0 / order_p1);
-            h1 = (T)pow((double)base, (double)ex);
-        }
-        h1 = A::abs(h1);
-        const T a = A::mul((T)100, h0);
-        const T r = (a != a || h1 != h1) ? (T)CUDART_NAN : (a < h1 ? a : h1);   // torch.min
-        dt = (double)r;
-    }
+    const double dt = tdq_initial_finish<T>(c.ratio_f64 != 0, c.order, c.ratio, c.h0, nd);
     c.dt = dt;
 }
 

@@ -1,0 +1,820 @@
+// tdq_rows.cu -- independent step-size control per batch row (include/tdq.h, "independent step-size control per batch row").
+//
+// The state is B rows of D contiguous elements; row r follows the reference's adaptive loop on its own (rk_common.py:213-369,
+// misc.py:36-95): its own dt, error ratio, accept/reject, output cursor and interpolant.  The shared control block keeps what
+// the rows share (tableau cast to T, options, output times, pointer table, loop handle, mailbox); per-row scalars live in the
+// caller's row buffer, one field of B entries per scalar.
+//
+// Work decomposition of every per-element kernel: a UNIT is one chunk of at most kChunk elements of one row and is taken by
+// one warp (8 units per block).  A unit reads its row's scalars once, so rows need no per-coefficient tables and a done or
+// not-fitting row costs one flag load.  Lane l of a unit takes the unit's elements l, l+32, ... -- for the norms that fixes
+// the order of every row's sum by D alone: lane-sequential, then the warp's shuffle tree, then (rows of several chunks)
+// chunk partials added in index order by the row's last unit to finish.  The streaming combines use 128-bit accesses inside a
+// row where the flat addresses allow it and scalar code at row edges.
+#include <climits>
+
+#include "tdq_common.cuh"
+#include "tdq_shape.cuh"
+#include "tdq_step.cuh"
+
+namespace {
+
+constexpr int kThreads = 256, kWarps = kThreads / 32;
+constexpr size_t kChunk = 1024;          // elements per unit
+constexpr size_t kHdr = 256;             // header bytes: int32 words [0] ticket, [1] active, [2] failing-row minimum, [3] result
+
+struct Rows {
+    unsigned char *base;
+    size_t slot;                          // bytes per field: 8*B rounded up to 256
+    int B;
+};
+inline size_t rows_slot(size_t B) { return (8 * B + 255) & ~size_t(255); }
+inline Rows make_rows(void *p, size_t B) { return Rows{(unsigned char *)p, rows_slot(B), (int)B}; }
+template <typename X> __device__ __forceinline__ X *fld(const Rows &R, int which) {
+    return reinterpret_cast<X *>(R.base + kHdr + (size_t)which * R.slot);
+}
+__device__ __forceinline__ int *hdr(const Rows &R) { return reinterpret_cast<int *>(R.base); }
+
+struct Geom {
+    size_t D;
+    size_t nch;                           // units per row
+    size_t units;                         // B * nch
+};
+inline Geom make_geom(size_t B, size_t D) {
+    Geom g;
+    g.D = D;
+    g.nch = (D + kChunk - 1) / kChunk;
+    g.units = B * g.nch;
+    return g;
+}
+inline unsigned unit_blocks(const Geom &g) { return tdq_grid(g.units, kWarps, 0); }
+inline unsigned row_blocks(size_t B) { return tdq_grid(B, kThreads, 0); }
+
+// This warp's unit: row r, elements [lo, hi) of the row.  False for the spare warps of the last block.
+__device__ __forceinline__ bool unit_of(const Geom &g, size_t &u, int &r, size_t &lo, size_t &hi) {
+    u = (size_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (u >= g.units) return false;
+    r = (int)(u / g.nch);
+    lo = (u % g.nch) * kChunk;
+    hi = lo + kChunk < g.D ? lo + kChunk : g.D;
+    return true;
+}
+
+// Elements [lo, hi) of the row starting at flat index `base`: scalar fs(i) at the edges, vector fv(i) (i = first element of a
+// 16-byte aligned vector) inside when `vec` (every operand's base address 16-byte aligned).
+template <typename T, typename FV, typename FS>
+__device__ __forceinline__ void row_span(size_t base, size_t lo, size_t hi, bool vec, FV &&fv, FS &&fs) {
+    constexpr size_t VN = Vec<T>::N;
+    const size_t lane = threadIdx.x & 31;
+    if (!vec) {
+        for (size_t i = lo + lane; i < hi; i += 32) fs(i);
+        return;
+    }
+    // flat indices, so that nothing wraps when the span is shorter than a vector
+    size_t fa = (base + lo + VN - 1) / VN * VN;                  // first vector-aligned element of the span
+    if (fa > base + hi) fa = base + hi;
+    size_t fb = (base + hi) / VN * VN;                           // end of the last whole vector
+    if (fb < fa) fb = fa;
+    const size_t a = fa - base, b = fb - base;
+    for (size_t i = lo + lane; i < a; i += 32) fs(i);
+    for (size_t i = a + lane * VN; i < b; i += 32 * VN) fv(i);
+    for (size_t i = b + lane; i < hi; i += 32) fs(i);
+}
+
+// ---- stage combines (rk_common.py:79, :83-89) -----------------------------------------------------------------------------
+template <typename T, int NK>
+__global__ void __launch_bounds__(kThreads)
+k_rows_combine(const TdqCtrl *__restrict__ c, Rows R, Geom g, int row, T *__restrict__ out, KPtrs kp, bool vec) {
+    if (c->halt) return;
+    using A = Ar<T>;
+    using V = Vec<T>;
+    size_t u, lo, hi;
+    int r;
+    if (!unit_of(g, u, r, lo, hi)) return;
+    const int par = fld<int>(R, TDQ_ROWS_PAR)[r];
+    const size_t base = (size_t)r * g.D;
+    const T *y0 = reinterpret_cast<const T *>(c->ybuf[par]) + base;
+    T *o = out + base;
+    if (fld<int>(R, TDQ_ROWS_DONE)[r]) {                                  // a done row: copies of its y0, no arithmetic
+        row_span<T>(base, lo, hi, vec, [&](size_t i) { st_vec<T>(o + i, ld_stream<T>(y0 + i)); },
+                    [&](size_t i) { o[i] = y0[i]; });
+        return;
+    }
+    const T dtT = (T)fld<double>(R, TDQ_ROWS_ATT_DT)[r], sgn = (T)c->t_sign;
+    T cf[NK];
+    const T *k[NK];
+#pragma unroll
+    for (int m = 0; m < NK; ++m) {
+        cf[m] = A::mul(sgn, A::mul((T)c->beta[row][m], dtT));             // t_sign * fl_T(beta_ij * T(dt_r))
+        k[m] = reinterpret_cast<const T *>(kp.p[m] ? kp.p[m] : c->kbuf[par]) + base;
+    }
+    auto one = [&](T y, const T *kv) {
+        T acc = A::mul(kv[0], cf[0]);
+#pragma unroll
+        for (int m = 1; m < NK; ++m) acc = A::add(acc, A::mul(kv[m], cf[m]));
+        return A::add(y, acc);
+    };
+    row_span<T>(base, lo, hi, vec,
+        [&](size_t i) {
+            V a = ld_stream<T>(y0 + i), kv[NK], res;
+#pragma unroll
+            for (int m = 0; m < NK; ++m) kv[m] = ld_stream<T>(k[m] + i);
+#pragma unroll
+            for (int e = 0; e < V::N; ++e) {
+                T ke[NK];
+#pragma unroll
+                for (int m = 0; m < NK; ++m) ke[m] = kv[m].v[e];
+                res.v[e] = one(a.v[e], ke);
+            }
+            st_vec<T>(o + i, res);
+        },
+        [&](size_t i) {
+            T ke[NK];
+#pragma unroll
+            for (int m = 0; m < NK; ++m) ke[m] = k[m][i];
+            o[i] = one(y0[i], ke);
+        });
+}
+
+struct RowFinalMap {
+    signed char rpos[TDQ_MAX_K];
+    signed char epos[TDQ_MAX_K];
+};
+
+template <typename T, int NU>
+__global__ void __launch_bounds__(kThreads)
+k_rows_combine_final(const TdqCtrl *__restrict__ c, Rows R, Geom g, int row, T *__restrict__ out, T *__restrict__ err_out,
+                     KPtrs kp, RowFinalMap fm, bool vec) {
+    if (c->halt) return;
+    using A = Ar<T>;
+    using V = Vec<T>;
+    size_t u, lo, hi;
+    int r;
+    if (!unit_of(g, u, r, lo, hi)) return;
+    const int par = fld<int>(R, TDQ_ROWS_PAR)[r];
+    const size_t base = (size_t)r * g.D;
+    const T *y0 = reinterpret_cast<const T *>(c->ybuf[par]) + base;
+    T *o = out + base, *eo = err_out + base;
+    if (fld<int>(R, TDQ_ROWS_DONE)[r]) {
+        row_span<T>(base, lo, hi, vec,
+            [&](size_t i) {
+                V z;
+#pragma unroll
+                for (int e = 0; e < V::N; ++e) z.v[e] = (T)0;
+                st_vec<T>(o + i, ld_stream<T>(y0 + i));
+                st_vec<T>(eo + i, z);
+            },
+            [&](size_t i) { o[i] = y0[i]; eo[i] = (T)0; });
+        return;
+    }
+    const T dtT = (T)fld<double>(R, TDQ_ROWS_ATT_DT)[r], sgn = (T)c->t_sign;
+    T cr[NU], ce[NU];
+    unsigned mask_r = 0, mask_e = 0;
+    const T *k[NU];
+#pragma unroll
+    for (int m = 0; m < NU; ++m) {
+        const bool ur = fm.rpos[m] >= 0, ue = fm.epos[m] >= 0;
+        if (ur) mask_r |= 1u << m;
+        if (ue) mask_e |= 1u << m;
+        cr[m] = ur ? A::mul(sgn, A::mul((T)c->beta[row][fm.rpos[m]], dtT)) : (T)0;
+        ce[m] = ue ? A::mul(sgn, A::mul(dtT, (T)c->c_err[fm.epos[m]])) : (T)0;
+        k[m] = reinterpret_cast<const T *>(kp.p[m] ? kp.p[m] : c->kbuf[par]) + base;
+    }
+    auto element = [&](T y, const T *kv, T &yo, T &ev) {
+        T ar = (T)0, ae = (T)0;
+        bool fr = true, fe = true;
+#pragma unroll
+        for (int m = 0; m < NU; ++m) {
+            if ((mask_r >> m) & 1u) {
+                const T p = A::mul(kv[m], cr[m]);
+                ar = fr ? p : A::add(ar, p);
+                fr = false;
+            }
+            if ((mask_e >> m) & 1u) {
+                const T p = A::mul(kv[m], ce[m]);
+                ae = fe ? p : A::add(ae, p);
+                fe = false;
+            }
+        }
+        yo = A::add(y, ar);
+        ev = ae;
+    };
+    row_span<T>(base, lo, hi, vec,
+        [&](size_t i) {
+            V a = ld_stream<T>(y0 + i), kv[NU], ry, re;
+#pragma unroll
+            for (int m = 0; m < NU; ++m) kv[m] = ld_stream<T>(k[m] + i);
+#pragma unroll
+            for (int e = 0; e < V::N; ++e) {
+                T ke[NU];
+#pragma unroll
+                for (int m = 0; m < NU; ++m) ke[m] = kv[m].v[e];
+                element(a.v[e], ke, ry.v[e], re.v[e]);
+            }
+            st_vec<T>(o + i, ry);
+            st_vec<T>(eo + i, re);
+        },
+        [&](size_t i) {
+            T ke[NU];
+#pragma unroll
+            for (int m = 0; m < NU; ++m) ke[m] = k[m][i];
+            element(y0[i], ke, o[i], eo[i]);
+        });
+}
+
+// ---- row norms (misc.py:55-58, :69, :80-82; MODE as in tdq_norm.cu) and the candidate commit (rk_common.py:338-352) ------
+struct RowNormArgs {
+    const void *x, *x2, *y1;
+    const double *rtol_v, *atol_v;
+    double *partials;                     // [0..1] unused; sums[units]; bad[units]; a uint32 ticket per row (rows of several units)
+    double *out;                          // [2B]: sums, then non-finite counts
+};
+
+template <typename T, int MODE, bool VTOL>
+__global__ void __launch_bounds__(kThreads)
+k_rows_norm(const TdqCtrl *__restrict__ c, Rows R, Geom g, RowNormArgs a) {
+    if (c->halt) return;
+    using A = Ar<T>;
+    using Q = typename std::conditional<VTOL, double, T>::type;
+    size_t u, lo, hi;
+    int r;
+    const bool have = unit_of(g, u, r, lo, hi);
+    const int lane = threadIdx.x & 31;
+    double acc = 0.0, bad = 0.0;
+    if (have && !(MODE == 0 && fld<int>(R, TDQ_ROWS_DONE)[r])) {
+        const int par = fld<int>(R, TDQ_ROWS_PAR)[r];
+        const size_t base = (size_t)r * g.D;
+        const T *y0 = reinterpret_cast<const T *>(c->ybuf[par]) + base;
+        const T *x = reinterpret_cast<const T *>(a.x) + base;
+        const T *x2 = (MODE != 1) ? reinterpret_cast<const T *>(a.x2) + base : nullptr;
+        const T *y1 = (MODE == 0) ? reinterpret_cast<const T *>(a.y1) + base : nullptr;
+        T *ycand = nullptr, *kcand = nullptr;
+        T ecS = (T)0;
+        bool ek = false;
+        if (MODE == 0) {
+            ycand = reinterpret_cast<T *>(c->ybuf[par ^ 1]) + base;
+            kcand = reinterpret_cast<T *>(c->kbuf[par ^ 1]) + base;
+            // the last error weight, when it belongs to k_S of an FSAL tableau, is not in the prefix
+            ek = c->fsal && c->err_nnz > 0 && c->err_idx[c->err_nnz - 1] == c->n_stages;
+            if (ek) ecS = A::mul((T)c->t_sign, A::mul((T)fld<double>(R, TDQ_ROWS_ATT_DT)[r], (T)c->c_err[c->err_nnz - 1]));
+        }
+        const T rtolT = (T)c->rtol, atolT = (T)c->atol;
+#pragma unroll 4
+        for (size_t i = lo + lane; i < hi; i += 32) {
+            const T v0 = y0[i], xa = x[i];
+            const T xb = (MODE != 1) ? x2[i] : (T)0;
+            const T v1 = (MODE == 0) ? y1[i] : (T)0;
+            if (MODE == 0) {
+                ycand[i] = v1;
+                kcand[i] = xb;
+                if (!A::finite(v1)) bad += 1.0;
+            }
+            if (MODE == 1 && !A::finite(v0)) bad += 1.0;
+            T num;
+            if (MODE == 0) num = ek ? A::add(xa, A::mul(xb, ecS)) : xa;
+            else num = (MODE == 2) ? A::sub(xa, xb) : xa;
+            Q q;
+            if (VTOL) {
+                const double rt = a.rtol_v[base + i], at = a.atol_v[base + i];
+                const double tol = (MODE == 0) ? at + rt * (double)A::max_nan(A::abs(v0), A::abs(v1))
+                                               : at + (double)A::abs(v0) * rt;
+                q = (Q)((double)num / tol);
+            } else {
+                const T tol = (MODE == 0) ? A::add(atolT, A::mul(rtolT, A::max_nan(A::abs(v0), A::abs(v1))))
+                                          : A::add(atolT, A::mul(A::abs(v0), rtolT));
+                q = (Q)A::div(num, tol);
+            }
+            acc += (double)Ar<Q>::mul(q, q);
+        }
+    }
+    acc = warp_sum(acc);
+    bad = warp_sum(bad);
+    if (have && lane == 0) {
+        if (g.nch == 1) {
+            a.out[r] = acc;
+            a.out[R.B + r] = bad;
+        } else {
+            a.partials[2 + u] = acc;
+            a.partials[2 + g.units + u] = bad;
+        }
+    }
+    if (g.nch == 1 || !have) return;
+    // rows of several units: the last unit of a row to finish adds that row's unit partials in index order (a ticket per
+    // row, so the serial sums of different rows run in different warps)
+    if (lane == 0) {
+        unsigned int *ticket = reinterpret_cast<unsigned int *>(a.partials + 2 + 2 * g.units) + r;
+        __threadfence();
+        if (atomicAdd(ticket, 1u) == (unsigned)g.nch - 1) {
+            __threadfence();
+            double s = 0.0, b = 0.0;
+            const double *ps = a.partials + 2 + (size_t)r * g.nch, *pb = ps + g.units;
+            for (size_t ch = 0; ch < g.nch; ++ch) {
+                s += __ldcg(ps + ch);
+                b += __ldcg(pb + ch);
+            }
+            a.out[r] = s;
+            a.out[R.B + r] = b;
+            *ticket = 0;                                                  // self-reset for the next launch
+        }
+    }
+}
+
+// ---- dense output (rk_common.py:363-369, interp.py:1-48) ------------------------------------------------------------------
+template <typename T> __device__ __forceinline__ T eval_poly(T e, T d, T cq, T b, T a, T x) {
+    using A = Ar<T>;
+    T total = A::add(e, A::mul(x, d));
+    T xp = A::mul(x, x);
+    total = A::add(total, A::mul(xp, cq));
+    xp = A::mul(xp, x);
+    total = A::add(total, A::mul(xp, b));
+    xp = A::mul(xp, x);
+    total = A::add(total, A::mul(xp, a));
+    return total;
+}
+
+template <typename T, int NK>
+__global__ void __launch_bounds__(kThreads)
+k_rows_fit_eval(const TdqCtrl *__restrict__ c, Rows R, Geom g, const T *__restrict__ y1p, const T *__restrict__ kSp,
+                KPtrs kmid, T *__restrict__ solution, size_t n) {
+    using A = Ar<T>;
+    size_t u, lo, hi;
+    int r;
+    if (!unit_of(g, u, r, lo, hi) || !fld<int>(R, TDQ_ROWS_FIT)[r]) return;
+    const int par = fld<int>(R, TDQ_ROWS_PAR)[r] ^ 1;                    // the pair the accepted step started from
+    const size_t base = (size_t)r * g.D;
+    const T *y0 = reinterpret_cast<const T *>(c->ybuf[par]) + base;
+    const T *f0p = reinterpret_cast<const T *>(c->kbuf[par]) + base;
+    const T *y1 = y1p + base, *f1p = kSp + base;
+    const T dtT = (T)fld<double>(R, TDQ_ROWS_FIT_DT)[r], sgn = (T)c->t_sign;
+    const T sdt = A::mul(sgn, dtT), two_sdt = A::mul((T)2, sdt);
+    T mf[NK];
+    const T *km[NK];
+#pragma unroll
+    for (int m = 0; m < NK; ++m) {
+        mf[m] = A::mul(sgn, A::mul(dtT, (T)c->c_mid[m]));
+        km[m] = kmid.p[m] ? reinterpret_cast<const T *>(kmid.p[m]) + base : f0p;
+    }
+    const int jlo = fld<int>(R, TDQ_ROWS_EMIT_LO)[r], jhi = fld<int>(R, TDQ_ROWS_EMIT_HI)[r];
+    const double t0 = fld<double>(R, TDQ_ROWS_T0)[r], t1 = fld<double>(R, TDQ_ROWS_T1)[r];
+    const int lane = threadIdx.x & 31;
+    for (size_t i = lo + lane; i < hi; i += 32) {
+        const T y0v = y0[i], y1v = y1[i], f0 = f0p[i], f1 = f1p[i];
+        T acc = A::mul(km[0][i], mf[0]);
+#pragma unroll
+        for (int m = 1; m < NK; ++m) acc = A::add(acc, A::mul(km[m][i], mf[m]));
+        const T ymid = A::add(y0v, acc);
+        const T a = A::add(A::sub(A::mul(two_sdt, A::sub(f1, f0)), A::mul((T)8, A::add(y1v, y0v))), A::mul((T)16, ymid));
+        const T b = A::sub(A::add(A::add(A::mul(sdt, A::sub(A::mul((T)5, f0), A::mul((T)3, f1))), A::mul((T)18, y0v)),
+                                  A::mul((T)14, y1v)),
+                           A::mul((T)32, ymid));
+        const T cq = A::add(A::sub(A::sub(A::mul(sdt, A::sub(f1, A::mul((T)4, f0))), A::mul((T)11, y0v)),
+                                   A::mul((T)5, y1v)),
+                            A::mul((T)16, ymid));
+        const T d = A::mul(sdt, f0);
+        for (int j = jlo; j < jhi; ++j) {
+            const T x = (T)((c->t_out[j] - t0) / (t1 - t0));
+            solution[(size_t)j * n + base + i] = eval_poly<T>(y0v, d, cq, b, a, x);
+        }
+    }
+}
+
+// ---- per-row scalar work: one thread per row ------------------------------------------------------------------------------
+// rk_common.py:246-247, :269-287 and the stage times of :72-78 for the attempt that starts at the row's t1.
+template <typename T> __device__ void row_prepare(const TdqCtrl &c, const Rows &R, int r, bool y0_bad) {
+    using A = Ar<T>;
+    int *status = fld<int>(R, TDQ_ROWS_STATUS);
+    if (fld<int64_t>(R, TDQ_ROWS_N_STEPS)[r] >= c.max_num_steps) {       // :247
+        status[r] = TDQ_RUN_MAX_STEPS;
+        return;
+    }
+    double dt = fld<double>(R, TDQ_ROWS_DT)[r];
+    if (!isfinite(dt)) dt = c.min_step;                                   // :269-270
+    dt = fmin(fmax(dt, c.min_step), c.max_step);                          // :271
+    const double t0 = fld<double>(R, TDQ_ROWS_T1)[r];
+    const double t1 = t0 + dt;                                            // :273
+    fld<double>(R, TDQ_ROWS_ATT_T0)[r] = t0;
+    fld<double>(R, TDQ_ROWS_ATT_DT)[r] = dt;
+    if (!(t0 + dt > t0)) {                                                // :286
+        status[r] = TDQ_RUN_DT_UNDERFLOW;
+        return;
+    }
+    if (y0_bad) {                                                         // :287 (later attempts: the controller)
+        status[r] = TDQ_RUN_NONFINITE;
+        return;
+    }
+    fld<double>(R, TDQ_ROWS_ATT_T1)[r] = t1;
+    const T t0T = (T)t0, dtT = (T)dt, t1T = (T)t1, sgn = (T)c.t_sign;
+    for (int i = 0; i < c.n_stages; ++i) {
+        const T a = (T)c.alpha[i];
+        const T ti = (a == (T)1) ? prev_repr<T>(t1T) : A::add(t0T, A::mul(a, dtT));
+        fld<T>(R, TDQ_ROWS_T_STAGE + i)[r] = A::mul(sgn, ti);
+    }
+}
+
+// rk_common.py:323-361 + misc.py:85-95 + solvers.py:33-34 for row r, then the row's next attempt.
+template <typename T> __device__ void row_control(const TdqCtrl &c, const Rows &R, int r, double sumsq, double n_bad,
+                                                  size_t D) {
+    double ratio = sqrt(sumsq / (double)D);                                // misc.py:22-23
+    if (!c.ratio_f64) ratio = (double)(T)ratio;
+    if (n_bad > 0.0) ratio = CUDART_NAN;                                   // a non-finite y1 poisons err/tol
+    fld<double>(R, TDQ_ROWS_RATIO)[r] = ratio;
+    const double dt = fld<double>(R, TDQ_ROWS_ATT_DT)[r];
+    bool accept = ratio <= 1.0;                                            // :324
+    if (dt > c.max_step) accept = false;                                   // :327-328
+    if (dt <= c.min_step) accept = true;                                   // :329-330
+    fld<int>(R, TDQ_ROWS_ACCEPT)[r] = accept ? 1 : 0;
+    const double att_t0 = fld<double>(R, TDQ_ROWS_ATT_T0)[r];
+    fld<double>(R, TDQ_ROWS_T0)[r] = att_t0;
+    int *status = fld<int>(R, TDQ_ROWS_STATUS);
+    if (accept) {                                                          // :338-352: the flip of the row's pair
+        fld<double>(R, TDQ_ROWS_T1)[r] = fld<double>(R, TDQ_ROWS_ATT_T1)[r];
+        fld<int64_t>(R, TDQ_ROWS_N_ACCEPT)[r] += 1;
+        fld<int>(R, TDQ_ROWS_PAR)[r] ^= 1;
+        fld<double>(R, TDQ_ROWS_FIT_DT)[r] = dt;
+        if (n_bad > 0.0) status[r] = TDQ_RUN_NONFINITE;                    // the next attempt would trip :287
+    } else {                                                               // :353-357
+        fld<double>(R, TDQ_ROWS_T1)[r] = att_t0;
+        fld<int64_t>(R, TDQ_ROWS_N_REJECT)[r] += 1;
+    }
+    fld<double>(R, TDQ_ROWS_DT)[r] = tdq_next_dt(ratio, dt, c.safety, c.ifactor, c.dfactor, c.order, c.min_step, c.max_step);
+    int cur = fld<int>(R, TDQ_ROWS_CURSOR)[r];
+    fld<int>(R, TDQ_ROWS_EMIT_LO)[r] = cur;
+    int64_t *steps = fld<int64_t>(R, TDQ_ROWS_N_STEPS);
+    steps[r] += 1;
+    if (accept) {
+        const double t1 = fld<double>(R, TDQ_ROWS_T1)[r];
+        const int c0 = cur;
+        while (cur < c.n_out && !(c.t_out[cur] > t1)) ++cur;
+        if (cur != c0) steps[r] = 0;
+        fld<int>(R, TDQ_ROWS_CURSOR)[r] = cur;
+    }
+    fld<int>(R, TDQ_ROWS_EMIT_HI)[r] = cur;
+    fld<int>(R, TDQ_ROWS_FIT)[r] = (accept && cur > fld<int>(R, TDQ_ROWS_EMIT_LO)[r]) ? 1 : 0;
+    const bool done = cur >= c.n_out;
+    fld<int>(R, TDQ_ROWS_DONE)[r] = done ? 1 : 0;
+    if (status[r] == TDQ_RUN_OK && !done) row_prepare<T>(c, R, r, false);
+}
+
+// End of a per-row launch: every block adds its count of rows still running and its smallest failing row; the last block
+// ends the solve when no row runs or some row failed, reports through the mailbox and keeps or ends the device-side loop.
+__device__ void rows_finish(TdqCtrl *c, const Rows &R, bool running, bool failed, int r, bool attempt) {
+    __shared__ int s_fail;
+    __shared__ bool is_last;
+    if (threadIdx.x == 0) s_fail = INT_MAX;
+    __syncthreads();
+    if (failed) atomicMin(&s_fail, r);
+    const int n_run = __syncthreads_count(running ? 1 : 0);
+    int *h = hdr(R);
+    if (threadIdx.x == 0) {
+        if (n_run) atomicAdd(&h[1], n_run);
+        if (s_fail != INT_MAX) atomicMin(&h[2], s_fail);
+        __threadfence();
+        is_last = atomicAdd(reinterpret_cast<unsigned int *>(&h[0]), 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!is_last || threadIdx.x != 0) return;
+    __threadfence();
+    const int total = atomicAdd(&h[1], 0), fail = atomicAdd(&h[2], 0);
+    if (fail != INT_MAX) {
+        c->status = fld<int>(R, TDQ_ROWS_STATUS)[fail];
+        c->halt = 1;
+        h[3] = fail;
+    } else if (total == 0) {
+        c->done = 1;
+        c->halt = 1;
+    }
+    h[0] = 0;
+    h[1] = 0;
+    h[2] = INT_MAX;
+    tdq_mailbox *m = c->mbox;
+    if (attempt) c->seq += 1;
+    if (m && (!attempt || c->loop_handle == 0ull || c->halt)) {
+        m->status = c->status;
+        m->accept = 0;
+        m->done = c->done;
+        m->on_jump_t = 0;
+        m->par = 0;
+        __threadfence_system();
+        if (attempt) m->seq = c->seq;
+    }
+    if (attempt && c->loop_handle != 0ull)
+        cudaGraphSetConditional((cudaGraphConditionalHandle)c->loop_handle, c->halt ? 0u : 1u);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_rows_init(const TdqCtrl *__restrict__ c, Rows R, double t_start) {
+    const int r = blockIdx.x * kThreads + threadIdx.x;
+    if (blockIdx.x == 0 && threadIdx.x < 4) hdr(R)[threadIdx.x] = threadIdx.x == 2 ? INT_MAX : (threadIdx.x == 3 ? -1 : 0);
+    if (r >= R.B) return;
+    for (int f = TDQ_ROWS_T0; f <= TDQ_ROWS_D1; ++f) fld<double>(R, f)[r] = 0.0;
+    fld<double>(R, TDQ_ROWS_T0)[r] = t_start;                             // rk_common.py:221
+    fld<double>(R, TDQ_ROWS_T1)[r] = t_start;
+    for (int f = TDQ_ROWS_PAR; f <= TDQ_ROWS_EMIT_HI; ++f) fld<int>(R, f)[r] = 0;
+    fld<int>(R, TDQ_ROWS_CURSOR)[r] = 1;                                  // solution[0] = y0 (solvers.py:30)
+    fld<int>(R, TDQ_ROWS_EMIT_LO)[r] = 1;
+    fld<int>(R, TDQ_ROWS_EMIT_HI)[r] = 1;
+    fld<int>(R, TDQ_ROWS_DONE)[r] = c->n_out <= 1 ? 1 : 0;
+    for (int f = TDQ_ROWS_N_STEPS; f <= TDQ_ROWS_N_REJECT; ++f) fld<int64_t>(R, f)[r] = 0;
+    fld<T>(R, TDQ_ROWS_T_FIRST)[r] = Ar<T>::mul((T)c->t_sign, (T)t_start);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+k_rows_h0(const TdqCtrl *__restrict__ c, Rows R, const double *s0, const double *s1, size_t D) {
+    const int r = blockIdx.x * kThreads + threadIdx.x;
+    if (r >= R.B) return;
+    double d0 = sqrt(s0[r] / (double)D), d1 = sqrt(s1[r] / (double)D);
+    if (!c->ratio_f64) {
+        d0 = (double)(T)d0;
+        d1 = (double)(T)d1;
+    }
+    const double h0 = tdq_initial_h0<T>(c->ratio_f64 != 0, d0, d1);
+    fld<double>(R, TDQ_ROWS_H0)[r] = h0;
+    fld<double>(R, TDQ_ROWS_D1)[r] = d1;
+    // probe time: t0 (f64) + h0 -> f64, cast to T by _PerturbFunc (misc.py:66-67, :187)
+    fld<T>(R, TDQ_ROWS_T_PROBE)[r] = Ar<T>::mul((T)c->t_sign, (T)(fld<double>(R, TDQ_ROWS_T1)[r] + h0));
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_rows_probe(const TdqCtrl *__restrict__ c, Rows R, Geom g, T *__restrict__ out) {
+    using A = Ar<T>;
+    size_t u, lo, hi;
+    int r;
+    if (!unit_of(g, u, r, lo, hi)) return;
+    const int par = fld<int>(R, TDQ_ROWS_PAR)[r];
+    const size_t base = (size_t)r * g.D;
+    const T *y0 = reinterpret_cast<const T *>(c->ybuf[par]) + base;
+    const T *f0 = reinterpret_cast<const T *>(c->kbuf[par]) + base;
+    const T h = A::mul((T)c->t_sign, (T)fld<double>(R, TDQ_ROWS_H0)[r]);   // y0 + h0 * f0, f0 = t_sign * k0 (misc.py:66)
+    for (size_t i = lo + (threadIdx.x & 31); i < hi; i += 32) out[base + i] = A::add(y0[i], A::mul(h, f0[i]));
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_rows_finish(const TdqCtrl *__restrict__ c, Rows R, const double *s2, size_t D) {
+    const int r = blockIdx.x * kThreads + threadIdx.x;
+    if (r >= R.B) return;
+    double nd = sqrt(s2[r] / (double)D);
+    if (!c->ratio_f64) nd = (double)(T)nd;
+    fld<double>(R, TDQ_ROWS_DT)[r] = tdq_initial_finish<T>(c->ratio_f64 != 0, c->order, fld<double>(R, TDQ_ROWS_D1)[r],
+                                                           fld<double>(R, TDQ_ROWS_H0)[r], nd);
+}
+
+__global__ void k_rows_first_step(Rows R, double dt) {
+    const int r = blockIdx.x * kThreads + threadIdx.x;
+    if (r < R.B) fld<double>(R, TDQ_ROWS_DT)[r] = dt;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_rows_prepare(TdqCtrl *c, Rows R, const double *y0_bad) {
+    const int r = blockIdx.x * kThreads + threadIdx.x;
+    bool running = false, failed = false;
+    if (!c->halt && r < R.B && !fld<int>(R, TDQ_ROWS_DONE)[r]) {
+        row_prepare<T>(*c, R, r, y0_bad != nullptr && y0_bad[R.B + r] > 0.0);
+        failed = fld<int>(R, TDQ_ROWS_STATUS)[r] != TDQ_RUN_OK;
+        running = true;
+    }
+    rows_finish(c, R, running, failed, r, false);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_rows_controller(TdqCtrl *c, Rows R, const double *norm_in, size_t D) {
+    const int r = blockIdx.x * kThreads + threadIdx.x;
+    if (c->halt) {
+        // attempts issued after the end are no-ops; the mailbox still ticks so that a host running ahead can account for
+        // every attempt it queued, and no row fits
+        if (r < R.B) fld<int>(R, TDQ_ROWS_FIT)[r] = 0;
+        if (r == 0) {
+            c->seq += 1;
+            if (c->mbox && c->loop_handle == 0ull) {
+                __threadfence_system();
+                c->mbox->seq = c->seq;
+            }
+            // a solve that had already ended when the device-side loop started (its first attempt failed in
+            // tdq_rows_prepare, or the attempt before the loop finished every row) must leave the loop here
+            if (c->loop_handle != 0ull) cudaGraphSetConditional((cudaGraphConditionalHandle)c->loop_handle, 0u);
+        }
+        return;
+    }
+    bool running = false, failed = false;
+    if (r < R.B) {
+        if (fld<int>(R, TDQ_ROWS_DONE)[r]) {
+            fld<int>(R, TDQ_ROWS_FIT)[r] = 0;
+        } else {
+            row_control<T>(*c, R, r, norm_in[r], norm_in[R.B + r], D);
+            failed = fld<int>(R, TDQ_ROWS_STATUS)[r] != TDQ_RUN_OK;
+            running = !fld<int>(R, TDQ_ROWS_DONE)[r];
+        }
+    }
+    rows_finish(c, R, running, failed, r, true);
+}
+
+// ---- host helpers -----------------------------------------------------------------------------------------------------------
+bool plan_kp(const int *idx, int nnz, const void *const *k, KPtrs &kp, bool &vec) {
+    return tdq_plan_terms(idx, nnz, k, kp.p, vec) == TDQ_PLAN_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t tdq_rows_size(size_t n_rows) { return kHdr + (size_t)TDQ_ROWS_N_FIELDS * rows_slot(n_rows); }
+
+size_t tdq_rows_offset(int32_t field, size_t n_rows) {
+    if (field == TDQ_ROWS_HEADER) return 0;
+    if (field < 0 || field >= TDQ_ROWS_N_FIELDS) return (size_t)-1;
+    return kHdr + (size_t)field * rows_slot(n_rows);
+}
+
+size_t tdq_rows_partials_len(size_t n_rows, size_t row_len) {
+    const Geom g = make_geom(n_rows, row_len);
+    return 2 + (g.nch > 1 ? 2 * g.units + (n_rows + 1) / 2 : 0);
+}
+
+#define TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len)                                                               \
+    TDQ_REQUIRE((n_rows) >= 1 && (n_rows) <= (size_t)INT_MAX, "n_rows out of range");                       \
+    TDQ_REQUIRE((row_len) >= 1, "row_len must be at least 1")
+
+int tdq_rows_init(void *ctrl_dev, void *rows_dev, int32_t dtype, size_t n_rows, double t_start, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev, "null argument");
+    TDQ_REQUIRE(n_rows >= 1 && n_rows <= (size_t)INT_MAX, "n_rows out of range");
+    TDQ_DISPATCH_T(dtype, (k_rows_init<T><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (const TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), t_start)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+static int rows_norm(int mode, void *ctrl_dev, void *rows_dev, int32_t dtype, RowNormArgs &a, size_t n_rows,
+                     size_t row_len, cudaStream_t st) {
+    const Geom g = make_geom(n_rows, row_len);
+    const Rows R = make_rows(rows_dev, n_rows);
+    const TdqCtrl *c = (const TdqCtrl *)ctrl_dev;
+    const bool vt = a.rtol_v != nullptr;
+    TDQ_DISPATCH_T(dtype, tdq_dispatch(TdqBool{}, vt, [&](auto VT) {
+        if (mode == 0) k_rows_norm<T, 0, VT><<<unit_blocks(g), kThreads, 0, st>>>(c, R, g, a);
+        else if (mode == 1) k_rows_norm<T, 1, VT><<<unit_blocks(g), kThreads, 0, st>>>(c, R, g, a);
+        else k_rows_norm<T, 2, VT><<<unit_blocks(g), kThreads, 0, st>>>(c, R, g, a);
+        return 0;
+    }));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_sumsq(void *ctrl_dev, void *rows_dev, int32_t dtype, const void *x, const void *x2, const double *rtol_vec,
+                   const double *atol_vec, size_t n_rows, size_t row_len, double *partials, double *out, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && x && partials && out, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_REQUIRE((rtol_vec == nullptr) == (atol_vec == nullptr), "rtol_vec and atol_vec go together");
+    RowNormArgs a{x, x2, nullptr, rtol_vec, atol_vec, partials, out};
+    return rows_norm(x2 ? 2 : 1, ctrl_dev, rows_dev, dtype, a, n_rows, row_len, (cudaStream_t)stream);
+}
+
+int tdq_rows_error_norm_commit(void *ctrl_dev, void *rows_dev, int32_t dtype, const void *err_pre, const void *k_last,
+                               const void *y1, const double *rtol_vec, const double *atol_vec, size_t n_rows,
+                               size_t row_len, double *partials, double *out, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && err_pre && k_last && y1 && partials && out, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_REQUIRE((rtol_vec == nullptr) == (atol_vec == nullptr), "rtol_vec and atol_vec go together");
+    RowNormArgs a{err_pre, k_last, y1, rtol_vec, atol_vec, partials, out};
+    return rows_norm(0, ctrl_dev, rows_dev, dtype, a, n_rows, row_len, (cudaStream_t)stream);
+}
+
+int tdq_rows_initial_h0(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *d0_sumsq, const double *d1_sumsq,
+                        size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && d0_sumsq && d1_sumsq, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_DISPATCH_T(dtype, (k_rows_h0<T><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (const TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), d0_sumsq, d1_sumsq, row_len)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_initial_probe(void *ctrl_dev, void *rows_dev, int32_t dtype, void *y_probe, size_t n_rows, size_t row_len,
+                           void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && y_probe, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    const Geom g = make_geom(n_rows, row_len);
+    TDQ_DISPATCH_T(dtype, (k_rows_probe<T><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(
+                               (const TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), g, (T *)y_probe)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_initial_finish(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *d2_sumsq, size_t n_rows,
+                            size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && d2_sumsq, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_DISPATCH_T(dtype, (k_rows_finish<T><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (const TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), d2_sumsq, row_len)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_set_first_step(void *rows_dev, size_t n_rows, double first_step, void *stream) {
+    TDQ_REQUIRE(rows_dev, "null argument");
+    TDQ_REQUIRE(n_rows >= 1 && n_rows <= (size_t)INT_MAX, "n_rows out of range");
+    k_rows_first_step<<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(make_rows(rows_dev, n_rows), first_step);
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_prepare(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *y0_nonfinite_dev, size_t n_rows,
+                     void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev, "null argument");
+    TDQ_REQUIRE(n_rows >= 1 && n_rows <= (size_t)INT_MAX, "n_rows out of range");
+    TDQ_DISPATCH_T(dtype, (k_rows_prepare<T><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), y0_nonfinite_dev)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_combine(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, int32_t row, void *y_out,
+                     const void *const *k, size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && tab && y_out && k, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TdqHostShape hs;
+    tdq_shape_from_tableau(tab, &hs);
+    TDQ_REQUIRE(row >= 0 && row <= hs.n_stages, "row out of range");
+    const int nk = hs.row_nnz[row];
+    TDQ_REQUIRE(nk >= 1, "empty tableau row");
+    KPtrs kp;
+    bool vec = tdq_aligned16(y_out);
+    TDQ_REQUIRE(plan_kp(hs.row_idx[row], nk, k, kp, vec), "missing stage slot for a non-zero tableau entry");
+    const Geom g = make_geom(n_rows, row_len);
+    const Rows R = make_rows(rows_dev, n_rows);
+    int rc = -1;
+    TDQ_DISPATCH_T(dtype, rc = tdq_dispatch(TdqRange<1, TDQ_MAX_K>{}, nk, [&](auto NK) {
+                       k_rows_combine<T, NK><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(
+                           (const TdqCtrl *)ctrl_dev, R, g, row, (T *)y_out, kp, vec);
+                       return 0;
+                   }));
+    TDQ_REQUIRE(rc == 0, "unsupported number of stage terms");
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_combine_final(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, void *y1_out,
+                           void *err_out, const void *const *k, size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && tab && y1_out && err_out && k, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TdqHostShape hs;
+    tdq_shape_from_tableau(tab, &hs);
+    const int S = hs.n_stages;
+    const int row = hs.fsal ? S - 1 : S;          // FSAL: y1 is the last stage value (rk_common.py:83-87)
+    const int avail = hs.fsal ? S - 1 : S;
+    KPtrs kp;
+    RowFinalMap fm;
+    int nu = 0;
+    bool vec = tdq_aligned16(y1_out) && tdq_aligned16(err_out);
+    TDQ_REQUIRE(tdq_plan_union(hs, row, avail, k, kp.p, fm, nu, vec) == TDQ_PLAN_OK,
+                "missing stage slot for a non-zero tableau entry");
+    TDQ_REQUIRE(nu >= 1, "empty tableau row");
+    const Geom g = make_geom(n_rows, row_len);
+    const Rows R = make_rows(rows_dev, n_rows);
+    int rc = -1;
+    TDQ_DISPATCH_T(dtype, rc = tdq_dispatch(TdqRange<1, TDQ_MAX_K>{}, nu, [&](auto NU) {
+                       k_rows_combine_final<T, NU><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(
+                           (const TdqCtrl *)ctrl_dev, R, g, row, (T *)y1_out, (T *)err_out, kp, fm, vec);
+                       return 0;
+                   }));
+    TDQ_REQUIRE(rc == 0, "unsupported number of stage terms");
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_controller(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in, size_t n_rows,
+                        size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && norm_in, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_DISPATCH_T(dtype, (k_rows_controller<T><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), norm_in, row_len)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_fit_eval(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, const void *y1,
+                      const void *const *k, void *solution, size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && tab && y1 && k && solution, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TdqHostShape hs;
+    tdq_shape_from_tableau(tab, &hs);
+    const int S = hs.n_stages, nk = hs.mid_nnz;
+    TDQ_REQUIRE(nk >= 1, "tableau has no mid-point weights");
+    TDQ_REQUIRE(k[S] != nullptr, "k_S is required");
+    KPtrs kmid;
+    bool vec = true;
+    TDQ_REQUIRE(plan_kp(hs.mid_idx, nk, k, kmid, vec), "missing stage slot for a non-zero mid-point weight");
+    const Geom g = make_geom(n_rows, row_len);
+    const Rows R = make_rows(rows_dev, n_rows);
+    int rc = -1;
+    TDQ_DISPATCH_T(dtype, rc = tdq_dispatch(TdqRange<1, TDQ_MAX_K>{}, nk, [&](auto NK) {
+                       k_rows_fit_eval<T, NK><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(
+                           (const TdqCtrl *)ctrl_dev, R, g, (const T *)y1, (const T *)k[S], kmid, (T *)solution,
+                           n_rows * row_len);
+                       return 0;
+                   }));
+    TDQ_REQUIRE(rc == 0, "unsupported number of mid-point terms");
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+}  // extern "C"

@@ -13,7 +13,7 @@ import warnings
 import torch
 
 from . import _lib
-from ._engine import AdaptiveEngine, Layout, on_solver_stream
+from ._engine import AdaptiveEngine, Layout, RowsEngine, on_solver_stream
 from ._adams import ADAMS_METHODS
 from ._fixed import FIXED_METHODS, grid_from_step_size, make_engine
 from ._implicit import IMPLICIT_METHODS
@@ -33,7 +33,8 @@ _ADAPTIVE_OPTIONS = {"min_step", "max_step", "first_step", "step_t", "jump_t", "
 _FIXED_OPTIONS = {"step_size", "grid_constructor", "interp", "perturb", "norm"}
 _ADAMS_OPTIONS = _FIXED_OPTIONS | {"max_iters", "max_order"}
 _IMPLICIT_OPTIONS = _FIXED_OPTIONS | {"max_iters"}                                  # rk_common.py:382-388
-_OUR_OPTIONS = {"graph", "run_ahead", "process_group", "cache", "exchange", "device_loop", "fused_linear", "fused_attempt"}
+_OUR_OPTIONS = {"graph", "run_ahead", "process_group", "cache", "exchange", "device_loop", "fused_linear", "fused_attempt",
+                 "independent_rows"}
 
 
 def _rms_norm(tensor):
@@ -303,6 +304,45 @@ def _make_adaptive_engine(p, method, rtol, atol, rtol_vec, atol_vec, options, fn
     return eng
 
 
+def _check_independent_rows(func, y0, t, method, options, event_fn):
+    """What options={'independent_rows': True} does not cover raises NotImplementedError before any work."""
+    def no(what):
+        raise NotImplementedError("options['independent_rows'] does not support %s" % what)
+    if not isinstance(y0, torch.Tensor):
+        no("tuple states")
+    if (method or "dopri5") not in ADAPTIVE_METHODS:
+        no("method %r: it is implemented for the adaptive methods %s" % (method, ", ".join(ADAPTIVE_METHODS)))
+    for name in ("step_t", "jump_t", "process_group"):
+        if options.get(name) is not None:
+            no("options['%s']" % name)
+    if options.get("norm") is not None and options["norm"] is not _rms_norm:
+        no("a custom norm callable (each row's error ratio is the RMS over its own elements)")
+    if any(getattr(func, name, None) is not None for name in _CALLBACK_NAMES):
+        no("callbacks")
+    if event_fn is not None:
+        no("event_fn / odeint_event")
+    if torch.is_grad_enabled():
+        from .backprop import discover_params
+        if y0.requires_grad or (isinstance(t, torch.Tensor) and t.requires_grad) or discover_params(func):
+            no("gradients (odeint under autograd with anything requiring grad); run it under torch.no_grad()")
+    if y0.dim() < 1 or y0.shape[0] < 1:
+        raise ValueError("options['independent_rows'] needs y0 of shape [B, ...] with B >= 1, got %s" % (tuple(y0.shape),))
+
+
+def _make_rows_engine(p):
+    o = p.options
+    _warn_unused(p.method, o, _ADAPTIVE_OPTIONS)
+    if o.get("dtype", torch.float64) != torch.float64:
+        raise NotImplementedError("time dtype other than float64 (options['dtype']) is not implemented")
+    return RowsEngine(
+        p.fn, p.shape, p.dtype, p.device, p.method, rtol=p.rtol, atol=p.atol, rtol_vec=p.rtol_vec, atol_vec=p.atol_vec,
+        t_sign=p.t_sign, min_step=o.get("min_step", 0), max_step=o.get("max_step", float("inf")),
+        first_step=o.get("first_step"), safety=o.get("safety", 0.9), ifactor=o.get("ifactor", 10.0),
+        dfactor=o.get("dfactor", 0.2), max_num_steps=o.get("max_num_steps", 2 ** 31 - 1),
+        graph=_resolve_graph(o.get("graph", "auto"), p.original_func), run_ahead=o.get("run_ahead", 2),
+        device_loop=o.get("device_loop", "auto"))
+
+
 # ---- engine cache -------------------------------------------------------------------------------
 # An engine owns ~10 state-sized buffers and, in graph mode, a captured step graph with its private
 # memory pool; building and tearing that down costs far more than a solve of the benchmark size.
@@ -452,6 +492,9 @@ def _solve(p):
         hit = _cache_get(key)
         if hit is not None:
             eng = hit[0]
+        elif p.options.get("independent_rows"):
+            eng = _make_rows_engine(p)
+            _cache_put(key, (eng, p.original_func))
         else:
             eng = _make_adaptive_engine(p, p.method, p.rtol, p.atol, p.rtol_vec, p.atol_vec, p.options,
                                         segs=p.segs, pieces=p.pieces, norm_fn=p.norm_fn, q_view=p.q_view,
@@ -625,6 +668,8 @@ def odeint_dense(func, y0, t0, t1, *, rtol=1e-7, atol=1e-9, method=None, options
     assert torch.is_tensor(y0)
     t0_, t1_ = torch.as_tensor(t0), torch.as_tensor(t1)
     t = torch.stack([t0_.reshape(()), t1_.reshape(()).to(t0_)]).to(t0_)
+    if options and options.get("independent_rows"):
+        raise NotImplementedError("options['independent_rows'] does not support odeint_dense")
     p = normalise(func, y0, t, rtol, atol, method, options, None)
     assert p.method == "dopri5"                                                        # odeint.py:119
     with torch.no_grad(), on_solver_stream(p.device) as ss:
@@ -713,7 +758,15 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
     call sequence) and `process_group` (batch-sharded solve with a common step size).
     Under autograd the result carries the gradient of the discrete solve w.r.t. y0, t and func's parameters
     (backprop.py); odeint_adjoint gives the continuous adjoint instead.
+
+    options={'independent_rows': True} (adaptive methods, tensor y0 of shape [B, *rest]): every row y0[r] gets its own step
+    size control, so row r's result is the reference's odeint(func, y0[r:r+1], t) for a row-wise func and does not depend
+    on the other rows.  In this mode func's time argument is a tensor of shape [B, 1, ..., 1] (y0.dim() dimensions, state
+    dtype) holding each row's time, so `t * y` and `torch.sin(t) + y` broadcast row by row.  last_stats() then also has
+    row_n_accept / row_n_reject (CPU int64 tensors of shape [B]).
     """
+    if options and options.get("independent_rows"):
+        _check_independent_rows(func, y0, t, method, options, event_fn)
     p = normalise(func, y0, t, rtol, atol, method, options, event_fn)
     if torch.is_grad_enabled():
         from .backprop import discover_params
@@ -744,6 +797,8 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
                        n_accept=getattr(eng, "n_accept", None), n_reject=getattr(eng, "n_reject", None),
                        fused_linear=getattr(eng, "linear", None) is not None,
                        fused_attempt=bool((getattr(eng, "linear", None) or {}).get("whole")))
+    if getattr(eng, "row_n_accept", None) is not None:
+        _LAST_STATS.update(row_n_accept=eng.row_n_accept, row_n_reject=eng.row_n_reject)
     if _stats is not None:               # private: solver counters for bench.py and the tests
         _stats["nfe"] = eng.nfe
         _stats["launches"] = _stats.get("launches", 0) + getattr(eng, "launches", 0)
