@@ -489,6 +489,40 @@ int tdq_rows_controller(void *ctrl_dev, void *rows_dev, int32_t dtype, const dou
 int tdq_rows_fit_eval(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, const void *y1,
                       const void *const *k, void *solution, size_t n_rows, size_t row_len, void *stream);
 
+/* ---- per-row events with independent step-size control (tdq_rows.cu) ---------------------------------------------------
+ * Row r stops at its own event as the reference's odeint_event does for y0[r:r+1] alone (rk_common.py:252-262,
+ * event_handling.py:5-35).  The event state is kept out of the row buffer, in caller-owned device arrays: event values
+ * ev_val [B, K] float64 (the event function's result widened; one call per launch that reads it), initial signs
+ * init_sign [B, K], sign0 [B] (float64), the "event in this attempt" flag [B] (int32), the bisection bracket lo / hi
+ * [2B] float64 each (the bracket after iteration i lives in half i & 1) and nitrs [B] (int32).  The solve runs with the
+ * output times [t0, inf], so the cursor never completes a row.  K: 1 .. 65536 components per row.
+ * tdq_rows_event_init:      after tdq_rows_init, before tdq_rows_prepare: from ev(t0, y0) the initial signs, sign0 =
+ *                           sign(min_k(val * init_sign)) (sign as torch.sign on the CPU: 0 for NaN; min: NaN if any product
+ *                           is NaN); a row whose combined value is exactly 0 is done at t0.
+ * tdq_rows_controller_event: tdq_rows_controller, where a row that accepts a candidate whose combined sign differs from
+ *                           sign0 (ev_val: ev(ATT_T1 * t_sign, y1)) is done with flag 1 and keeps the step as T0 / T1; that
+ *                           decision comes before the non-finite-y1 and max_num_steps failures of its next attempt.  The
+ *                           flag is 0 for every other row, done rows and attempts after the end included.
+ * tdq_rows_fit_store:       for flagged rows, the quartic of the step (e, d, c, b, a) into coeff [5, B*D] (the arithmetic of
+ *                           tdq_rows_fit_eval).
+ * tdq_rows_event_bisect:    iteration iter of the bisection for every row with iter <= nitrs[r]: for iter > 0 the bracket
+ *                           update from ev_val (the previous iteration's values); then for iter < nitrs[r] t_ev[r] =
+ *                           t_mid * t_sign and y_mid's row = interp(t_mid), for iter == nitrs[r] event_t[r] = event_t *
+ *                           t_sign and y_event's row = interp(event_t).  Rows done at t0 (no accepted step) have nitrs 0
+ *                           and write (t0, y_start). */
+int tdq_rows_event_init(void *rows_dev, const double *ev_val, double *init_sign, double *sign0, int32_t *flag,
+                        size_t n_rows, int32_t K, void *stream);
+int tdq_rows_controller_event(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in, const double *ev_val,
+                              const double *init_sign, const double *sign0, int32_t *flag, size_t n_rows, size_t row_len,
+                              int32_t K, void *stream);
+int tdq_rows_fit_store(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, const void *y1,
+                       const void *const *k, const int32_t *flag, void *coeff, size_t n_rows, size_t row_len,
+                       void *stream);
+int tdq_rows_event_bisect(void *ctrl_dev, void *rows_dev, int32_t dtype, int32_t iter, const double *ev_val,
+                          const double *init_sign, const double *sign0, const int32_t *nitrs, double *lo, double *hi,
+                          const void *coeff, const void *y_start, void *y_mid, double *t_ev, double *event_t,
+                          void *y_event, size_t n_rows, size_t row_len, int32_t K, void *stream);
+
 /* ---- adjoint augmented state (adjoint.py:72-105, misc.py:137-165) ------------------------- */
 /* dst[offset_i .. offset_i + len_i) = scale_i * src_i for i < n_src, one launch
  * (the torch.cat of _TupleFunc, the unary minus on adj_y and the *(-1) of _ReverseFunc).

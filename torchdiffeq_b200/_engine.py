@@ -26,6 +26,7 @@ Execution modes (options of our path only, SURVEY.md section 5 "config"):
     device_loop True/False/'auto' run the captured attempt inside the device-side while loop.
 """
 import ctypes as C
+import math
 import time
 
 import torch
@@ -920,6 +921,19 @@ class AdaptiveEngine:
         self._launch(self.lib.tdq_set_first_step(self.ctrl.data_ptr(), dt, _stream()))
 
 
+def bisect_iterations(lo, hi, tol):
+    """event_handling.py:13 per row: ceil(log((hi - lo) / tol) / log 2) in float64 on the CPU, as the reference computes
+    it.  The vectorised log may differ from the scalar one the reference runs on a 0-dim tensor in the last bit, which
+    can move the ceiling only when the quotient is within rounding of an integer: those rows are recomputed one at a
+    time.  A negative or non-finite count (an empty bracket: a row done at t0) runs no iteration, as range() of it does
+    not.  Returns int32 [B]."""
+    v = torch.log((hi - lo) / tol) / math.log(2.0)
+    for r in ((v - v.round()).abs() < 1e-6).nonzero().view(-1).tolist():
+        v[r] = torch.log((hi[r] - lo[r]) / tol[r]) / math.log(2.0)
+    n = torch.ceil(v)
+    return torch.where(torch.isfinite(n) & (n > 0), n, torch.zeros_like(n)).to(torch.int32)
+
+
 class RowsEngine(AdaptiveEngine):
     """Independent step-size control per batch row (odeint's options={'independent_rows': True}).
 
@@ -952,6 +966,7 @@ class RowsEngine(AdaptiveEngine):
         self.row_norm = torch.zeros(2 * B, **f64)                   # sums of squares, then non-finite counts
         self.row_dsum = [torch.zeros(2 * B, **f64) for _ in range(3)]
         self.row_n_accept = self.row_n_reject = None
+        self.ev_fn = None                # set by solve_until_event: the attempt then tests each row's event
 
     def _rows_sumsq(self, x, x2, out):
         self._launch(self.lib.tdq_rows_sumsq(
@@ -987,13 +1002,82 @@ class RowsEngine(AdaptiveEngine):
             self.rtol_vec.data_ptr() if self.rtol_vec is not None else None,
             self.atol_vec.data_ptr() if self.atol_vec is not None else None,
             B, D, self.row_partials.data_ptr(), self.row_norm.data_ptr(), st))
-        self._launch(lib.tdq_rows_controller(ctrl, rows, dc, self.row_norm.data_ptr(), B, D, st))
+        if self.ev_fn is None:
+            self._launch(lib.tdq_rows_controller(ctrl, rows, dc, self.row_norm.data_ptr(), B, D, st))
+        else:
+            # each row's event value at its candidate (ATT_T1, y1), then the controller with the sign test inside it
+            torch.mul(self.row_field(_lib.ROWS_ATT_T1, torch.float64), self.opt.t_sign, out=self.ev_t)
+            self._ev_call(self.y1)
+            self._launch(lib.tdq_rows_controller_event(ctrl, rows, dc, self.row_norm.data_ptr(), self.ev_val.data_ptr(),
+                                                       self.ev_init.data_ptr(), self.ev_sign0.data_ptr(),
+                                                       self.ev_flag.data_ptr(), B, D, self.K, st))
         return k, kp, keep
 
     def _attempt_back(self, kp):
+        if self.ev_fn is not None:                  # the interpolant of a row's event step, kept for the bisection
+            self._launch(self.lib.tdq_rows_fit_store(self.ctrl.data_ptr(), self.rows.data_ptr(), C.byref(self.tab),
+                                                     self.dt_code, self.y1.data_ptr(), kp, self.ev_flag.data_ptr(),
+                                                     self.ev_coeff.data_ptr(), self.B, self.D, _stream()))
+            return
         self._launch(self.lib.tdq_rows_fit_eval(self.ctrl.data_ptr(), self.rows.data_ptr(), C.byref(self.tab),
                                                 self.dt_code, self.y1.data_ptr(), kp, self.solution.data_ptr(),
                                                 self.B, self.D, _stream()))
+
+    # ---- per-row events (rk_common.py:252-262, event_handling.py:5-35) ------------------------------------------------
+    def _ev_call(self, y_flat):
+        """ev on the whole batch at the times in ev_t; its values, widened to float64 [B, K], into ev_val.  Values of rows
+        that did not accept in this attempt, or are done, are ignored by the kernels."""
+        self.n_ev += 1
+        v = self.ev_fn(self.ev_t_view, y_flat.view(self.B, *self.row_shape))
+        if not isinstance(v, torch.Tensor) or v.dim() == 0 or v.shape[0] != self.B or v.numel() != self.B * self.K:
+            raise ValueError("event_fn returned %s; with independent rows it must keep the shape of its first result, "
+                             "[B, K...] with B = %d and K = %d" % (tuple(getattr(v, "shape", ())), self.B, self.K))
+        self.ev_val.copy_(v.reshape(self.B, self.K))
+
+    def solve_until_event(self, y0_flat, t_start, ev, ev0, tol):
+        """Row r integrates from t_start until the sign of its combined event value changes, then bisects on the
+        interpolant of its last step: the reference's odeint_event on y0[r:r+1] alone.  ev(t, y): t is a float64 tensor
+        [B, 1, ...] of each row's time in the caller's direction, y the [B, *rest] state.  ev0 = ev(t_start, y0), already
+        evaluated (shape [B, K...]); tol: float64 [B] CPU tensor, each row's bisection tolerance.  The stepping phase runs
+        with the usual drivers (run-ahead, graph capture, device-side loop, lock step); the bisection is max(nitrs) + 1
+        launches with one ev call between two of them and no synchronisation.  Returns (event_t float64 [B] in the
+        caller's time, solution [2, n]); both are engine buffers."""
+        B, dev = self.B, self.device
+        K = int(ev0.numel()) // B
+        f64 = dict(dtype=torch.float64, device=dev)
+        self.ev_fn, self.K = ev, K
+        self.ev_val = torch.zeros(B, K, **f64)
+        self.ev_init = torch.zeros(B, K, **f64)
+        self.ev_sign0 = torch.zeros(B, **f64)
+        self.ev_flag = torch.zeros(B, dtype=torch.int32, device=dev)
+        self.ev_lo = torch.zeros(2 * B, **f64)
+        self.ev_hi = torch.zeros(2 * B, **f64)
+        self.ev_nitrs = torch.zeros(B, dtype=torch.int32, device=dev)
+        self.ev_coeff = torch.zeros(5, self.n, dtype=self.dtype, device=dev)
+        sign = self.opt.t_sign
+        self.ev_t = torch.full((B,), t_start * sign, **f64)
+        self.ev_t_view = self.ev_t.view(B, *([1] * len(self.row_shape)))
+        self.ev_event_t = torch.zeros(B, **f64)
+        self.ev_val.copy_(ev0.reshape(B, K))
+        self.n_ev = 1                                          # ev0
+        t64 = torch.tensor([t_start, float("inf")], **f64)     # the cursor never completes a row
+        self.solve(y0_flat, t64, t_start)
+        # nitrs from each row's last step, on the host as the reference computes it (one copy of 2 B doubles)
+        o0, o1 = self.lib.tdq_rows_offset(_lib.ROWS_T0, B), self.lib.tdq_rows_offset(_lib.ROWS_T1, B)
+        tt = self.rows[o0:o1 + 8 * B].view(torch.float64).cpu()
+        nitrs = bisect_iterations(tt[:B], tt[(o1 - o0) // 8:], tol)
+        self.ev_nitrs.copy_(nitrs)
+        self.bisect_iters = int(nitrs.max())
+        lib, ctrl, rows, dc, st = self.lib, self.ctrl.data_ptr(), self.rows.data_ptr(), self.dt_code, _stream()
+        for it in range(self.bisect_iters + 1):
+            self._launch(lib.tdq_rows_event_bisect(
+                ctrl, rows, dc, it, self.ev_val.data_ptr(), self.ev_init.data_ptr(), self.ev_sign0.data_ptr(),
+                self.ev_nitrs.data_ptr(), self.ev_lo.data_ptr(), self.ev_hi.data_ptr(), self.ev_coeff.data_ptr(),
+                self.solution[0].data_ptr(), self.ytmp.data_ptr(), self.ev_t.data_ptr(), self.ev_event_t.data_ptr(),
+                self.solution[1].data_ptr(), B, self.D, K, st))
+            if it < self.bisect_iters:
+                self._ev_call(self.ytmp)
+        return self.ev_event_t, self.solution
 
     def _begin(self, y0_flat, t64, t_start=None, loop=False):
         """rk_common.py:166-241 for every row: f0 on the whole batch, then each row's initial step."""
@@ -1036,6 +1120,9 @@ class RowsEngine(AdaptiveEngine):
             self._launch(lib.tdq_rows_initial_finish(ctrl, rows, dc, d[2].data_ptr(), B, D, st))
         else:
             self._launch(lib.tdq_rows_set_first_step(rows, B, float(self.first_step), st))
+        if self.ev_fn is not None:                                  # rows done at t0 take no attempt
+            self._launch(lib.tdq_rows_event_init(rows, self.ev_val.data_ptr(), self.ev_init.data_ptr(),
+                                                 self.ev_sign0.data_ptr(), self.ev_flag.data_ptr(), B, self.K, st))
         self._launch(lib.tdq_rows_prepare(ctrl, rows, dc, d[0].data_ptr() if n_out > 1 else None, B, st))
         return n_out
 

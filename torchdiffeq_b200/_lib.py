@@ -143,6 +143,11 @@ _SIGNATURES = {
     "tdq_rows_error_norm_commit": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _vp, _vp, _vp]),
     "tdq_rows_controller": (C.c_int, [_vp, _vp, _i32, _vp, _sz, _sz, _vp]),
     "tdq_rows_fit_eval": (C.c_int, [_vp, _vp, _ptab, _i32, _vp, _pp, _vp, _sz, _sz, _vp]),
+    "tdq_rows_event_init": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _sz, _i32, _vp]),
+    "tdq_rows_controller_event": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _i32, _vp]),
+    "tdq_rows_fit_store": (C.c_int, [_vp, _vp, _ptab, _i32, _vp, _pp, _vp, _vp, _sz, _sz, _vp]),
+    "tdq_rows_event_bisect": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                        _sz, _sz, _i32, _vp]),
     "tdq_xchg_create": (C.c_int, [_pp, C.POINTER(IpcHandle)]),
     "tdq_xchg_open": (C.c_int, [C.POINTER(IpcHandle), _pp]),
     "tdq_xchg_close": (C.c_int, [_vp]),

@@ -332,48 +332,66 @@ template <typename T> __device__ __forceinline__ T eval_poly(T e, T d, T cq, T b
     return total;
 }
 
-template <typename T, int NK>
-__global__ void __launch_bounds__(kThreads)
-k_rows_fit_eval(const TdqCtrl *__restrict__ c, Rows R, Geom g, const T *__restrict__ y1p, const T *__restrict__ kSp,
-                KPtrs kmid, T *__restrict__ solution, size_t n) {
-    using A = Ar<T>;
-    size_t u, lo, hi;
-    int r;
-    if (!unit_of(g, u, r, lo, hi) || !fld<int>(R, TDQ_ROWS_FIT)[r]) return;
-    const int par = fld<int>(R, TDQ_ROWS_PAR)[r] ^ 1;                    // the pair the accepted step started from
-    const size_t base = (size_t)r * g.D;
-    const T *y0 = reinterpret_cast<const T *>(c->ybuf[par]) + base;
-    const T *f0p = reinterpret_cast<const T *>(c->kbuf[par]) + base;
-    const T *y1 = y1p + base, *f1p = kSp + base;
-    const T dtT = (T)fld<double>(R, TDQ_ROWS_FIT_DT)[r], sgn = (T)c->t_sign;
-    const T sdt = A::mul(sgn, dtT), two_sdt = A::mul((T)2, sdt);
-    T mf[NK];
-    const T *km[NK];
+// The quartic [e, d, c, b, a] of row r's accepted step (rk_common.py:363-369, interp.py:1-22), element by element: shared
+// by the output kernel and the event kernels' coefficient store, so both use one arithmetic.
+template <typename T, int NK> struct RowQuartic {
+    const T *y0, *f0, *y1, *f1, *km[NK];
+    T mf[NK], sdt, two_sdt;
+
+    __device__ __forceinline__ RowQuartic(const TdqCtrl *c, const Rows &R, int r, size_t base, const T *y1p, const T *kSp,
+                                          const KPtrs &kmid) {
+        using A = Ar<T>;
+        const int par = fld<int>(R, TDQ_ROWS_PAR)[r] ^ 1;                // the pair the accepted step started from
+        y0 = reinterpret_cast<const T *>(c->ybuf[par]) + base;
+        f0 = reinterpret_cast<const T *>(c->kbuf[par]) + base;
+        y1 = y1p + base;
+        f1 = kSp + base;
+        const T dtT = (T)fld<double>(R, TDQ_ROWS_FIT_DT)[r], sgn = (T)c->t_sign;
+        sdt = A::mul(sgn, dtT);
+        two_sdt = A::mul((T)2, sdt);
 #pragma unroll
-    for (int m = 0; m < NK; ++m) {
-        mf[m] = A::mul(sgn, A::mul(dtT, (T)c->c_mid[m]));
-        km[m] = kmid.p[m] ? reinterpret_cast<const T *>(kmid.p[m]) + base : f0p;
+        for (int m = 0; m < NK; ++m) {
+            mf[m] = A::mul(sgn, A::mul(dtT, (T)c->c_mid[m]));
+            km[m] = kmid.p[m] ? reinterpret_cast<const T *>(kmid.p[m]) + base : f0;
+        }
     }
-    const int jlo = fld<int>(R, TDQ_ROWS_EMIT_LO)[r], jhi = fld<int>(R, TDQ_ROWS_EMIT_HI)[r];
-    const double t0 = fld<double>(R, TDQ_ROWS_T0)[r], t1 = fld<double>(R, TDQ_ROWS_T1)[r];
-    const int lane = threadIdx.x & 31;
-    for (size_t i = lo + lane; i < hi; i += 32) {
-        const T y0v = y0[i], y1v = y1[i], f0 = f0p[i], f1 = f1p[i];
+
+    __device__ __forceinline__ void at(size_t i, T &e, T &d, T &cq, T &b, T &a) const {
+        using A = Ar<T>;
+        const T y0v = y0[i], y1v = y1[i], f0v = f0[i], f1v = f1[i];
         T acc = A::mul(km[0][i], mf[0]);
 #pragma unroll
         for (int m = 1; m < NK; ++m) acc = A::add(acc, A::mul(km[m][i], mf[m]));
         const T ymid = A::add(y0v, acc);
-        const T a = A::add(A::sub(A::mul(two_sdt, A::sub(f1, f0)), A::mul((T)8, A::add(y1v, y0v))), A::mul((T)16, ymid));
-        const T b = A::sub(A::add(A::add(A::mul(sdt, A::sub(A::mul((T)5, f0), A::mul((T)3, f1))), A::mul((T)18, y0v)),
-                                  A::mul((T)14, y1v)),
-                           A::mul((T)32, ymid));
-        const T cq = A::add(A::sub(A::sub(A::mul(sdt, A::sub(f1, A::mul((T)4, f0))), A::mul((T)11, y0v)),
-                                   A::mul((T)5, y1v)),
-                            A::mul((T)16, ymid));
-        const T d = A::mul(sdt, f0);
+        a = A::add(A::sub(A::mul(two_sdt, A::sub(f1v, f0v)), A::mul((T)8, A::add(y1v, y0v))), A::mul((T)16, ymid));
+        b = A::sub(A::add(A::add(A::mul(sdt, A::sub(A::mul((T)5, f0v), A::mul((T)3, f1v))), A::mul((T)18, y0v)),
+                          A::mul((T)14, y1v)),
+                   A::mul((T)32, ymid));
+        cq = A::add(A::sub(A::sub(A::mul(sdt, A::sub(f1v, A::mul((T)4, f0v))), A::mul((T)11, y0v)), A::mul((T)5, y1v)),
+                    A::mul((T)16, ymid));
+        d = A::mul(sdt, f0v);
+        e = y0v;
+    }
+};
+
+template <typename T, int NK>
+__global__ void __launch_bounds__(kThreads)
+k_rows_fit_eval(const TdqCtrl *__restrict__ c, Rows R, Geom g, const T *__restrict__ y1p, const T *__restrict__ kSp,
+                KPtrs kmid, T *__restrict__ solution, size_t n) {
+    size_t u, lo, hi;
+    int r;
+    if (!unit_of(g, u, r, lo, hi) || !fld<int>(R, TDQ_ROWS_FIT)[r]) return;
+    const size_t base = (size_t)r * g.D;
+    const RowQuartic<T, NK> q(c, R, r, base, y1p, kSp, kmid);
+    const int jlo = fld<int>(R, TDQ_ROWS_EMIT_LO)[r], jhi = fld<int>(R, TDQ_ROWS_EMIT_HI)[r];
+    const double t0 = fld<double>(R, TDQ_ROWS_T0)[r], t1 = fld<double>(R, TDQ_ROWS_T1)[r];
+    const int lane = threadIdx.x & 31;
+    for (size_t i = lo + lane; i < hi; i += 32) {
+        T e, d, cq, b, a;
+        q.at(i, e, d, cq, b, a);
         for (int j = jlo; j < jhi; ++j) {
             const T x = (T)((c->t_out[j] - t0) / (t1 - t0));
-            solution[(size_t)j * n + base + i] = eval_poly<T>(y0v, d, cq, b, a, x);
+            solution[(size_t)j * n + base + i] = eval_poly<T>(e, d, cq, b, a, x);
         }
     }
 }
@@ -411,9 +429,17 @@ template <typename T> __device__ void row_prepare(const TdqCtrl &c, const Rows &
     }
 }
 
-// rk_common.py:323-361 + misc.py:85-95 + solvers.py:33-34 for row r, then the row's next attempt.
-template <typename T> __device__ void row_control(const TdqCtrl &c, const Rows &R, int r, double sumsq, double n_bad,
-                                                  size_t D) {
+struct NoEvent {
+    __device__ bool operator()(bool) const { return false; }
+};
+
+// rk_common.py:323-361 + misc.py:85-95 + solvers.py:33-34 for row r, then the row's next attempt.  event(accept) says
+// whether the row's event fires in this attempt (rk_common.py:259): such a row is done, keeps the accepted step as
+// [T0, T1] and takes no next attempt, so neither a non-finite y1 nor max_num_steps can fail it (the reference tests the
+// sign before it would take that attempt).
+template <typename T, typename Event = NoEvent>
+__device__ void row_control(const TdqCtrl &c, const Rows &R, int r, double sumsq, double n_bad, size_t D,
+                            Event event = Event{}) {
     double ratio = sqrt(sumsq / (double)D);                                // misc.py:22-23
     if (!c.ratio_f64) ratio = (double)(T)ratio;
     if (n_bad > 0.0) ratio = CUDART_NAN;                                   // a non-finite y1 poisons err/tol
@@ -423,6 +449,7 @@ template <typename T> __device__ void row_control(const TdqCtrl &c, const Rows &
     if (dt > c.max_step) accept = false;                                   // :327-328
     if (dt <= c.min_step) accept = true;                                   // :329-330
     fld<int>(R, TDQ_ROWS_ACCEPT)[r] = accept ? 1 : 0;
+    const bool fired = event(accept);
     const double att_t0 = fld<double>(R, TDQ_ROWS_ATT_T0)[r];
     fld<double>(R, TDQ_ROWS_T0)[r] = att_t0;
     int *status = fld<int>(R, TDQ_ROWS_STATUS);
@@ -431,7 +458,7 @@ template <typename T> __device__ void row_control(const TdqCtrl &c, const Rows &
         fld<int64_t>(R, TDQ_ROWS_N_ACCEPT)[r] += 1;
         fld<int>(R, TDQ_ROWS_PAR)[r] ^= 1;
         fld<double>(R, TDQ_ROWS_FIT_DT)[r] = dt;
-        if (n_bad > 0.0) status[r] = TDQ_RUN_NONFINITE;                    // the next attempt would trip :287
+        if (n_bad > 0.0 && !fired) status[r] = TDQ_RUN_NONFINITE;          // the next attempt would trip :287
     } else {                                                               // :353-357
         fld<double>(R, TDQ_ROWS_T1)[r] = att_t0;
         fld<int64_t>(R, TDQ_ROWS_N_REJECT)[r] += 1;
@@ -450,7 +477,7 @@ template <typename T> __device__ void row_control(const TdqCtrl &c, const Rows &
     }
     fld<int>(R, TDQ_ROWS_EMIT_HI)[r] = cur;
     fld<int>(R, TDQ_ROWS_FIT)[r] = (accept && cur > fld<int>(R, TDQ_ROWS_EMIT_LO)[r]) ? 1 : 0;
-    const bool done = cur >= c.n_out;
+    const bool done = cur >= c.n_out || fired;
     fld<int>(R, TDQ_ROWS_DONE)[r] = done ? 1 : 0;
     if (status[r] == TDQ_RUN_OK && !done) row_prepare<T>(c, R, r, false);
 }
@@ -576,13 +603,42 @@ __global__ void __launch_bounds__(kThreads) k_rows_prepare(TdqCtrl *c, Rows R, c
     rows_finish(c, R, running, failed, r, false);
 }
 
-template <typename T>
-__global__ void __launch_bounds__(kThreads) k_rows_controller(TdqCtrl *c, Rows R, const double *norm_in, size_t D) {
+// ---- per-row events (rk_common.py:252-262, event_handling.py:5-35) ---------------------------------------------------------
+// Event values arrive widened to float64 [B, K]; sign, the product with the initial signs (+-1 or 0) and the minimum are
+// exact in float64, so they equal the reference's in the event function's own dtype.
+struct RowEvents {
+    const double *val;                    // [B, K] event values of this attempt's candidate (or of the bisection's y_mid)
+    const double *init;                   // [B, K] initial signs
+    const double *sign0;                  // [B]
+    int *flag;                            // [B] the row's event fired in this attempt
+    int K;
+};
+
+// torch.sign as the reference runs it on the CPU: 0 for NaN (and for +-0)
+__device__ __forceinline__ double sign_of(double v) { return v > 0.0 ? 1.0 : (v < 0.0 ? -1.0 : 0.0); }
+
+// torch.min(c * initial_signs) over row r's K components: NaN as soon as one product is NaN
+__device__ __forceinline__ double ev_combined(const double *val, const double *init, int K, int r) {
+    const double *v = val + (size_t)r * K, *s = init + (size_t)r * K;
+    double m = v[0] * s[0];
+    for (int k = 1; k < K; ++k) {
+        const double p = v[k] * s[k];
+        if (p < m || isnan(p)) m = p;
+    }
+    return m;
+}
+
+template <typename T, bool EVENT>
+__global__ void __launch_bounds__(kThreads)
+k_rows_controller(TdqCtrl *c, Rows R, const double *norm_in, size_t D, RowEvents ev) {
     const int r = blockIdx.x * kThreads + threadIdx.x;
     if (c->halt) {
         // attempts issued after the end are no-ops; the mailbox still ticks so that a host running ahead can account for
         // every attempt it queued, and no row fits
-        if (r < R.B) fld<int>(R, TDQ_ROWS_FIT)[r] = 0;
+        if (r < R.B) {
+            fld<int>(R, TDQ_ROWS_FIT)[r] = 0;
+            if (EVENT) ev.flag[r] = 0;
+        }
         if (r == 0) {
             c->seq += 1;
             if (c->mbox && c->loop_handle == 0ull) {
@@ -599,13 +655,120 @@ __global__ void __launch_bounds__(kThreads) k_rows_controller(TdqCtrl *c, Rows R
     if (r < R.B) {
         if (fld<int>(R, TDQ_ROWS_DONE)[r]) {
             fld<int>(R, TDQ_ROWS_FIT)[r] = 0;
+            if (EVENT) ev.flag[r] = 0;
         } else {
-            row_control<T>(*c, R, r, norm_in[r], norm_in[R.B + r], D);
+            if (EVENT) {
+                // an accepted candidate whose combined sign differs from sign0 ends the row
+                row_control<T>(*c, R, r, norm_in[r], norm_in[R.B + r], D, [&](bool accept) {
+                    const bool fired = accept && !(sign_of(ev_combined(ev.val, ev.init, ev.K, r)) == ev.sign0[r]);
+                    ev.flag[r] = fired ? 1 : 0;
+                    return fired;
+                });
+            } else {
+                row_control<T>(*c, R, r, norm_in[r], norm_in[R.B + r], D);
+            }
             failed = fld<int>(R, TDQ_ROWS_STATUS)[r] != TDQ_RUN_OK;
             running = !fld<int>(R, TDQ_ROWS_DONE)[r];
         }
     }
     rows_finish(c, R, running, failed, r, true);
+}
+
+// ev(t0, y0) -> initial signs, sign0 and the rows done at t0: combined value exactly 0 (rk_common.py:254-255).  A NaN
+// combined value is not 0; its sign, and so sign0, is 0, and the row steps until its combined sign is no longer 0.
+__global__ void __launch_bounds__(kThreads) k_rows_event_init(Rows R, const double *val, double *init, double *sign0,
+                                                               int *flag, int K) {
+    const int r = blockIdx.x * kThreads + threadIdx.x;
+    if (r >= R.B) return;
+    for (int k = 0; k < K; ++k) init[(size_t)r * K + k] = sign_of(val[(size_t)r * K + k]);
+    const double m = ev_combined(val, init, K, r);
+    sign0[r] = sign_of(m);
+    flag[r] = 0;
+    if (m == 0.0) fld<int>(R, TDQ_ROWS_DONE)[r] = 1;
+}
+
+// The quartic of each flagged row's event step into coeff[5][n] (e, d, c, b, a).
+template <typename T, int NK>
+__global__ void __launch_bounds__(kThreads)
+k_rows_fit_store(const TdqCtrl *__restrict__ c, Rows R, Geom g, const T *__restrict__ y1p, const T *__restrict__ kSp,
+                 KPtrs kmid, const int *__restrict__ flag, T *__restrict__ coeff, size_t n) {
+    size_t u, lo, hi;
+    int r;
+    if (!unit_of(g, u, r, lo, hi) || !flag[r]) return;
+    const size_t base = (size_t)r * g.D;
+    const RowQuartic<T, NK> q(c, R, r, base, y1p, kSp, kmid);
+    for (size_t i = lo + (threadIdx.x & 31); i < hi; i += 32) {
+        T e, d, cq, b, a;
+        q.at(i, e, d, cq, b, a);
+        coeff[base + i] = e;
+        coeff[n + base + i] = d;
+        coeff[2 * n + base + i] = cq;
+        coeff[3 * n + base + i] = b;
+        coeff[4 * n + base + i] = a;
+    }
+}
+
+struct BisectArgs {
+    RowEvents ev;                         // val: the event values of the previous iteration's y_mid
+    const int *nitrs;                     // [B]
+    double *lo, *hi;                      // [2B] each: the bracket after iteration i lives in half i & 1
+    const void *coeff;                    // [5, n]
+    const void *y_start;                  // [n] y0 of the solve
+    void *y_mid;                          // [n] what ev reads
+    double *t_ev;                         // [B] what ev's time aliases: t_mid * t_sign
+    double *event_t;                      // [B] event_t * t_sign
+    void *y_event;                        // [n] the state at the event
+    size_t n;
+};
+
+// Bisection iteration `iter` of find_event (event_handling.py:5-20) for every row with iter <= nitrs_r: the bracket
+// update from the previous iteration's event values, then t_mid and y_mid (iter < nitrs_r), or event_t and the state
+// there (iter == nitrs_r).  Every unit of a row forms the same bracket; the row's first unit stores it.  A row done at t0
+// (no accepted step: its event value was 0 there) has nitrs 0 and returns (t0, y_start).
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+k_rows_event_bisect(const TdqCtrl *__restrict__ c, Rows R, Geom g, BisectArgs a, int iter) {
+    size_t u, lo, hi;
+    int r;
+    if (!unit_of(g, u, r, lo, hi)) return;
+    const int nit = a.nitrs[r];
+    if (iter > nit) return;
+    const double s0 = a.ev.sign0[r], t0 = fld<double>(R, TDQ_ROWS_T0)[r], t1 = fld<double>(R, TDQ_ROWS_T1)[r];
+    double blo = t0, bhi = t1;
+    if (iter > 0) {
+        const int p = (iter - 1) & 1;
+        blo = a.lo[(size_t)p * R.B + r];
+        bhi = a.hi[(size_t)p * R.B + r];
+        const double mid = (bhi + blo) / 2.0;
+        if (s0 == sign_of(ev_combined(a.ev.val, a.ev.init, a.ev.K, r))) blo = mid;   // torch.where(same, mid, lo)
+        else bhi = mid;
+    }
+    const int lane = threadIdx.x & 31;
+    const bool first = lane == 0 && lo == 0;
+    if (first) {
+        a.lo[(size_t)(iter & 1) * R.B + r] = blo;
+        a.hi[(size_t)(iter & 1) * R.B + r] = bhi;
+    }
+    const size_t base = (size_t)r * g.D;
+    const T *y0 = reinterpret_cast<const T *>(a.y_start) + base;
+    if (fld<int64_t>(R, TDQ_ROWS_N_ACCEPT)[r] == 0) {                    // done at t0 (rk_common.py:254-255)
+        if (first) a.event_t[r] = t0 * c->t_sign;
+        T *out = reinterpret_cast<T *>(a.y_event) + base;
+        for (size_t i = lo + lane; i < hi; i += 32) out[i] = y0[i];
+        return;
+    }
+    const double tq = (bhi + blo) / 2.0;                                  // t_mid, or event_t = (lo + hi) / 2
+    const bool last = iter == nit;
+    if (first) {
+        if (last) a.event_t[r] = tq * c->t_sign;
+        else a.t_ev[r] = tq * c->t_sign;
+    }
+    const T x = (T)((tq - t0) / (t1 - t0));
+    T *out = reinterpret_cast<T *>(last ? a.y_event : a.y_mid) + base;
+    const T *cf = reinterpret_cast<const T *>(a.coeff) + base;
+    const size_t n = a.n;
+    for (size_t i = lo + lane; i < hi; i += 32)
+        out[i] = eval_poly<T>(cf[i], cf[n + i], cf[2 * n + i], cf[3 * n + i], cf[4 * n + i], x);
 }
 
 // ---- host helpers -----------------------------------------------------------------------------------------------------------
@@ -785,8 +948,80 @@ int tdq_rows_controller(void *ctrl_dev, void *rows_dev, int32_t dtype, const dou
                         size_t row_len, void *stream) {
     TDQ_REQUIRE(ctrl_dev && rows_dev && norm_in, "null argument");
     TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
-    TDQ_DISPATCH_T(dtype, (k_rows_controller<T><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
-                               (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), norm_in, row_len)));
+    TDQ_DISPATCH_T(dtype, (k_rows_controller<T, false><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), norm_in, row_len, RowEvents{})));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+#define TDQ_ROWS_REQUIRE_K(K) TDQ_REQUIRE((K) >= 1 && (K) <= 65536, "K out of range")
+
+int tdq_rows_event_init(void *rows_dev, const double *ev_val, double *init_sign, double *sign0, int32_t *flag,
+                        size_t n_rows, int32_t K, void *stream) {
+    TDQ_REQUIRE(rows_dev && ev_val && init_sign && sign0 && flag, "null argument");
+    TDQ_REQUIRE(n_rows >= 1 && n_rows <= (size_t)INT_MAX, "n_rows out of range");
+    TDQ_ROWS_REQUIRE_K(K);
+    k_rows_event_init<<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(make_rows(rows_dev, n_rows), ev_val,
+                                                                                 init_sign, sign0, flag, K);
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_controller_event(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in, const double *ev_val,
+                              const double *init_sign, const double *sign0, int32_t *flag, size_t n_rows, size_t row_len,
+                              int32_t K, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && norm_in && ev_val && init_sign && sign0 && flag, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_ROWS_REQUIRE_K(K);
+    const RowEvents ev{ev_val, init_sign, sign0, flag, K};
+    TDQ_DISPATCH_T(dtype, (k_rows_controller<T, true><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), norm_in, row_len, ev)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_fit_store(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, const void *y1,
+                       const void *const *k, const int32_t *flag, void *coeff, size_t n_rows, size_t row_len,
+                       void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && tab && y1 && k && flag && coeff, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TdqHostShape hs;
+    tdq_shape_from_tableau(tab, &hs);
+    const int S = hs.n_stages, nk = hs.mid_nnz;
+    TDQ_REQUIRE(nk >= 1, "tableau has no mid-point weights");
+    TDQ_REQUIRE(k[S] != nullptr, "k_S is required");
+    KPtrs kmid;
+    bool vec = true;
+    TDQ_REQUIRE(plan_kp(hs.mid_idx, nk, k, kmid, vec), "missing stage slot for a non-zero mid-point weight");
+    const Geom g = make_geom(n_rows, row_len);
+    const Rows R = make_rows(rows_dev, n_rows);
+    int rc = -1;
+    TDQ_DISPATCH_T(dtype, rc = tdq_dispatch(TdqRange<1, TDQ_MAX_K>{}, nk, [&](auto NK) {
+                       k_rows_fit_store<T, NK><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(
+                           (const TdqCtrl *)ctrl_dev, R, g, (const T *)y1, (const T *)k[S], kmid, flag, (T *)coeff,
+                           n_rows * row_len);
+                       return 0;
+                   }));
+    TDQ_REQUIRE(rc == 0, "unsupported number of mid-point terms");
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_event_bisect(void *ctrl_dev, void *rows_dev, int32_t dtype, int32_t iter, const double *ev_val,
+                          const double *init_sign, const double *sign0, const int32_t *nitrs, double *lo, double *hi,
+                          const void *coeff, const void *y_start, void *y_mid, double *t_ev, double *event_t,
+                          void *y_event, size_t n_rows, size_t row_len, int32_t K, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && ev_val && init_sign && sign0 && nitrs && lo && hi && coeff && y_start && y_mid &&
+                    t_ev && event_t && y_event,
+                "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_ROWS_REQUIRE_K(K);
+    TDQ_REQUIRE(iter >= 0, "iter must be at least 0");
+    BisectArgs a{RowEvents{ev_val, init_sign, sign0, nullptr, K}, nitrs, lo, hi, coeff, y_start, y_mid, t_ev, event_t,
+                 y_event, n_rows * row_len};
+    const Geom g = make_geom(n_rows, row_len);
+    TDQ_DISPATCH_T(dtype, (k_rows_event_bisect<T><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(
+                               (const TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), g, a, iter)));
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
 }

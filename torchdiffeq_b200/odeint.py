@@ -319,17 +319,31 @@ def _check_independent_rows(func, y0, t, method, options, event_fn):
         no("a custom norm callable (each row's error ratio is the RMS over its own elements)")
     if any(getattr(func, name, None) is not None for name in _CALLBACK_NAMES):
         no("callbacks")
-    if event_fn is not None:
-        no("event_fn / odeint_event")
     if torch.is_grad_enabled():
         from .backprop import discover_params
         if y0.requires_grad or (isinstance(t, torch.Tensor) and t.requires_grad) or discover_params(func):
             no("gradients (odeint under autograd with anything requiring grad); run it under torch.no_grad()")
     if y0.dim() < 1 or y0.shape[0] < 1:
         raise ValueError("options['independent_rows'] needs y0 of shape [B, ...] with B >= 1, got %s" % (tuple(y0.shape),))
+    if event_fn is None:
+        return None
+    # event_fn(t, y) is called with t a float64 [B, 1, ...] tensor of each row's time and must give one value, or K,
+    # per row; this first call at t0 also starts the solve
+    if len(t) != 2:                                                                    # misc.py:203-204
+        raise ValueError(f"We require len(t) == 2 when in event handling mode, but got len(t)={len(t)}.")
+    B = y0.shape[0]
+    t0 = torch.full((B,) + (1,) * (y0.dim() - 1), float(t[0]), dtype=torch.float64, device=y0.device)
+    with torch.no_grad():
+        v = event_fn(t0, y0)
+    if not isinstance(v, torch.Tensor) or v.dim() == 0:
+        no("an event function with a 0-dim result: it must return one value per row, [B] or [B, K...]")
+    if v.shape[0] != B or v.numel() == 0:
+        raise ValueError("with options['independent_rows'] event_fn must return a tensor of shape [B] or [B, K...] with "
+                         "B = %d, got %s" % (B, tuple(v.shape)))
+    return v
 
 
-def _make_rows_engine(p):
+def _make_rows_engine(p, graph=None):
     o = p.options
     _warn_unused(p.method, o, _ADAPTIVE_OPTIONS)
     if o.get("dtype", torch.float64) != torch.float64:
@@ -339,8 +353,27 @@ def _make_rows_engine(p):
         t_sign=p.t_sign, min_step=o.get("min_step", 0), max_step=o.get("max_step", float("inf")),
         first_step=o.get("first_step"), safety=o.get("safety", 0.9), ifactor=o.get("ifactor", 10.0),
         dfactor=o.get("dfactor", 0.2), max_num_steps=o.get("max_num_steps", 2 ** 31 - 1),
-        graph=_resolve_graph(o.get("graph", "auto"), p.original_func), run_ahead=o.get("run_ahead", 2),
-        device_loop=o.get("device_loop", "auto"))
+        graph=_resolve_graph(o.get("graph", "auto"), p.original_func) if graph is None else graph,
+        run_ahead=o.get("run_ahead", 2), device_loop=o.get("device_loop", "auto"))
+
+
+def _solve_rows_event(p, event_fn, ev0):
+    """Every row until its own event (options={'independent_rows': True}); returns (event_t float64 [B] in the caller's
+    time, solution [2, n], engine).  The captured attempt runs event_fn's Python once, so graph='auto' captures only when
+    func and event_fn are both nn.Modules.  Event engines are not cached."""
+    graph = _resolve_graph(p.options.get("graph", "auto"), p.original_func)
+    if graph == "auto" and not isinstance(event_fn, torch.nn.Module):
+        graph = False
+    eng = _make_rows_engine(p, graph=graph)
+    B, shape = p.shape[0], p.shape
+    # the bisection tolerance: atol, or with a per-element atol the smallest of the row's own elements
+    if p.atol_vec is not None:
+        tol = p.atol_vec.view(B, -1).min(dim=1).values.cpu()
+    else:
+        tol = torch.full((B,), float(p.atol), dtype=torch.float64)
+    event_t, sol = eng.solve_until_event(p.y0_flat, float(p.t_cpu[0]), lambda t_, y_: event_fn(t_, y_.view(shape)), ev0,
+                                         tol)
+    return event_t, sol, eng
 
 
 # ---- engine cache -------------------------------------------------------------------------------
@@ -632,6 +665,10 @@ def odeint_event(func, y0, t0, *, event_fn, reverse_time=False, odeint_interface
         t = torch.cat([t0.reshape(-1), t0.reshape(-1).detach() - 1.0])
     else:
         t = torch.cat([t0.reshape(-1), t0.reshape(-1).detach() + 1.0])
+    if (kwargs.get("options") or {}).get("independent_rows"):
+        # one event time per row: the implicit-function rerouting below assumes one scalar event time, and this mode
+        # refuses gradients anyway
+        return odeint_interface(func, y0, t, event_fn=event_fn, **kwargs)
     event_t, solution = odeint_interface(func, y0, t, event_fn=event_fn, **kwargs)
     p = normalise(func, y0, t, 0.0, 0.0, kwargs.get("method"), None, event_fn)        # flat func / event_fn, :172
     sign_ = p.t_sign
@@ -764,9 +801,22 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
     on the other rows.  In this mode func's time argument is a tensor of shape [B, 1, ..., 1] (y0.dim() dimensions, state
     dtype) holding each row's time, so `t * y` and `torch.sin(t) + y` broadcast row by row.  last_stats() then also has
     row_n_accept / row_n_reject (CPU int64 tensors of shape [B]).
+
+    With independent rows, event_fn (and odeint_event) finds each row's own event: row r's (event_t[r], solution[:, r])
+    is the reference's odeint_event(func, y0[r:r+1], t[0], event_fn) for the event function restricted to that row.
+    event_fn(t, y) gets t as a float64 [B, 1, ..., 1] tensor of each row's time (caller's direction) and returns [B] or
+    [B, K...] (K components per row, combined per row as the reference combines them).  It is called on the whole batch:
+    once at t[0], once per attempt and once per bisection iteration; values of rows that did not accept, or are done, are
+    ignored.  event_t has shape [B] and the solution [2, B, ...].  The bisection tolerance is atol; with a per-element atol
+    tensor row r uses the smallest of its own elements (the reference refuses a tensor atol there).  last_stats() adds
+    event_calls and bisect_iters (the largest per-row bisection count).
     """
+    row_ev0 = row_event_fn = None
     if options and options.get("independent_rows"):
-        _check_independent_rows(func, y0, t, method, options, event_fn)
+        row_ev0 = _check_independent_rows(func, y0, t, method, options, event_fn)
+        if row_ev0 is not None:
+            # normalise must not call it: the row engine combines each row's own components
+            row_event_fn, event_fn = event_fn, None
     p = normalise(func, y0, t, rtol, atol, method, options, event_fn)
     if torch.is_grad_enabled():
         from .backprop import discover_params
@@ -790,8 +840,13 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
             event_t, sol, eng = _solve_event(p)
             ss.publish(sol)
             return torch.tensor(event_t, dtype=t.dtype, device=t.device), _unflatten(p, sol)     # odeint.py:98, :105-108
-        sol, eng = _solve(p)
-        ss.publish(sol)
+        if row_event_fn is not None:
+            row_event_t, sol, eng = _solve_rows_event(p, row_event_fn, row_ev0)
+            row_event_t = row_event_t.to(device=t.device, dtype=t.dtype, copy=True)
+            ss.publish(row_event_t, sol)
+        else:
+            sol, eng = _solve(p)
+            ss.publish(sol)
     _LAST_STATS.clear()
     _LAST_STATS.update(nfe=eng.nfe, launches=getattr(eng, "launches", 0), attempts=getattr(eng, "n_attempts", None),
                        n_accept=getattr(eng, "n_accept", None), n_reject=getattr(eng, "n_reject", None),
@@ -799,10 +854,14 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
                        fused_attempt=bool((getattr(eng, "linear", None) or {}).get("whole")))
     if getattr(eng, "row_n_accept", None) is not None:
         _LAST_STATS.update(row_n_accept=eng.row_n_accept, row_n_reject=eng.row_n_reject)
+    if row_event_fn is not None:
+        _LAST_STATS.update(event_calls=eng.n_ev, bisect_iters=eng.bisect_iters)
     if _stats is not None:               # private: solver counters for bench.py and the tests
         _stats["nfe"] = eng.nfe
         _stats["launches"] = _stats.get("launches", 0) + getattr(eng, "launches", 0)
         _stats["attempts"] = getattr(eng, "n_attempts", None)
         _stats["n_accept"], _stats["n_reject"] = getattr(eng, "n_accept", None), getattr(eng, "n_reject", None)
         _stats["fused_linear"], _stats["fused_attempt"] = _LAST_STATS["fused_linear"], _LAST_STATS["fused_attempt"]
+    if row_event_fn is not None:
+        return row_event_t, _unflatten(p, sol)
     return _unflatten(p, sol)
