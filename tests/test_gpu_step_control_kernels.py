@@ -132,7 +132,10 @@ INIT_CASES = {
 
 
 @pytest.mark.parametrize("t_sign", [1.0, -1.0])
-@pytest.mark.parametrize("dtype,ratio_f64", [(torch.float32, False), (torch.float32, True), (torch.float64, True)])
+@pytest.mark.parametrize("dtype,ratio_f64", [(torch.float32, False),
+                                             # h0 = (T)1e-6 stays a float32 tensor: misc.py:72 and :77 round to float32
+                                             pytest.param(torch.float32, True, id="float32-tensor_tols"),
+                                             (torch.float64, True)])
 @pytest.mark.parametrize("case", list(INIT_CASES))
 def test_initial_step_branches(case, dtype, ratio_f64, t_sign):
     """tdq_initial_step_h0 / _finish on hand-made segment sums, so that every branch and boundary of misc.py:60-77 is
@@ -159,15 +162,17 @@ def test_initial_step_branches(case, dtype, ratio_f64, t_sign):
 
     d0, d1, nd = _norm(d0s, T, ratio_f64), _norm(d1s, T, ratio_f64), _norm(d2s, T, ratio_f64)
     pow_decides = False
-    if ratio_f64:                                                    # everything in float64
-        h0 = float(torch.tensor(1e-6, dtype=T)) if (d0 < 1e-5 or d1 < 1e-5) else abs(0.01 * d0 / d1)
+    if ratio_f64:                                                    # the norms in float64
+        h0_T = d0 < 1e-5 or d1 < 1e-5                                # misc.py:61: h0 is then a tensor of T
+        h0 = float(torch.tensor(1e-6, dtype=T)) if h0_T else abs(0.01 * d0 / d1)
         d2 = abs(nd / h0)
+        h100 = float(100 * torch.tensor(h0, dtype=T)) if h0_T else 100.0 * h0
         if d1 <= 1e-15 and d2 <= 1e-15:
-            h1 = max(float(torch.tensor(1e-6, dtype=T)), h0 * 1e-3)
+            h1 = max(float(torch.tensor(1e-6, dtype=T)), float(torch.tensor(h0, dtype=T) * 1e-3) if h0_T else h0 * 1e-3)
         else:
             h1 = abs((torch.tensor(0.01, dtype=torch.float64) / max(d1, d2)) ** (1.0 / order)).item()
-            pow_decides = h1 < 100.0 * h0
-        want_dt = min(100.0 * h0, h1)
+            pow_decides = h1 < h100
+        want_dt = min(h100, h1)
     else:                                                            # misc.py:55-77 with 0-dim tensors of T
         d0t, d1t = torch.tensor(d0, dtype=T), torch.tensor(d1, dtype=T)
         h0t = torch.tensor(1e-6, dtype=T) if (d0t < 1e-5 or d1t < 1e-5) else 0.01 * d0t / d1t

@@ -47,12 +47,17 @@ template <typename T>
 __device__ __forceinline__ double tdq_initial_finish(bool ratio_f64, int order_p1, double d1d, double h0d, double nd) {
     using A = Ar<T>;
     if (ratio_f64) {
+        // h0 is a tensor of T when :60-61 chose the constant 1e-6 (d0 or d1 below 1e-5; then h0d is exactly (T)1e-6),
+        // and its products of :72 and :77 round to T; the quotient of :63 is float64.  A quotient that lands exactly
+        // on (T)1e-6 with d1 >= 1e-5 is taken for the constant.
+        const bool h0_T = d1d < 1e-5 || h0d == (double)(T)1e-6;
         const double d2 = fabs(nd / h0d);
         double h1;
-        if (d1d <= 1e-15 && d2 <= 1e-15) h1 = fmax((double)(T)1e-6, h0d * 1e-3);
+        if (d1d <= 1e-15 && d2 <= 1e-15)
+            h1 = fmax((double)(T)1e-6, h0_T ? (double)A::mul((T)h0d, (T)1e-3) : h0d * 1e-3);
         else h1 = pow(0.01 / ((d2 > d1d) ? d2 : d1d), 1.0 / (double)order_p1);
         h1 = fabs(h1);
-        return fmin(100.0 * h0d, h1);
+        return fmin(h0_T ? (double)A::mul((T)100, (T)h0d) : 100.0 * h0d, h1);
     }
     const T d1 = (T)d1d, h0 = (T)h0d;
     const T d2 = A::abs(A::div((T)nd, h0));
