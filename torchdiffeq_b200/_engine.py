@@ -514,19 +514,22 @@ class AdaptiveEngine:
         return mb
 
     def _raise_if_failed(self, mb):
-        s = mb.status
-        if s == _lib.RUN_OK:
-            return
-        torch.cuda.current_stream().synchronize()
+        if mb.status != _lib.RUN_OK:
+            torch.cuda.current_stream().synchronize()
+            self._raise_status(mb.status, mb.next_dt, self.y0w)
+
+    def _raise_status(self, s, dt, y, where=""):
+        """The reference's failure for run status `s` of the attempt with step `dt` from state `y`."""
         if s == _lib.RUN_DT_UNDERFLOW:
-            raise SolverFailure("underflow in dt {}".format(mb.next_dt))
+            raise SolverFailure("underflow in dt {}".format(dt) + where)
         if s == _lib.RUN_NONFINITE:
-            raise SolverFailure("non-finite values in state `y`: {}".format(self.y0w))
+            raise SolverFailure("non-finite values in state `y`: {}".format(y) + where)
         if s == _lib.RUN_EXCHANGE_TIMEOUT:
             raise _lib.TdqError("a peer rank did not deliver its norm partials within 10 s (sharded solve)")
         if s == _lib.RUN_MAX_STEPS:
-            raise SolverFailure("max_num_steps exceeded ({}>={})".format(self.opt.max_num_steps, self.opt.max_num_steps))
-        raise SolverFailure("solver failed with status %d" % s)
+            m = self.opt.max_num_steps
+            raise SolverFailure("max_num_steps exceeded ({}>={})".format(m, m) + where)
+        raise SolverFailure("solver failed with status %d" % s + where)
 
     def _lockstep_mode(self):
         return bool(self.callbacks) or self.run_ahead == 0
@@ -578,7 +581,8 @@ class AdaptiveEngine:
         return self._graph is not None
 
     def _begin(self, y0_flat, t64, t_start=None, loop=False):
-        """Everything of a solve that precedes the first attempt (rk_common.py:166-241)."""
+        """Everything of a solve that precedes the first attempt (rk_common.py:166-241): the per-solve reset of the
+        engine and the control block, then `_start`.  Returns the number of output times."""
         lib = self.lib
         self.nfe_total += self.nfe
         self.nfe, self.launches = 0, 0                  # per-solve counters (engines are reused)
@@ -601,6 +605,13 @@ class AdaptiveEngine:
         self.opt.loop_handle = self._loop_handle if loop else 0
         _lib.check(lib.tdq_ctrl_init(self.ctrl.data_ptr(), C.byref(self.tab), C.byref(self.opt),
                                      self.t_out.data_ptr(), float(t_start), n_out, self.mbox_dev, st))
+        self._start(float(t_start), n_out)
+        return n_out
+
+    def _start(self, t_start, n_out):
+        """The solve's start after the reset: the time grids, f0, the initial step and the first attempt's prepare."""
+        lib = self.lib
+        st = _stream()
         if self.exchange is not None:
             self.exchange.arm(self.ctrl.data_ptr(), st)
         if self.jump_t is not None and self.jump_t.numel() > 0:
@@ -639,7 +650,6 @@ class AdaptiveEngine:
             self._launch(lib.tdq_set_first_step(ctrl, float(self.first_step), st))
         bad_ptr = self.dsum[0].data_ptr() + 8 * self.n_seg if n_out > 1 else None
         self._launch(lib.tdq_prepare_attempt(ctrl, dc, bad_ptr, st))
-        return n_out
 
     # ---- lock step: the reference's exact call sequence --------------------------------------
     def _lockstep_attempt(self, issued, mb):
@@ -1079,31 +1089,11 @@ class RowsEngine(AdaptiveEngine):
                 self._ev_call(self.ytmp)
         return self.ev_event_t, self.solution
 
-    def _begin(self, y0_flat, t64, t_start=None, loop=False):
-        """rk_common.py:166-241 for every row: f0 on the whole batch, then each row's initial step."""
-        lib = self.lib
-        self.nfe_total += self.nfe
-        self.nfe, self.launches = 0, 0
-        n_out = int(t64.numel())
-        self.t_out = t64.contiguous()
-        if getattr(self, "solution", None) is None or self.solution.shape[0] != n_out:
-            self.solution = torch.empty(n_out, self.n, dtype=self.dtype, device=self.device)
-            self._drop_graph()
-            self._own_ptrs = None
-            loop = False
-        self.solution[0].copy_(y0_flat)
-        self.ybuf[0].copy_(y0_flat)
-        st = _stream()
-        mb = self.mbox_host.contents
-        mb.seq, mb.status, mb.done, mb.par, mb.accept = 0, 0, 0, 0, 0
-        mb.n_accept, mb.n_reject = 0, 0
-        if t_start is None:
-            t_start = float(t64[0])
-        self.opt.loop_handle = self._loop_handle if loop else 0
+    def _start(self, t_start, n_out):
+        """rk_common.py:213-241 for every row: f0 on the whole batch, then each row's initial step."""
+        lib, st = self.lib, _stream()
         ctrl, rows, dc, B, D = self.ctrl.data_ptr(), self.rows.data_ptr(), self.dt_code, self.B, self.D
-        _lib.check(lib.tdq_ctrl_init(ctrl, C.byref(self.tab), C.byref(self.opt), self.t_out.data_ptr(), float(t_start),
-                                     n_out, self.mbox_dev, st))
-        self._launch(lib.tdq_rows_init(ctrl, rows, dc, B, float(t_start), st))
+        self._launch(lib.tdq_rows_init(ctrl, rows, dc, B, t_start, st))
         f0 = self._call_fn(self.t_first, self.ybuf[0], 0, dst=self.kbuf[0])
         if f0.data_ptr() != self.kbuf[0].data_ptr():
             self.kbuf[0].copy_(f0)
@@ -1124,29 +1114,18 @@ class RowsEngine(AdaptiveEngine):
             self._launch(lib.tdq_rows_event_init(rows, self.ev_val.data_ptr(), self.ev_init.data_ptr(),
                                                  self.ev_sign0.data_ptr(), self.ev_flag.data_ptr(), B, self.K, st))
         self._launch(lib.tdq_rows_prepare(ctrl, rows, dc, d[0].data_ptr() if n_out > 1 else None, B, st))
-        return n_out
 
     def row_field(self, which, dtype):
         return self._field(which, dtype, torch.empty((), dtype=dtype).element_size())
 
     def _raise_if_failed(self, mb):
-        s = mb.status
-        if s == _lib.RUN_OK:
+        if mb.status == _lib.RUN_OK:
             return
         torch.cuda.current_stream().synchronize()
         r = int(self.rows[:16].view(torch.int32)[3])               # the smallest failing row
-        where = " (row %d)" % r
-        if s == _lib.RUN_DT_UNDERFLOW:
-            raise SolverFailure("underflow in dt {}".format(float(self.row_field(_lib.ROWS_ATT_DT, torch.float64)[r]))
-                                + where)
-        if s == _lib.RUN_NONFINITE:
-            par = int(self.row_field(_lib.ROWS_PAR, torch.int32)[r])
-            y = self.ybuf[par][r * self.D:(r + 1) * self.D].view(1, *self.row_shape)      # y0[r:r+1]
-            raise SolverFailure("non-finite values in state `y`: {}".format(y) + where)
-        if s == _lib.RUN_MAX_STEPS:
-            m = self.opt.max_num_steps
-            raise SolverFailure("max_num_steps exceeded ({}>={})".format(m, m) + where)
-        raise SolverFailure("solver failed with status %d" % s + where)
+        par = int(self.row_field(_lib.ROWS_PAR, torch.int32)[r])
+        y = self.ybuf[par][r * self.D:(r + 1) * self.D].view(1, *self.row_shape)      # y0[r:r+1]
+        self._raise_status(mb.status, float(self.row_field(_lib.ROWS_ATT_DT, torch.float64)[r]), y, " (row %d)" % r)
 
     def solve(self, y0_flat, t64, t_start=None):
         sol = super().solve(y0_flat, t64, t_start)

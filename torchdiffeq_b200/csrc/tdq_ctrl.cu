@@ -25,9 +25,7 @@ template <typename T> __device__ void prepare_scalar(TdqCtrl &c) {
         c.halt = 1;
         return;
     }
-    double dt = c.dt;
-    if (!isfinite(dt)) dt = c.min_step;                               // :269-270
-    dt = fmin(fmax(dt, c.min_step), c.max_step);                      // :271
+    double dt = tdq_clamp_dt(c.dt, c.min_step, c.max_step);           // :269-271
     const double t0 = c.t1;
     double t1 = t0 + dt;                                              // :273
     c.att_t0 = t0;
@@ -68,24 +66,18 @@ template <typename T> __device__ void prepare_scalar(TdqCtrl &c) {
 
 template <typename T> __device__ void prepare_tables(TdqCtrl &c, int tid, int nthreads) {
     if (c.halt) return;
-    using A = Ar<T>;
     const T t0T = (T)c.att_t0, dtT = (T)c.att_dt, t1T = (T)c.att_t1;  // :61-65
     const T sgn = (T)c.t_sign;
     const int S = c.n_stages;
-    for (int i = tid; i < S; i += nthreads) {                         // :72-78
-        const T a = (T)c.alpha[i];
-        T ti;
-        if (a == (T)1) ti = prev_repr<T>(t1T);
-        else ti = A::add(t0T, A::mul(a, dtT));
-        store_T<T>(c.tstage, i, A::mul(sgn, ti));
-    }
+    for (int i = tid; i < S; i += nthreads)                           // :72-78
+        store_T<T>(c.tstage, i, tdq_stage_time<T>((T)c.alpha[i], t0T, dtT, t1T, sgn));
     const int rows = c.fsal ? S : S + 1;
     for (int e = tid; e < rows * TDQ_MAX_K; e += nthreads) {          // :79 (beta_i * dt), :85 (dt * c_sol)
         const int r = e / TDQ_MAX_K, m = e % TDQ_MAX_K;
-        if (m < c.row_nnz[r]) c.coef[r][m] = (double)A::mul(sgn, A::mul((T)c.beta[r][m], dtT));
+        if (m < c.row_nnz[r]) c.coef[r][m] = (double)tdq_coef<T>(sgn, (T)c.beta[r][m], dtT);
     }
     for (int m = tid; m < c.err_nnz; m += nthreads)                   // :89
-        c.ecoef[m] = (double)A::mul(sgn, A::mul(dtT, (T)c.c_err[m]));
+        c.ecoef[m] = (double)tdq_coef<T>(sgn, (T)c.c_err[m], dtT);
 }
 
 template <typename T> __device__ void prepare_attempt(TdqCtrl &c) {
@@ -105,8 +97,7 @@ __device__ double block_norm_from_sums(const TdqCtrl &c, const double *sums, con
     for (int s = threadIdx.x; s < n_seg; s += THREADS) {
         const double cnt = counts ? (double)counts[s] : (double)c.n_global;
         if (cnt <= 0.0) continue;
-        double r = sqrt(sums[s] / cnt);
-        if (!c.ratio_f64) r = (double)(T)r;
+        const double r = tdq_rms<T>(sums[s], cnt, c.ratio_f64);
         if (r != r) nan = 1;
         if (r > best) best = r;
     }
@@ -189,9 +180,7 @@ __device__ void controller(TdqCtrl &c, const double *norm_in, int n_seg, const v
     c.ratio = ratio;
 
     const double dt = c.att_dt;
-    bool accept = ratio <= 1.0;                                       // :324
-    if (dt > c.max_step) accept = false;                              // :327-328
-    if (dt <= c.min_step) accept = true;                              // :329-330
+    const bool accept = tdq_accept(ratio, dt, c.min_step, c.max_step);   // :324-330
     c.accept = accept ? 1 : 0;
 
     if (accept) {                                                     // :338-352
@@ -214,7 +203,7 @@ __device__ void controller(TdqCtrl &c, const double *norm_in, int n_seg, const v
         const T dtT = (T)c.att_dtT, sgn = (T)c.t_sign;
         c.fit_sdt = (double)A::mul(sgn, dtT);
         for (int m = 0; m < c.mid_nnz; ++m)
-            c.fit_mcoef[m] = (double)A::mul(sgn, A::mul(dtT, (T)c.c_mid[m]));
+            c.fit_mcoef[m] = (double)tdq_coef<T>(sgn, (T)c.c_mid[m], dtT);
         if (y1_nonfinite) {                                           // the next attempt would trip :287
             c.status = TDQ_RUN_NONFINITE;
             c.halt = 1;
@@ -233,8 +222,7 @@ __device__ void controller(TdqCtrl &c, const double *norm_in, int n_seg, const v
     c.emit_lo = c.out_cursor;
     c.n_steps_interval += 1;
     if (accept) {
-        int cur = c.out_cursor;
-        while (cur < c.n_out && !(c.t_out[cur] > c.t1)) ++cur;
+        const int cur = tdq_cursor_after(c.t_out, c.n_out, c.out_cursor, c.t1);
         if (cur != c.out_cursor) c.n_steps_interval = 0;
         c.out_cursor = cur;
     }

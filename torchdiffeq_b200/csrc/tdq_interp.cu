@@ -13,23 +13,11 @@
 // for them.  The arithmetic, and hence every output bit, is that of interp.py:17-22, :39-46.
 #include "tdq_common.cuh"
 #include "tdq_shape.cuh"
+#include "tdq_step.cuh"
 
 namespace {
 
 constexpr int kThreads = 256;
-
-// x = T((t - t0)/(t1 - t0)) in float64 then cast (interp.py:39-40); running powers, not Horner (interp.py:42-46).
-template <typename T> __device__ __forceinline__ T eval_poly(T e, T d, T cq, T b, T a, T x) {
-    using A = Ar<T>;
-    T total = A::add(e, A::mul(x, d));
-    T xp = A::mul(x, x);
-    total = A::add(total, A::mul(xp, cq));
-    xp = A::mul(xp, x);
-    total = A::add(total, A::mul(xp, b));
-    xp = A::mul(xp, x);
-    total = A::add(total, A::mul(xp, a));
-    return total;
-}
 
 template <typename T, int NK, bool VECTOR, bool STORE>
 __global__ void __launch_bounds__(kThreads)
@@ -53,21 +41,7 @@ k_fit_eval(const TdqCtrl *__restrict__ c, const T *__restrict__ y1p, const T *__
     const double t0 = c->t0, t1 = c->t1;
 
     auto fit = [&](T y0v, T y1v, T f0, T f1, const T *kv, T &e, T &d, T &cq, T &b, T &a) {
-        T acc = A::mul(kv[0], mf[0]);
-#pragma unroll
-        for (int m = 1; m < NK; ++m) acc = A::add(acc, A::mul(kv[m], mf[m]));
-        const T ymid = A::add(y0v, acc);
-        // a = 2*dt*(f1 - f0) - 8*(y1 + y0) + 16*y_mid
-        a = A::add(A::sub(A::mul(two_sdt, A::sub(f1, f0)), A::mul((T)8, A::add(y1v, y0v))), A::mul((T)16, ymid));
-        // b = dt*(5*f0 - 3*f1) + 18*y0 + 14*y1 - 32*y_mid
-        b = A::sub(A::add(A::add(A::mul(sdt, A::sub(A::mul((T)5, f0), A::mul((T)3, f1))), A::mul((T)18, y0v)),
-                          A::mul((T)14, y1v)),
-                   A::mul((T)32, ymid));
-        // c = dt*(f1 - 4*f0) - 11*y0 - 5*y1 + 16*y_mid
-        cq = A::add(A::sub(A::sub(A::mul(sdt, A::sub(f1, A::mul((T)4, f0))), A::mul((T)11, y0v)), A::mul((T)5, y1v)),
-                    A::mul((T)16, ymid));
-        d = A::mul(sdt, f0);
-        e = y0v;
+        tdq_quartic<T>(y0v, y1v, f0, f1, tdq_combine<T, NK>(y0v, kv, mf), sdt, two_sdt, e, d, cq, b, a);
     };
     auto xof = [&](int j) -> T { return (T)((c->t_out[j] - t0) / (t1 - t0)); };
 
@@ -97,7 +71,7 @@ k_fit_eval(const TdqCtrl *__restrict__ c, const T *__restrict__ y1p, const T *__
                 const T x = xof(j);
                 V r;
 #pragma unroll
-                for (int l = 0; l < V::N; ++l) r.v[l] = eval_poly<T>(re.v[l], rd.v[l], rc.v[l], rb.v[l], ra.v[l], x);
+                for (int l = 0; l < V::N; ++l) r.v[l] = tdq_eval_poly<T>(re.v[l], rd.v[l], rc.v[l], rb.v[l], ra.v[l], x);
                 st_vec<T>(solution + (size_t)j * n + i0, r);
             }
         }
@@ -110,7 +84,7 @@ k_fit_eval(const TdqCtrl *__restrict__ c, const T *__restrict__ y1p, const T *__
                 T e, d, cq, b, a;
                 fit(y0p[i], y1p[i], k0p[i], kSp[i], ke, e, d, cq, b, a);
                 if (STORE) { ce[i] = e; cd[i] = d; cc[i] = cq; cb[i] = b; ca[i] = a; }
-                for (int j = lo; j < hi; ++j) solution[(size_t)j * n + i] = eval_poly<T>(e, d, cq, b, a, xof(j));
+                for (int j = lo; j < hi; ++j) solution[(size_t)j * n + i] = tdq_eval_poly<T>(e, d, cq, b, a, xof(j));
             }
         }
     } else {
@@ -121,7 +95,7 @@ k_fit_eval(const TdqCtrl *__restrict__ c, const T *__restrict__ y1p, const T *__
             T e, d, cq, b, a;
             fit(y0p[i], y1p[i], k0p[i], kSp[i], ke, e, d, cq, b, a);
             if (STORE) { ce[i] = e; cd[i] = d; cc[i] = cq; cb[i] = b; ca[i] = a; }
-            for (int j = lo; j < hi; ++j) solution[(size_t)j * n + i] = eval_poly<T>(e, d, cq, b, a, xof(j));
+            for (int j = lo; j < hi; ++j) solution[(size_t)j * n + i] = tdq_eval_poly<T>(e, d, cq, b, a, xof(j));
         }
     }
 }
@@ -151,7 +125,7 @@ k_poly_eval(const T *__restrict__ ce, const T *__restrict__ cd, const T *__restr
             const T *__restrict__ ca, T *__restrict__ out, double x64, size_t n) {
     const T x = (T)x64;
     for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += (size_t)gridDim.x * kThreads)
-        out[i] = eval_poly<T>(ce[i], cd[i], cc[i], cb[i], ca[i], x);
+        out[i] = tdq_eval_poly<T>(ce[i], cd[i], cc[i], cb[i], ca[i], x);
 }
 
 // The stored interpolant of the last accepted step at a device-resident time (event bisection).
@@ -163,19 +137,18 @@ k_interp_eval_at(const TdqCtrl *__restrict__ c, const T *__restrict__ ce, const 
     const double t0 = c->t0, t1 = c->t1;
     const T x = (T)((*t_at - t0) / (t1 - t0));
     for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += (size_t)gridDim.x * kThreads)
-        out[i] = eval_poly<T>(ce[i], cd[i], cc[i], cb[i], ca[i], x);
+        out[i] = tdq_eval_poly<T>(ce[i], cd[i], cc[i], cb[i], ca[i], x);
 }
 
 // y_probe = y0 + h0*f0 with f0 = s*k0 (misc.py:66)
 template <typename T>
 __global__ void __launch_bounds__(kThreads)
 k_probe(const TdqCtrl *__restrict__ c, T *__restrict__ out, const T *y0, const T *f0, size_t n) {
-    using A = Ar<T>;
     if (y0 == nullptr) y0 = reinterpret_cast<const T *>(c->y0_cur);
     if (f0 == nullptr) f0 = reinterpret_cast<const T *>(c->k0_cur);
-    const T h = A::mul((T)c->t_sign, (T)c->h0);
+    const T h = tdq_probe_h<T>(c->t_sign, c->h0);
     for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += (size_t)gridDim.x * kThreads)
-        out[i] = A::add(y0[i], A::mul(h, f0[i]));
+        out[i] = tdq_probe<T>(y0[i], h, f0[i]);
 }
 
 }  // namespace

@@ -18,6 +18,7 @@
 // partials in index order, so a result depends on n and the segment list only -- not on the schedule.
 #include "tdq_common.cuh"
 #include "tdq_shape.cuh"
+#include "tdq_step.cuh"
 
 namespace {
 
@@ -25,9 +26,6 @@ constexpr int kThreads = 256;
 constexpr int kChunk = 2048;            // elements per chunk of the multi-segment path
 constexpr int kMaxGrid = 132 * 4;       // persistent grid of the single-segment path (H100 SXM: 132 SMs); a constant,
                                         // so that partial sums do not depend on the device the library runs on
-
-template <typename T, bool VTOL> struct TolT { using type = T; };
-template <typename T> struct TolT<T, true> { using type = double; };
 
 struct NormArgs {
     const void *x;          // MODE 0: err_pre          MODE 1/2: x
@@ -49,7 +47,7 @@ __global__ void __launch_bounds__(kThreads)
 k_norm(const TdqCtrl *__restrict__ c, NormArgs a) {
     if (c->halt) return;
     using A = Ar<T>;
-    using Q = typename TolT<T, VTOL>::type;     // dtype of tol and of err/tol (float64 with vector tolerances)
+    using Q = typename std::conditional<VTOL, double, T>::type;   // dtype of tol and of err/tol (float64 with vector tolerances)
     using V = Vec<T>;
     constexpr int VN = VECTOR ? V::N : 1;
     __shared__ double red[kThreads / 32];
@@ -76,22 +74,7 @@ k_norm(const TdqCtrl *__restrict__ c, NormArgs a) {
         if (MODE == 0 && !A::finite(v1)) bad += 1.0;
         if (MODE == 1 && !A::finite(v0)) bad += 1.0;      // d0's pass over y0 doubles as rk_common.py:287's check
         if (!in_seg) return;
-        T num;
-        if (MODE == 0) num = ek ? A::add(xa, A::mul(xb, ecS)) : xa;
-        else num = (MODE == 2) ? A::sub(xa, xb) : xa;
-        Q q;
-        if (VTOL) {
-            const double rt = a.rtol_v[i], at = a.atol_v[i];
-            double tol;
-            if (MODE == 0) tol = at + rt * (double)A::max_nan(A::abs(v0), A::abs(v1));
-            else tol = at + (double)A::abs(v0) * rt;
-            q = (Q)((double)num / tol);
-        } else {
-            T tol;
-            if (MODE == 0) tol = A::add(atolT, A::mul(rtolT, A::max_nan(A::abs(v0), A::abs(v1))));
-            else tol = A::add(atolT, A::mul(A::abs(v0), rtolT));
-            q = (Q)A::div(num, tol);
-        }
+        const Q q = tdq_err_q<T, MODE, VTOL>(v0, v1, xa, xb, ek, ecS, rtolT, atolT, a.rtol_v, a.atol_v, i);
         if (WRITEQ) reinterpret_cast<Q *>(a.q_out)[i] = q;
         const Q q2 = Ar<Q>::mul(q, q);                 // .abs().pow(2)
         acc += (double)q2;

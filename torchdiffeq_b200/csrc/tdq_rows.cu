@@ -86,7 +86,6 @@ template <typename T, int NK>
 __global__ void __launch_bounds__(kThreads)
 k_rows_combine(const TdqCtrl *__restrict__ c, Rows R, Geom g, int row, T *__restrict__ out, KPtrs kp, bool vec) {
     if (c->halt) return;
-    using A = Ar<T>;
     using V = Vec<T>;
     size_t u, lo, hi;
     int r;
@@ -105,15 +104,9 @@ k_rows_combine(const TdqCtrl *__restrict__ c, Rows R, Geom g, int row, T *__rest
     const T *k[NK];
 #pragma unroll
     for (int m = 0; m < NK; ++m) {
-        cf[m] = A::mul(sgn, A::mul((T)c->beta[row][m], dtT));             // t_sign * fl_T(beta_ij * T(dt_r))
+        cf[m] = tdq_coef<T>(sgn, (T)c->beta[row][m], dtT);
         k[m] = reinterpret_cast<const T *>(kp.p[m] ? kp.p[m] : c->kbuf[par]) + base;
     }
-    auto one = [&](T y, const T *kv) {
-        T acc = A::mul(kv[0], cf[0]);
-#pragma unroll
-        for (int m = 1; m < NK; ++m) acc = A::add(acc, A::mul(kv[m], cf[m]));
-        return A::add(y, acc);
-    };
     row_span<T>(base, lo, hi, vec,
         [&](size_t i) {
             V a = ld_stream<T>(y0 + i), kv[NK], res;
@@ -124,7 +117,7 @@ k_rows_combine(const TdqCtrl *__restrict__ c, Rows R, Geom g, int row, T *__rest
                 T ke[NK];
 #pragma unroll
                 for (int m = 0; m < NK; ++m) ke[m] = kv[m].v[e];
-                res.v[e] = one(a.v[e], ke);
+                res.v[e] = tdq_combine<T, NK>(a.v[e], ke, cf);
             }
             st_vec<T>(o + i, res);
         },
@@ -132,7 +125,7 @@ k_rows_combine(const TdqCtrl *__restrict__ c, Rows R, Geom g, int row, T *__rest
             T ke[NK];
 #pragma unroll
             for (int m = 0; m < NK; ++m) ke[m] = k[m][i];
-            o[i] = one(y0[i], ke);
+            o[i] = tdq_combine<T, NK>(y0[i], ke, cf);
         });
 }
 
@@ -146,7 +139,6 @@ __global__ void __launch_bounds__(kThreads)
 k_rows_combine_final(const TdqCtrl *__restrict__ c, Rows R, Geom g, int row, T *__restrict__ out, T *__restrict__ err_out,
                      KPtrs kp, RowFinalMap fm, bool vec) {
     if (c->halt) return;
-    using A = Ar<T>;
     using V = Vec<T>;
     size_t u, lo, hi;
     int r;
@@ -176,29 +168,10 @@ k_rows_combine_final(const TdqCtrl *__restrict__ c, Rows R, Geom g, int row, T *
         const bool ur = fm.rpos[m] >= 0, ue = fm.epos[m] >= 0;
         if (ur) mask_r |= 1u << m;
         if (ue) mask_e |= 1u << m;
-        cr[m] = ur ? A::mul(sgn, A::mul((T)c->beta[row][fm.rpos[m]], dtT)) : (T)0;
-        ce[m] = ue ? A::mul(sgn, A::mul(dtT, (T)c->c_err[fm.epos[m]])) : (T)0;
+        cr[m] = ur ? tdq_coef<T>(sgn, (T)c->beta[row][fm.rpos[m]], dtT) : (T)0;
+        ce[m] = ue ? tdq_coef<T>(sgn, (T)c->c_err[fm.epos[m]], dtT) : (T)0;
         k[m] = reinterpret_cast<const T *>(kp.p[m] ? kp.p[m] : c->kbuf[par]) + base;
     }
-    auto element = [&](T y, const T *kv, T &yo, T &ev) {
-        T ar = (T)0, ae = (T)0;
-        bool fr = true, fe = true;
-#pragma unroll
-        for (int m = 0; m < NU; ++m) {
-            if ((mask_r >> m) & 1u) {
-                const T p = A::mul(kv[m], cr[m]);
-                ar = fr ? p : A::add(ar, p);
-                fr = false;
-            }
-            if ((mask_e >> m) & 1u) {
-                const T p = A::mul(kv[m], ce[m]);
-                ae = fe ? p : A::add(ae, p);
-                fe = false;
-            }
-        }
-        yo = A::add(y, ar);
-        ev = ae;
-    };
     row_span<T>(base, lo, hi, vec,
         [&](size_t i) {
             V a = ld_stream<T>(y0 + i), kv[NU], ry, re;
@@ -209,7 +182,7 @@ k_rows_combine_final(const TdqCtrl *__restrict__ c, Rows R, Geom g, int row, T *
                 T ke[NU];
 #pragma unroll
                 for (int m = 0; m < NU; ++m) ke[m] = kv[m].v[e];
-                element(a.v[e], ke, ry.v[e], re.v[e]);
+                tdq_combine_final<T, NU>(a.v[e], ke, cr, ce, mask_r, mask_e, ry.v[e], re.v[e]);
             }
             st_vec<T>(o + i, ry);
             st_vec<T>(eo + i, re);
@@ -218,7 +191,7 @@ k_rows_combine_final(const TdqCtrl *__restrict__ c, Rows R, Geom g, int row, T *
             T ke[NU];
 #pragma unroll
             for (int m = 0; m < NU; ++m) ke[m] = k[m][i];
-            element(y0[i], ke, o[i], eo[i]);
+            tdq_combine_final<T, NU>(y0[i], ke, cr, ce, mask_r, mask_e, o[i], eo[i]);
         });
 }
 
@@ -256,7 +229,7 @@ k_rows_norm(const TdqCtrl *__restrict__ c, Rows R, Geom g, RowNormArgs a) {
             kcand = reinterpret_cast<T *>(c->kbuf[par ^ 1]) + base;
             // the last error weight, when it belongs to k_S of an FSAL tableau, is not in the prefix
             ek = c->fsal && c->err_nnz > 0 && c->err_idx[c->err_nnz - 1] == c->n_stages;
-            if (ek) ecS = A::mul((T)c->t_sign, A::mul((T)fld<double>(R, TDQ_ROWS_ATT_DT)[r], (T)c->c_err[c->err_nnz - 1]));
+            if (ek) ecS = tdq_coef<T>((T)c->t_sign, (T)c->c_err[c->err_nnz - 1], (T)fld<double>(R, TDQ_ROWS_ATT_DT)[r]);
         }
         const T rtolT = (T)c->rtol, atolT = (T)c->atol;
 #pragma unroll 4
@@ -270,20 +243,7 @@ k_rows_norm(const TdqCtrl *__restrict__ c, Rows R, Geom g, RowNormArgs a) {
                 if (!A::finite(v1)) bad += 1.0;
             }
             if (MODE == 1 && !A::finite(v0)) bad += 1.0;
-            T num;
-            if (MODE == 0) num = ek ? A::add(xa, A::mul(xb, ecS)) : xa;
-            else num = (MODE == 2) ? A::sub(xa, xb) : xa;
-            Q q;
-            if (VTOL) {
-                const double rt = a.rtol_v[base + i], at = a.atol_v[base + i];
-                const double tol = (MODE == 0) ? at + rt * (double)A::max_nan(A::abs(v0), A::abs(v1))
-                                               : at + (double)A::abs(v0) * rt;
-                q = (Q)((double)num / tol);
-            } else {
-                const T tol = (MODE == 0) ? A::add(atolT, A::mul(rtolT, A::max_nan(A::abs(v0), A::abs(v1))))
-                                          : A::add(atolT, A::mul(A::abs(v0), rtolT));
-                q = (Q)A::div(num, tol);
-            }
+            const Q q = tdq_err_q<T, MODE, VTOL>(v0, v1, xa, xb, ek, ecS, rtolT, atolT, a.rtol_v, a.atol_v, base + i);
             acc += (double)Ar<Q>::mul(q, q);
         }
     }
@@ -320,18 +280,6 @@ k_rows_norm(const TdqCtrl *__restrict__ c, Rows R, Geom g, RowNormArgs a) {
 }
 
 // ---- dense output (rk_common.py:363-369, interp.py:1-48) ------------------------------------------------------------------
-template <typename T> __device__ __forceinline__ T eval_poly(T e, T d, T cq, T b, T a, T x) {
-    using A = Ar<T>;
-    T total = A::add(e, A::mul(x, d));
-    T xp = A::mul(x, x);
-    total = A::add(total, A::mul(xp, cq));
-    xp = A::mul(xp, x);
-    total = A::add(total, A::mul(xp, b));
-    xp = A::mul(xp, x);
-    total = A::add(total, A::mul(xp, a));
-    return total;
-}
-
 // The quartic [e, d, c, b, a] of row r's accepted step (rk_common.py:363-369, interp.py:1-22), element by element: shared
 // by the output kernel and the event kernels' coefficient store, so both use one arithmetic.
 template <typename T, int NK> struct RowQuartic {
@@ -351,26 +299,14 @@ template <typename T, int NK> struct RowQuartic {
         two_sdt = A::mul((T)2, sdt);
 #pragma unroll
         for (int m = 0; m < NK; ++m) {
-            mf[m] = A::mul(sgn, A::mul(dtT, (T)c->c_mid[m]));
+            mf[m] = tdq_coef<T>(sgn, (T)c->c_mid[m], dtT);
             km[m] = kmid.p[m] ? reinterpret_cast<const T *>(kmid.p[m]) + base : f0;
         }
     }
 
     __device__ __forceinline__ void at(size_t i, T &e, T &d, T &cq, T &b, T &a) const {
-        using A = Ar<T>;
         const T y0v = y0[i], y1v = y1[i], f0v = f0[i], f1v = f1[i];
-        T acc = A::mul(km[0][i], mf[0]);
-#pragma unroll
-        for (int m = 1; m < NK; ++m) acc = A::add(acc, A::mul(km[m][i], mf[m]));
-        const T ymid = A::add(y0v, acc);
-        a = A::add(A::sub(A::mul(two_sdt, A::sub(f1v, f0v)), A::mul((T)8, A::add(y1v, y0v))), A::mul((T)16, ymid));
-        b = A::sub(A::add(A::add(A::mul(sdt, A::sub(A::mul((T)5, f0v), A::mul((T)3, f1v))), A::mul((T)18, y0v)),
-                          A::mul((T)14, y1v)),
-                   A::mul((T)32, ymid));
-        cq = A::add(A::sub(A::sub(A::mul(sdt, A::sub(f1v, A::mul((T)4, f0v))), A::mul((T)11, y0v)), A::mul((T)5, y1v)),
-                    A::mul((T)16, ymid));
-        d = A::mul(sdt, f0v);
-        e = y0v;
+        tdq_quartic<T>(y0v, y1v, f0v, f1v, tdq_combine<T, NK>(y0v, TdqTerms<T>{km, i}, mf), sdt, two_sdt, e, d, cq, b, a);
     }
 };
 
@@ -391,7 +327,7 @@ k_rows_fit_eval(const TdqCtrl *__restrict__ c, Rows R, Geom g, const T *__restri
         q.at(i, e, d, cq, b, a);
         for (int j = jlo; j < jhi; ++j) {
             const T x = (T)((c->t_out[j] - t0) / (t1 - t0));
-            solution[(size_t)j * n + base + i] = eval_poly<T>(e, d, cq, b, a, x);
+            solution[(size_t)j * n + base + i] = tdq_eval_poly<T>(e, d, cq, b, a, x);
         }
     }
 }
@@ -399,15 +335,12 @@ k_rows_fit_eval(const TdqCtrl *__restrict__ c, Rows R, Geom g, const T *__restri
 // ---- per-row scalar work: one thread per row ------------------------------------------------------------------------------
 // rk_common.py:246-247, :269-287 and the stage times of :72-78 for the attempt that starts at the row's t1.
 template <typename T> __device__ void row_prepare(const TdqCtrl &c, const Rows &R, int r, bool y0_bad) {
-    using A = Ar<T>;
     int *status = fld<int>(R, TDQ_ROWS_STATUS);
     if (fld<int64_t>(R, TDQ_ROWS_N_STEPS)[r] >= c.max_num_steps) {       // :247
         status[r] = TDQ_RUN_MAX_STEPS;
         return;
     }
-    double dt = fld<double>(R, TDQ_ROWS_DT)[r];
-    if (!isfinite(dt)) dt = c.min_step;                                   // :269-270
-    dt = fmin(fmax(dt, c.min_step), c.max_step);                          // :271
+    const double dt = tdq_clamp_dt(fld<double>(R, TDQ_ROWS_DT)[r], c.min_step, c.max_step);   // :269-271
     const double t0 = fld<double>(R, TDQ_ROWS_T1)[r];
     const double t1 = t0 + dt;                                            // :273
     fld<double>(R, TDQ_ROWS_ATT_T0)[r] = t0;
@@ -422,11 +355,8 @@ template <typename T> __device__ void row_prepare(const TdqCtrl &c, const Rows &
     }
     fld<double>(R, TDQ_ROWS_ATT_T1)[r] = t1;
     const T t0T = (T)t0, dtT = (T)dt, t1T = (T)t1, sgn = (T)c.t_sign;
-    for (int i = 0; i < c.n_stages; ++i) {
-        const T a = (T)c.alpha[i];
-        const T ti = (a == (T)1) ? prev_repr<T>(t1T) : A::add(t0T, A::mul(a, dtT));
-        fld<T>(R, TDQ_ROWS_T_STAGE + i)[r] = A::mul(sgn, ti);
-    }
+    for (int i = 0; i < c.n_stages; ++i)                                  // :72-78
+        fld<T>(R, TDQ_ROWS_T_STAGE + i)[r] = tdq_stage_time<T>((T)c.alpha[i], t0T, dtT, t1T, sgn);
 }
 
 struct NoEvent {
@@ -440,14 +370,11 @@ struct NoEvent {
 template <typename T, typename Event = NoEvent>
 __device__ void row_control(const TdqCtrl &c, const Rows &R, int r, double sumsq, double n_bad, size_t D,
                             Event event = Event{}) {
-    double ratio = sqrt(sumsq / (double)D);                                // misc.py:22-23
-    if (!c.ratio_f64) ratio = (double)(T)ratio;
+    double ratio = tdq_rms<T>(sumsq, (double)D, c.ratio_f64);
     if (n_bad > 0.0) ratio = CUDART_NAN;                                   // a non-finite y1 poisons err/tol
     fld<double>(R, TDQ_ROWS_RATIO)[r] = ratio;
     const double dt = fld<double>(R, TDQ_ROWS_ATT_DT)[r];
-    bool accept = ratio <= 1.0;                                            // :324
-    if (dt > c.max_step) accept = false;                                   // :327-328
-    if (dt <= c.min_step) accept = true;                                   // :329-330
+    const bool accept = tdq_accept(ratio, dt, c.min_step, c.max_step);     // :324-330
     fld<int>(R, TDQ_ROWS_ACCEPT)[r] = accept ? 1 : 0;
     const bool fired = event(accept);
     const double att_t0 = fld<double>(R, TDQ_ROWS_ATT_T0)[r];
@@ -471,7 +398,7 @@ __device__ void row_control(const TdqCtrl &c, const Rows &R, int r, double sumsq
     if (accept) {
         const double t1 = fld<double>(R, TDQ_ROWS_T1)[r];
         const int c0 = cur;
-        while (cur < c.n_out && !(c.t_out[cur] > t1)) ++cur;
+        cur = tdq_cursor_after(c.t_out, c.n_out, cur, t1);
         if (cur != c0) steps[r] = 0;
         fld<int>(R, TDQ_ROWS_CURSOR)[r] = cur;
     }
@@ -550,11 +477,7 @@ __global__ void __launch_bounds__(kThreads)
 k_rows_h0(const TdqCtrl *__restrict__ c, Rows R, const double *s0, const double *s1, size_t D) {
     const int r = blockIdx.x * kThreads + threadIdx.x;
     if (r >= R.B) return;
-    double d0 = sqrt(s0[r] / (double)D), d1 = sqrt(s1[r] / (double)D);
-    if (!c->ratio_f64) {
-        d0 = (double)(T)d0;
-        d1 = (double)(T)d1;
-    }
+    const double d0 = tdq_rms<T>(s0[r], (double)D, c->ratio_f64), d1 = tdq_rms<T>(s1[r], (double)D, c->ratio_f64);
     const double h0 = tdq_initial_h0<T>(c->ratio_f64 != 0, d0, d1);
     fld<double>(R, TDQ_ROWS_H0)[r] = h0;
     fld<double>(R, TDQ_ROWS_D1)[r] = d1;
@@ -564,7 +487,6 @@ k_rows_h0(const TdqCtrl *__restrict__ c, Rows R, const double *s0, const double 
 
 template <typename T>
 __global__ void __launch_bounds__(kThreads) k_rows_probe(const TdqCtrl *__restrict__ c, Rows R, Geom g, T *__restrict__ out) {
-    using A = Ar<T>;
     size_t u, lo, hi;
     int r;
     if (!unit_of(g, u, r, lo, hi)) return;
@@ -572,16 +494,15 @@ __global__ void __launch_bounds__(kThreads) k_rows_probe(const TdqCtrl *__restri
     const size_t base = (size_t)r * g.D;
     const T *y0 = reinterpret_cast<const T *>(c->ybuf[par]) + base;
     const T *f0 = reinterpret_cast<const T *>(c->kbuf[par]) + base;
-    const T h = A::mul((T)c->t_sign, (T)fld<double>(R, TDQ_ROWS_H0)[r]);   // y0 + h0 * f0, f0 = t_sign * k0 (misc.py:66)
-    for (size_t i = lo + (threadIdx.x & 31); i < hi; i += 32) out[base + i] = A::add(y0[i], A::mul(h, f0[i]));
+    const T h = tdq_probe_h<T>(c->t_sign, fld<double>(R, TDQ_ROWS_H0)[r]);
+    for (size_t i = lo + (threadIdx.x & 31); i < hi; i += 32) out[base + i] = tdq_probe<T>(y0[i], h, f0[i]);
 }
 
 template <typename T>
 __global__ void __launch_bounds__(kThreads) k_rows_finish(const TdqCtrl *__restrict__ c, Rows R, const double *s2, size_t D) {
     const int r = blockIdx.x * kThreads + threadIdx.x;
     if (r >= R.B) return;
-    double nd = sqrt(s2[r] / (double)D);
-    if (!c->ratio_f64) nd = (double)(T)nd;
+    const double nd = tdq_rms<T>(s2[r], (double)D, c->ratio_f64);
     fld<double>(R, TDQ_ROWS_DT)[r] = tdq_initial_finish<T>(c->ratio_f64 != 0, c->order, fld<double>(R, TDQ_ROWS_D1)[r],
                                                            fld<double>(R, TDQ_ROWS_H0)[r], nd);
 }
@@ -768,7 +689,7 @@ k_rows_event_bisect(const TdqCtrl *__restrict__ c, Rows R, Geom g, BisectArgs a,
     const T *cf = reinterpret_cast<const T *>(a.coeff) + base;
     const size_t n = a.n;
     for (size_t i = lo + lane; i < hi; i += 32)
-        out[i] = eval_poly<T>(cf[i], cf[n + i], cf[2 * n + i], cf[3 * n + i], cf[4 * n + i], x);
+        out[i] = tdq_eval_poly<T>(cf[i], cf[n + i], cf[2 * n + i], cf[3 * n + i], cf[4 * n + i], x);
 }
 
 // ---- host helpers -----------------------------------------------------------------------------------------------------------

@@ -15,6 +15,7 @@
 // Arithmetic is contraction free and follows the reference's order of roundings (SURVEY.md 8(a)).
 #include "tdq_common.cuh"
 #include "tdq_shape.cuh"
+#include "tdq_step.cuh"
 
 namespace {
 
@@ -33,7 +34,6 @@ template <typename T, int NK, int THREADS, int U, bool VECTOR>
 __global__ void __launch_bounds__(THREADS)
 k_combine(const TdqCtrl *__restrict__ c, int row, T *__restrict__ out, const T *y0, KPtrs kp, size_t n) {
     if (c->halt) return;
-    using A = Ar<T>;
     T cf[NK];
     const T *k[NK];
     if (y0 == nullptr) y0 = reinterpret_cast<const T *>(c->y0_cur);
@@ -65,10 +65,10 @@ k_combine(const TdqCtrl *__restrict__ c, int row, T *__restrict__ out, const T *
                     V r;
 #pragma unroll
                     for (int e = 0; e < V::N; ++e) {
-                        T acc = A::mul(kv[u][0].v[e], cf[0]);
+                        T ke[NK];
 #pragma unroll
-                        for (int m = 1; m < NK; ++m) acc = A::add(acc, A::mul(kv[u][m].v[e], cf[m]));
-                        r.v[e] = A::add(a[u].v[e], acc);
+                        for (int m = 0; m < NK; ++m) ke[m] = kv[u][m].v[e];
+                        r.v[e] = tdq_combine<T, NK>(a[u].v[e], ke, cf);
                     }
                     st_vec<T>(out + v * V::N, r);
                 }
@@ -77,19 +77,11 @@ k_combine(const TdqCtrl *__restrict__ c, int row, T *__restrict__ out, const T *
         // scalar tail (n not a multiple of the vector width): first threads of block 0
         if (blockIdx.x == 0) {
             const size_t i = nvec * V::N + threadIdx.x;
-            if (i < n) {
-                T acc = A::mul(k[0][i], cf[0]);
-#pragma unroll
-                for (int m = 1; m < NK; ++m) acc = A::add(acc, A::mul(k[m][i], cf[m]));
-                out[i] = A::add(y0[i], acc);
-            }
+            if (i < n) out[i] = tdq_combine<T, NK>(y0[i], TdqTerms<T>{k, i}, cf);
         }
     } else {
         for (size_t i = (size_t)blockIdx.x * THREADS + threadIdx.x; i < n; i += (size_t)gridDim.x * THREADS) {
-            T acc = A::mul(k[0][i], cf[0]);
-#pragma unroll
-            for (int m = 1; m < NK; ++m) acc = A::add(acc, A::mul(k[m][i], cf[m]));
-            out[i] = A::add(y0[i], acc);
+            out[i] = tdq_combine<T, NK>(y0[i], TdqTerms<T>{k, i}, cf);
         }
     }
 }
@@ -130,7 +122,6 @@ __global__ void __launch_bounds__(256)
 k_combine_final(const TdqCtrl *__restrict__ c, int row, T *__restrict__ out, T *__restrict__ err_out, const T *y0,
                 KPtrs kp, FinalMap fm, size_t n) {
     if (c->halt) return;
-    using A = Ar<T>;
     // two vectors per operand per thread for every row width: on dopri8/float64 (NU = 9) one vector per operand measured
     // at about half the bandwidth even at twice the occupancy (another GPU) -- bytes in flight per thread matter
     constexpr int THREADS = 256, U = 2;
@@ -150,25 +141,6 @@ k_combine_final(const TdqCtrl *__restrict__ c, int row, T *__restrict__ out, T *
         k[m] = tdq_detach(reinterpret_cast<const T *>(kp.p[m] ? kp.p[m] : c->k0_cur), n);
     }
     y0 = tdq_detach(y0, n);
-    auto element = [&](T y, const T *kv, T &yo, T &eo) {
-        T ar = (T)0, ae = (T)0;
-        bool fr = true, fe = true;
-#pragma unroll
-        for (int m = 0; m < NU; ++m) {
-            if ((mask_r >> m) & 1u) {
-                const T p = A::mul(kv[m], cr[m]);
-                ar = fr ? p : A::add(ar, p);
-                fr = false;
-            }
-            if ((mask_e >> m) & 1u) {
-                const T p = A::mul(kv[m], ce[m]);
-                ae = fe ? p : A::add(ae, p);
-                fe = false;
-            }
-        }
-        yo = A::add(y, ar);
-        eo = ae;
-    };
     if (VECTOR) {
         using V = Vec<T>;
         const size_t nvec = n / V::N;
@@ -194,7 +166,7 @@ k_combine_final(const TdqCtrl *__restrict__ c, int row, T *__restrict__ out, T *
                         T ke[NU];
 #pragma unroll
                         for (int m = 0; m < NU; ++m) ke[m] = kv[u][m].v[e];
-                        element(a[u].v[e], ke, r.v[e], q.v[e]);
+                        tdq_combine_final<T, NU>(a[u].v[e], ke, cr, ce, mask_r, mask_e, r.v[e], q.v[e]);
                     }
                     st_vec<T>(out + v * V::N, r);
                     st_vec<T>(err_out + v * V::N, q);
@@ -207,7 +179,7 @@ k_combine_final(const TdqCtrl *__restrict__ c, int row, T *__restrict__ out, T *
                 T ke[NU];
 #pragma unroll
                 for (int m = 0; m < NU; ++m) ke[m] = k[m][i];
-                element(y0[i], ke, out[i], err_out[i]);
+                tdq_combine_final<T, NU>(y0[i], ke, cr, ce, mask_r, mask_e, out[i], err_out[i]);
             }
         }
     } else {
@@ -215,7 +187,7 @@ k_combine_final(const TdqCtrl *__restrict__ c, int row, T *__restrict__ out, T *
             T ke[NU];
 #pragma unroll
             for (int m = 0; m < NU; ++m) ke[m] = k[m][i];
-            element(y0[i], ke, out[i], err_out[i]);
+            tdq_combine_final<T, NU>(y0[i], ke, cr, ce, mask_r, mask_e, out[i], err_out[i]);
         }
     }
 }

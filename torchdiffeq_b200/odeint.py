@@ -244,14 +244,24 @@ def _resolve_graph(graph, func):
     return graph
 
 
+def _step_control(name, o):
+    """The step-control options of an adaptive solve (rk_common.py:166-205) as engine keywords, after warning about
+    the options `name` does not use."""
+    _warn_unused(name, o, _ADAPTIVE_OPTIONS)
+    if o.get("dtype", torch.float64) != torch.float64:
+        raise NotImplementedError("time dtype other than float64 (options['dtype']) is not implemented")
+    return dict(min_step=o.get("min_step", 0), max_step=o.get("max_step", float("inf")), first_step=o.get("first_step"),
+                safety=o.get("safety", 0.9), ifactor=o.get("ifactor", 10.0), dfactor=o.get("dfactor", 0.2),
+                max_num_steps=o.get("max_num_steps", 2 ** 31 - 1), run_ahead=o.get("run_ahead", 2),
+                device_loop=o.get("device_loop", "auto"))
+
+
 def _make_adaptive_engine(p, method, rtol, atol, rtol_vec, atol_vec, options, fn=None, n=None, segs=None,
                           pieces=None, norm_fn=None, q_view=None, callbacks=None, solver_name=None,
                           keep_interp=False, replicated=(), post_fn=None):
     o = options
-    _warn_unused(solver_name or method, o, _ADAPTIVE_OPTIONS)
+    control = _step_control(solver_name or method, o)
     graph = _resolve_graph(o.get("graph", "auto"), getattr(p, "original_func", None))
-    if o.get("dtype", torch.float64) != torch.float64:
-        raise NotImplementedError("time dtype other than float64 (options['dtype']) is not implemented")
     def _tvals(v):                                                                     # rk_common.py:372-375
         v = torch.as_tensor(v, dtype=torch.float64).to("cpu")
         return torch.sort(v[v >= p.t_cpu[0].double()]).values
@@ -286,15 +296,10 @@ def _make_adaptive_engine(p, method, rtol, atol, rtol_vec, atol_vec, options, fn
     eng = AdaptiveEngine(
         fn if fn is not None else p.fn, n if n is not None else p.n, p.dtype, p.device, method,
         rtol=rtol, atol=atol, rtol_vec=rtol_vec, atol_vec=atol_vec,
-        segs=segs, t_sign=p.t_sign, pieces=pieces,
-        min_step=o.get("min_step", 0), max_step=o.get("max_step", float("inf")),
-        first_step=o.get("first_step"), step_t=step_t, jump_t=jump_t,
-        safety=o.get("safety", 0.9), ifactor=o.get("ifactor", 10.0), dfactor=o.get("dfactor", 0.2),
-        max_num_steps=o.get("max_num_steps", 2 ** 31 - 1),
-        norm_fn=norm_fn, q_view=q_view, graph=graph, run_ahead=o.get("run_ahead", 2),
+        segs=segs, t_sign=p.t_sign, pieces=pieces, step_t=step_t, jump_t=jump_t,
+        norm_fn=norm_fn, q_view=q_view, graph=graph,
         reduce_fn=reduce_fn, n_global=n_global, seg_counts_global=seg_counts_global, agree_fn=agree_fn,
-        exchange=exchange, callbacks=callbacks, keep_interp=keep_interp, device_loop=o.get("device_loop", "auto"),
-        post_fn=post_fn)
+        exchange=exchange, callbacks=callbacks, keep_interp=keep_interp, post_fn=post_fn, **control)
     if fn is None and not p.is_tuple and o.get("fused_linear", True):
         # func is a torchdiffeq_b200.LinearField on a float32 [..., 128] state: stages run as one wgmma kernel each
         from .fields import fusable
@@ -345,16 +350,11 @@ def _check_independent_rows(func, y0, t, method, options, event_fn):
 
 def _make_rows_engine(p, graph=None):
     o = p.options
-    _warn_unused(p.method, o, _ADAPTIVE_OPTIONS)
-    if o.get("dtype", torch.float64) != torch.float64:
-        raise NotImplementedError("time dtype other than float64 (options['dtype']) is not implemented")
+    control = _step_control(p.method, o)
     return RowsEngine(
         p.fn, p.shape, p.dtype, p.device, p.method, rtol=p.rtol, atol=p.atol, rtol_vec=p.rtol_vec, atol_vec=p.atol_vec,
-        t_sign=p.t_sign, min_step=o.get("min_step", 0), max_step=o.get("max_step", float("inf")),
-        first_step=o.get("first_step"), safety=o.get("safety", 0.9), ifactor=o.get("ifactor", 10.0),
-        dfactor=o.get("dfactor", 0.2), max_num_steps=o.get("max_num_steps", 2 ** 31 - 1),
-        graph=_resolve_graph(o.get("graph", "auto"), p.original_func) if graph is None else graph,
-        run_ahead=o.get("run_ahead", 2), device_loop=o.get("device_loop", "auto"))
+        t_sign=p.t_sign, graph=_resolve_graph(o.get("graph", "auto"), p.original_func) if graph is None else graph,
+        **control)
 
 
 def _solve_rows_event(p, event_fn, ev0):
