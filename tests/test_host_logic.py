@@ -41,6 +41,47 @@ def test_tol_vector():
     assert v.shape == (8,) and v[1] == float(torch.tensor(1e-6))   # float32 tensor -> float64, like rk_common.py:186
 
 
+def test_step_jump_times():
+    """rk_common.py:372-375 and :233-236: points before the start dropped, the rest sorted, a point in both step_t and
+    jump_t refused.  odeint hands over a tensor in the caller's dtype (negated for reverse time), the plug-in whatever
+    the seam passes (here a list): the same points come out as float64."""
+    from torchdiffeq_b200.odeint import step_jump_times
+    cpu = torch.device("cpu")
+    assert step_jump_times(None, None, 0.0, cpu) == (None, None)
+    st, jt = step_jump_times(torch.tensor([0.75, -1.0, 0.25, 0.5], dtype=torch.float64), None, 0.25, cpu)
+    assert jt is None and st.dtype == torch.float64 and st.tolist() == [0.25, 0.5, 0.75]
+    st, jt = step_jump_times(None, torch.tensor([-0.5]), -0.25, cpu)     # given, but all before t0: empty, not None
+    assert st is None and jt.dtype == torch.float64 and jt.numel() == 0
+    for form in (torch.tensor([-0.5, -0.75, -0.25]), [-0.5, -0.75, -0.25], torch.tensor([-0.5, -0.75, -0.25]).double()):
+        st, jt = step_jump_times(form, [-0.375], -1.0, cpu)
+        assert st.tolist() == [-0.75, -0.5, -0.25] and jt.tolist() == [-0.375]
+    # float32 step points are widened, not rounded: 0.3f stays above a float64 t0 of 0.3
+    assert step_jump_times(torch.tensor([0.3]), None, 0.3, cpu)[0].tolist() == [float(torch.tensor(0.3))]
+    for st, jt in (([0.5], [0.5]), ([0.5, 0.5], None), ([0.25, 0.5], [0.75, 0.5])):
+        with pytest.raises(ValueError, match="`step_t` and `jump_t` must not have any repeated elements between them."):
+            step_jump_times(st, jt, 0.0, cpu)
+    st, jt = step_jump_times([-0.5, 0.5], [-0.5, 0.75], 0.0, cpu)           # a repeat before t0 is dropped first
+    assert st.tolist() == [0.5] and jt.tolist() == [0.75]
+
+
+def test_choose_grid_constructor():
+    """solvers.py:70-79: t itself, a user grid_constructor or the step_size grid; step_size and grid_constructor
+    together are refused, and odeint's fixed_grid goes through the same choice."""
+    from torchdiffeq_b200._fixed import choose_grid_constructor
+    from torchdiffeq_b200.odeint import fixed_grid
+    t = torch.tensor([0.0, 0.25, 1.0], dtype=torch.float64)
+    assert torch.equal(choose_grid_constructor(None, None)(None, None, t), t)
+    gc = lambda f, y0, t_: torch.linspace(float(t_[0]), float(t_[-1]), 9, dtype=t_.dtype)
+    assert choose_grid_constructor(None, gc) is gc
+    assert torch.equal(choose_grid_constructor(0.3, None)(None, None, t), grid_from_step_size(0.3)(None, None, t))
+    with pytest.raises(ValueError, match="step_size and grid_constructor are mutually exclusive arguments."):
+        choose_grid_constructor(0.3, gc)
+    assert torch.equal(fixed_grid("rk4", {"step_size": 0.3}, None, None, t), grid_from_step_size(0.3)(None, None, t))
+    assert torch.equal(fixed_grid("rk4", {"grid_constructor": gc}, None, None, t), gc(None, None, t))
+    with pytest.raises(ValueError, match="mutually exclusive"):
+        fixed_grid("rk4", {"step_size": 0.3, "grid_constructor": gc}, None, None, t)
+
+
 def _reference_fixed_loop(grid, t):
     """solvers.py:108-126 as written: which output index is produced in which step, and how."""
     recs, j = [], 1

@@ -220,6 +220,11 @@ class AdaptiveEngine:
             self.norm_table = torch.tensor(words, dtype=torch.int64, device=device)
             self.n_chunks, self.table_aligned = int(words[1]), int(words[3])
 
+        if (rtol_vec is None) != (atol_vec is None):            # a scalar tolerance next to a per-element one
+            if rtol_vec is None:
+                rtol_vec = torch.full_like(atol_vec, rtol)
+            else:
+                atol_vec = torch.full_like(rtol_vec, atol)
         self.rtol_vec = rtol_vec
         self.atol_vec = atol_vec
         vtol = rtol_vec is not None
@@ -545,12 +550,13 @@ class AdaptiveEngine:
         solution [len(t), n] (solvers.py:28-35).  The returned tensor is owned by the engine and is
         overwritten by the next solve() with the same number of output times."""
         try:
-            n_out = self._begin(y0_flat, t64, t_start, loop=self._use_loop())
-            if n_out > 1:
-                if self._lockstep_mode():
-                    self._loop_lockstep()
-                else:
+            if self._lockstep_mode():
+                for _ in self._lockstep(y0_flat, t64, t_start):
+                    pass
+            else:
+                if self._begin(y0_flat, t64, t_start, loop=self._use_loop()) > 1:
                     self._loop_run_ahead()
+                self._read_counters()
         except BaseException:
             # attempts may still be queued: let them drain before anybody resets the mailbox, and do not let a
             # half-finished engine be reused (the caller evicts it from the cache)
@@ -560,10 +566,13 @@ class AdaptiveEngine:
             except Exception:
                 pass
             raise
+        return self.solution
+
+    def _read_counters(self):
+        """n_accept / n_reject / n_attempts of the solve that just ended."""
         mb = self.mbox_host.contents
         self.n_accept, self.n_reject = int(mb.n_accept), int(mb.n_reject)
         self.n_attempts = self.n_accept + self.n_reject
-        return self.solution
 
     def prime(self, y0_flat, t64, t_start=None):
         """Warm up and capture the attempt graph ahead of time on representative inputs (one eager
@@ -677,34 +686,37 @@ class AdaptiveEngine:
             del f
         return issued, mb
 
-    def _loop_lockstep(self):
-        issued = 0
+    def _lockstep(self, y0_flat, t64, t_start=None):
+        """A lock-step solve: yields the mailbox once after the start and once after every attempt, until the solve is
+        done or the caller closes the generator after an attempt; it then synchronises and reads the counters."""
+        n_out = self._begin(y0_flat, t64, t_start)
         torch.cuda.current_stream().synchronize()          # first attempt's (t0, dt) and status are in the mailbox
         mb = self.mbox_host.contents
         self._raise_if_failed(mb)
-        while True:
-            issued, mb = self._lockstep_attempt(issued, mb)
-            if mb.done:
-                break
+        issued = 0
+        yield mb                                           # closed here: no attempt was made, nothing to read
+        try:
+            while n_out > 1:
+                issued, mb = self._lockstep_attempt(issued, mb)
+                yield mb
+                if mb.done:
+                    break
+        except GeneratorExit:                              # the caller stopped the solve
+            pass
         torch.cuda.current_stream().synchronize()
+        self._read_counters()
 
     # ---- dense output (odeint.py:111-157) ------------------------------------------------------------
     def solve_dense(self, y0_flat, t64):
         """Lock-step solve that keeps the interpolant of EVERY accepted step: returns (solution, times, coeffs)
         with times[i], times[i+1] bounding accepted step i and coeffs[i] its five coefficient arrays."""
-        n_out = self._begin(y0_flat, t64)
-        torch.cuda.current_stream().synchronize()
-        mb = self.mbox_host.contents
-        self._raise_if_failed(mb)
-        times, coeffs, issued = [float(t64[0])], [], 0
-        while n_out > 1:
-            issued, mb = self._lockstep_attempt(issued, mb)
+        steps = self._lockstep(y0_flat, t64)
+        next(steps)
+        times, coeffs = [float(t64[0])], []
+        for mb in steps:
             if mb.accept:                                                   # odeint.py:141-145
                 times.append(float(mb.t1))
                 coeffs.append([c.clone() for c in self.coeff])
-            if mb.done:
-                break
-        torch.cuda.current_stream().synchronize()
         return self.solution, times, coeffs
 
     # ---- taped solve for the differentiable (non-adjoint) odeint (torchdiffeq_b200/backprop.py) ------------------
@@ -712,13 +724,10 @@ class AdaptiveEngine:
         """Lock-step solve that records every ACCEPTED step: start time, step size, the (y0, k_0) pair it started from
         (clones: 2 n elements per step), the output rows it produced and whether it followed a jump_t re-evaluation.
         Returns (solution, tape)."""
-        n_out = self._begin(y0_flat, t64, t_start)
-        torch.cuda.current_stream().synchronize()
-        mb = self.mbox_host.contents
-        self._raise_if_failed(mb)
-        tape, issued, cursor, first, jumped = [], 0, 1, True, None
-        while n_out > 1:
-            issued, mb = self._lockstep_attempt(issued, mb)
+        steps = self._lockstep(y0_flat, t64, t_start)
+        next(steps)
+        tape, cursor, first, jumped = [], 1, True, None
+        for mb in steps:
             if mb.accept:
                 prev = (mb.par ^ 1) & 1                                     # the pair the accepted step started from
                 k0 = self.kbuf[prev]
@@ -726,11 +735,6 @@ class AdaptiveEngine:
                                  out_lo=cursor, out_hi=int(mb.out_cursor), first=first, jumped_into=jumped))
                 cursor, first = int(mb.out_cursor), False
                 jumped = True if mb.on_jump_t else None
-            if mb.done:
-                break
-        torch.cuda.current_stream().synchronize()
-        self.n_accept, self.n_reject = int(mb.n_accept), int(mb.n_reject)
-        self.n_attempts = self.n_accept + self.n_reject
         return self.solution, tape
 
     # ---- event handling (solvers.py:38-49, rk_common.py:252-264, event_handling.py:5-20) ----------------
@@ -739,25 +743,19 @@ class AdaptiveEngine:
         step.  event_fn takes a 0-dim float64 device tensor (ascending solver time) and the flat state.
         Host driven by nature (a sign test per step); returns (event_t as float, y(event_t) tensor)."""
         t64 = torch.tensor([float(t0), float("inf")], dtype=torch.float64, device=self.device)
-        self._begin(y0_flat, t64, float(t0))
-        torch.cuda.current_stream().synchronize()
-        mb = self.mbox_host.contents
-        self._raise_if_failed(mb)
+        steps = self._lockstep(y0_flat, t64, float(t0))
+        mb = next(steps)
         tt = lambda v: torch.tensor(v, dtype=torch.float64, device=self.device)
         t_cur = float(t0)
         if bool(event_fn(tt(t_cur), self.y0w) == 0):                         # rk_common.py:254-255
             return t_cur, self.y0w.clone()
         sign0 = torch.sign(event_fn(tt(t_cur), self.y0w))
-        issued = 0
         while bool(sign0 == torch.sign(event_fn(tt(t_cur), self.y0w))):      # :259
-            issued, mb = self._lockstep_attempt(issued, mb)
+            mb = next(steps)
             t_cur = mb.t1
-        torch.cuda.current_stream().synchronize()
-        self.n_accept, self.n_reject = int(mb.n_accept), int(mb.n_reject)
-        self.n_attempts = self.n_accept + self.n_reject
+        steps.close()
         # find_event (event_handling.py:5-20): bisection on [t0, t1] of the last accepted step
         lo, hi = float(mb.t0), float(mb.t1)
-        import math
         nitrs = int(math.ceil(math.log((hi - lo) / float(tol)) / math.log(2.0)))
         y_mid = torch.empty(self.n, dtype=self.dtype, device=self.device)
 
@@ -1127,10 +1125,8 @@ class RowsEngine(AdaptiveEngine):
         y = self.ybuf[par][r * self.D:(r + 1) * self.D].view(1, *self.row_shape)      # y0[r:r+1]
         self._raise_status(mb.status, float(self.row_field(_lib.ROWS_ATT_DT, torch.float64)[r]), y, " (row %d)" % r)
 
-    def solve(self, y0_flat, t64, t_start=None):
-        sol = super().solve(y0_flat, t64, t_start)
+    def _read_counters(self):
         self.row_n_accept = self.row_field(_lib.ROWS_N_ACCEPT, torch.int64).cpu()
         self.row_n_reject = self.row_field(_lib.ROWS_N_REJECT, torch.int64).cpu()
         self.n_accept, self.n_reject = int(self.row_n_accept.sum()), int(self.row_n_reject.sum())
         self.n_attempts = int((self.row_n_accept + self.row_n_reject).max())   # loop iterations that did work
-        return sol

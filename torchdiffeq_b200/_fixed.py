@@ -34,6 +34,15 @@ def grid_from_step_size(step_size):
     return _grid_constructor
 
 
+def choose_grid_constructor(step_size, grid_constructor):
+    """solvers.py:70-79: the grid constructor of a fixed-grid solve from its step_size / grid_constructor options."""
+    if step_size is None:
+        return grid_constructor if grid_constructor is not None else (lambda f, y0, t: t)
+    if grid_constructor is not None:
+        raise ValueError("step_size and grid_constructor are mutually exclusive arguments.")
+    return grid_from_step_size(step_size)
+
+
 def stage_times(method, t0, dt, t1, perturb, dtype):
     """Func times of the four evaluations of a step (zero where the method makes fewer): the reference's expressions in
     the dtypes of t0, dt and t1, then _PerturbFunc's cast to the state dtype (misc.py:187) and its Perturb.NEXT / PREV

@@ -156,10 +156,6 @@ class _BackwardSolver:
         # t[i-1:i+1].flip(0)).  The engine integrates ascending s = bsign * t, bsign = -fwd_sign.
         fwd_sign = -1.0 if p.t_reversed else 1.0
         self.bsign = -fwd_sign
-        bp = Problem()                       # the backward problem as the engine factory sees it
-        bp.t_sign, bp.device, bp.dtype, bp.n, bp.fn = self.bsign, dev, T, lay.n, aug_fn
-        bp.original_func = p.original_func          # decides graph='auto' (only nn.Module funcs are captured)
-        bp.t_cpu = (p.t_cpu.to(torch.float64) * fwd_sign * self.bsign).flip(0)
         self.fixed = adjoint_method in FIXED_METHODS or adjoint_method in IMPLICIT_METHODS
         self.fixed_method = adjoint_method
         if self.fixed and opts.get("process_group") is not None:
@@ -202,17 +198,15 @@ class _BackwardSolver:
             replicated = (0,) + tuple(range(1 + n_state_segs, len(segs)))
         self.dist_group = None if pg is None else (None if pg is True else pg)
         self.sharded = pg is not None
-        rtol_s, rtol_v = _adj_tol(adjoint_rtol, lay, dev)
-        atol_s, atol_v = _adj_tol(adjoint_atol, lay, dev)
-        if (rtol_v is None) != (atol_v is None):
-            if rtol_v is None:
-                rtol_v = torch.full_like(atol_v, rtol_s)
-            else:
-                atol_v = torch.full_like(rtol_v, atol_s)
-        self.eng = _make_adaptive_engine(bp, adjoint_method, rtol_s, atol_s, rtol_v, atol_v, opts, fn=aug_fn,
-                                         n=lay.n, segs=segs, pieces=pieces, norm_fn=norm_fn, q_view=q_view,
-                                         callbacks=callbacks, solver_name=adjoint_method, replicated=replicated,
-                                         post_fn=post_fn)
+        bp = Problem()                       # the backward problem as the engine factory sees it
+        bp.method, bp.options, bp.callbacks = adjoint_method, opts, callbacks
+        bp.t_sign, bp.device, bp.dtype, bp.n, bp.fn, bp.shape = self.bsign, dev, T, lay.n, aug_fn, None
+        bp.original_func = p.original_func          # decides graph='auto' (only nn.Module funcs are captured)
+        bp.t_cpu = (p.t_cpu.to(torch.float64) * fwd_sign * self.bsign).flip(0)
+        bp.segs, bp.pieces, bp.norm_fn, bp.q_view = segs, pieces, norm_fn, q_view
+        bp.rtol, bp.rtol_vec = _adj_tol(adjoint_rtol, lay, dev)
+        bp.atol, bp.atol_vec = _adj_tol(adjoint_atol, lay, dev)
+        self.eng = _make_adaptive_engine(bp, replicated=replicated, post_fn=post_fn)
         # solves run inside autograd's backward: never capture there (see AdaptiveEngine.prime)
         self.eng.capture_in_solve = False
 

@@ -15,7 +15,7 @@ import torch
 from . import _lib
 from ._engine import AdaptiveEngine, Layout, RowsEngine, on_solver_stream
 from ._adams import ADAMS_METHODS
-from ._fixed import FIXED_METHODS, grid_from_step_size, make_engine
+from ._fixed import FIXED_METHODS, choose_grid_constructor, make_engine
 from ._implicit import IMPLICIT_METHODS
 
 ADAPTIVE_METHODS = ("dopri5", "dopri8", "tsit5", "bosh3", "fehlberg2", "adaptive_heun")
@@ -160,11 +160,6 @@ def normalise(func, y0, t, rtol, atol, method, options, event_fn, adjoint=False)
     shape_ = None if p.is_tuple else y0.shape
     p.rtol, p.rtol_vec = _tol_vector('rtol', rtol, p.layout, shape_, p.device)
     p.atol, p.atol_vec = _tol_vector('atol', atol, p.layout, shape_, p.device)
-    if (p.rtol_vec is None) != (p.atol_vec is None):                                   # mixed scalar/vector
-        if p.rtol_vec is None:
-            p.rtol_vec = torch.full_like(p.atol_vec, p.rtol)
-        else:
-            p.atol_vec = torch.full_like(p.rtol_vec, p.atol)
 
     # callbacks (misc.py:313-343)
     p.callbacks = {}
@@ -256,37 +251,45 @@ def _step_control(name, o):
                 device_loop=o.get("device_loop", "auto"))
 
 
-def _make_adaptive_engine(p, method, rtol, atol, rtol_vec, atol_vec, options, fn=None, n=None, segs=None,
-                          pieces=None, norm_fn=None, q_view=None, callbacks=None, solver_name=None,
-                          keep_interp=False, replicated=(), post_fn=None):
-    o = options
-    control = _step_control(solver_name or method, o)
-    graph = _resolve_graph(o.get("graph", "auto"), getattr(p, "original_func", None))
-    def _tvals(v):                                                                     # rk_common.py:372-375
+def step_jump_times(step_t, jump_t, t0, device):
+    """rk_common.py:372-375 and :233-236: the step_t / jump_t points at or after the ascending start time t0, sorted, as
+    float64 tensors on `device` (None where not given); a point in both raises."""
+    def points(v):
         v = torch.as_tensor(v, dtype=torch.float64).to("cpu")
-        return torch.sort(v[v >= p.t_cpu[0].double()]).values
-    step_t, jump_t = o.get("step_t"), o.get("jump_t")
-    st = _tvals(step_t) if step_t is not None else torch.tensor([], dtype=torch.float64)
-    jt = _tvals(jump_t) if jump_t is not None else torch.tensor([], dtype=torch.float64)
-    if (torch.cat([st, jt]).unique(return_counts=True)[1] > 1).any():                  # :233-236
+        return torch.sort(v[v >= t0]).values
+    st = points(step_t) if step_t is not None else torch.tensor([], dtype=torch.float64)
+    jt = points(jump_t) if jump_t is not None else torch.tensor([], dtype=torch.float64)
+    if (torch.cat([st, jt]).unique(return_counts=True)[1] > 1).any():
         raise ValueError("`step_t` and `jump_t` must not have any repeated elements between them.")
-    step_t = st.to(p.device) if step_t is not None else None
-    jump_t = jt.to(p.device) if jump_t is not None else None
+    return (st.to(device) if step_t is not None else None), (jt.to(device) if jump_t is not None else None)
+
+
+def _make_adaptive_engine(p, lockstep=False, keep_interp=False, graph=None, replicated=(), post_fn=None):
+    """The adaptive engine of a Problem: method, tolerances, step control, norm, callbacks and state come from `p`.
+    lockstep: the reference's exact call sequence (run_ahead=0, no graph).  graph: instead of options['graph']."""
+    o = p.options
+    control = _step_control(p.method, o)
+    graph = _resolve_graph(o.get("graph", "auto") if graph is None else graph, p.original_func)
+    if lockstep:
+        control["run_ahead"], graph = 0, False
+    tol = dict(rtol=p.rtol, atol=p.atol, rtol_vec=p.rtol_vec, atol_vec=p.atol_vec, t_sign=p.t_sign)
+    if o.get("independent_rows"):
+        return RowsEngine(p.fn, p.shape, p.dtype, p.device, p.method, graph=graph, **tol, **control)
+    step_t, jump_t = step_jump_times(o.get("step_t"), o.get("jump_t"), float(p.t_cpu[0]), p.device)
     reduce_fn, n_global, seg_counts_global, agree_fn, exchange = None, None, None, None, None
     pg = o.get("process_group")
     if pg is not None:
         from .dist import make_agree, make_reduce
-        if norm_fn is not None:
+        if p.norm_fn is not None:
             raise NotImplementedError("a custom norm callable cannot be evaluated on a batch-sharded state "
                                       "(SURVEY.md section 8(e): replicas only); use the default norm or 'seminorm'")
-        reduce_fn, n_global, seg_counts_global = make_reduce(pg, segs if segs is not None else
-                                                             [(0, n if n is not None else p.n)], p.device,
+        reduce_fn, n_global, seg_counts_global = make_reduce(pg, p.segs if p.segs is not None else [(0, p.n)], p.device,
                                                              replicated=replicated)
         agree_fn = make_agree(pg)
-        if o.get("exchange", "peer") == "peer" and norm_fn is None:
+        if o.get("exchange", "peer") == "peer" and p.norm_fn is None:
             try:
                 from .dist import PeerExchange
-                n_seg_ = len(segs) if segs is not None else 1
+                n_seg_ = len(p.segs) if p.segs is not None else 1
                 if n_seg_ > _lib.TDQ_MAX_SEGS:
                     raise _lib.TdqError("more than %d norm segments" % _lib.TDQ_MAX_SEGS)
                 exchange = PeerExchange(pg, p.device)
@@ -294,16 +297,15 @@ def _make_adaptive_engine(p, method, rtol, atol, rtol_vec, atol_vec, options, fn
                 warnings.warn("torchdiffeq_b200: NVLink peer exchange unavailable (%s: %s); using the process "
                               "group's all-reduce" % (type(e).__name__, e))
     eng = AdaptiveEngine(
-        fn if fn is not None else p.fn, n if n is not None else p.n, p.dtype, p.device, method,
-        rtol=rtol, atol=atol, rtol_vec=rtol_vec, atol_vec=atol_vec,
-        segs=segs, t_sign=p.t_sign, pieces=pieces, step_t=step_t, jump_t=jump_t,
-        norm_fn=norm_fn, q_view=q_view, graph=graph,
+        p.fn, p.n, p.dtype, p.device, p.method, segs=p.segs, pieces=p.pieces, step_t=step_t, jump_t=jump_t,
+        norm_fn=p.norm_fn, q_view=p.q_view, graph=graph,
         reduce_fn=reduce_fn, n_global=n_global, seg_counts_global=seg_counts_global, agree_fn=agree_fn,
-        exchange=exchange, callbacks=callbacks, keep_interp=keep_interp, post_fn=post_fn, **control)
-    if fn is None and not p.is_tuple and o.get("fused_linear", True):
-        # func is a torchdiffeq_b200.LinearField on a float32 [..., 128] state: stages run as one wgmma kernel each
+        exchange=exchange, callbacks=p.callbacks, keep_interp=keep_interp, post_fn=post_fn, **tol, **control)
+    if p.shape is not None and o.get("fused_linear", True):
+        # func is a torchdiffeq_b200.LinearField on a float32 [..., 128] tensor state (not a tuple state, not the
+        # adjoint's augmented one): stages run as one wgmma kernel each
         from .fields import fusable
-        w = fusable(getattr(p, "original_func", None), tuple(p.shape), p.dtype, p.device, eng.lib)
+        w = fusable(p.original_func, tuple(p.shape), p.dtype, p.device, eng.lib)
         if w is not None:
             eng.set_linear(w, whole_attempt=o.get("fused_attempt", True))
     return eng
@@ -348,23 +350,14 @@ def _check_independent_rows(func, y0, t, method, options, event_fn):
     return v
 
 
-def _make_rows_engine(p, graph=None):
-    o = p.options
-    control = _step_control(p.method, o)
-    return RowsEngine(
-        p.fn, p.shape, p.dtype, p.device, p.method, rtol=p.rtol, atol=p.atol, rtol_vec=p.rtol_vec, atol_vec=p.atol_vec,
-        t_sign=p.t_sign, graph=_resolve_graph(o.get("graph", "auto"), p.original_func) if graph is None else graph,
-        **control)
-
-
 def _solve_rows_event(p, event_fn, ev0):
     """Every row until its own event (options={'independent_rows': True}); returns (event_t float64 [B] in the caller's
     time, solution [2, n], engine).  The captured attempt runs event_fn's Python once, so graph='auto' captures only when
     func and event_fn are both nn.Modules.  Event engines are not cached."""
-    graph = _resolve_graph(p.options.get("graph", "auto"), p.original_func)
+    graph = p.options.get("graph", "auto")
     if graph == "auto" and not isinstance(event_fn, torch.nn.Module):
         graph = False
-    eng = _make_rows_engine(p, graph=graph)
+    eng = _make_adaptive_engine(p, graph=graph)
     B, shape = p.shape[0], p.shape
     # the bisection tolerance: atol, or with a per-element atol the smallest of the row's own elements
     if p.atol_vec is not None:
@@ -463,7 +456,8 @@ def _func_signature(func, explicit=False):
 
 def _cache_key(p, extra=()):
     o = p.options
-    if o.get("cache", True) is False or p.callbacks or p.norm_fn is not None or p.rtol_vec is not None:
+    if (o.get("cache", True) is False or p.callbacks or p.norm_fn is not None or p.rtol_vec is not None
+            or p.atol_vec is not None):
         return None
     fsig = _func_signature(p.original_func, explicit=o.get("cache", None) is True)
     if fsig is None:
@@ -525,13 +519,8 @@ def _solve(p):
         hit = _cache_get(key)
         if hit is not None:
             eng = hit[0]
-        elif p.options.get("independent_rows"):
-            eng = _make_rows_engine(p)
-            _cache_put(key, (eng, p.original_func))
         else:
-            eng = _make_adaptive_engine(p, p.method, p.rtol, p.atol, p.rtol_vec, p.atol_vec, p.options,
-                                        segs=p.segs, pieces=p.pieces, norm_fn=p.norm_fn, q_view=p.q_view,
-                                        callbacks=p.callbacks)
+            eng = _make_adaptive_engine(p)
             _cache_put(key, (eng, p.original_func))     # the func reference keeps id(func) from being recycled
         t64 = p.t_cpu.to(torch.float64).to(p.device)                                   # solvers.py:31
         try:
@@ -587,13 +576,7 @@ def fixed_grid(method, o, func, y0_view, t_cpu, keep_graph=False):
     """Option handling and time grid of FixedGridODESolver (solvers.py:55-79, :85-96, :103-104) for an
     ascending CPU `t_cpu`; the caller has already wrapped a user grid_constructor for reversed time."""
     _warn_unused(_FIXED_NAMES[method], o, _fixed_options(method))
-    step_size, gc = o.get("step_size"), o.get("grid_constructor")
-    if step_size is None:
-        grid_constructor = gc if gc is not None else (lambda f, y0, t: t)
-    else:
-        if gc is not None:
-            raise ValueError("step_size and grid_constructor are mutually exclusive arguments.")   # solvers.py:79
-        grid_constructor = grid_from_step_size(step_size)
+    grid_constructor = choose_grid_constructor(o.get("step_size"), o.get("grid_constructor"))
     _cubic_or_linear(o.get("interp", "linear"))
     grid = grid_constructor(func, y0_view, t_cpu)
     grid = grid.to("cpu") if keep_graph else grid.detach().to("cpu")
@@ -609,16 +592,13 @@ def _solve_event(p):
         if o.get("step_size") is None:
             raise AssertionError("Event handling for fixed step solvers currently requires `step_size` to be provided "
                                  "in options.")
-        if o.get("grid_constructor") is not None:
-            raise ValueError("step_size and grid_constructor are mutually exclusive arguments.")
+        choose_grid_constructor(o["step_size"], o.get("grid_constructor"))          # refuses both at once
         eng = _fixed_engine(p, graph=False)
         tol = p.atol if p.atol is not None else float(p.atol_vec.min())
         event_t, y_event = eng.solve_until_event(p.y0_flat, p.t_cpu[0], o["step_size"], p.event_fn, tol)
         sol = torch.stack([p.y0_flat.to(p.dtype), y_event], dim=0)
         return float(event_t) * p.t_sign, sol, eng
-    eng = _make_adaptive_engine(p, p.method, p.rtol, p.atol, p.rtol_vec, p.atol_vec,
-                                dict(p.options, run_ahead=0, graph=False), segs=p.segs, pieces=p.pieces,
-                                norm_fn=p.norm_fn, q_view=p.q_view, callbacks=p.callbacks, keep_interp=True)
+    eng = _make_adaptive_engine(p, lockstep=True, keep_interp=True)
     tol = p.atol if p.atol is not None else float(p.atol_vec.min())
     event_t, y_event = eng.solve_until_event(p.y0_flat, float(p.t_cpu[0]), p.event_fn, tol)
     sol = torch.stack([p.y0_flat.to(p.dtype), y_event], dim=0)                         # solvers.py:48
@@ -710,9 +690,7 @@ def odeint_dense(func, y0, t0, t1, *, rtol=1e-7, atol=1e-9, method=None, options
     p = normalise(func, y0, t, rtol, atol, method, options, None)
     assert p.method == "dopri5"                                                        # odeint.py:119
     with torch.no_grad(), on_solver_stream(p.device) as ss:
-        eng = _make_adaptive_engine(p, p.method, p.rtol, p.atol, p.rtol_vec, p.atol_vec,
-                                    dict(p.options, run_ahead=0, graph=False), segs=p.segs, pieces=p.pieces,
-                                    norm_fn=p.norm_fn, q_view=p.q_view, callbacks=p.callbacks, keep_interp=True)
+        eng = _make_adaptive_engine(p, lockstep=True, keep_interp=True)
         t64 = p.t_cpu.to(torch.float64).to(p.device)
         _, times, coeffs = eng.solve_dense(p.y0_flat, t64)
     lib, dc, n, sign_, shape, dtype, dev = eng.lib, eng.dt_code, p.n, p.t_sign, p.shape, p.dtype, p.device
@@ -745,9 +723,7 @@ def _odeint_backprop(p, func, y0, t, params, _stats):
 
     def run():
         if p.method in ADAPTIVE_METHODS:
-            eng = _make_adaptive_engine(p, p.method, p.rtol, p.atol, p.rtol_vec, p.atol_vec,
-                                        dict(p.options, run_ahead=0, graph=False), segs=p.segs, pieces=p.pieces,
-                                        norm_fn=p.norm_fn, q_view=p.q_view, callbacks=p.callbacks)
+            eng = _make_adaptive_engine(p, lockstep=True)
             t64 = p.t_cpu.to(torch.float64).to(p.device)
             sol, tape = eng.solve_taped(p.y0_flat, t64, t_start=float(p.t_cpu[0]))
             holder["eng"] = eng
@@ -777,14 +753,23 @@ def _odeint_backprop(p, func, y0, t, params, _stats):
         ss.publish(sol)
     eng = holder.get("eng")
     if eng is not None:
-        _LAST_STATS.clear()
-        _LAST_STATS.update(nfe=eng.nfe, launches=getattr(eng, "launches", 0), attempts=getattr(eng, "n_attempts", None),
-                           n_accept=getattr(eng, "n_accept", None), n_reject=getattr(eng, "n_reject", None),
+        _publish_stats(eng, _stats, add_launches=False)
+    return _unflatten(p, sol)
+
+
+def _publish_stats(eng, _stats, add_launches):
+    """last_stats() of the solve `eng` just ran.  `_stats` (private: solver counters for bench.py and the tests) gets
+    the same counters except the per-row ones; its launches are added to what it holds when add_launches is set."""
+    _LAST_STATS.clear()
+    _LAST_STATS.update(nfe=eng.nfe, launches=getattr(eng, "launches", 0), attempts=getattr(eng, "n_attempts", None),
+                       n_accept=getattr(eng, "n_accept", None), n_reject=getattr(eng, "n_reject", None),
                        fused_linear=getattr(eng, "linear", None) is not None,
                        fused_attempt=bool((getattr(eng, "linear", None) or {}).get("whole")))
-        if _stats is not None:
-            _stats.update(_LAST_STATS)
-    return _unflatten(p, sol)
+    if _stats is not None:
+        launches = _stats.get("launches", 0) if add_launches else 0
+        _stats.update(_LAST_STATS, launches=launches + _LAST_STATS["launches"])
+    if getattr(eng, "row_n_accept", None) is not None:
+        _LAST_STATS.update(row_n_accept=eng.row_n_accept, row_n_reject=eng.row_n_reject)
 
 
 def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, event_fn=None, _stats=None):
@@ -847,21 +832,8 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
         else:
             sol, eng = _solve(p)
             ss.publish(sol)
-    _LAST_STATS.clear()
-    _LAST_STATS.update(nfe=eng.nfe, launches=getattr(eng, "launches", 0), attempts=getattr(eng, "n_attempts", None),
-                       n_accept=getattr(eng, "n_accept", None), n_reject=getattr(eng, "n_reject", None),
-                       fused_linear=getattr(eng, "linear", None) is not None,
-                       fused_attempt=bool((getattr(eng, "linear", None) or {}).get("whole")))
-    if getattr(eng, "row_n_accept", None) is not None:
-        _LAST_STATS.update(row_n_accept=eng.row_n_accept, row_n_reject=eng.row_n_reject)
+    _publish_stats(eng, _stats, add_launches=True)
     if row_event_fn is not None:
         _LAST_STATS.update(event_calls=eng.n_ev, bisect_iters=eng.bisect_iters)
-    if _stats is not None:               # private: solver counters for bench.py and the tests
-        _stats["nfe"] = eng.nfe
-        _stats["launches"] = _stats.get("launches", 0) + getattr(eng, "launches", 0)
-        _stats["attempts"] = getattr(eng, "n_attempts", None)
-        _stats["n_accept"], _stats["n_reject"] = getattr(eng, "n_accept", None), getattr(eng, "n_reject", None)
-        _stats["fused_linear"], _stats["fused_attempt"] = _LAST_STATS["fused_linear"], _LAST_STATS["fused_attempt"]
-    if row_event_fn is not None:
         return row_event_t, _unflatten(p, sol)
     return _unflatten(p, sol)

@@ -32,10 +32,11 @@ import warnings
 import torch
 
 from . import _lib
-from ._engine import AdaptiveEngine, on_solver_stream
+from ._engine import on_solver_stream
 from ._adams import ADAMS_METHODS
-from ._fixed import FIXED_METHODS, grid_from_step_size, make_engine
+from ._fixed import FIXED_METHODS, choose_grid_constructor, make_engine
 from ._implicit import IMPLICIT_METHODS
+from .odeint import Problem, _make_adaptive_engine
 
 ADAPTIVE = ("dopri5", "dopri8", "tsit5", "bosh3", "fehlberg2", "adaptive_heun")
 _CB = ("callback_step", "callback_accept_step", "callback_reject_step")
@@ -101,67 +102,48 @@ def make_adaptive(method, **defaults):
             unused = {k: v for k, v in opts.items() if k not in _ADAPTIVE_KEYS + _OUR_KEYS}
             if unused:                                                         # misc.py:13-15
                 warnings.warn('{}: Unexpected arguments {}'.format(self.__class__.__name__, unused))
-            self.opts = opts
-            self.rtol, self.rtol_vec = _tol(rtol, y0.device)
-            self.atol, self.atol_vec = _tol(atol, y0.device)
-            if (self.rtol_vec is None) != (self.atol_vec is None):
-                if self.rtol_vec is None:
-                    self.rtol_vec = torch.full_like(self.atol_vec, self.rtol)
-                else:
-                    self.atol_vec = torch.full_like(self.rtol_vec, self.atol)
-            self.norm = None if (norm is None or _is_default_rms(norm)) else norm
-            self.callbacks = _callbacks_of(func, _CB)
+            # the problem as the engine factory sees it; the seam hands over the reference's wrapper of func, so
+            # 'auto' graph resolution sees an nn.Module, and the fused LinearField path is never taken
+            self.p = p = Problem()
+            p.method, p.original_func, p.callbacks = method, func, _callbacks_of(func, _CB)
+            p.options = dict({k: v for k, v in opts.items() if k not in unused}, fused_linear=False)
+            p.fn, p.n, p.shape, p.dtype, p.device = (lambda t_, yf: self.base(t_, yf.view(y0.shape))), y0.numel(), \
+                y0.shape, y0.dtype, y0.device
+            p.t_sign, p.segs, p.pieces = 1.0, None, None
+            p.rtol, p.rtol_vec = _tol(rtol, y0.device)
+            p.atol, p.atol_vec = _tol(atol, y0.device)
+            p.norm_fn = None if (norm is None or _is_default_rms(norm)) else norm
+            p.q_view = (lambda q: q.view(y0.shape)) if p.norm_fn is not None else None
             self.engine = None
 
         @classmethod
         def valid_callbacks(cls):                                              # rk_common.py:207-211
             return set(_CB)
 
-        def _engine(self, keep_interp):
-            o, dev, shape = self.opts, self.y0.device, self.shape
-            base = self.base
-
-            def tvals(v):                                                      # rk_common.py:372-375 happens on the device
-                return None if v is None else torch.as_tensor(v, dtype=torch.float64).to(dev)
-            step_t, jump_t = tvals(o.get("step_t")), tvals(o.get("jump_t"))
-            t0 = self._t0
-            if step_t is not None:
-                step_t = torch.sort(step_t[step_t >= t0]).values
-            if jump_t is not None:
-                jump_t = torch.sort(jump_t[jump_t >= t0]).values
-            both = torch.cat([x for x in (step_t, jump_t) if x is not None]) if (step_t is not None or jump_t is not None) \
-                else None
-            if both is not None and (both.unique(return_counts=True)[1] > 1).any():        # rk_common.py:233-236
-                raise ValueError("`step_t` and `jump_t` must not have any repeated elements between them.")
-            lock = "graph" not in o and "run_ahead" not in o                   # default: the reference's call sequence
-            return AdaptiveEngine(
-                lambda t_, yf: base(t_, yf.view(shape)), self.y0.numel(), self.y0.dtype, dev, method,
-                rtol=self.rtol, atol=self.atol, rtol_vec=self.rtol_vec, atol_vec=self.atol_vec,
-                min_step=o.get("min_step", 0), max_step=o.get("max_step", float("inf")), first_step=o.get("first_step"),
-                step_t=step_t, jump_t=jump_t, safety=o.get("safety", 0.9), ifactor=o.get("ifactor", 10.0),
-                dfactor=o.get("dfactor", 0.2), max_num_steps=o.get("max_num_steps", 2 ** 31 - 1),
-                norm_fn=self.norm, q_view=(lambda q: q.view(shape)) if self.norm is not None else None,
-                graph=False if lock else o.get("graph", False), run_ahead=0 if lock else o.get("run_ahead", 2),
-                device_loop=o.get("device_loop", "auto"), callbacks=self.callbacks, keep_interp=keep_interp)
+        def _engine(self, t_cpu, keep_interp):
+            """Lock step (the reference's call sequence) unless options give graph or run_ahead; graph defaults to
+            False."""
+            o, self.p.t_cpu = self.p.options, t_cpu
+            return _make_adaptive_engine(self.p, lockstep="graph" not in o and "run_ahead" not in o,
+                                         keep_interp=keep_interp, graph=o.get("graph", False))
 
         def integrate(self, t):                                                # solvers.py:28-35
             t_cpu = t.detach().to("cpu", torch.float64)
-            self._t0 = float(t_cpu[0])
             with torch.no_grad(), on_solver_stream(self.y0.device) as ss:
-                self.engine = eng = self._engine(False)
-                sol = eng.solve(self.y0.detach().reshape(-1), t_cpu.to(self.y0.device), t_start=self._t0)
+                self.engine = eng = self._engine(t_cpu, False)
+                sol = eng.solve(self.y0.detach().reshape(-1), t_cpu.to(self.y0.device), t_start=float(t_cpu[0]))
                 sol = sol.view(len(t), *self.shape).clone()
                 ss.publish(sol)
             return sol
 
         def integrate_until_event(self, t0, event_fn):                         # solvers.py:41-49, rk_common.py:252-264
-            self._t0 = float(t0)
-            shape = self.shape
-            tol = self.atol if self.atol is not None else float(self.atol_vec.min())
+            t0 = float(t0)
+            shape, p = self.shape, self.p
+            tol = p.atol if p.atol is not None else float(p.atol_vec.min())
             with torch.no_grad(), on_solver_stream(self.y0.device) as ss:
-                self.engine = eng = self._engine(True)
+                self.engine = eng = self._engine(torch.tensor([t0], dtype=torch.float64), True)
                 ev = lambda t_, yf: event_fn(t_, yf.view(shape))
-                event_t, y1 = eng.solve_until_event(self.y0.detach().reshape(-1), self._t0, ev, tol)
+                event_t, y1 = eng.solve_until_event(self.y0.detach().reshape(-1), t0, ev, tol)
                 sol = torch.stack([self.y0.detach(), y1.view(shape)], dim=0)
                 ss.publish(sol)
             return torch.tensor(event_t, dtype=torch.float64, device=self.y0.device), sol
@@ -197,12 +179,7 @@ def make_fixed(method, **defaults):
             self.func, self.y0, self.shape = func, y0, y0.shape
             self.base = _unwrap_perturb(func)
             self.step_size, self.interp, self.perturb = step_size, interp, perturb
-            if step_size is None:                                              # solvers.py:70-79
-                self.grid_constructor = grid_constructor if grid_constructor is not None else (lambda f, y0, t: t)
-            else:
-                if grid_constructor is not None:
-                    raise ValueError("step_size and grid_constructor are mutually exclusive arguments.")
-                self.grid_constructor = grid_from_step_size(step_size)
+            self.grid_constructor = choose_grid_constructor(step_size, grid_constructor)
             self.callbacks = _callbacks_of(func, ("callback_step",))
 
         @classmethod
