@@ -82,6 +82,109 @@ def test_choose_grid_constructor():
         fixed_grid("rk4", {"step_size": 0.3, "grid_constructor": gc}, None, None, t)
 
 
+def test_fixed_grid_option_check():
+    """The option check warns about unused options under the solver class's name, refuses an unknown interp, and for an
+    event solve requires step_size first (solvers.py:55-79, :125, :131); the grid build asserts the end points."""
+    import warnings
+    from torchdiffeq_b200.odeint import build_grid, fixed_grid_constructor
+    t = torch.tensor([0.0, 1.0], dtype=torch.float64)
+    with warnings.catch_warnings(record=True) as w:
+        warnings.simplefilter("always")
+        fixed_grid_constructor("rk4", {"step_size": 0.5, "max_iters": 3, "graph": False})
+        fixed_grid_constructor("implicit_adams", {"step_size": 0.5, "max_iters": 3, "max_order": 4})
+    assert [str(x.message) for x in w] == ["RK4: Unexpected arguments {'max_iters': 3}"]
+    with pytest.raises(ValueError, match="Unknown interpolation method quadratic"):
+        fixed_grid_constructor("rk4", {"interp": "quadratic"})
+    with pytest.raises(AssertionError, match="requires `step_size`"):
+        fixed_grid_constructor("rk4", {"interp": "quadratic"}, event=True)
+    fixed_grid_constructor("rk4", {"step_size": 0.5}, event=True)
+    with pytest.raises(AssertionError):
+        build_grid(lambda f, y0, t_: torch.tensor([0.0, 0.5]), None, None, t)
+
+
+@pytest.mark.parametrize("sign", [1.0, -1.0])
+def test_signed_grid_constructor(sign):
+    """misc.py:283-289: in engine time s = sign * t the user's constructor is called with the caller's times, and its
+    grid comes back in engine time."""
+    from torchdiffeq_b200._fixed import signed_grid_constructor
+    seen = []
+
+    def gc(func, y0, t_):
+        seen.append((func, y0, t_.clone()))
+        return torch.linspace(float(t_[0]), float(t_[-1]), 5, dtype=t_.dtype)
+    caller_t = torch.tensor([0.5, 1.5] if sign > 0 else [1.5, 0.5], dtype=torch.float64)
+    s = caller_t * sign                                              # ascending engine time
+    grid = signed_grid_constructor(gc, sign)("f", "y0", s)
+    assert seen[0][:2] == ("f", "y0") and torch.equal(seen[0][2], caller_t)
+    assert torch.equal(grid, sign * gc(None, None, caller_t))
+    assert (grid[1:] > grid[:-1]).all() and grid[0] == s[0] and grid[-1] == s[-1]
+
+
+def test_find_event_iteration_count():
+    """event_handling.py:5-20: ceil(log((t1 - t0) / tol) / log 2) bisection steps, evaluated in the bounds' dtype.  With
+    float32 bounds 0 and 0.05 and tol = 0.00625 the float32 quotient is exactly 8 (3 steps); on float64 values it lies
+    just above 8 (4 steps)."""
+    import math
+    from torchdiffeq_b200._engine import find_event
+
+    def count(t0, t1, tol, t_event):
+        calls = []
+
+        def event_fn(t_, y_):
+            calls.append(float(t_))
+            return t_ - t_event
+        ev_t, y = find_event(lambda t_: t_ * 2.0, torch.tensor(-1.0), t0, t1, event_fn, tol)
+        assert torch.equal(y, ev_t * 2.0) and ev_t.dtype == t0.dtype
+        return len(calls), ev_t
+    reference = lambda t0, t1, tol: int(torch.ceil(torch.log((t1 - t0) / tol) / math.log(2.0)).long())
+    f32 = lambda v: torch.tensor(v, dtype=torch.float32)
+    n, _ = count(f32(0.0), f32(0.05), 0.00625, 0.03)
+    assert n == reference(f32(0.0), f32(0.05), 0.00625) == 3
+    assert math.ceil(math.log(float(f32(0.05)) / 0.00625) / math.log(2.0)) == 4
+    f64 = lambda v: torch.tensor(v, dtype=torch.float64)
+    for lo, hi, tol in ((0.0, 1.0, 1e-9), (0.25, 0.75, 0.5 / 1024), (0.1, 0.3, 0.2 / 3)):
+        n, ev_t = count(f64(lo), f64(hi), tol, 0.3 * lo + 0.7 * hi)
+        assert n == reference(f64(lo), f64(hi), tol)
+        assert abs(float(ev_t) - (0.3 * lo + 0.7 * hi)) <= tol
+    assert count(f64(0.0), f64(1.0), 2.0, 0.5)[0] == 0               # tolerance wider than the interval: no bisection
+
+
+def test_valid_callbacks():
+    """misc.py:339-343: every callback for the adaptive methods, callback_step for the fixed-grid ones; the others are
+    dropped with the reference's warning."""
+    import warnings
+    from torchdiffeq_b200.odeint import valid_callbacks
+    cbs = {"callback_step": 1, "callback_accept_step": 2, "callback_reject_step": 3}
+    with warnings.catch_warnings(record=True) as w:
+        warnings.simplefilter("always")
+        assert valid_callbacks("dopri5", cbs) == cbs
+        assert valid_callbacks("rk4", {"callback_step": 1}) == {"callback_step": 1}
+        assert not w
+        assert valid_callbacks("sdirk2", dict(cbs)) == {"callback_step": 1}
+    assert len(w) == 1
+    msg = str(w[0].message)
+    assert msg.startswith("Solver 'sdirk2' does not support callbacks {")
+    assert "'callback_accept_step'" in msg and "'callback_reject_step'" in msg and "'callback_step'" not in msg
+
+
+def test_problem_defaults():
+    """A Problem needs its method, options, func, state and device; everything else has the default of a tensor state
+    solved forward in time with scalar tolerances."""
+    from torchdiffeq_b200.odeint import Problem
+    p = Problem(method="rk4", options={}, original_func=None, fn=None, n=3, dtype=torch.float32,
+                device=torch.device("cpu"))
+    assert p.t_sign == 1.0 and p.callbacks == {} and p.is_tuple is False
+    for name in ("rtol", "atol", "rtol_vec", "atol_vec", "segs", "pieces", "norm_fn", "q_view", "event_fn", "layout",
+                 "shape", "t_cpu", "y0_flat"):
+        assert getattr(p, name) is None, name
+    q = Problem(method="rk4", options={}, original_func=None, fn=None, n=3, dtype=torch.float32,
+                device=torch.device("cpu"))
+    q.callbacks["callback_step"] = None
+    assert p.callbacks == {}                                         # not shared between problems
+    with pytest.raises(TypeError):
+        Problem(method="rk4", options={})
+
+
 def _reference_fixed_loop(grid, t):
     """solvers.py:108-126 as written: which output index is produced in which step, and how."""
     recs, j = [], 1

@@ -145,6 +145,7 @@ class AdamsEngine(FixedGridEngine):
                 converged = bool((err / tol).abs().max() < 1)
                 if converged:
                     break
+            self._hist_alive.extend(alive)       # ... also through the cubic emit, which runs after this returns
             if not converged:
                 warnings.warn('Functional iteration did not converge. Solution may be incorrect.')
                 self.prev_f.pop()

@@ -158,6 +158,21 @@ def pack_pieces(lib, dt_code, dtype, buf, f, pieces):
     return n_launch
 
 
+def find_event(interp_fn, sign0, t0, t1, event_fn, tol):
+    """event_handling.py:5-20: bisect [t0, t1] (0-dim CPU tensors) for the point where event_fn, evaluated on the
+    interpolant interp_fn, leaves sign0; returns (event_t, interp_fn(event_t)).  The iteration count is the reference's
+    expression, evaluated in the dtype of the bounds."""
+    nitrs = torch.ceil(torch.log((t1 - t0) / tol) / math.log(2.0))
+    for _ in range(int(nitrs.long())):
+        t_mid = (t1 + t0) / 2.0
+        if bool(sign0 == torch.sign(event_fn(t_mid, interp_fn(t_mid)))):
+            t0 = t_mid
+        else:
+            t1 = t_mid
+    event_t = (t0 + t1) / 2.0
+    return event_t, interp_fn(event_t)
+
+
 class AdaptiveEngine:
     """One adaptive explicit-RK solve on a flat state vector, all state on the device.
 
@@ -754,24 +769,18 @@ class AdaptiveEngine:
             mb = next(steps)
             t_cur = mb.t1
         steps.close()
-        # find_event (event_handling.py:5-20): bisection on [t0, t1] of the last accepted step
-        lo, hi = float(mb.t0), float(mb.t1)
-        nitrs = int(math.ceil(math.log((hi - lo) / float(tol)) / math.log(2.0)))
+        # bisection on [t0, t1] of the last accepted step, on its dense output
         y_mid = torch.empty(self.n, dtype=self.dtype, device=self.device)
 
         def interp(t_eval):
             self._launch(self.lib.tdq_interp_eval_at(self.ctrl.data_ptr(), self.dt_code, self.coeff_ptrs,
-                                                     tt(t_eval).data_ptr(), y_mid.data_ptr(), self.n, _stream()))
+                                                     t_eval.to(self.device).data_ptr(), y_mid.data_ptr(), self.n,
+                                                     _stream()))
             return y_mid
-        for _ in range(max(nitrs, 0)):
-            t_mid = (hi + lo) / 2.0
-            same = bool(sign0 == torch.sign(event_fn(tt(t_mid), interp(t_mid))))
-            if same:
-                lo = t_mid
-            else:
-                hi = t_mid
-        event_t = (lo + hi) / 2.0
-        return event_t, interp(event_t).clone()
+        bound = lambda v: torch.tensor(float(v), dtype=torch.float64)
+        event_t, y_event = find_event(interp, sign0, bound(mb.t0), bound(mb.t1),
+                                      lambda t_, y_: event_fn(t_.to(self.device), y_), tol)
+        return float(event_t), y_event.clone()
 
     def _with_y(self, t0, dt):
         t0, dt = self._scalars(t0, dt)

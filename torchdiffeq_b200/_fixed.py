@@ -14,7 +14,7 @@ from typing import NamedTuple
 import torch
 
 from . import _lib
-from ._engine import _DTYPES, _RetryWithCopies, _stream, pack_pieces, solver_stream
+from ._engine import _DTYPES, _RetryWithCopies, _stream, find_event, pack_pieces, solver_stream
 
 _ONE_THIRD = 1 / 3      # rk_common.py:94-96
 _TWO_THIRDS = 2 / 3
@@ -41,6 +41,12 @@ def choose_grid_constructor(step_size, grid_constructor):
     if grid_constructor is not None:
         raise ValueError("step_size and grid_constructor are mutually exclusive arguments.")
     return grid_from_step_size(step_size)
+
+
+def signed_grid_constructor(grid_constructor, sign):
+    """misc.py:283-289: a user grid_constructor for a solve in engine time s = sign * t.  The user's function sees
+    and returns the caller's times."""
+    return lambda func, y0, t: sign * grid_constructor(func, y0, sign * t)
 
 
 def stage_times(method, t0, dt, t1, perturb, dtype):
@@ -390,7 +396,6 @@ class FixedGridEngine:
         """Step with dt = step_size from t0 until event_fn(t, y) changes sign, then bisect on the step's interpolant
         (event_handling.py:5-20).  event_fn takes a 0-dim tensor of the state dtype (solver time, ascending) and the
         flat state.  Host driven by nature: one sign test per step.  Returns (event_t tensor, y(event_t))."""
-        import math
         dev, T = self.device, self.dtype
         t0c = torch.as_tensor(t0).detach().to("cpu").to(T).reshape(())              # t0.type_as(y0.abs())
         dt = step_size.detach().to("cpu") if torch.is_tensor(step_size) else step_size
@@ -435,17 +440,9 @@ class FixedGridEngine:
                     return y1
                 slope = (t - t0c) / (t1c - t0c)
                 return y0 + float(slope) * (y1 - y0)
-        lo, hi = t0c, t1c                                                          # event_handling.py:5-20
-        nitrs = torch.ceil(torch.log((hi - lo) / atol) / math.log(2.0))
-        for _ in range(int(nitrs.long())):
-            t_mid = (hi + lo) / 2.0
-            same = bool(sign0 == torch.sign(event_fn(t_mid.to(dev), interp_fn(t_mid))))
-            if same:
-                lo = t_mid
-            else:
-                hi = t_mid
-        event_t = (lo + hi) / 2.0
-        y_ev = interp_fn(event_t).clone()
+        ev = lambda t, y: event_fn(t.to(dev), y)
+        event_t, y_ev = find_event(interp_fn, sign0, t0c, t1c, ev, atol)
+        y_ev = y_ev.clone()
         torch.cuda.current_stream().synchronize()
         return event_t.to(dev), y_ev
 

@@ -21,11 +21,11 @@ import torch.nn as nn
 
 from . import _lib
 from ._engine import Layout, on_solver_stream
-from ._fixed import FIXED_METHODS, make_engine
+from ._fixed import FIXED_METHODS, signed_grid_constructor
 from ._implicit import IMPLICIT_METHODS
 from .odeint import (ADAPTIVE_METHODS, _ADJOINT_CALLBACK_NAMES, _CALLBACK_NAMES, _cache_drop, _cache_get,
-                     _cache_key, _cache_put, _make_adaptive_engine, _mixed_norm, _rms_norm, _solve, _solve_event, _unflatten,
-                     fixed_grid, normalise, Problem)
+                     _cache_key, _cache_put, _make_adaptive_engine, _make_fixed_engine, _mixed_norm, _rms_norm, _solve,
+                     _solve_event, _unflatten, fixed_grid, normalise, Problem, valid_callbacks)
 
 
 def find_parameters(module):
@@ -153,27 +153,16 @@ class _BackwardSolver:
                 callbacks[name] = _cb
 
         # The backward solve always runs against the forward time direction (adjoint.py:136
-        # t[i-1:i+1].flip(0)).  The engine integrates ascending s = bsign * t, bsign = -fwd_sign.
-        fwd_sign = -1.0 if p.t_reversed else 1.0
-        self.bsign = -fwd_sign
+        # t[i-1:i+1].flip(0)).  The engine integrates ascending s = bsign * t, bsign = -p.t_sign.
+        self.bsign = -p.t_sign
         self.fixed = adjoint_method in FIXED_METHODS or adjoint_method in IMPLICIT_METHODS
-        self.fixed_method = adjoint_method
-        if self.fixed and opts.get("process_group") is not None:
-            raise NotImplementedError("sharded adjoint with a fixed-grid adjoint_method is not implemented")
         if self.fixed:
-            # fixed-grid backward (adjoint.py:134-138 with a FixedGridODESolver): the same step kernels; the grid of
-            # every interval comes from adjoint_options (step_size / grid_constructor), solvers.py:85-104
-            self.fixed_opts = {k: v for k, v in opts.items() if k not in ("graph", "run_ahead", "cache", "exchange",
-                                                                           "process_group")}
-            self.aug_fn = aug_fn
-            valid = {k: v for k, v in callbacks.items() if k == "callback_step"}
-            if set(callbacks) - set(valid):
-                warnings.warn("Solver '{}' does not support callbacks {}".format(adjoint_method, set(callbacks) - set(valid)))
-            # never capture inside autograd's backward (see AdaptiveEngine.prime): eager launches
-            self.eng = make_engine(adjoint_method, aug_fn, lay.n, T, dev, t_sign=self.bsign,
-                                   perturb=opts.get("perturb", False), graph=False, callbacks=valid, pieces=pieces,
-                                   max_iters=opts.get("max_iters"))
-            return
+            # fixed-grid backward (adjoint.py:134-138 with a FixedGridODESolver): the grid of every interval comes from
+            # adjoint_options (step_size / grid_constructor, solvers.py:85-104); the user's constructor sees true times
+            if opts.get("process_group") is not None:
+                raise NotImplementedError("sharded adjoint with a fixed-grid adjoint_method is not implemented")
+            if "grid_constructor" in opts:                                   # misc.py:283-289
+                opts["grid_constructor"] = signed_grid_constructor(opts["grid_constructor"], self.bsign)
         # ---- batch-sharded backward solve (SURVEY.md section 8(e)) -------------------------------------------------
         # y and adj_y are this rank's rows; vjp_t and the parameter gradients every evaluation produces are PARTIAL
         # sums over the local rows.  They are all-reduced right after the pack (two contiguous ranges of the slot:
@@ -198,14 +187,23 @@ class _BackwardSolver:
             replicated = (0,) + tuple(range(1 + n_state_segs, len(segs)))
         self.dist_group = None if pg is None else (None if pg is True else pg)
         self.sharded = pg is not None
-        bp = Problem()                       # the backward problem as the engine factory sees it
-        bp.method, bp.options, bp.callbacks = adjoint_method, opts, callbacks
-        bp.t_sign, bp.device, bp.dtype, bp.n, bp.fn, bp.shape = self.bsign, dev, T, lay.n, aug_fn, None
-        bp.original_func = p.original_func          # decides graph='auto' (only nn.Module funcs are captured)
-        bp.t_cpu = (p.t_cpu.to(torch.float64) * fwd_sign * self.bsign).flip(0)
-        bp.segs, bp.pieces, bp.norm_fn, bp.q_view = segs, pieces, norm_fn, q_view
-        bp.rtol, bp.rtol_vec = _adj_tol(adjoint_rtol, lay, dev)
-        bp.atol, bp.atol_vec = _adj_tol(adjoint_atol, lay, dev)
+        if self.fixed:
+            rtol = atol = (None, None)                 # no error control: the tolerances are not read
+        else:
+            rtol, atol = _adj_tol(adjoint_rtol, lay, dev), _adj_tol(adjoint_atol, lay, dev)
+        # the backward problem as the engine factories see it; original_func decides graph='auto' (only nn.Module funcs
+        # are captured)
+        self.bp = bp = Problem(
+            method=adjoint_method, options=opts, original_func=p.original_func, fn=aug_fn, n=lay.n, dtype=T, device=dev,
+            rtol=rtol[0], rtol_vec=rtol[1], atol=atol[0], atol_vec=atol[1], t_sign=self.bsign,
+            t_cpu=(p.t_cpu.to(torch.float64) * p.t_sign * self.bsign).flip(0),
+            callbacks=valid_callbacks(adjoint_method, callbacks), segs=segs, pieces=pieces, norm_fn=norm_fn, q_view=q_view)
+        if self.fixed:
+            # Eager launches: never capture inside autograd's backward (see AdaptiveEngine.prime).  Outputs are linear
+            # whatever adjoint_options['interp'] says; with interp='cubic' the reference interpolates cubically here,
+            # one more func call per output time.
+            self.eng = _make_fixed_engine(bp, graph=False, interp="linear")
+            return
         self.eng = _make_adaptive_engine(bp, replicated=replicated, post_fn=post_fn)
         # solves run inside autograd's backward: never capture there (see AdaptiveEngine.prime)
         self.eng.capture_in_solve = False
@@ -241,18 +239,15 @@ class _BackwardSolver:
                 if isinstance(fe, tuple):
                     fe = self.fwd_layout.flatten([f_.detach() for f_ in fe])
                 dLd_cur_t = fe.reshape(-1).dot(grad_sol[i].reshape(-1))
-                if getattr(self, "sharded", False):                  # a sum over ALL rows of the batch
+                if self.sharded:                                     # a sum over ALL rows of the batch
                     import torch.distributed as dist
                     dist.all_reduce(dLd_cur_t, group=self.dist_group)
                 aug[o_t] -= dLd_cur_t
                 time_vjps[i] = dLd_cur_t
             if self.fixed:
                 pair = (t[i - 1:i + 1].detach().flip(0) * self.bsign).to("cpu")      # ascending engine time, t's own dtype
-                opts = dict(self.fixed_opts)
-                if "grid_constructor" in opts:                       # the user sees the true times (misc.py:283-289)
-                    gc, sgn = opts["grid_constructor"], self.bsign
-                    opts["grid_constructor"] = lambda f_, y_, t_: sgn * gc(f_, y_, sgn * t_)
-                grid = fixed_grid(self.fixed_method, opts, self.aug_fn, aug, pair)
+                # the options are checked per interval, where the reference builds its solver
+                grid = fixed_grid(self.bp.method, self.bp.options, self.bp.fn, aug, pair)
                 sol = eng.solve(aug, grid, pair)
             else:
                 sol = eng.solve(aug, pairs[i - 1], t_start=float(s_cpu[i]))   # ascending for the engine
@@ -298,7 +293,7 @@ class _AdjointFunction(torch.autograd.Function):
         with torch.no_grad():
             if ctx.event_mode:                                           # adjoint.py:30-31
                 ev, sol, _ = _solve_event(p)
-                event_t = torch.tensor(ev, dtype=t.dtype, device=t.device)
+                event_t = torch.tensor(float(ev) * p.t_sign, dtype=t.dtype, device=t.device)
                 ctx.save_for_backward(t, sol, event_t, *adjoint_params)
                 return event_t, sol
             sol, _ = _solve(p)                                          # adjoint.py:23-24

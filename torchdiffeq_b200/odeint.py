@@ -8,6 +8,7 @@ misc.py:200-345 (_check_inputs) with two differences that are not observable in 
     the sign is folded into the Runge-Kutta coefficients on the device.
 """
 import collections
+import dataclasses
 import warnings
 
 import torch
@@ -15,7 +16,7 @@ import torch
 from . import _lib
 from ._engine import AdaptiveEngine, Layout, RowsEngine, on_solver_stream
 from ._adams import ADAMS_METHODS
-from ._fixed import FIXED_METHODS, choose_grid_constructor, make_engine
+from ._fixed import FIXED_METHODS, choose_grid_constructor, make_engine, signed_grid_constructor
 from ._implicit import IMPLICIT_METHODS
 
 ADAPTIVE_METHODS = ("dopri5", "dopri8", "tsit5", "bosh3", "fehlberg2", "adaptive_heun")
@@ -49,9 +50,33 @@ def _mixed_norm(tensor_tuple):
     return max([_rms_norm(tensor) for tensor in tensor_tuple])
 
 
+@dataclasses.dataclass(eq=False)
 class Problem:
-    """Normalised inputs of one solve (what misc.py:200-345 returns as a 10-tuple)."""
-    pass
+    """Normalised inputs of one solve (what misc.py:200-345 returns as a 10-tuple), as the engine factories read them.
+    Times are the solver's ascending ones; fn and event_fn take the flat state."""
+    method: str
+    options: dict
+    original_func: object               # the caller's func: decides graph='auto' and the fused linear path
+    fn: object                          # func on the flat state
+    n: int
+    dtype: torch.dtype
+    device: torch.device
+    rtol: float = None                  # scalar tolerances, or None next to a per-element vector
+    atol: float = None
+    rtol_vec: torch.Tensor = None
+    atol_vec: torch.Tensor = None
+    t_sign: float = 1.0                 # -1.0: the caller's time runs backwards
+    t_cpu: torch.Tensor = None          # output times, ascending
+    y0_flat: torch.Tensor = None
+    callbacks: dict = dataclasses.field(default_factory=dict)
+    is_tuple: bool = False
+    layout: Layout = None
+    shape: torch.Size = None            # a tensor state's shape
+    segs: list = None                   # norm segments (offset, length); None: one over the whole state
+    pieces: tuple = None                # fn returns a tuple of pieces at these (offsets, lens, scales)
+    norm_fn: object = None              # a norm callable on the compatibility path ...
+    q_view: object = None               # ... and how err/tol is presented to it
+    event_fn: object = None
 
 
 def _combine_event_functions(event_fn, t0, y0):
@@ -110,18 +135,16 @@ def normalise(func, y0, t, rtol, atol, method, options, event_fn, adjoint=False)
         if len(t) != 2:                                                                # misc.py:203-204
             raise ValueError(f"We require len(t) == 2 when in event handling mode, but got len(t)={len(t)}.")
         event_fn = _combine_event_functions(event_fn, t[0], y0)                        # misc.py:207
-    p = Problem()
-    p.original_func = func
-    p.is_tuple = not isinstance(y0, torch.Tensor)
-    if p.is_tuple:
+    is_tuple = not isinstance(y0, torch.Tensor)
+    if is_tuple:
         assert isinstance(y0, tuple), 'y0 must be either a torch.Tensor or a tuple'   # misc.py:216
-        p.layout = Layout([y_.shape for y_ in y0], y0[0].dtype)
-        p.device = y0[0].device
-        p.dtype = y0[0].dtype
+        layout, shape = Layout([y_.shape for y_ in y0], y0[0].dtype), None
+        device, dtype = y0[0].device, y0[0].dtype
+        unflat = layout.views
     else:
-        p.layout = None
-        p.device = y0.device
-        p.dtype = y0.dtype
+        layout, shape = None, y0.shape
+        device, dtype = y0.device, y0.dtype
+        unflat = lambda yf: yf.view(shape)
     options = {} if options is None else options.copy()                               # misc.py:226-229
     if method is None:
         method = 'dopri5'
@@ -131,96 +154,75 @@ def normalise(func, y0, t, rtol, atol, method, options, event_fn, adjoint=False)
     if method not in ADAPTIVE_METHODS + FIXED_METHODS + tuple(ADAMS_METHODS) + IMPLICIT_METHODS:
         raise NotImplementedError('method "{}" is not part of the CUDA hot path; implemented: {}'.format(
             method, ADAPTIVE_METHODS + FIXED_METHODS + tuple(ADAMS_METHODS) + IMPLICIT_METHODS))
-    p.method, p.options = method, options
-    if p.device.type != "cuda":
-        raise _lib.TdqError("torchdiffeq_b200 runs on CUDA devices only (got %s); there is no CPU path" % p.device)
+    if device.type != "cuda":
+        raise _lib.TdqError("torchdiffeq_b200 runs on CUDA devices only (got %s); there is no CPU path" % device)
     _lib.load()                                   # fail loudly, before any work, if libtdq.so is missing
 
     t_cpu = t.detach().to("cpu") if isinstance(t, torch.Tensor) else t                 # the one host read of t
     _check_timelike('t', t, True, values=t_cpu)
-    p.t_reversed = bool(len(t_cpu) > 1 and t_cpu[0] > t_cpu[1])                        # misc.py:270-271
-    p.t_sign = -1.0 if p.t_reversed else 1.0
-    p.t_cpu = -t_cpu if p.t_reversed else t_cpu                                        # ascending from here on
-    if p.t_reversed:
+    t_reversed = bool(len(t_cpu) > 1 and t_cpu[0] > t_cpu[1])                          # misc.py:270-271
+    t_sign = -1.0 if t_reversed else 1.0
+    if t_reversed:
+        t_cpu = -t_cpu                                                                 # ascending from here on
         for name in ("step_t", "jump_t"):                                              # misc.py:292-293
             if isinstance(options.get(name), torch.Tensor):
                 options[name] = -options[name]
-        if "grid_constructor" in options:                                             # misc.py:283-289
-            _gc = options["grid_constructor"]
-            options["grid_constructor"] = lambda func, y0, t: -_gc(func, y0, -t)
-    assert (p.t_cpu[1:] > p.t_cpu[:-1]).all(), 't must be strictly increasing or decreasing'   # misc.py:296
+        if "grid_constructor" in options:
+            options["grid_constructor"] = signed_grid_constructor(options["grid_constructor"], t_sign)
+    assert (t_cpu[1:] > t_cpu[:-1]).all(), 't must be strictly increasing or decreasing'   # misc.py:296
 
     if torch.is_tensor(rtol):                                                          # misc.py:299-302
         assert not rtol.requires_grad, "rtol cannot require gradient"
     if torch.is_tensor(atol):
         assert not atol.requires_grad, "atol cannot require gradient"
-    if t.device != p.device:                                                           # misc.py:305-307
+    if t.device != device:                                                             # misc.py:305-307
         warnings.warn("t is not on the same device as y0. Coercing to y0.device.")
+    rtol, rtol_vec = _tol_vector('rtol', rtol, layout, shape, device)
+    atol, atol_vec = _tol_vector('atol', atol, layout, shape, device)
 
-    shape_ = None if p.is_tuple else y0.shape
-    p.rtol, p.rtol_vec = _tol_vector('rtol', rtol, p.layout, shape_, p.device)
-    p.atol, p.atol_vec = _tol_vector('atol', atol, p.layout, shape_, p.device)
+    # callbacks (misc.py:313-343), in the caller's time and shapes
+    callbacks = {name: getattr(func, name, None) for name in _CALLBACK_NAMES}
+    callbacks = valid_callbacks(method, {k: v for k, v in callbacks.items() if v is not None})
 
-    # callbacks (misc.py:313-343)
-    p.callbacks = {}
-    for name in _CALLBACK_NAMES:
-        cb = getattr(func, name, None)
-        if cb is not None:
-            p.callbacks[name] = cb
-    valid = set(_CALLBACK_NAMES) if method in ADAPTIVE_METHODS else {"callback_step"}     # solvers.py:81-83
-    invalid = set(p.callbacks) - valid
-    if invalid:
-        warnings.warn("Solver '{}' does not support callbacks {}".format(method, invalid))
-        for name in invalid:
-            del p.callbacks[name]
-    if p.callbacks:
-        layout, sign = p.layout, p.t_sign
-        def _wrap(cb):
-            def _cb(t0, y0_flat, dt):
-                y_ = layout.views(y0_flat) if layout is not None else y0_flat.view(p.shape)
-                return cb(t0 * sign, y_, dt)                                           # misc.py:326-331
-            return _cb
-        p.callbacks = {k: _wrap(v) for k, v in p.callbacks.items()}
+    def _wrap(cb):
+        return lambda t0, y0_flat, dt: cb(t0 * t_sign, unflat(y0_flat), dt)           # misc.py:326-331
+    callbacks = {k: _wrap(v) for k, v in callbacks.items()}
 
     # flat state + flat func
-    if p.is_tuple:
-        p.shape = None
-        p.y0_flat = p.layout.flatten([y_.detach() for y_ in y0])
-        p.n = p.layout.n
-        layout = p.layout
-        def fn(t_, y_flat):
-            f = func(t_, layout.views(y_flat))                                         # misc.py:143-145
-            return tuple(f)
-        p.fn = fn
-        p.pieces = (list(layout.offsets), list(layout.lens), [1.0] * len(layout.lens))
-        p.segs = list(zip(layout.offsets, layout.lens))                                # misc.py:247 _mixed_norm
+    if is_tuple:
+        y0_flat = layout.flatten([y_.detach() for y_ in y0])
+        fn = lambda t_, y_flat: tuple(func(t_, layout.views(y_flat)))                  # misc.py:143-145
+        pieces = (list(layout.offsets), list(layout.lens), [1.0] * len(layout.lens))
+        segs = list(zip(layout.offsets, layout.lens))                                  # misc.py:247 _mixed_norm
     else:
-        p.shape = y0.shape
-        p.y0_flat = y0.detach().reshape(-1)
-        p.n = p.y0_flat.numel()
-        shape = p.shape
-        p.fn = lambda t_, y_flat: func(t_, y_flat.view(shape))
-        p.pieces = None
-        p.segs = None
+        y0_flat = y0.detach().reshape(-1)
+        fn = lambda t_, y_flat: func(t_, y_flat.view(shape))
+        pieces = segs = None
 
     # event function on the flat state, in the solver's ascending time (misc.py:224-225, :281-282)
-    p.event_fn = None
+    flat_event_fn = None
     if event_fn is not None:
-        unflat = (lambda yf: p.layout.views(yf)) if p.is_tuple else (lambda yf: yf.view(p.shape))
-        sign_ = p.t_sign
-        p.event_fn = lambda t_, y_flat: event_fn(t_ * sign_, unflat(y_flat))
+        flat_event_fn = lambda t_, y_flat: event_fn(t_ * t_sign, unflat(y_flat))
 
     # norm (misc.py:237-266): the defaults stay fused; a user callable takes the compatibility path
-    p.norm_fn = None
-    p.q_view = None
-    user_norm = options.get("norm", None)
-    if user_norm is not None and user_norm is not _rms_norm and not (p.is_tuple and user_norm is _mixed_norm):
-        p.norm_fn = user_norm
-        if p.is_tuple:
-            p.q_view = lambda q: layout.views(q)
-        else:
-            p.q_view = lambda q: q.view(shape)
-    return p
+    norm_fn = options.get("norm", None)
+    if norm_fn is _rms_norm or (is_tuple and norm_fn is _mixed_norm):
+        norm_fn = None
+    return Problem(method=method, options=options, original_func=func, fn=fn, n=y0_flat.numel(), dtype=dtype,
+                   device=device, rtol=rtol, atol=atol, rtol_vec=rtol_vec, atol_vec=atol_vec, t_sign=t_sign,
+                   t_cpu=t_cpu, y0_flat=y0_flat, callbacks=callbacks, is_tuple=is_tuple, layout=layout, shape=shape,
+                   segs=segs, pieces=pieces, norm_fn=norm_fn, q_view=unflat if norm_fn is not None else None,
+                   event_fn=flat_event_fn)
+
+
+def valid_callbacks(method, callbacks):
+    """misc.py:339-343: the callbacks `method` accepts -- every one for the adaptive methods (rk_common.py:207-211),
+    callback_step for the fixed-grid ones (solvers.py:81-83); the others are dropped with the reference's warning."""
+    valid = set(_CALLBACK_NAMES) if method in ADAPTIVE_METHODS else {"callback_step"}
+    invalid = set(callbacks) - valid
+    if invalid:
+        warnings.warn("Solver '{}' does not support callbacks {}".format(method, invalid))
+    return {k: v for k, v in callbacks.items() if k in valid}
 
 
 def _warn_unused(solver_name, options, known):                                        # misc.py:13-15
@@ -309,6 +311,20 @@ def _make_adaptive_engine(p, lockstep=False, keep_interp=False, graph=None, repl
         if w is not None:
             eng.set_linear(w, whole_attempt=o.get("fused_attempt", True))
     return eng
+
+
+def _make_fixed_engine(p, *, graph=None, interp=None):
+    """The fixed-grid engine of a Problem (explicit Runge-Kutta, Adams or implicit Runge-Kutta): method, func, state,
+    time direction, callbacks and tolerances come from `p`, perturb, interp, max_iters and max_order from its options.
+    graph, interp: instead of options['graph'] / options['interp']."""
+    o = p.options
+    if graph is None:
+        graph = _resolve_graph(o.get("graph", "auto"), p.original_func)
+    return make_engine(p.method, p.fn, p.n, p.dtype, p.device, t_sign=p.t_sign, perturb=o.get("perturb", False),
+                       callbacks=p.callbacks, pieces=p.pieces,
+                       interp=_cubic_or_linear(o.get("interp", "linear") if interp is None else interp),
+                       graph=graph, rtol=p.rtol, atol=p.atol, max_iters=o.get("max_iters"), max_order=o.get("max_order"),
+                       sharded=o.get("process_group") is not None)
 
 
 def _check_independent_rows(func, y0, t, method, options, event_fn):
@@ -531,11 +547,10 @@ def _solve(p):
         if key is not None:
             sol = sol.clone()                           # the engine reuses its solution buffer
         return sol, eng
-    # fixed grid: euler / midpoint / heun2 / heun3 / rk4 (solvers.py:55-128, fixed_grid.py:6-60)
-    o = p.options
+    # fixed grid: explicit Runge-Kutta, Adams and implicit Runge-Kutta (solvers.py:55-128)
     y0_view = p.layout.views(p.y0_flat) if p.is_tuple else p.y0_flat.view(p.shape)
-    grid = fixed_grid(p.method, o, p.original_func, y0_view, p.t_cpu)
-    eng = _fixed_engine(p)
+    grid = fixed_grid(p.method, p.options, p.original_func, y0_view, p.t_cpu)
+    eng = _make_fixed_engine(p)
     sol = eng.solve(p.y0_flat, grid, p.t_cpu)
     return sol, eng
 
@@ -561,23 +576,27 @@ def _fixed_options(method):
     return _IMPLICIT_OPTIONS if method in IMPLICIT_METHODS else _FIXED_OPTIONS
 
 
-def _fixed_engine(p, graph=None):
-    """The fixed-grid engine of a normalised problem: explicit Runge-Kutta, Adams or implicit Runge-Kutta."""
-    o = p.options
-    if graph is None:
-        graph = _resolve_graph(o.get("graph", "auto"), p.original_func)
-    return make_engine(p.method, p.fn, p.n, p.dtype, p.device, t_sign=p.t_sign, perturb=o.get("perturb", False),
-                       callbacks=p.callbacks, pieces=p.pieces, interp=_cubic_or_linear(o.get("interp", "linear")),
-                       graph=graph, rtol=p.rtol, atol=p.atol, max_iters=o.get("max_iters"), max_order=o.get("max_order"),
-                       sharded=o.get("process_group") is not None)
+def fixed_grid_constructor(method, o, event=False):
+    """Option handling of FixedGridODESolver (solvers.py:55-79, :125, :131): the unused-option warning, step_size and
+    grid_constructor refused together, an unknown interp refused; with event=True step_size is required.  Returns the
+    grid constructor."""
+    _warn_unused(_FIXED_NAMES[method], o, _fixed_options(method))
+    if event and o.get("step_size") is None:
+        raise AssertionError("Event handling for fixed step solvers currently requires `step_size` to be provided in "
+                             "options.")
+    grid_constructor = choose_grid_constructor(o.get("step_size"), o.get("grid_constructor"))
+    _cubic_or_linear(o.get("interp", "linear"))
+    return grid_constructor
 
 
 def fixed_grid(method, o, func, y0_view, t_cpu, keep_graph=False):
-    """Option handling and time grid of FixedGridODESolver (solvers.py:55-79, :85-96, :103-104) for an
-    ascending CPU `t_cpu`; the caller has already wrapped a user grid_constructor for reversed time."""
-    _warn_unused(_FIXED_NAMES[method], o, _fixed_options(method))
-    grid_constructor = choose_grid_constructor(o.get("step_size"), o.get("grid_constructor"))
-    _cubic_or_linear(o.get("interp", "linear"))
+    """Option check (fixed_grid_constructor) and time grid of one fixed-grid solve."""
+    return build_grid(fixed_grid_constructor(method, o), func, y0_view, t_cpu, keep_graph)
+
+
+def build_grid(grid_constructor, func, y0_view, t_cpu, keep_graph=False):
+    """The time grid of one fixed-grid solve (solvers.py:103-104) for an ascending CPU `t_cpu`, on the CPU; a user
+    grid_constructor has already been wrapped for reversed time (signed_grid_constructor)."""
     grid = grid_constructor(func, y0_view, t_cpu)
     grid = grid.to("cpu") if keep_graph else grid.detach().to("cpu")
     assert grid[0] == t_cpu[0] and grid[-1] == t_cpu[-1]                               # solvers.py:104
@@ -585,24 +604,19 @@ def fixed_grid(method, o, func, y0_view, t_cpu, keep_graph=False):
 
 
 def _solve_event(p):
-    """odeint.py:97-100 + solvers.py:41-49: integrate until the event; returns (event_t tensor like t, [2, n])."""
-    if p.method in FIXED_METHODS or p.method in ADAMS_METHODS or p.method in IMPLICIT_METHODS:   # solvers.py:130-164
-        o = p.options
-        _warn_unused(_FIXED_NAMES[p.method], o, _fixed_options(p.method))
-        if o.get("step_size") is None:
-            raise AssertionError("Event handling for fixed step solvers currently requires `step_size` to be provided "
-                                 "in options.")
-        choose_grid_constructor(o["step_size"], o.get("grid_constructor"))          # refuses both at once
-        eng = _fixed_engine(p, graph=False)
-        tol = p.atol if p.atol is not None else float(p.atol_vec.min())
-        event_t, y_event = eng.solve_until_event(p.y0_flat, p.t_cpu[0], o["step_size"], p.event_fn, tol)
-        sol = torch.stack([p.y0_flat.to(p.dtype), y_event], dim=0)
-        return float(event_t) * p.t_sign, sol, eng
-    eng = _make_adaptive_engine(p, lockstep=True, keep_interp=True)
+    """odeint.py:97-100 with solvers.py:41-49 (adaptive) or :130-164 (fixed grid): integrate until the event.  Returns
+    the engine's event time (solver time: a float, or a device tensor of the state dtype on a fixed grid), the flat
+    [y0, y(event)] and the engine."""
+    if p.method in ADAPTIVE_METHODS:
+        eng = _make_adaptive_engine(p, lockstep=True, keep_interp=True)
+        args = (float(p.t_cpu[0]),)
+    else:
+        fixed_grid_constructor(p.method, p.options, event=True)
+        eng = _make_fixed_engine(p, graph=False)
+        args = (p.t_cpu[0], p.options["step_size"])
     tol = p.atol if p.atol is not None else float(p.atol_vec.min())
-    event_t, y_event = eng.solve_until_event(p.y0_flat, float(p.t_cpu[0]), p.event_fn, tol)
-    sol = torch.stack([p.y0_flat.to(p.dtype), y_event], dim=0)                         # solvers.py:48
-    return event_t * p.t_sign, sol, eng                                                # odeint.py:99-100
+    event_t, y_event = eng.solve_until_event(p.y0_flat, *args, p.event_fn, tol)
+    return event_t, torch.stack([p.y0_flat.to(p.dtype), y_event], dim=0), eng            # solvers.py:48
 
 
 def _unflatten(p, sol):
@@ -743,8 +757,7 @@ def _odeint_backprop(p, func, y0, t, params, _stats):
             t_req = p.t_cpu.detach().clone().requires_grad_(True)
             grid_req = fixed_grid(p.method, o, p.original_func, y0_view, t_req, keep_graph=True)
         grid = grid_req.detach()
-        eng = make_engine(p.method, p.fn, p.n, p.dtype, p.device, t_sign=p.t_sign, perturb=o.get("perturb", False),
-                          graph=False, callbacks=p.callbacks, pieces=p.pieces)
+        eng = _make_fixed_engine(p, graph=False)
         sol, tape = eng.solve_taped(p.y0_flat, grid, p.t_cpu)
         holder["eng"] = eng
         return sol, {"kind": "fixed", "tape": tape, "grid": grid, "grid_req": grid_req, "t_req": t_req}
@@ -824,7 +837,8 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
         if p.event_fn is not None:
             event_t, sol, eng = _solve_event(p)
             ss.publish(sol)
-            return torch.tensor(event_t, dtype=t.dtype, device=t.device), _unflatten(p, sol)     # odeint.py:98, :105-108
+            event_t = torch.tensor(float(event_t) * p.t_sign, dtype=t.dtype, device=t.device)  # odeint.py:98-100
+            return event_t, _unflatten(p, sol)                                                   # :105-108
         if row_event_fn is not None:
             row_event_t, sol, eng = _solve_rows_event(p, row_event_fn, row_ev0)
             row_event_t = row_event_t.to(device=t.device, dtype=t.dtype, copy=True)

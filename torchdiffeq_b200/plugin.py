@@ -34,9 +34,9 @@ import torch
 from . import _lib
 from ._engine import on_solver_stream
 from ._adams import ADAMS_METHODS
-from ._fixed import FIXED_METHODS, choose_grid_constructor, make_engine
+from ._fixed import FIXED_METHODS
 from ._implicit import IMPLICIT_METHODS
-from .odeint import Problem, _make_adaptive_engine
+from .odeint import Problem, _make_adaptive_engine, _make_fixed_engine, _solve_event, fixed_grid, fixed_grid_constructor
 
 ADAPTIVE = ("dopri5", "dopri8", "tsit5", "bosh3", "fehlberg2", "adaptive_heun")
 _CB = ("callback_step", "callback_accept_step", "callback_reject_step")
@@ -104,48 +104,36 @@ def make_adaptive(method, **defaults):
                 warnings.warn('{}: Unexpected arguments {}'.format(self.__class__.__name__, unused))
             # the problem as the engine factory sees it; the seam hands over the reference's wrapper of func, so
             # 'auto' graph resolution sees an nn.Module, and the fused LinearField path is never taken
-            self.p = p = Problem()
-            p.method, p.original_func, p.callbacks = method, func, _callbacks_of(func, _CB)
-            p.options = dict({k: v for k, v in opts.items() if k not in unused}, fused_linear=False)
-            p.fn, p.n, p.shape, p.dtype, p.device = (lambda t_, yf: self.base(t_, yf.view(y0.shape))), y0.numel(), \
-                y0.shape, y0.dtype, y0.device
-            p.t_sign, p.segs, p.pieces = 1.0, None, None
-            p.rtol, p.rtol_vec = _tol(rtol, y0.device)
-            p.atol, p.atol_vec = _tol(atol, y0.device)
-            p.norm_fn = None if (norm is None or _is_default_rms(norm)) else norm
-            p.q_view = (lambda q: q.view(y0.shape)) if p.norm_fn is not None else None
+            rtol, rtol_vec = _tol(rtol, y0.device)
+            atol, atol_vec = _tol(atol, y0.device)
+            norm_fn = None if (norm is None or _is_default_rms(norm)) else norm
+            self.p = Problem(method=method, options=dict({k: v for k, v in opts.items() if k not in unused},
+                                                         fused_linear=False),
+                             original_func=func, fn=lambda t_, yf: self.base(t_, yf.view(y0.shape)), n=y0.numel(),
+                             dtype=y0.dtype, device=y0.device, rtol=rtol, atol=atol, rtol_vec=rtol_vec,
+                             atol_vec=atol_vec, callbacks=_callbacks_of(func, _CB), shape=y0.shape, norm_fn=norm_fn,
+                             q_view=(lambda q: q.view(y0.shape)) if norm_fn is not None else None)
             self.engine = None
 
         @classmethod
         def valid_callbacks(cls):                                              # rk_common.py:207-211
             return set(_CB)
 
-        def _engine(self, t_cpu, keep_interp):
+        def integrate(self, t):                                                # solvers.py:28-35
             """Lock step (the reference's call sequence) unless options give graph or run_ahead; graph defaults to
             False."""
-            o, self.p.t_cpu = self.p.options, t_cpu
-            return _make_adaptive_engine(self.p, lockstep="graph" not in o and "run_ahead" not in o,
-                                         keep_interp=keep_interp, graph=o.get("graph", False))
-
-        def integrate(self, t):                                                # solvers.py:28-35
-            t_cpu = t.detach().to("cpu", torch.float64)
+            o, t_cpu = self.p.options, t.detach().to("cpu", torch.float64)
+            self.p.t_cpu = t_cpu
             with torch.no_grad(), on_solver_stream(self.y0.device) as ss:
-                self.engine = eng = self._engine(t_cpu, False)
+                self.engine = eng = _make_adaptive_engine(self.p, lockstep="graph" not in o and "run_ahead" not in o,
+                                                          graph=o.get("graph", False))
                 sol = eng.solve(self.y0.detach().reshape(-1), t_cpu.to(self.y0.device), t_start=float(t_cpu[0]))
                 sol = sol.view(len(t), *self.shape).clone()
                 ss.publish(sol)
             return sol
 
         def integrate_until_event(self, t0, event_fn):                         # solvers.py:41-49, rk_common.py:252-264
-            t0 = float(t0)
-            shape, p = self.shape, self.p
-            tol = p.atol if p.atol is not None else float(p.atol_vec.min())
-            with torch.no_grad(), on_solver_stream(self.y0.device) as ss:
-                self.engine = eng = self._engine(torch.tensor([t0], dtype=torch.float64), True)
-                ev = lambda t_, yf: event_fn(t_, yf.view(shape))
-                event_t, y1 = eng.solve_until_event(self.y0.detach().reshape(-1), t0, ev, tol)
-                sol = torch.stack([self.y0.detach(), y1.view(shape)], dim=0)
-                ss.publish(sol)
+            event_t, sol = _integrate_until_event(self, t0, event_fn)
             return torch.tensor(event_t, dtype=torch.float64, device=self.y0.device), sol
 
     B200AdaptiveSolver.__name__ = B200AdaptiveSolver.__qualname__ = "B200_" + method
@@ -167,62 +155,58 @@ def make_fixed(method, **defaults):
                      **unused_kwargs):
             if not y0.is_cuda:
                 raise _lib.TdqError("torchdiffeq_b200.plugin solvers take CUDA tensors (got %s)" % y0.device)
-            self.atol = unused_kwargs.pop("atol", None)                        # solvers.py:58-61
-            self.rtol = unused_kwargs.pop("rtol", None)
-            self.iter_kw = {k: unused_kwargs.pop(k) for k in iter_keys if k in unused_kwargs}
+            atol = unused_kwargs.pop("atol", None)                             # solvers.py:58-61
+            rtol = unused_kwargs.pop("rtol", None)
+            iter_kw = {k: unused_kwargs.pop(k) for k in iter_keys if k in unused_kwargs}
             unused_kwargs.pop("norm", None)
-            self.our = {k: unused_kwargs.pop(k) for k in _OUR_KEYS if k in unused_kwargs}
-            for k, v in defaults.items():
-                self.our.setdefault(k, v)
+            our = {k: unused_kwargs.pop(k) for k in _OUR_KEYS if k in unused_kwargs}
             if unused_kwargs:
                 warnings.warn('{}: Unexpected arguments {}'.format(self.__class__.__name__, unused_kwargs))
-            self.func, self.y0, self.shape = func, y0, y0.shape
-            self.base = _unwrap_perturb(func)
-            self.step_size, self.interp, self.perturb = step_size, interp, perturb
-            self.grid_constructor = choose_grid_constructor(step_size, grid_constructor)
-            self.callbacks = _callbacks_of(func, ("callback_step",))
+            self.y0 = y0
+            self.graph = our.get("graph", defaults.get("graph", False))
+            # solvers.py:70-79 refuses step_size with grid_constructor here; interp is checked when integrating (:125)
+            fixed_grid_constructor(method, dict(step_size=step_size, grid_constructor=grid_constructor))
+            # the Adams corrector's tolerances default to fixed_adams.py:164's
+            rtol, rtol_vec = _tol(rtol if rtol is not None else 1e-3, y0.device)
+            atol, atol_vec = _tol(atol if atol is not None else 1e-4, y0.device)
+            base = _unwrap_perturb(func)
+            self.p = Problem(method=method, options=dict(step_size=step_size, grid_constructor=grid_constructor,
+                                                         interp=interp, perturb=perturb, **iter_kw),
+                             original_func=func, fn=lambda t_, yf: base(t_, yf.view(y0.shape)), n=y0.numel(),
+                             dtype=y0.dtype, device=y0.device, rtol=rtol, atol=atol, rtol_vec=rtol_vec,
+                             atol_vec=atol_vec, callbacks=_callbacks_of(func, ("callback_step",)), shape=y0.shape)
 
         @classmethod
         def valid_callbacks(cls):                                              # solvers.py:81-83
             return {"callback_step"}
 
-        def _make_engine(self, interp, graph):
-            shape, base = self.shape, self.base
-            fn = lambda t_, yf: base(t_, yf.view(shape))
-            return make_engine(method, fn, self.y0.numel(), self.y0.dtype, self.y0.device, perturb=self.perturb,
-                               graph=graph, callbacks=self.callbacks, interp=interp,
-                               rtol=self.rtol if self.rtol is not None else 1e-3,
-                               atol=self.atol if self.atol is not None else 1e-4, **self.iter_kw)
-
         def integrate(self, t):                                                # solvers.py:102-128
-            from .odeint import _cubic_or_linear
-            interp = _cubic_or_linear(self.interp)
-            shape = self.shape
             t_cpu = t.detach().to("cpu")
-            grid = self.grid_constructor(self.func, self.y0, t_cpu).detach().to("cpu")
-            assert grid[0] == t_cpu[0] and grid[-1] == t_cpu[-1]
-            lock = "graph" not in self.our
+            grid = fixed_grid(method, self.p.options, self.p.original_func, self.y0, t_cpu)
             with torch.no_grad(), on_solver_stream(self.y0.device) as ss:
-                eng = self._make_engine(interp, False if lock else self.our.get("graph", False))
-                sol = eng.solve(self.y0.detach().reshape(-1), grid, t_cpu).view(len(t), *shape)
+                eng = _make_fixed_engine(self.p, graph=self.graph)
+                sol = eng.solve(self.y0.detach().reshape(-1), grid, t_cpu).view(len(t), *self.y0.shape)
                 ss.publish(sol)
             return sol
 
         def integrate_until_event(self, t0, event_fn):                         # solvers.py:130-164
-            from .odeint import _cubic_or_linear
-            assert self.step_size is not None, ("Event handling for fixed step solvers currently requires `step_size` "
-                                                "to be provided in options.")
-            shape = self.shape
-            with torch.no_grad(), on_solver_stream(self.y0.device) as ss:
-                eng = self._make_engine(_cubic_or_linear(self.interp), False)
-                ev = lambda t_, yf: event_fn(t_, yf.view(shape))
-                event_t, y1 = eng.solve_until_event(self.y0.detach().reshape(-1), t0, self.step_size, ev, float(self.atol))
-                sol = torch.stack([self.y0.detach(), y1.view(shape)], dim=0)
-                ss.publish(sol)
-            return event_t, sol
+            return _integrate_until_event(self, t0, event_fn)
 
     B200FixedSolver.__name__ = B200FixedSolver.__qualname__ = "B200_" + method
     return B200FixedSolver
+
+
+def _integrate_until_event(solver, t0, event_fn):
+    """integrate_until_event of both solver classes through odeint's event solve; returns (the engine's event time,
+    [y0, y(event)] in y0's shape)."""
+    p, y0 = solver.p, solver.y0
+    p.t_cpu, p.y0_flat = torch.as_tensor(t0).detach().to("cpu").reshape(1), y0.detach().reshape(-1)
+    p.event_fn = lambda t_, yf: event_fn(t_, yf.view(y0.shape))
+    with torch.no_grad(), on_solver_stream(y0.device) as ss:
+        event_t, sol, solver.engine = _solve_event(p)
+        sol = sol.view(2, *y0.shape)
+        ss.publish(sol)
+    return event_t, sol
 
 
 class _Dispatch:
