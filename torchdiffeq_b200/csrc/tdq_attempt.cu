@@ -33,6 +33,7 @@
 #include "tdq_shape.cuh"
 #include "tdq_tc.cuh"
 
+#include <cstddef>
 #include <type_traits>
 
 namespace {
@@ -56,16 +57,24 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
     return v;
 }
 
+__device__ __forceinline__ uint64_t lds_u64(uint32_t addr) {
+    uint64_t v;
+    asm volatile("ld.shared.u64 %0, [%1];" : "=l"(v) : "r"(addr) : "memory");
+    return v;
+}
+// ld.volatile: ptxas keeps the load where it is written.  A plain load of a coefficient can be merged with its neighbours
+// into a vector load or moved away from the block that uses it; either keeps more registers live across the stage window,
+// and the dopri5 instantiation (255 registers) then spills.
+__device__ __forceinline__ float lds_pinned_f32(uint32_t addr) {
+    float v;
+    asm volatile("ld.volatile.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+    return v;
+}
+
 struct AttOut {
     float *k[AT_MAX_S + 1];                    // k[i], i = 1..S: where k_i goes when the attempt's stages are kept
     float *y1, *err;
 };
-
-__host__ __device__ constexpr int popc_below(unsigned mask, int j) {
-    int n = 0;
-    for (int b = 0; b < j; ++b) n += (mask >> b) & 1u;
-    return n;
-}
 
 // S: stages of an FSAL tableau (rows 0..S-1, the last one is c_sol and yields y1).  RM: 8 bits per row, bit j set <=> slot j has
 // a non-zero coefficient in that row.  EM: the same for the error weights of slots 0..S-1 (k_S always carries the last one).
@@ -78,33 +87,52 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
     uint8_t *aux = smem + W_BYTES + AT_STAGE + AT_Y0;
     int *s_flag = reinterpret_cast<int *>(aux);
-    float *s_cr = reinterpret_cast<float *>(aux + 64);                    // [S][8]: coef[i][m] as float32
-    float *s_ce = s_cr + AT_MAX_S * 8;                                    // [8]:    ecoef[m]
+    // per-attempt pointers and tolerances, read where they are used rather than held in registers through the tile loop
+    struct Scalars {
+        const float *y0, *k0;
+        float *ycand, *kcand;                                             // candidate commit (nullptr: none)
+        AttOut out;
+        float rtol, atol;
+    };
+    Scalars *s_sc = reinterpret_cast<Scalars *>(aux + 320);
+    static_assert(320 + sizeof(Scalars) <= 512, "aux layout");
+    // this attempt's coefficients (prepare_tables) as float32, laid out by slot: the coefficient of k_j in row i at
+    // s_cr[8 i + j], the error weight of k_j at s_ce[j] (j = 0..S), zero where the tableau has none.  Every index the tile
+    // loop uses is then a compile-time constant of RM / EM: each block loads the few it needs once, with a 32-bit
+    // ld.shared (coef()), instead of finding the ordinal of a slot at run time for every element.
+    float *s_cr = reinterpret_cast<float *>(aux + 64);                    // [AT_MAX_S][8]
+    float *s_ce = s_cr + AT_MAX_S * 8;                                    // [8]
     double *s_red = reinterpret_cast<double *>(aux + 512);                // [2][32]
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);                  // warp-uniform for the compiler as well
     const int n_rows = (int)n_rows_sz;
 
-    if (tid < AT_MAX_S * 8) {                                             // this attempt's coefficients (prepare_tables)
-        const int i = tid >> 3, m = tid & 7;
-        s_cr[i * 8 + m] = (i < S) ? (float)c->coef[i][m] : 0.f;
-        if (i == 0) s_ce[m] = (float)c->ecoef[m];
+    if (tid < AT_MAX_S * 8) {
+        const int i = tid >> 3, j = tid & 7;
+        const unsigned mask = i < S ? (unsigned)((RM >> (8 * i)) & 0xffull) : 0u, below = (1u << j) - 1u;
+        s_cr[i * 8 + j] = ((mask >> j) & 1u) ? (float)c->coef[i][__popc(mask & below)] : 0.f;
+        if (i == 0) s_ce[j] = j == S ? (float)c->ecoef[__popc(EM)] : ((EM >> j) & 1u) ? (float)c->ecoef[__popc(EM & below)] : 0.f;
+    }
+    const bool fold = partials != nullptr;                                // squared error norm + candidate commit in here
+    if (tid == 0) {
+        Scalars sc;
+        sc.y0 = tdq_detach(y0 != nullptr ? y0 : reinterpret_cast<const float *>(c->y0_cur), n_rows_sz);
+        sc.k0 = tdq_detach(k0 != nullptr ? k0 : reinterpret_cast<const float *>(c->k0_cur), n_rows_sz);
+        sc.ycand = sc.kcand = nullptr;
+        if (fold && c->ybuf[0] != nullptr) {
+            sc.ycand = tdq_detach(reinterpret_cast<float *>(c->ybuf[c->par ^ 1]), n_rows_sz);
+            sc.kcand = tdq_detach(reinterpret_cast<float *>(c->kbuf[c->par ^ 1]), n_rows_sz);
+        }
+        sc.out = out;
+        sc.rtol = (float)c->rtol;
+        sc.atol = (float)c->atol;
+        *s_sc = sc;
     }
     load_weights(smem, wt, tid, AT_THREADS);
     fence_async_smem();
     __syncthreads();
 
     // ---- per-attempt scalars ---------------------------------------------------------------------------------
-    if (y0 == nullptr) y0 = reinterpret_cast<const float *>(c->y0_cur);
-    if (k0 == nullptr) k0 = reinterpret_cast<const float *>(c->k0_cur);
-    y0 = tdq_detach(y0, n_rows_sz);
-    k0 = tdq_detach(k0, n_rows_sz);
-    const bool fold = partials != nullptr;                                // squared error norm + candidate commit in here
-    float *ycand = nullptr, *kcand = nullptr;
-    if (fold && c->ybuf[0] != nullptr) {
-        ycand = tdq_detach(reinterpret_cast<float *>(c->ybuf[c->par ^ 1]), n_rows_sz);
-        kcand = tdq_detach(reinterpret_cast<float *>(c->kbuf[c->par ^ 1]), n_rows_sz);
-    }
     // the stages of this attempt are needed afterwards only if an output time can fall into it (the controller's
     // test `!(t_out[cursor] > t1)` for t1 = att_t1, rk_common.py:246) or the caller keeps every step
     bool store = store_always != 0 || c->always_fit != 0;
@@ -112,13 +140,13 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
         const int cur = c->out_cursor;
         store = cur < c->n_out && !(c->t_out[cur] > c->att_t1);
     }
-    const float rtolT = (float)c->rtol, atolT = (float)c->atol;
-    constexpr int EK = popc_below(EM, S);                                 // index of k_S's error weight in ecoef
-    const float ecS = s_ce[EK];
-
     // h = the warpgroup's half of the output features; w = warp inside the warpgroup
     const int h = warp >> 2, w = warp & 3;
     const uint32_t wsm = smem_u32(smem);
+    const uint32_t ssc = wsm + (uint32_t)(reinterpret_cast<uint8_t *>(s_sc) - smem);
+    const uint32_t scoef = wsm + (uint32_t)(reinterpret_cast<uint8_t *>(s_cr) - smem);
+    // the coefficient of k_j in row i (i = AT_MAX_S: the error weights); i and j are compile-time constants at every use
+    auto coef = [scoef](int i, int j) { return lds_pinned_f32(scoef + 4 * (8 * i + j)); };
     const uint32_t wsm_h = wsm + h * 8 * SBO;                             // the weight rows of features [64 h, 64 h + 64)
     const uint32_t stage = wsm + W_BYTES;
     const uint32_t sy0 = stage + AT_STAGE + tid * 4;                      // element e at sy0 + 1024 e: this thread's only
@@ -163,6 +191,8 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
         float A[NACC > 0 ? NACC : 1][16];                             // A[q - KEEP]: running sum of row q
         float AE[16], PRE[16], KN[16], Y1[16];
         {
+            const float *y0 = reinterpret_cast<const float *>(lds_u64(ssc + offsetof(Scalars, y0)));
+            const float *k0 = reinterpret_cast<const float *>(lds_u64(ssc + offsetof(Scalars, k0)));
             float Y0[16];
 #pragma unroll
             for (int e = 0; e < 16; ++e) {
@@ -181,7 +211,7 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
             const unsigned mask = row_mask(i);
             const bool last = i == S - 1;
             const bool has_prefix = (mask & ((1u << i) - 1u)) != 0u, has_new = ((mask >> i) & 1u) != 0u;
-            const float c_new = has_new ? s_cr[i * 8 + popc_below(mask, i)] : 0.f;
+            const float c_new = has_new ? coef(i, i) : 0.f;
             if (i < KEEP) {
 #pragma unroll
                 for (int e = 0; e < 16; ++e) K[i < KEEP ? i : 0][e] = KN[e];
@@ -216,7 +246,7 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
 #pragma unroll
                 for (int j = 0; j <= i; ++j) {
                     if ((mn >> j) & 1u) {
-                        const float cj = s_cr[(i + 1) * 8 + popc_below(mn, j)];
+                        const float cj = coef(i + 1, j);
 #pragma unroll
                         for (int e = 0; e < 16; ++e) {
                             const float p = K[j < KEEP ? j : 0][e] * cj;
@@ -229,7 +259,15 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
             }
             if (i == KEEP - 1) {
                 // every kept slot is known: the remaining rows and the error estimate become running sums (element by element,
-                // so that the kept slots die as the sums are born)
+                // so that the kept slots die as the sums are born); their coefficients are loaded once, before the element loop
+                float cq[NACC > 0 ? NACC : 1][KEEP], ce[KEEP];
+#pragma unroll
+                for (int j = 0; j < KEEP; ++j) {
+#pragma unroll
+                    for (int qrow = KEEP; qrow < S; ++qrow)
+                        if ((row_mask(qrow) >> j) & 1u) cq[qrow - KEEP][j] = coef(qrow, j);
+                    if ((EM >> j) & 1u) ce[j] = coef(AT_MAX_S, j);
+                }
 #pragma unroll
                 for (int e = 0; e < 16; ++e) {
 #pragma unroll
@@ -240,7 +278,7 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
 #pragma unroll
                         for (int j = 0; j <= i; ++j) {
                             if ((mq >> j) & 1u) {
-                                const float p = K[j < KEEP ? j : 0][e] * s_cr[qrow * 8 + popc_below(mq, j)];
+                                const float p = K[j < KEEP ? j : 0][e] * cq[qrow - KEEP][j];
                                 a_ = first ? p : a_ + p;
                                 first = false;
                             }
@@ -252,7 +290,7 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
 #pragma unroll
                     for (int j = 0; j <= i; ++j) {
                         if ((EM >> j) & 1u) {
-                            const float p = K[j < KEEP ? j : 0][e] * s_ce[popc_below(EM, j)];
+                            const float p = K[j < KEEP ? j : 0][e] * ce[j];
                             e_ = first ? p : e_ + p;
                             first = false;
                         }
@@ -269,7 +307,7 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
                 for (int qrow = i + 1; qrow < S; ++qrow) {
                     const unsigned mq = row_mask(qrow);
                     if ((mq >> i) & 1u) {
-                        const float cj = s_cr[qrow * 8 + popc_below(mq, i)];
+                        const float cj = coef(qrow, i);
                         const bool started = (mq & ((1u << i) - 1u)) != 0u;
 #pragma unroll
                         for (int e = 0; e < 16; ++e) {
@@ -279,7 +317,7 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
                     }
                 }
                 if ((EM >> i) & 1u) {
-                    const float cj = s_ce[popc_below(EM, i)];
+                    const float cj = coef(AT_MAX_S, i);
                     const bool started = (EM & ((1u << i) - 1u)) != 0u;
 #pragma unroll
                     for (int e = 0; e < 16; ++e) {
@@ -294,6 +332,8 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
             if (last) {
                 // y1: non-finite count, candidate commit, (optional) y1 and the error prefix; tol = atol + rtol * max(|y0|, |y1|)
                 // (misc.py:81) replaces y1 in its registers
+                float *ycand = reinterpret_cast<float *>(lds_u64(ssc + offsetof(Scalars, ycand)));
+                const float rtolT = lds_f32(ssc + offsetof(Scalars, rtol)), atolT = lds_f32(ssc + offsetof(Scalars, atol));
 #pragma unroll
                 for (int e = 0; e < 16; ++e) {
                     const float y1v = Y1[e];
@@ -302,8 +342,8 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
                         const size_t o = base + elem_offset<AT_ROWS>(e);
                         if (ycand) ycand[o] = y1v;
                         if (store) {
-                            out.y1[o] = y1v;
-                            out.err[o] = AE[e];
+                            reinterpret_cast<float *>(lds_u64(ssc + offsetof(Scalars, out.y1)))[o] = y1v;
+                            reinterpret_cast<float *>(lds_u64(ssc + offsetof(Scalars, out.err)))[o] = AE[e];
                         }
                     }
                     Y1[e] = Ar<float>::add(atolT, Ar<float>::mul(rtolT, Ar<float>::max_nan(fabsf(lds_f32(sy0 + e * 1024)), fabsf(y1v))));
@@ -313,12 +353,15 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
             wgmma_wait();
             tile_result(tacc, KN);
             if (store) {
+                float *ko = reinterpret_cast<float *>(lds_u64(ssc + offsetof(Scalars, out.k) + 8 * (i + 1)));
 #pragma unroll
                 for (int e = 0; e < 16; ++e)
-                    if (FULL || elem_row<AT_ROWS>(e, lane) < rows_here) out.k[i + 1][base + elem_offset<AT_ROWS>(e)] = KN[e];
+                    if (FULL || elem_row<AT_ROWS>(e, lane) < rows_here) ko[base + elem_offset<AT_ROWS>(e)] = KN[e];
             }
             if (last) {
                 // ---- k_S: candidate commit, error ratio (misc.py:80-82 up to the mean) ----
+                float *kcand = reinterpret_cast<float *>(lds_u64(ssc + offsetof(Scalars, kcand)));
+                const float ecS = coef(AT_MAX_S, S);
 #pragma unroll
                 for (int e = 0; e < 16; ++e) {
                     if (FULL || elem_row<AT_ROWS>(e, lane) < rows_here) {
@@ -340,6 +383,8 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
             const int tn = t + (int)gridDim.x;
             const long long prow = (long long)tn * AT_ROWS + lane;
             if (tn < tiles && prow < (long long)n_rows) {
+                const float *y0 = reinterpret_cast<const float *>(lds_u64(ssc + offsetof(Scalars, y0)));
+                const float *k0 = reinterpret_cast<const float *>(lds_u64(ssc + offsetof(Scalars, k0)));
                 const size_t o = (size_t)prow * LD + 64 * h + 16 * w;
                 asm volatile("prefetch.global.L2 [%0];" :: "l"(y0 + o));
                 asm volatile("prefetch.global.L2 [%0];" :: "l"(k0 + o));
