@@ -434,7 +434,17 @@ int tdq_ctrl_set_exchange(void *ctrl_dev, const void *const *peer_ptrs, int32_t 
  * that depends on D only (not on B or the row's position), so a row's results do not depend on the rest of the batch.
  * TDQ_ROWS_T_FIRST / _T_PROBE / _T_STAGE + i hold, in the state dtype, the time func sees for f0, the initial-step probe
  * and stage i of the attempt in flight (t_sign applied): what func's time argument aliases.
- * tdq_rows_init:            per-row state at t_start (rk_common.py:213-221).  Not needed again until the next solve.
+ * tdq_rows_init:            per-row state at t_start (rk_common.py:213-221).  Not needed again until the next solve.  Every
+ *                           row reads the control block's output times; a per-row table left by tdq_rows_init_grid is
+ *                           cleared.
+ * tdq_rows_init_grid:       tdq_rows_init with per-row output times: t_grid is [B, n_out] float64, row r ascending in solver
+ *                           time (t_sign applied), and row r starts at t_grid[r, 0], ends at t_grid[r, n_out - 1] and emits
+ *                           solution[j, r, :] at t_grid[r, j] when the solve's attempts use tdq_rows_controller_grid
+ *                           (or _controller_event_grid) and tdq_rows_fit_eval_grid in place of the launchers without
+ *                           _grid, which have the same arguments.  Those read the table until the next init (its address
+ *                           is kept in the control block, which tdq_ctrl_init and tdq_rows_init clear), so it must stay
+ *                           alive and unchanged for the solve; with no table set they read the control block's t_out.
+ *                           The launchers without _grid never read the table.
  * tdq_rows_sumsq:           out[r] = sum over row r of (x/scale)^2, or ((x - x2)/scale)^2 with x2; scale = atol + |y0|*rtol;
  *                           without x2 out[B + r] = number of non-finite y0 elements of row r (misc.py:55-58, :69).
  * tdq_rows_initial_h0 / _probe / _finish: misc.py:60-77 per row from tdq_rows_sumsq's sums; _set_first_step: options
@@ -466,6 +476,8 @@ size_t tdq_rows_size(size_t n_rows);
 size_t tdq_rows_offset(int32_t field, size_t n_rows);                     /* (size_t)-1 for an unknown field             */
 size_t tdq_rows_partials_len(size_t n_rows, size_t row_len);
 int tdq_rows_init(void *ctrl_dev, void *rows_dev, int32_t dtype, size_t n_rows, double t_start, void *stream);
+int tdq_rows_init_grid(void *ctrl_dev, void *rows_dev, int32_t dtype, size_t n_rows, const double *t_grid, int32_t n_out,
+                       void *stream);
 int tdq_rows_sumsq(void *ctrl_dev, void *rows_dev, int32_t dtype, const void *x, const void *x2, const double *rtol_vec,
                    const double *atol_vec, size_t n_rows, size_t row_len, double *partials, double *out, void *stream);
 int tdq_rows_initial_h0(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *d0_sumsq, const double *d1_sumsq,
@@ -488,6 +500,10 @@ int tdq_rows_controller(void *ctrl_dev, void *rows_dev, int32_t dtype, const dou
                         size_t row_len, void *stream);
 int tdq_rows_fit_eval(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, const void *y1,
                       const void *const *k, void *solution, size_t n_rows, size_t row_len, void *stream);
+int tdq_rows_controller_grid(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in, size_t n_rows,
+                             size_t row_len, void *stream);
+int tdq_rows_fit_eval_grid(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, const void *y1,
+                           const void *const *k, void *solution, size_t n_rows, size_t row_len, void *stream);
 
 /* ---- per-row events with independent step-size control (tdq_rows.cu) ---------------------------------------------------
  * Row r stops at its own event as the reference's odeint_event does for y0[r:r+1] alone (rk_common.py:252-262,
@@ -515,6 +531,9 @@ int tdq_rows_event_init(void *rows_dev, const double *ev_val, double *init_sign,
 int tdq_rows_controller_event(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in, const double *ev_val,
                               const double *init_sign, const double *sign0, int32_t *flag, size_t n_rows, size_t row_len,
                               int32_t K, void *stream);
+int tdq_rows_controller_event_grid(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in,
+                                   const double *ev_val, const double *init_sign, const double *sign0, int32_t *flag,
+                                   size_t n_rows, size_t row_len, int32_t K, void *stream);
 int tdq_rows_fit_store(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, const void *y1,
                        const void *const *k, const int32_t *flag, void *coeff, size_t n_rows, size_t row_len,
                        void *stream);

@@ -984,6 +984,36 @@ class RowsEngine(AdaptiveEngine):
         self.row_dsum = [torch.zeros(2 * B, **f64) for _ in range(3)]
         self.row_n_accept = self.row_n_reject = None
         self.ev_fn = None                # set by solve_until_event: the attempt then tests each row's event
+        self.grid = None                 # per-row output times [B, T] of the solve in progress, or None
+        self._next_grid = None           # what solve(grid=...) hands to the next _begin
+        self._graph_grid = False         # the captured attempt launches the per-row-table kernels
+
+    def solve(self, y0_flat, t64, t_start=None, grid=None):
+        """AdaptiveEngine.solve, or with `grid` (an ascending float64 [B, T] device tensor) per-row output times: row r
+        starts at grid[r, 0], ends at grid[r, T-1] and solution[j] holds row r at grid[r, j].  t64 is then not read: the
+        control block gets row 0's times, so its n_out is T.  The engine keeps the grid alive until the next solve."""
+        if grid is not None:
+            if grid.dim() != 2 or grid.shape[0] != self.B or grid.dtype != torch.float64 or grid.device != self.device:
+                raise ValueError("grid must be a float64 [%d, T] tensor on %s, got %s %s on %s"
+                                 % (self.B, self.device, grid.dtype, tuple(grid.shape), grid.device))
+            grid = grid.contiguous()
+            t64 = grid[0]
+        self._next_grid = grid
+        try:
+            return super().solve(y0_flat, t64, t_start)
+        finally:
+            self._next_grid = None
+
+    def _begin(self, y0_flat, t64, t_start=None, loop=False):
+        """AdaptiveEngine._begin with the grid solve() was given, or none: every other way into a solve (prime, a direct
+        _begin) runs on the shared times.  The per-row-table and shared-times attempts launch different kernels, so a
+        captured attempt of the other kind is dropped."""
+        self.grid = self._next_grid
+        if (self.grid is not None) != self._graph_grid:
+            self._drop_graph()
+            self._graph_grid = self.grid is not None
+            loop = False
+        return super()._begin(y0_flat, t64, t_start, loop)
 
     def _rows_sumsq(self, x, x2, out):
         self._launch(self.lib.tdq_rows_sumsq(
@@ -1019,15 +1049,18 @@ class RowsEngine(AdaptiveEngine):
             self.rtol_vec.data_ptr() if self.rtol_vec is not None else None,
             self.atol_vec.data_ptr() if self.atol_vec is not None else None,
             B, D, self.row_partials.data_ptr(), self.row_norm.data_ptr(), st))
+        grid = self.grid is not None                 # the per-row-table kernels read each row's own times
         if self.ev_fn is None:
-            self._launch(lib.tdq_rows_controller(ctrl, rows, dc, self.row_norm.data_ptr(), B, D, st))
+            controller = lib.tdq_rows_controller_grid if grid else lib.tdq_rows_controller
+            self._launch(controller(ctrl, rows, dc, self.row_norm.data_ptr(), B, D, st))
         else:
             # each row's event value at its candidate (ATT_T1, y1), then the controller with the sign test inside it
             torch.mul(self.row_field(_lib.ROWS_ATT_T1, torch.float64), self.opt.t_sign, out=self.ev_t)
             self._ev_call(self.y1)
-            self._launch(lib.tdq_rows_controller_event(ctrl, rows, dc, self.row_norm.data_ptr(), self.ev_val.data_ptr(),
-                                                       self.ev_init.data_ptr(), self.ev_sign0.data_ptr(),
-                                                       self.ev_flag.data_ptr(), B, D, self.K, st))
+            controller = lib.tdq_rows_controller_event_grid if grid else lib.tdq_rows_controller_event
+            self._launch(controller(ctrl, rows, dc, self.row_norm.data_ptr(), self.ev_val.data_ptr(),
+                                    self.ev_init.data_ptr(), self.ev_sign0.data_ptr(), self.ev_flag.data_ptr(), B, D,
+                                    self.K, st))
         return k, kp, keep
 
     def _attempt_back(self, kp):
@@ -1036,9 +1069,9 @@ class RowsEngine(AdaptiveEngine):
                                                      self.dt_code, self.y1.data_ptr(), kp, self.ev_flag.data_ptr(),
                                                      self.ev_coeff.data_ptr(), self.B, self.D, _stream()))
             return
-        self._launch(self.lib.tdq_rows_fit_eval(self.ctrl.data_ptr(), self.rows.data_ptr(), C.byref(self.tab),
-                                                self.dt_code, self.y1.data_ptr(), kp, self.solution.data_ptr(),
-                                                self.B, self.D, _stream()))
+        fit_eval = self.lib.tdq_rows_fit_eval_grid if self.grid is not None else self.lib.tdq_rows_fit_eval
+        self._launch(fit_eval(self.ctrl.data_ptr(), self.rows.data_ptr(), C.byref(self.tab), self.dt_code,
+                              self.y1.data_ptr(), kp, self.solution.data_ptr(), self.B, self.D, _stream()))
 
     # ---- per-row events (rk_common.py:252-262, event_handling.py:5-35) ------------------------------------------------
     def _ev_call(self, y_flat):
@@ -1051,8 +1084,9 @@ class RowsEngine(AdaptiveEngine):
                              "[B, K...] with B = %d and K = %d" % (tuple(getattr(v, "shape", ())), self.B, self.K))
         self.ev_val.copy_(v.reshape(self.B, self.K))
 
-    def solve_until_event(self, y0_flat, t_start, ev, ev0, tol):
-        """Row r integrates from t_start until the sign of its combined event value changes, then bisects on the
+    def solve_until_event(self, y0_flat, t_start, ev, ev0, tol, t_starts=None):
+        """Row r integrates from t_start (or t_starts[r], a float64 [B] device tensor in ascending solver time) until the
+        sign of its combined event value changes, then bisects on the
         interpolant of its last step: the reference's odeint_event on y0[r:r+1] alone.  ev(t, y): t is a float64 tensor
         [B, 1, ...] of each row's time in the caller's direction, y the [B, *rest] state.  ev0 = ev(t_start, y0), already
         evaluated (shape [B, K...]); tol: float64 [B] CPU tensor, each row's bisection tolerance.  The stepping phase runs
@@ -1072,13 +1106,15 @@ class RowsEngine(AdaptiveEngine):
         self.ev_nitrs = torch.zeros(B, dtype=torch.int32, device=dev)
         self.ev_coeff = torch.zeros(5, self.n, dtype=self.dtype, device=dev)
         sign = self.opt.t_sign
-        self.ev_t = torch.full((B,), t_start * sign, **f64)
+        self.ev_t = torch.full((B,), t_start * sign, **f64) if t_starts is None else t_starts * sign
         self.ev_t_view = self.ev_t.view(B, *([1] * len(self.row_shape)))
         self.ev_event_t = torch.zeros(B, **f64)
         self.ev_val.copy_(ev0.reshape(B, K))
         self.n_ev = 1                                          # ev0
-        t64 = torch.tensor([t_start, float("inf")], **f64)     # the cursor never completes a row
-        self.solve(y0_flat, t64, t_start)
+        # the cursor never completes a row: output times [t0, inf], one row of them per row with per-row starts
+        t64 = torch.tensor([t_start, float("inf")], **f64)
+        grid = None if t_starts is None else torch.stack([t_starts, torch.full_like(t_starts, float("inf"))], dim=1)
+        self.solve(y0_flat, t64, t_start, grid=grid)
         # nitrs from each row's last step, on the host as the reference computes it (one copy of 2 B doubles)
         o0, o1 = self.lib.tdq_rows_offset(_lib.ROWS_T0, B), self.lib.tdq_rows_offset(_lib.ROWS_T1, B)
         tt = self.rows[o0:o1 + 8 * B].view(torch.float64).cpu()
@@ -1100,7 +1136,10 @@ class RowsEngine(AdaptiveEngine):
         """rk_common.py:213-241 for every row: f0 on the whole batch, then each row's initial step."""
         lib, st = self.lib, _stream()
         ctrl, rows, dc, B, D = self.ctrl.data_ptr(), self.rows.data_ptr(), self.dt_code, self.B, self.D
-        self._launch(lib.tdq_rows_init(ctrl, rows, dc, B, t_start, st))
+        if self.grid is not None:                                   # each row from its own grid[r, 0]
+            self._launch(lib.tdq_rows_init_grid(ctrl, rows, dc, B, self.grid.data_ptr(), n_out, st))
+        else:
+            self._launch(lib.tdq_rows_init(ctrl, rows, dc, B, t_start, st))
         f0 = self._call_fn(self.t_first, self.ybuf[0], 0, dst=self.kbuf[0])
         if f0.data_ptr() != self.kbuf[0].data_ptr():
             self.kbuf[0].copy_(f0)

@@ -132,6 +132,7 @@ _SIGNATURES = {
     "tdq_rows_offset": (_sz, [_i32, _sz]),
     "tdq_rows_partials_len": (_sz, [_sz, _sz]),
     "tdq_rows_init": (C.c_int, [_vp, _vp, _i32, _sz, _dbl, _vp]),
+    "tdq_rows_init_grid": (C.c_int, [_vp, _vp, _i32, _sz, _vp, _i32, _vp]),
     "tdq_rows_sumsq": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _sz, _sz, _vp, _vp, _vp]),
     "tdq_rows_initial_h0": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _sz, _sz, _vp]),
     "tdq_rows_initial_probe": (C.c_int, [_vp, _vp, _i32, _vp, _sz, _sz, _vp]),
@@ -142,9 +143,12 @@ _SIGNATURES = {
     "tdq_rows_combine_final": (C.c_int, [_vp, _vp, _ptab, _i32, _vp, _vp, _pp, _sz, _sz, _vp]),
     "tdq_rows_error_norm_commit": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _vp, _vp, _vp]),
     "tdq_rows_controller": (C.c_int, [_vp, _vp, _i32, _vp, _sz, _sz, _vp]),
+    "tdq_rows_controller_grid": (C.c_int, [_vp, _vp, _i32, _vp, _sz, _sz, _vp]),
     "tdq_rows_fit_eval": (C.c_int, [_vp, _vp, _ptab, _i32, _vp, _pp, _vp, _sz, _sz, _vp]),
+    "tdq_rows_fit_eval_grid": (C.c_int, [_vp, _vp, _ptab, _i32, _vp, _pp, _vp, _sz, _sz, _vp]),
     "tdq_rows_event_init": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _sz, _i32, _vp]),
     "tdq_rows_controller_event": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _i32, _vp]),
+    "tdq_rows_controller_event_grid": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _i32, _vp]),
     "tdq_rows_fit_store": (C.c_int, [_vp, _vp, _ptab, _i32, _vp, _pp, _vp, _vp, _sz, _sz, _vp]),
     "tdq_rows_event_bisect": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                         _sz, _sz, _i32, _vp]),

@@ -67,6 +67,9 @@ struct TdqCtrl {
     // ---- state-dtype scalars torch views alias (func's time argument) ----------------------
     alignas(16) unsigned char tstage[8 * TDQ_MAX_K];
     alignas(16) unsigned char taux[8 * 4];
+    // ---- independent rows: per-row output times (tdq_rows_init_grid), cleared by tdq_ctrl_init and tdq_rows_init ----
+    const double *row_t;                     // [B, row_n] float64, row r ascending, or NULL: every row reads t_out
+    int32_t row_n, row_pad;
 };
 
 // Exchange buffer of one rank.  Four slots: (solve epoch parity, attempt parity).  Within a solve a rank can be at

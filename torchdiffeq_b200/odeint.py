@@ -103,6 +103,39 @@ def _check_timelike(name, timelike, can_grad, values=None):                     
     assert diff.all() or (~diff).all(), '{} must be strictly increasing or decreasing'.format(name)
 
 
+def check_row_shape(t, B):
+    """A 2-D t with options={'independent_rows': True} must have one row of times per batch row."""
+    if t.dim() != 2 or B is None or t.shape[0] != B:
+        raise ValueError("options['independent_rows'] with per-row output times needs t of shape [B, T] with B = "
+                         "y0.shape[0] = %s, got %s" % (B, tuple(t.shape)))
+
+
+def check_row_times(t, t_cpu, B):
+    """Per-row output times t [B, T] (options={'independent_rows': True}) from their host copy t_cpu: the reference's checks
+    and conversions of a 1-D t (misc.py:110-112, :270-296) applied to every row, with ` (row r)` added to its messages.
+    All rows must run in the same direction (a row with T == 1 has none).  Returns (t_sign, the rows in ascending solver
+    time)."""
+    if not torch.is_floating_point(t):                                                 # misc.py:110-112
+        raise TypeError('`t` must be a floating point Tensor but is a {}'.format(t.type()))
+    check_row_shape(t, B)
+    if t_cpu.shape[1] == 0:
+        raise ValueError("options['independent_rows'] with per-row output times needs at least one time per row")
+    msg = 't must be strictly increasing or decreasing (row {})'
+    diff = t_cpu[:, 1:] > t_cpu[:, :-1]                                                # misc.py:373 row by row
+    bad = (~(diff.all(dim=1) | (~diff).all(dim=1))).nonzero().view(-1)
+    assert bad.numel() == 0, msg.format(int(bad[0]))
+    if t_cpu.shape[1] == 1:
+        return 1.0, t_cpu
+    rev = t_cpu[:, 0] > t_cpu[:, 1]                                                    # misc.py:270-271 row by row
+    t_asc = torch.where(rev[:, None], -t_cpu, t_cpu)
+    bad = (~(t_asc[:, 1:] > t_asc[:, :-1]).all(dim=1)).nonzero().view(-1)              # misc.py:296 row by row
+    assert bad.numel() == 0, msg.format(int(bad[0]))
+    if bool(rev.any()) and not bool(rev.all()):
+        raise ValueError("options['independent_rows']: every row of t must run in the same direction, but row %d increases "
+                         "and row %d decreases" % (int((~rev).nonzero()[0]), int(rev.nonzero()[0])))
+    return (-1.0 if bool(rev[0]) else 1.0), t_asc
+
+
 def _tol_vector(name, tol, layout, shape, device):
     """Scalar tolerance -> (float, None).  Tuple of tolerances for a tuple state (misc.py:115-123
     _tuple_tol) or a tensor broadcastable to a tensor state -> (None, per-element float64 vector), the
@@ -159,17 +192,7 @@ def normalise(func, y0, t, rtol, atol, method, options, event_fn, adjoint=False)
     _lib.load()                                   # fail loudly, before any work, if libtdq.so is missing
 
     t_cpu = t.detach().to("cpu") if isinstance(t, torch.Tensor) else t                 # the one host read of t
-    _check_timelike('t', t, True, values=t_cpu)
-    t_reversed = bool(len(t_cpu) > 1 and t_cpu[0] > t_cpu[1])                          # misc.py:270-271
-    t_sign = -1.0 if t_reversed else 1.0
-    if t_reversed:
-        t_cpu = -t_cpu                                                                 # ascending from here on
-        for name in ("step_t", "jump_t"):                                              # misc.py:292-293
-            if isinstance(options.get(name), torch.Tensor):
-                options[name] = -options[name]
-        if "grid_constructor" in options:
-            options["grid_constructor"] = signed_grid_constructor(options["grid_constructor"], t_sign)
-    assert (t_cpu[1:] > t_cpu[:-1]).all(), 't must be strictly increasing or decreasing'   # misc.py:296
+    t_sign, t_cpu = normalise_times(t, t_cpu, options, shape[0] if shape else None)
 
     if torch.is_tensor(rtol):                                                          # misc.py:299-302
         assert not rtol.requires_grad, "rtol cannot require gradient"
@@ -213,6 +236,26 @@ def normalise(func, y0, t, rtol, atol, method, options, event_fn, adjoint=False)
                    t_cpu=t_cpu, y0_flat=y0_flat, callbacks=callbacks, is_tuple=is_tuple, layout=layout, shape=shape,
                    segs=segs, pieces=pieces, norm_fn=norm_fn, q_view=unflat if norm_fn is not None else None,
                    event_fn=flat_event_fn)
+
+
+def normalise_times(t, t_cpu, options, B):
+    """The checks and conversions of t (misc.py:270-296) from its host copy t_cpu: returns (t_sign, the output times in
+    ascending solver time).  With options['independent_rows'] a 2-D t holds per-row times [B, T] (check_row_times);
+    otherwise t must be 1-D, and reversed time also negates options' step_t / jump_t and wraps its grid_constructor."""
+    if options.get("independent_rows") and isinstance(t, torch.Tensor) and t.dim() == 2:
+        return check_row_times(t, t_cpu, B)
+    _check_timelike('t', t, True, values=t_cpu)
+    t_reversed = bool(len(t_cpu) > 1 and t_cpu[0] > t_cpu[1])                          # misc.py:270-271
+    t_sign = -1.0 if t_reversed else 1.0
+    if t_reversed:
+        t_cpu = -t_cpu                                                                 # ascending from here on
+        for name in ("step_t", "jump_t"):                                              # misc.py:292-293
+            if isinstance(options.get(name), torch.Tensor):
+                options[name] = -options[name]
+        if "grid_constructor" in options:
+            options["grid_constructor"] = signed_grid_constructor(options["grid_constructor"], t_sign)
+    assert (t_cpu[1:] > t_cpu[:-1]).all(), 't must be strictly increasing or decreasing'   # misc.py:296
+    return t_sign, t_cpu
 
 
 def valid_callbacks(method, callbacks):
@@ -352,10 +395,19 @@ def _check_independent_rows(func, y0, t, method, options, event_fn):
         return None
     # event_fn(t, y) is called with t a float64 [B, 1, ...] tensor of each row's time and must give one value, or K,
     # per row; this first call at t0 also starts the solve
-    if len(t) != 2:                                                                    # misc.py:203-204
-        raise ValueError(f"We require len(t) == 2 when in event handling mode, but got len(t)={len(t)}.")
     B = y0.shape[0]
-    t0 = torch.full((B,) + (1,) * (y0.dim() - 1), float(t[0]), dtype=torch.float64, device=y0.device)
+    tshape = (B,) + (1,) * (y0.dim() - 1)
+    if isinstance(t, torch.Tensor) and t.dim() == 2:                                   # per-row start times t[:, 0]
+        check_row_shape(t, B)
+        if t.shape[1] != 2:
+            raise ValueError(f"We require t.shape[1] == 2 when in event handling mode with per-row times, but got "
+                             f"t.shape[1]={t.shape[1]}.")
+        check_row_times(t, t.detach().to("cpu"), B)       # a refused table runs no user code (normalise checks it again)
+        t0 = t[:, 0].detach().to(device=y0.device, dtype=torch.float64, copy=True).view(tshape)
+    else:
+        if len(t) != 2:                                                                # misc.py:203-204
+            raise ValueError(f"We require len(t) == 2 when in event handling mode, but got len(t)={len(t)}.")
+        t0 = torch.full(tshape, float(t[0]), dtype=torch.float64, device=y0.device)
     with torch.no_grad():
         v = event_fn(t0, y0)
     if not isinstance(v, torch.Tensor) or v.dim() == 0:
@@ -380,8 +432,10 @@ def _solve_rows_event(p, event_fn, ev0):
         tol = p.atol_vec.view(B, -1).min(dim=1).values.cpu()
     else:
         tol = torch.full((B,), float(p.atol), dtype=torch.float64)
-    event_t, sol = eng.solve_until_event(p.y0_flat, float(p.t_cpu[0]), lambda t_, y_: event_fn(t_, y_.view(shape)), ev0,
-                                         tol)
+    t0 = p.t_cpu[..., 0]                                  # [B]: each row's own start (per-row times), or one start
+    t_starts = t0.to(torch.float64).to(p.device) if t0.dim() == 1 else None
+    event_t, sol = eng.solve_until_event(p.y0_flat, float(t0.view(-1)[0]), lambda t_, y_: event_fn(t_, y_.view(shape)),
+                                         ev0, tol, t_starts=t_starts)
     return event_t, sol, eng
 
 
@@ -531,7 +585,8 @@ def last_stats():
 def _solve(p):
     """Run the normalised problem; returns the flat solution [len(t), n] and the engine."""
     if p.method in ADAPTIVE_METHODS:
-        key = _cache_key(p)
+        row_grid = p.t_cpu.dim() == 2                   # per-row output times (independent rows): data, not part of the key
+        key = _cache_key(p, extra=("row_grid",) if row_grid else ())
         hit = _cache_get(key)
         if hit is not None:
             eng = hit[0]
@@ -540,7 +595,10 @@ def _solve(p):
             _cache_put(key, (eng, p.original_func))     # the func reference keeps id(func) from being recycled
         t64 = p.t_cpu.to(torch.float64).to(p.device)                                   # solvers.py:31
         try:
-            sol = eng.solve(p.y0_flat, t64, t_start=float(p.t_cpu[0]))
+            if row_grid:
+                sol = eng.solve(p.y0_flat, None, t_start=float(p.t_cpu[0, 0]), grid=t64)
+            else:
+                sol = eng.solve(p.y0_flat, t64, t_start=float(p.t_cpu[0]))
         except BaseException:
             _cache_drop(key)                            # a half-finished engine is never reused
             raise
@@ -655,11 +713,15 @@ def odeint_event(func, y0, t0, *, event_fn, reverse_time=False, odeint_interface
     Pass odeint_interface=odeint_adjoint for gradients with respect to func's parameters and y0."""
     if odeint_interface is None:
         odeint_interface = odeint
-    if reverse_time:
+    rows = bool((kwargs.get("options") or {}).get("independent_rows"))
+    if rows and torch.is_tensor(t0) and t0.dim() == 1 and t0.numel() > 1:
+        # one start time per row: t of shape [B, 2], row r from t0[r]
+        t = torch.stack([t0, t0.detach() - 1.0 if reverse_time else t0.detach() + 1.0], dim=1)
+    elif reverse_time:
         t = torch.cat([t0.reshape(-1), t0.reshape(-1).detach() - 1.0])
     else:
         t = torch.cat([t0.reshape(-1), t0.reshape(-1).detach() + 1.0])
-    if (kwargs.get("options") or {}).get("independent_rows"):
+    if rows:
         # one event time per row: the implicit-function rerouting below assumes one scalar event time, and this mode
         # refuses gradients anyway
         return odeint_interface(func, y0, t, event_fn=event_fn, **kwargs)
@@ -800,8 +862,16 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
     dtype) holding each row's time, so `t * y` and `torch.sin(t) + y` broadcast row by row.  last_stats() then also has
     row_n_accept / row_n_reject (CPU int64 tensors of shape [B]).
 
+    With independent rows t may also be a [B, T] tensor of per-row output times: row r is integrated from t[r, 0] over its
+    own times to t[r, T-1], solution[j, r] is its state at t[r, j], and row r's result is the reference's
+    odeint(func, y0[r:r+1], t[r]).  Each row must be strictly increasing or strictly decreasing (the reference's check,
+    failing with the row named) and all rows must run in the same direction (ValueError otherwise); max_num_steps counts
+    per interval of the row's own times.  Every row still needs the same T.  func is called on the whole batch until the
+    last row ends: rows that ended early see copies of their last state.
+
     With independent rows, event_fn (and odeint_event) finds each row's own event: row r's (event_t[r], solution[:, r])
     is the reference's odeint_event(func, y0[r:r+1], t[0], event_fn) for the event function restricted to that row.
+    Per-row start times: t of shape [B, 2] (row r from t[r, 0]), or odeint_event with t0 of shape [B].
     event_fn(t, y) gets t as a float64 [B, 1, ..., 1] tensor of each row's time (caller's direction) and returns [B] or
     [B, K...] (K components per row, combined per row as the reference combines them).  It is called on the whole batch:
     once at t[0], once per attempt and once per bisection iteration; values of rows that did not accept, or are done, are
