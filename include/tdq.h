@@ -46,7 +46,8 @@ typedef enum {
     TDQ_RUN_DT_UNDERFLOW = 1,   /* rk_common.py:286  assert t0 + dt > t0                          */
     TDQ_RUN_NONFINITE = 2,      /* rk_common.py:287  assert isfinite(y0).all()                     */
     TDQ_RUN_MAX_STEPS = 3,      /* rk_common.py:247  assert n_steps < max_num_steps                */
-    TDQ_RUN_EXCHANGE_TIMEOUT = 4 /* a peer rank never delivered its norm partials (sharded solves)  */
+    TDQ_RUN_EXCHANGE_TIMEOUT = 4, /* a peer rank never delivered its norm partials (sharded solves) */
+    TDQ_RUN_BARRIER_TIMEOUT = 5 /* a CTA of tdq_linear_solve missed a grid barrier by 10 s          */
 } tdq_run_status;
 
 /* Butcher tableau of an explicit embedded RK method, float64 as in the reference
@@ -349,6 +350,23 @@ int tdq_linear_attempt_supported(const tdq_tableau *tab, int32_t dtype, int32_t 
 int tdq_linear_attempt(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, void *const *k_out, void *y1_out, void *err_out,
                        const void *y0, const void *k0, const void *planes, int32_t width, size_t n, double *partials,
                        double *norm_out, const int64_t *seg_counts_dev, int32_t store_always, void *stream);
+
+/* ---- A WHOLE fused solve in one launch (tdq_attempt.cu) ---------------------------------------------------------------------
+ * Every attempt of a solve whose attempts tdq_linear_attempt can run with the norm folded in (partials given, scalar tolerances,
+ * one segment), with the controller step and the lazy interpolant fit in between: what the loop
+ *   tdq_linear_attempt(..., partials, norm_out, NULL, 0) ; tdq_controller(ctrl, dtype, norm_out, seg_counts_dev, 1, NULL) ;
+ *   tdq_interp_fit_eval(ctrl, tab, dtype, y1_out, k, NULL, solution, n)     (k[0] = NULL, k[i] = k_out[i])
+ * does until the solve ends, bit for bit, in one cooperative launch whose CTAs stay resident (k_linear_solve).  Call it after
+ * tdq_prepare_attempt, as that loop's first attempt.  The mailbox is written once, by the attempt that ends the solve (seq = the
+ * number of attempts, as inside the device-side loop); the control block must not keep every step (always_fit).
+ * scratch: tdq_linear_solve_scratch_len() doubles, engine-owned, not shared with a concurrent solve; its barrier words are
+ * reset before the launch.  TDQ_ERR_UNSUPPORTED, with nothing launched, when the device refuses the cooperative launch or
+ * a buffer is not 16-byte aligned: the caller then runs the loop above.  A CTA that misses a grid barrier by 10 s ends the
+ * solve with TDQ_RUN_BARRIER_TIMEOUT. */
+size_t tdq_linear_solve_scratch_len(void);
+int tdq_linear_solve(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, void *const *k_out, void *y1_out, void *err_out,
+                     const void *planes, int32_t width, size_t n, double *scratch, size_t scratch_len,
+                     const int64_t *seg_counts_dev, void *solution, void *stream);
 
 /* interp='cubic' (solvers.py:120-125, :166-173): for records r in [rec_lo, rec_hi) of one step
  * solution[out_idx[r]] = h00*y0 + (h10*dt)*f0 + h01*y1 + (h11*dt)*f1 with the four weights of record r at

@@ -293,6 +293,8 @@ class AdaptiveEngine:
         self._loop = None                # tdq_loop handle: the captured attempt inside a device-side while
         self._loop_handle = 0
         self._loop_failed = False
+        self._solve_scratch = None       # tdq_linear_solve's barrier words and partials (engine-owned)
+        self._solve_refused = False      # the device refused its cooperative launch: attempts take the loop below
         self._always_copy = False        # set when func is seen to reuse its output buffer (see _call_fn)
         self.linear = None               # set_linear(): every stage fused with a linear field (csrc/tdq_linear.cu)
         self.capture_in_solve = True     # False: only a prime()d graph is used (solves run inside autograd backward)
@@ -546,6 +548,8 @@ class AdaptiveEngine:
             raise SolverFailure("non-finite values in state `y`: {}".format(y) + where)
         if s == _lib.RUN_EXCHANGE_TIMEOUT:
             raise _lib.TdqError("a peer rank did not deliver its norm partials within 10 s (sharded solve)")
+        if s == _lib.RUN_BARRIER_TIMEOUT:
+            raise _lib.TdqError("a block of the persistent linear solve missed a grid barrier by 10 s")
         if s == _lib.RUN_MAX_STEPS:
             m = self.opt.max_num_steps
             raise SolverFailure("max_num_steps exceeded ({}>={})".format(m, m) + where)
@@ -793,6 +797,8 @@ class AdaptiveEngine:
 
     # ---- bounded run-ahead: no host sync, optional CUDA graph -----------------------------------
     def _loop_run_ahead(self):
+        if self._linear_solve_ready() and self._linear_solve():
+            return
         D = max(1, self.run_ahead)
         mb = self.mbox_host.contents
         issued = 0
@@ -845,6 +851,38 @@ class AdaptiveEngine:
         mb = self._wait_seq(issued)
         self._raise_if_failed(mb)
         torch.cuda.current_stream().synchronize()
+
+    persistent_linear = True             # RowsEngine: per-row control blocks, no persistent solve
+
+    def _linear_solve_ready(self):
+        """Can this solve's attempts run as ONE persistent launch (tdq_linear_solve)?  Whole-attempt linear field with the
+        norm folded in, and a solve the device loop would run: no host work between attempts and no stored interpolants."""
+        L = self.linear
+        return (L is not None and L["whole"] and L["fold"] and self.persistent_linear and not self._solve_refused
+                and self.device_loop in (True, "auto") and not self._lockstep_mode() and self.agree_fn is None
+                and self.norm_fn is None and self.exchange is None and not self.keep_interp)
+
+    def _linear_solve(self):
+        """Every attempt of the solve in one cooperative launch (csrc/tdq_attempt.cu k_linear_solve): the attempt, the
+        controller step and the lazy fit, until the solve ends.  False (nothing launched) if the device refuses the launch."""
+        lib, L = self.lib, self.linear
+        if self._solve_scratch is None:
+            self._solve_scratch = torch.zeros(int(lib.tdq_linear_solve_scratch_len()), dtype=torch.float64,
+                                              device=self.device)
+        k = [None] + [L["k"][i].data_ptr() for i in range(self.S)]
+        rc = lib.tdq_linear_solve(self.ctrl.data_ptr(), C.byref(self.tab), self.dt_code, _lib.ptr_array(k),
+                                  self.y1.data_ptr(), self.errp.data_ptr(), L["planes"].data_ptr(), L["width"], self.n,
+                                  self._solve_scratch.data_ptr(), self._solve_scratch.numel(), self.seg_counts.data_ptr(),
+                                  self.solution.data_ptr(), _stream())
+        if rc == _lib.TDQ_ERR_UNSUPPORTED:
+            self._solve_refused = True
+            return False
+        self._launch(rc)
+        torch.cuda.current_stream().synchronize()
+        mb = self.mbox_host.contents
+        self.nfe += self.S * int(mb.seq)
+        self._raise_if_failed(mb)
+        return True
 
     def _launch_loop(self, first=0):
         _lib.check(self.lib.tdq_loop_launch(self._loop, _stream()))
@@ -959,6 +997,8 @@ class RowsEngine(AdaptiveEngine):
     (csrc/tdq_rows.cu).  func is still called on the whole batch, with t a tensor of shape [B, 1, ...] holding each row's
     time; finished rows see copies of their last state.  Stage slots, capture, the device-side loop and the run-ahead and
     lock-step drivers are AdaptiveEngine's; only the launches differ."""
+
+    persistent_linear = False
 
     def __init__(self, fn, shape, dtype, device, method, **kw):
         shape = torch.Size(shape)

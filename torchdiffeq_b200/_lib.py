@@ -10,7 +10,8 @@ TDQ_MAX_STAGES = 16
 TDQ_MAX_K = TDQ_MAX_STAGES + 1
 TDQ_MAX_SEGS = 64
 TDQ_F32, TDQ_F64 = 0, 1
-RUN_OK, RUN_DT_UNDERFLOW, RUN_NONFINITE, RUN_MAX_STEPS, RUN_EXCHANGE_TIMEOUT = 0, 1, 2, 3, 4
+TDQ_ERR_UNSUPPORTED = 3
+RUN_OK, RUN_DT_UNDERFLOW, RUN_NONFINITE, RUN_MAX_STEPS, RUN_EXCHANGE_TIMEOUT, RUN_BARRIER_TIMEOUT = 0, 1, 2, 3, 4, 5
 TDQ_MAX_RANKS = 16
 # tdq_rows_field (include/tdq.h)
 (ROWS_T0, ROWS_T1, ROWS_DT, ROWS_RATIO, ROWS_ATT_T0, ROWS_ATT_DT, ROWS_ATT_T1, ROWS_FIT_DT, ROWS_H0, ROWS_D1, ROWS_PAR,
@@ -120,6 +121,8 @@ _SIGNATURES = {
     "tdq_linear_stage": (C.c_int, [_vp, _ptab, _i32, _i32, _vp, _vp, _vp, _vp, _pp, _vp, _i32, _sz, _vp]),
     "tdq_linear_attempt_supported": (C.c_int, [_ptab, _i32, _i32]),
     "tdq_linear_attempt": (C.c_int, [_vp, _ptab, _i32, _pp, _vp, _vp, _vp, _vp, _vp, _i32, _sz, _vp, _vp, _vp, _i32, _vp]),
+    "tdq_linear_solve_scratch_len": (_sz, []),
+    "tdq_linear_solve": (C.c_int, [_vp, _ptab, _i32, _pp, _vp, _vp, _vp, _i32, _sz, _vp, _sz, _vp, _vp, _vp]),
     "tdq_fixed_emit_cubic": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _sz, _vp]),
     "tdq_pack_segments": (C.c_int, [_i32, _vp, _pp, _pi64, _pi64, _pdbl, _i32, _vp]),
     "tdq_implicit_partials_len": (_sz, [_i32]),

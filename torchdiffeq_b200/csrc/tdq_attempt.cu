@@ -26,12 +26,15 @@
 // fence.proxy.async, bar.sync (all 256 threads: the product needs both halves), 48 wgmma + commits per warpgroup; while they
 // run, the prefix of the next row's sum; then wgmma.wait and k_{i+1} = small + big.  The chain of a tile is serial by nature
 // (stage i+1 needs k_i).  The last block to finish adds the per-block partials of the squared error norm; the controller
-// step is the next launch (tdq_controller, tdq_ctrl.cu).
+// step is the next launch (tdq_controller, tdq_ctrl.cu).  k_linear_solve, at the end of this file, runs the same tile code
+// for every attempt of a solve in one resident launch, with the controller step and the fit in between.
 //
 // Stage derivatives, y1 and the error prefix are written to HBM only for attempts that can contain an output time (the
 // lazy interpolant fit needs them, tdq_interp.cu) or when the caller keeps every step (dense output, events).
 #include "tdq_shape.cuh"
 #include "tdq_tc.cuh"
+#include "tdq_ctrl_step.cuh"
+#include "tdq_fit.cuh"
 
 #include <cstddef>
 #include <type_traits>
@@ -76,44 +79,43 @@ struct AttOut {
     float *y1, *err;
 };
 
-// S: stages of an FSAL tableau (rows 0..S-1, the last one is c_sol and yields y1).  RM: 8 bits per row, bit j set <=> slot j has
-// a non-zero coefficient in that row.  EM: the same for the error weights of slots 0..S-1 (k_S always carries the last one).
-template <int S, unsigned long long RM, unsigned EM>
-__global__ void __launch_bounds__(AT_THREADS, 1)
-k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const uint32_t *__restrict__ wt,
-                 double *partials, double *norm_out, int store_always, size_t n_rows_sz) {
-    if (c->halt) return;                                  // an attempt issued after the end of the solve is a no-op
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
-    uint8_t *aux = smem + W_BYTES + AT_STAGE + AT_Y0;
-    int *s_flag = reinterpret_cast<int *>(aux);
-    // per-attempt pointers and tolerances, read where they are used rather than held in registers through the tile loop
-    struct Scalars {
-        const float *y0, *k0;
-        float *ycand, *kcand;                                             // candidate commit (nullptr: none)
-        AttOut out;
-        float rtol, atol;
-    };
-    Scalars *s_sc = reinterpret_cast<Scalars *>(aux + 320);
-    static_assert(320 + sizeof(Scalars) <= 512, "aux layout");
-    // this attempt's coefficients (prepare_tables) as float32, laid out by slot: the coefficient of k_j in row i at
-    // s_cr[8 i + j], the error weight of k_j at s_ce[j] (j = 0..S), zero where the tableau has none.  Every index the tile
-    // loop uses is then a compile-time constant of RM / EM: each block loads the few it needs once, with a 32-bit
-    // ld.shared (coef()), instead of finding the ordinal of a slot at run time for every element.
-    float *s_cr = reinterpret_cast<float *>(aux + 64);                    // [AT_MAX_S][8]
-    float *s_ce = s_cr + AT_MAX_S * 8;                                    // [8]
-    double *s_red = reinterpret_cast<double *>(aux + 512);                // [2][32]
-    const int tid = threadIdx.x, lane = tid & 31;
-    const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);                  // warp-uniform for the compiler as well
-    const int n_rows = (int)n_rows_sz;
+// per-attempt pointers and tolerances, read where they are used rather than held in registers through the tile loop
+struct Scalars {
+    const float *y0, *k0;
+    float *ycand, *kcand;                                             // candidate commit (nullptr: none)
+    AttOut out;
+    float rtol, atol;
+};
 
+// The auxiliary shared-memory area (AT_AUX bytes after the tile's y0)
+constexpr int AUX_CR = 64;                     // float s_cr[AT_MAX_S][8], s_ce[8]: this attempt's coefficients
+constexpr int AUX_SC = 320;                    // Scalars
+constexpr int AUX_RED = 512;                   // double [2][32]: reduction scratch
+constexpr int AUX_SOLVE = 1024;                // k_linear_solve's words (SolveAux)
+static_assert(AUX_SC + sizeof(Scalars) <= AUX_RED, "aux layout");
+
+__device__ __forceinline__ uint8_t *at_smem() {
+    extern __shared__ uint8_t smem_raw[];
+    return reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
+}
+__device__ __forceinline__ uint8_t *at_aux(uint8_t *smem) { return smem + W_BYTES + AT_STAGE + AT_Y0; }
+
+// This attempt's coefficients (prepare_tables) as float32, laid out by slot: the coefficient of k_j in row i at s_cr[8 i + j],
+// the error weight of k_j at s_ce[j] (j = 0..S), zero where the tableau has none.  Every index the tile loop uses is then a
+// compile-time constant of RM / EM: each block loads the few it needs once, with a 32-bit ld.shared (coef()), instead of
+// finding the ordinal of a slot at run time for every element.  Then the attempt's pointers and tolerances (thread 0).
+// The caller synchronises the block before the tiles read them.
+template <int S, unsigned long long RM, unsigned EM>
+__device__ __forceinline__ void attempt_prologue(const TdqCtrl *c, const float *y0, const float *k0, const AttOut &out,
+                                                 bool fold, size_t n_rows_sz, uint8_t *aux, int tid) {
+    float *s_cr = reinterpret_cast<float *>(aux + AUX_CR);              // [AT_MAX_S][8]
+    float *s_ce = s_cr + AT_MAX_S * 8;                                    // [8]
     if (tid < AT_MAX_S * 8) {
         const int i = tid >> 3, j = tid & 7;
         const unsigned mask = i < S ? (unsigned)((RM >> (8 * i)) & 0xffull) : 0u, below = (1u << j) - 1u;
         s_cr[i * 8 + j] = ((mask >> j) & 1u) ? (float)c->coef[i][__popc(mask & below)] : 0.f;
         if (i == 0) s_ce[j] = j == S ? (float)c->ecoef[__popc(EM)] : ((EM >> j) & 1u) ? (float)c->ecoef[__popc(EM & below)] : 0.f;
     }
-    const bool fold = partials != nullptr;                                // squared error norm + candidate commit in here
     if (tid == 0) {
         Scalars sc;
         sc.y0 = tdq_detach(y0 != nullptr ? y0 : reinterpret_cast<const float *>(c->y0_cur), n_rows_sz);
@@ -126,33 +128,27 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
         sc.out = out;
         sc.rtol = (float)c->rtol;
         sc.atol = (float)c->atol;
-        *s_sc = sc;
+        *reinterpret_cast<Scalars *>(aux + AUX_SC) = sc;
     }
-    load_weights(smem, wt, tid, AT_THREADS);
-    fence_async_smem();
-    __syncthreads();
+}
 
-    // ---- per-attempt scalars ---------------------------------------------------------------------------------
-    // the stages of this attempt are needed afterwards only if an output time can fall into it (the controller's
-    // test `!(t_out[cursor] > t1)` for t1 = att_t1, rk_common.py:246) or the caller keeps every step
+// the stages of this attempt are needed afterwards only if an output time can fall into it (the controller's test
+// `!(t_out[cursor] > t1)` for t1 = att_t1, rk_common.py:246) or the caller keeps every step
+__device__ __forceinline__ bool attempt_store(const TdqCtrl *c, int store_always) {
     bool store = store_always != 0 || c->always_fit != 0;
     if (!store) {
         const int cur = c->out_cursor;
         store = cur < c->n_out && !(c->t_out[cur] > c->att_t1);
     }
-    // h = the warpgroup's half of the output features; w = warp inside the warpgroup
+    return store;
+}
+
+// the hi weight plane of the warpgroup's features as the register A operand of every hi.* product (k-step ks: ahi[ks]);
+// the weight image is in shared memory and the block has synchronised since
+__device__ __forceinline__ void load_ahi(uint32_t (&ahi)[LD / 16][4], const uint8_t *smem) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int h = warp >> 2, w = warp & 3;
-    const uint32_t wsm = smem_u32(smem);
-    const uint32_t ssc = wsm + (uint32_t)(reinterpret_cast<uint8_t *>(s_sc) - smem);
-    const uint32_t scoef = wsm + (uint32_t)(reinterpret_cast<uint8_t *>(s_cr) - smem);
-    // the coefficient of k_j in row i (i = AT_MAX_S: the error weights); i and j are compile-time constants at every use
-    auto coef = [scoef](int i, int j) { return lds_pinned_f32(scoef + 4 * (8 * i + j)); };
-    const uint32_t wsm_h = wsm + h * 8 * SBO;                             // the weight rows of features [64 h, 64 h + 64)
-    const uint32_t stage = wsm + W_BYTES;
-    const uint32_t sy0 = stage + AT_STAGE + tid * 4;                      // element e at sy0 + 1024 e: this thread's only
-    const uint64_t dw = make_desc(wsm_h), dy = make_desc(stage);          // every wgmma descriptor is one of these + offset
-    // the hi weight plane of the warpgroup's features as the register A operand of every hi.* product (k-step ks: ahi[ks])
-    uint32_t ahi[LD / 16][4];
+    const uint32_t wsm_h = smem_u32(smem) + h * 8 * SBO;
 #pragma unroll
     for (int ks = 0; ks < LD / 16; ++ks) {
 #pragma unroll
@@ -162,11 +158,29 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
                          : "r"(wsm_h + (f >> 3) * SBO + (k >> 3) * LBO + (f & 7) * 16 + (k & 7) * 2));
         }
     }
+}
+
+// This CTA's tiles of one attempt (tiles blockIdx.x, blockIdx.x + gridDim.x, ...) through all S stages.  tid = threadIdx.x.
+// acc / nbad: this thread's share of the squared error norm (fold) and of the non-finite y1 count.
+template <int S, unsigned long long RM, unsigned EM>
+__device__ __forceinline__ void attempt_tiles(uint8_t *smem, const uint32_t (&ahi)[LD / 16][4], bool store, bool fold, int n_rows,
+                                              int tid, double &acc, int &nbad) {
+    const int lane = tid & 31;
+    const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);                  // warp-uniform for the compiler as well
+    // h = the warpgroup's half of the output features; w = warp inside the warpgroup
+    const int h = warp >> 2, w = warp & 3;
+    const uint32_t wsm = smem_u32(smem);
+    const uint32_t ssc = wsm + (uint32_t)(at_aux(smem) - smem) + AUX_SC;
+    const uint32_t scoef = wsm + (uint32_t)(at_aux(smem) - smem) + AUX_CR;
+    // the coefficient of k_j in row i (i = AT_MAX_S: the error weights); i and j are compile-time constants at every use
+    auto coef = [scoef](int i, int j) { return lds_pinned_f32(scoef + 4 * (8 * i + j)); };
+    const uint32_t wsm_h = wsm + h * 8 * SBO;                             // the weight rows of features [64 h, 64 h + 64)
+    const uint32_t stage = wsm + W_BYTES;
+    const uint32_t sy0 = stage + AT_STAGE + tid * 4;                      // element e at sy0 + 1024 e: this thread's only
+    const uint64_t dw = make_desc(wsm_h), dy = make_desc(stage);          // every wgmma descriptor is one of these + offset
     const int toff = thread_offset(w, lane) + 64 * h;
 
     const int tiles = (n_rows + AT_ROWS - 1) / AT_ROWS;
-    double acc = 0.0;
-    int nbad = 0;
 
     // One tile through all S stages.  FULL: all 32 rows exist (no per-row predicates); the one partial tile of a launch
     // takes the predicated copy of the same code.
@@ -393,21 +407,19 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
         if (n_rows - t * AT_ROWS >= AT_ROWS) do_tile(std::true_type{}, t);
         else do_tile(std::false_type{}, t);
     }
-    const double bad = (double)nbad;
+}
 
-    // ---- per-CTA partial of the squared norm and of the non-finite count; the last CTA adds them in index order ----
-    if (!fold) return;
+// Per-CTA partial of the squared norm and of the non-finite count: p_sum[blockIdx.x], p_bad[blockIdx.x] (thread 0 stores).
+__device__ __forceinline__ void cta_partial(double acc, int nbad, double *s_red, double *p_sum, double *p_bad) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     {
-        const double wa = warp_sum(acc), wb = warp_sum(bad);
+        const double wa = warp_sum(acc), wb = warp_sum((double)nbad);
         if (lane == 0) {
             s_red[warp] = wa;
             s_red[32 + warp] = wb;
         }
     }
     __syncthreads();
-    const int P = (int)gridDim.x;
-    double *p_sum = partials + 2, *p_bad = p_sum + P;
-    unsigned int *ticket = reinterpret_cast<unsigned int *>(partials);
     if (tid == 0) {
         double a = 0.0, b = 0.0;
         for (int w_ = 0; w_ < AT_THREADS / 32; ++w_) {
@@ -416,6 +428,53 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
         }
         p_sum[blockIdx.x] = a;
         p_bad[blockIdx.x] = b;
+    }
+}
+
+// The P partials added in index order by one warp; the sums are valid in lane 0.
+__device__ __forceinline__ void sum_partials(const double *p_sum, const double *p_bad, int P, double &a, double &b) {
+    const int lane = threadIdx.x & 31;
+    a = 0.0;
+    b = 0.0;
+    for (int i = lane; i < P; i += 32) {
+        a += __ldcg(&p_sum[i]);
+        b += __ldcg(&p_bad[i]);
+    }
+    a = warp_sum(a);
+    b = warp_sum(b);
+}
+
+// S: stages of an FSAL tableau (rows 0..S-1, the last one is c_sol and yields y1).  RM: 8 bits per row, bit j set <=> slot j has
+// a non-zero coefficient in that row.  EM: the same for the error weights of slots 0..S-1 (k_S always carries the last one).
+template <int S, unsigned long long RM, unsigned EM>
+__global__ void __launch_bounds__(AT_THREADS, 1)
+k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const uint32_t *__restrict__ wt,
+                 double *partials, double *norm_out, int store_always, size_t n_rows_sz) {
+    if (c->halt) return;                                  // an attempt issued after the end of the solve is a no-op
+    uint8_t *smem = at_smem();
+    uint8_t *aux = at_aux(smem);
+    int *s_flag = reinterpret_cast<int *>(aux);
+    double *s_red = reinterpret_cast<double *>(aux + AUX_RED);            // [2][32]
+    const int tid = threadIdx.x;
+    const bool fold = partials != nullptr;                                // squared error norm + candidate commit in here
+    attempt_prologue<S, RM, EM>(c, y0, k0, out, fold, n_rows_sz, aux, tid);
+    load_weights(smem, wt, tid, AT_THREADS);
+    fence_async_smem();
+    __syncthreads();
+    const bool store = attempt_store(c, store_always);
+    uint32_t ahi[LD / 16][4];
+    load_ahi(ahi, smem);
+    double acc = 0.0;
+    int nbad = 0;
+    attempt_tiles<S, RM, EM>(smem, ahi, store, fold, (int)n_rows_sz, tid, acc, nbad);
+
+    // ---- per-CTA partial of the squared norm and of the non-finite count; the last CTA adds them in index order ----
+    if (!fold) return;
+    const int P = (int)gridDim.x;
+    double *p_sum = partials + 2, *p_bad = p_sum + P;
+    unsigned int *ticket = reinterpret_cast<unsigned int *>(partials);
+    cta_partial(acc, nbad, s_red, p_sum, p_bad);
+    if (tid == 0) {
         __threadfence();
         const unsigned int tk = atomicAdd(ticket, 1u);
         *s_flag = (tk == gridDim.x - 1) ? 1 : 0;
@@ -423,19 +482,194 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
     __syncthreads();
     if (!*s_flag) return;
     __threadfence();
-    if (warp == 0) {
-        double a = 0.0, b = 0.0;
-        for (int i = lane; i < P; i += 32) {
-            a += __ldcg(&p_sum[i]);
-            b += __ldcg(&p_bad[i]);
-        }
-        a = warp_sum(a);
-        b = warp_sum(b);
-        if (lane == 0) {
+    if ((tid >> 5) == 0) {
+        double a, b;
+        sum_partials(p_sum, p_bad, P, a, b);
+        if (tid == 0) {
             norm_out[0] = a;
             norm_out[1] = b;
             *ticket = 0;                                                  // self-reset for the next launch
         }
+    }
+}
+
+// ---- a whole fused solve in one launch ---------------------------------------------------------------------------------
+// k_linear_solve runs every attempt of a solve: the CTAs stay resident (cooperative launch), keep the weight image in shared
+// memory and the hi plane in registers, and meet at a grid barrier after each attempt.  There CTA 0 adds the partials and
+// runs the controller step on a shared-memory copy of the control block (tdq_ctrl_step.cuh, what k_controller runs), then
+// releases the others.  When an output time fell into the step, every CTA runs the fit (tdq_fit.cuh, k_fit_eval's body)
+// and they meet once more: the next attempt overwrites the pair the fit reads.
+//
+// Barrier words (engine-owned, zeroed by tdq_linear_solve before the launch): arrivals after an attempt, the attempt whose
+// controller step is published, arrivals after a fit, abort.  A wait is an ld.acquire.gpu spin bounded by %globaltimer: after
+// 10 s (only a bug can make a co-resident CTA that late) the CTA aborts the solve with TDQ_RUN_BARRIER_TIMEOUT instead of
+// hanging the device.
+enum { BAR_ARRIVE = 0, BAR_RELEASE = 1, BAR_FIT = 2, BAR_ABORT = 3, BAR_WORDS = 4 };
+
+struct SolveAux {                                 // in the aux area of shared memory, at AUX_SOLVE
+    double norm[2];                               // the attempt's squared norm and non-finite count (CTA 0)
+    double nsm[AT_THREADS / 32 + 1];              // block_norm_from_sums scratch
+    int attempt, fits, fit_now, halt, was_halted, ok;
+    // the fit's operands and this block's place in the grid, read back (volatile) where the fit runs: the compiler cannot
+    // hoist what it derives from them out of the attempt loop, where it would hold registers through the tile loop
+    KPtrs kmid;
+    const float *y1s, *kSs;
+    float *solution;
+    unsigned long long n;
+    unsigned block, blocks;
+};
+static_assert(AUX_SOLVE + sizeof(SolveAux) <= AT_AUX, "aux layout");
+constexpr int SV_CTRL = (AT_SMEM + 15) & ~15;     // the staged control block follows the attempt's shared memory
+constexpr int SV_SMEM = SV_CTRL + (int)sizeof(TdqCtrl);
+
+// threadIdx.x through a volatile asm: what the attempt loop derives from it is recomputed in every iteration instead of being
+// hoisted out of the loop, where it would hold registers through the tile loop (the dopri5 instantiation then spills)
+__device__ __forceinline__ int opaque_tid() {
+    int t;
+    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+    return t;
+}
+
+__device__ __forceinline__ unsigned ld_acquire_u32(const unsigned *p) {
+    unsigned v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ unsigned long long global_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+
+// thread 0: wait until *word >= target; false after an abort or 10 s, with the solve aborted
+__device__ __forceinline__ bool bar_wait(TdqCtrl *c, unsigned *bar, int which, unsigned target) {
+    const unsigned long long t0 = global_ns();
+    for (;;) {
+        if ((int)(ld_acquire_u32(bar + which) - target) >= 0) return true;
+        if (ld_acquire_u32(bar + BAR_ABORT) != 0u) return false;
+        if (global_ns() - t0 > 10000000000ull) break;                       // 10 s
+    }
+    if (atomicExch(bar + BAR_ABORT, 1u) == 0u) {
+        c->status = TDQ_RUN_BARRIER_TIMEOUT;
+        c->halt = 1;
+        if (c->mbox) {
+            c->mbox->status = TDQ_RUN_BARRIER_TIMEOUT;
+            __threadfence_system();
+        }
+    }
+    return false;
+}
+
+// thread 0 arrives: everything the block wrote before the caller's __syncthreads is visible to whoever acquires the count
+__device__ __forceinline__ void bar_arrive(unsigned *bar, int which) {
+    __threadfence();
+    atomicAdd(bar + which, 1u);
+}
+
+// CTA 0: the controller step of the attempt just finished (norm = its squared norm and non-finite count), as k_controller
+// runs it, on the control block staged in shared memory; only the attempt that ends the solve writes the mailbox
+__device__ __forceinline__ void solve_controller_step(TdqCtrl *c, uint8_t *smem, SolveAux *sx, const int64_t *cnt) {
+    unsigned char *raw = smem + SV_CTRL;
+    ctrl_stage_in(c, raw);
+    ctrl_decide<float, AT_THREADS>(*reinterpret_cast<TdqCtrl *>(raw), sx->norm, cnt, 1, nullptr, true, sx->nsm, &sx->was_halted,
+                                    opaque_tid());
+    ctrl_stage_out(c, raw);
+}
+
+// NK: the tableau's non-zero mid-point weights (the fit's stage terms).  kmid, y1s, kSs: the fit's operands as
+// tdq_interp_fit_eval plans them.  part: two slots (attempt parity) of P sums and P non-finite counts.
+template <int S, unsigned long long RM, unsigned EM, int NK>
+__global__ void __launch_bounds__(AT_THREADS, 1)
+k_linear_solve(TdqCtrl *c, AttOut out, const uint32_t *__restrict__ wt, unsigned *bar, double *part, const int64_t *cnt,
+               KPtrs kmid, const float *y1s, const float *kSs, float *solution, size_t n_rows_sz) {
+    uint8_t *smem = at_smem();
+    uint8_t *aux = at_aux(smem);
+    double *s_red = reinterpret_cast<double *>(aux + AUX_RED);
+    volatile SolveAux *sxv = reinterpret_cast<volatile SolveAux *>(aux + AUX_SOLVE);
+    SolveAux *sx = reinterpret_cast<SolveAux *>(aux + AUX_SOLVE);
+    const int tid = threadIdx.x;
+    const unsigned P = gridDim.x;
+    if (c->halt) {
+        // the start already ended the solve (k_prepare): the controller step of the one no-op attempt, as the device loop runs it
+        if (blockIdx.x == 0) solve_controller_step(c, smem, sx, cnt);
+        return;
+    }
+    // ---- once per launch: the weight image, the hi plane ----
+    load_weights(smem, wt, tid, AT_THREADS);
+    fence_async_smem();
+    if (tid == 0) {
+        sx->attempt = 0;
+        sx->fits = 0;
+        sx->kmid = kmid;
+        sx->y1s = y1s;
+        sx->kSs = kSs;
+        sx->solution = solution;
+        sx->n = n_rows_sz * LD;
+        sx->block = blockIdx.x;
+        sx->blocks = gridDim.x;
+    }
+    __syncthreads();
+    uint32_t ahi[LD / 16][4];
+    load_ahi(ahi, smem);
+    for (;;) {
+        // ---- the attempt: same prologue, tiles and per-CTA partial as k_linear_attempt ----
+        attempt_prologue<S, RM, EM>(c, nullptr, nullptr, out, true, n_rows_sz, aux, opaque_tid());
+        __syncthreads();
+        const bool store = attempt_store(c, 0);
+        double acc = 0.0;
+        int nbad = 0;
+        attempt_tiles<S, RM, EM>(smem, ahi, store, true, (int)n_rows_sz, opaque_tid(), acc, nbad);
+        const unsigned a = (unsigned)sxv->attempt;
+        double *p_sum = part + (a & 1u) * 2 * P, *p_bad = p_sum + P;
+        cta_partial(acc, nbad, s_red, p_sum, p_bad);
+        if (tid == 0) bar_arrive(bar, BAR_ARRIVE);
+        // ---- controller step: CTA 0 once every partial is in, the others wait for its release ----
+        if (blockIdx.x == 0) {
+            if (tid == 0) sxv->ok = bar_wait(c, bar, BAR_ARRIVE, P * (a + 1u));
+            __syncthreads();
+            if (!sxv->ok) return;
+            if ((tid >> 5) == 0) {
+                double sa, sb;
+                sum_partials(p_sum, p_bad, (int)P, sa, sb);
+                if (tid == 0) {
+                    sxv->norm[0] = sa;
+                    sxv->norm[1] = sb;
+                }
+            }
+            __syncthreads();
+            solve_controller_step(c, smem, sx, cnt);
+            __syncthreads();
+            if (tid == 0) {
+                __threadfence();
+                asm volatile("st.release.gpu.global.u32 [%0], %1;" :: "l"(bar + BAR_RELEASE), "r"(a + 1u) : "memory");
+            }
+        } else if (tid == 0) {
+            sxv->ok = bar_wait(c, bar, BAR_RELEASE, a + 1u);
+        }
+        if (tid == 0) {
+            sxv->fit_now = c->fit_now;
+            sxv->halt = c->halt;
+            sxv->attempt = (int)(a + 1u);
+        }
+        __syncthreads();
+        if (!sxv->ok) return;
+        // ---- the lazy fit of the accepted step, grid-stride over the whole grid ----
+        if (sxv->fit_now) {
+            KPtrs km;
+#pragma unroll
+            for (int m = 0; m < NK; ++m) km.p[m] = sxv->kmid.p[m];
+            fit_eval_body<float, NK, true, false>(c, sxv->y1s, sxv->kSs, km, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                                  sxv->solution, (size_t)sxv->n, sxv->block, sxv->blocks);
+            __syncthreads();
+            if (tid == 0) {
+                bar_arrive(bar, BAR_FIT);
+                sxv->fits = sxv->fits + 1;
+                sxv->ok = bar_wait(c, bar, BAR_FIT, P * (unsigned)sxv->fits);
+            }
+            __syncthreads();
+            if (!sxv->ok) return;
+        }
+        if (sxv->halt) return;
     }
 }
 
@@ -450,6 +684,29 @@ int launch_attempt(TdqCtrl *c, const float *y0, const float *k0, const AttOut &o
     auto kern = k_linear_attempt<S, RM, EM>;
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM) != cudaSuccess) return -2;
     kern<<<tdq_grid(n_rows, AT_ROWS, 1), AT_THREADS, AT_SMEM, st>>>(c, y0, k0, out, wt, partials, norm_out, store_always, n_rows);
+    return 0;
+}
+
+// Cooperative launch: every CTA must be resident at once for the grid barrier, or the launch is refused (-3).
+template <int S, unsigned long long RM, unsigned EM, int NK>
+int launch_solve(TdqCtrl *c, const AttOut &out, const uint32_t *wt, unsigned *bar, double *part, const int64_t *cnt,
+                 const KPtrs &kmid, const float *y1, const float *kS, float *solution, size_t n_rows, cudaStream_t st) {
+    auto kern = k_linear_solve<S, RM, EM, NK>;
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SV_SMEM) != cudaSuccess) return -2;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(tdq_grid(n_rows, AT_ROWS, 1));
+    cfg.blockDim = dim3(AT_THREADS);
+    cfg.dynamicSmemBytes = SV_SMEM;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeCooperative;
+    attr[0].val.cooperative = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    if (cudaLaunchKernelEx(&cfg, kern, c, out, wt, bar, part, cnt, kmid, y1, kS, solution, n_rows) != cudaSuccess) {
+        (void)cudaGetLastError();                                         // not sticky: the caller takes the per-attempt path
+        return -3;
+    }
     return 0;
 }
 
@@ -526,6 +783,65 @@ int tdq_linear_attempt(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, vo
         rc = launch_attempt<3, RM_BOSH3, 0x07u>(c, (const float *)y0, (const float *)k0, out, wt, partials, norm_out, store_always, n_rows, st);
     TDQ_REQUIRE(rc != -1, "no whole-attempt kernel for this tableau (tdq_linear_attempt_supported)");
     TDQ_REQUIRE(rc == 0, "launch configuration failed");
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+size_t tdq_linear_solve_scratch_len(void) { return (size_t)(2 + 4 * tdq_sm_count()); }
+
+int tdq_linear_solve(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, void *const *k_out, void *y1_out, void *err_out,
+                     const void *planes, int32_t width, size_t n, double *scratch, size_t scratch_len,
+                     const int64_t *seg_counts_dev, void *solution, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && tab && k_out && y1_out && err_out && planes && scratch && seg_counts_dev && solution, "null argument");
+    TDQ_REQUIRE(dtype == TDQ_F32 && width == LD, "the fused linear field is float32, width 128");
+    TDQ_REQUIRE(n % (size_t)width == 0 && n > 0, "state size is not a positive multiple of the field width");
+    const size_t n_rows = n / (size_t)width;
+    TDQ_REQUIRE(n_rows < ((size_t)1 << 31) - 64, "too many rows");
+    TDQ_REQUIRE(scratch_len >= tdq_linear_solve_scratch_len(), "scratch is shorter than tdq_linear_solve_scratch_len()");
+    TdqHostShape hs;
+    tdq_shape_from_tableau(tab, &hs);
+    unsigned long long rm = 0;
+    unsigned em = 0;
+    TDQ_REQUIRE(attempt_masks(hs, &rm, &em), "the whole-attempt kernel takes FSAL tableaus of at most 7 stages");
+    const int S = hs.n_stages;
+    AttOut out;
+    memset(&out, 0, sizeof(out));
+    const void *k[TDQ_MAX_K] = {nullptr};                                 // k[0] = NULL: the fit reads k_0 from the pointer table
+    for (int i = 1; i <= S; ++i) {
+        TDQ_REQUIRE(k_out[i] != nullptr, "missing stage slot");
+        out.k[i] = (float *)k_out[i];
+        k[i] = k_out[i];
+    }
+    out.y1 = (float *)y1_out;
+    out.err = (float *)err_out;
+    // the fit's operands, planned as tdq_interp_fit_eval plans them; the solve runs its vector (16-byte) body only
+    KPtrs kmid;
+    bool vec = tdq_aligned16(y1_out) && tdq_aligned16(k_out[S]) && tdq_aligned16(solution) && (n * 4) % 16 == 0;
+    TDQ_REQUIRE(hs.mid_nnz >= 1 && tdq_plan_terms(hs.mid_idx, hs.mid_nnz, k, kmid.p, vec) == TDQ_PLAN_OK,
+                "missing stage slot for a non-zero mid-point weight");
+    if (!vec) {
+        tdq_set_error("tdq_linear_solve: the stage, y1 and solution buffers must be 16-byte aligned");
+        return TDQ_ERR_UNSUPPORTED;
+    }
+    // barrier words in the first 16 bytes, then two slots of per-CTA partials
+    unsigned *bar = reinterpret_cast<unsigned *>(scratch);
+    cudaStream_t st = (cudaStream_t)stream;
+    TDQ_CHECK_CUDA(cudaMemsetAsync(bar, 0, BAR_WORDS * sizeof(unsigned), st));
+    TdqCtrl *c = (TdqCtrl *)ctrl_dev;
+    const uint32_t *wt = (const uint32_t *)planes;
+    int rc = -1;
+    if (S == 6 && rm == RM_DOPRI5 && em == 0x3du && hs.mid_nnz == 6)
+        rc = launch_solve<6, RM_DOPRI5, 0x3du, 6>(c, out, wt, bar, scratch + 2, seg_counts_dev, kmid, (const float *)y1_out,
+                                                 (const float *)k_out[S], (float *)solution, n_rows, st);
+    else if (S == 3 && rm == RM_BOSH3 && em == 0x07u && hs.mid_nnz == 1)
+        rc = launch_solve<3, RM_BOSH3, 0x07u, 1>(c, out, wt, bar, scratch + 2, seg_counts_dev, kmid, (const float *)y1_out,
+                                                (const float *)k_out[S], (float *)solution, n_rows, st);
+    TDQ_REQUIRE(rc != -1, "no persistent solve kernel for this tableau (tdq_linear_attempt_supported)");
+    TDQ_REQUIRE(rc != -2, "launch configuration failed");
+    if (rc == -3) {
+        tdq_set_error("tdq_linear_solve: the cooperative launch was refused (the CTAs cannot all be resident)");
+        return TDQ_ERR_UNSUPPORTED;
+    }
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
 }
