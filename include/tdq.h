@@ -331,6 +331,26 @@ int tdq_linear_stage(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, int3
                      void *err_out, const void *y0, const void *const *k, const void *planes, int32_t width, size_t n,
                      void *stream);
 
+/* ---- The adjoint's augmented field of a LINEAR vector field on the tensor cores (tdq_linear_adjoint.cu) ----------------------
+ * For f(t, y) = y W^T and a = adj_y, g = grad(f, ., +a) has the closed form g_y = a W, g_W = a^T y (summed over rows), g_t = 0.
+ * One evaluation of the backward augmented field (adjoint.py:72-105) in one pass over y and a:
+ *   out_y = s_y (y W^T)   bitwise tdq_linear_apply(y, planes_w) when s_y = 1
+ *   out_a = s_a (a W)     bitwise s_a * tdq_linear_apply(a, planes_wt)
+ *   out_w = s_W (a^T y)   128 x 128, six split-bf16 products per tile into float32 accumulators, one float32 partial per fixed
+ *                         chunk of 512 rows, the partials added in chunk order in float64 and rounded once: the result
+ *                         depends on n_rows and the operands only, and |out_w - s_W a^T y| <= 76 u S + 8 n_rows FLT_MIN with
+ *                         u = 2^-24, S = sum_r |a_r||y_r| (tests/test_gpu_linear_adjoint.py, DESIGN.md section 3d).
+ * y, a: [n_rows][width] float32; planes_w / planes_wt: tdq_linear_prepare of W and of W^T.  scales: HOST array {s_y, s_a, s_W}.
+ * out_w NULL: the weight gradient is not formed (partials may then be NULL); otherwise partials holds
+ * tdq_linear_adjoint_partials_len(n_rows) floats of scratch (no initial value needed; not shared with a concurrent call).
+ * A non-finite row stays in its own row of out_y / out_a; it may make out_w non-finite.  Every pointer 16-byte aligned.
+ * Two launches on `stream` (the row products and the partials; the chunk sum). */
+int tdq_linear_adjoint_supported(int32_t dtype, int32_t width);
+size_t tdq_linear_adjoint_partials_len(size_t n_rows);
+int tdq_linear_adjoint_field(int32_t dtype, const void *y, const void *a, const void *planes_w, const void *planes_wt,
+                             int32_t width, size_t n_rows, void *out_y, void *out_a, void *out_w, const float *scales,
+                             void *partials, void *stream);
+
 /* ---- A WHOLE attempt of a linear vector field in one launch (tdq_attempt.cu) ---------------------------------------------
  * For f(t, y) = y W^T an attempt is row-local, so one kernel takes every tile of 32 state rows through all S stages on chip:
  * rk_common.py:43-90 (_runge_kutta_step: every y_i, every k_i, y1, the error estimate), the squared error ratio of

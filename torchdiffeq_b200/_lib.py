@@ -119,6 +119,10 @@ _SIGNATURES = {
     "tdq_linear_prepare": (C.c_int, [_i32, _vp, _i32, _vp, _vp]),
     "tdq_linear_apply": (C.c_int, [_i32, _vp, _vp, _i32, _sz, _vp, _vp]),
     "tdq_linear_stage": (C.c_int, [_vp, _ptab, _i32, _i32, _vp, _vp, _vp, _vp, _pp, _vp, _i32, _sz, _vp]),
+    "tdq_linear_adjoint_supported": (C.c_int, [_i32, _i32]),
+    "tdq_linear_adjoint_partials_len": (_sz, [_sz]),
+    "tdq_linear_adjoint_field": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _i32, _sz, _vp, _vp, _vp, C.POINTER(C.c_float), _vp,
+                                           _vp]),
     "tdq_linear_attempt_supported": (C.c_int, [_ptab, _i32, _i32]),
     "tdq_linear_attempt": (C.c_int, [_vp, _ptab, _i32, _pp, _vp, _vp, _vp, _vp, _vp, _i32, _sz, _vp, _vp, _vp, _i32, _vp]),
     "tdq_linear_solve_scratch_len": (_sz, []),

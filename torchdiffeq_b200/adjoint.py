@@ -13,17 +13,27 @@ the minus of `-adj_y` (adjoint.py:96) and the *(-1) of reverse time (misc.py:165
 tdq_pack_segments launch per evaluation.  The default adjoint norm
 max(|t|, rms(y), rms(adj_y), max_i rms(theta_i)) (adjoint.py:247-250) and 'seminorm' (:267-271) are
 segments of the fused error-norm kernel.  One engine (and one captured graph) serves all intervals.
+
+When func is a torchdiffeq_b200.LinearField (f = y W^T, float32 [..., 128]) the augmented field has a closed form --
+g_y = a W, g_W = a^T y, g_t = 0 -- and each evaluation is one tensor-core kernel that writes the raw slot directly
+(csrc/tdq_linear_adjoint.cu): no autograd graph, no GEMM through torch, no pack.  It is opt-in, with
+adjoint_options={'fused_linear': True}: its products round like the forward's tensor-core ones rather than like the
+float32 GEMMs of the autograd backward, so the gradients differ from the default's at float32 rounding, amplified by the
+conditioning of the problem (DESIGN.md section 3d).  last_stats()['fused_adjoint'] tells which one the last backward
+pass ran.
 """
+import ctypes as C
 import warnings
 
 import torch
 import torch.nn as nn
 
 from . import _lib
-from ._engine import Layout, on_solver_stream
+from ._engine import Layout, _stream, on_solver_stream
 from ._fixed import FIXED_METHODS, signed_grid_constructor
 from ._implicit import IMPLICIT_METHODS
-from .odeint import (ADAPTIVE_METHODS, _ADJOINT_CALLBACK_NAMES, _CALLBACK_NAMES, _cache_drop, _cache_get,
+from .fields import fusable
+from .odeint import (ADAPTIVE_METHODS, _ADJOINT_CALLBACK_NAMES, _CALLBACK_NAMES, _LAST_STATS, _cache_drop, _cache_get,
                      _cache_key, _cache_put, _make_adaptive_engine, _make_fixed_engine, _mixed_norm, _rms_norm, _solve,
                      _solve_event, _unflatten, fixed_grid, normalise, Problem, valid_callbacks)
 
@@ -101,6 +111,12 @@ class _BackwardSolver:
         lens = [1] + f_lens + [n] + list(lay.lens[3:])
         scales = [-1.0] + [1.0] * len(f_offs) + [-1.0] + [-1.0] * len(adjoint_params)
         pieces = (offs, lens, scales)
+
+        # ---- the closed-form augmented field of a LinearField (csrc/tdq_linear_adjoint.cu) -----------------------------
+        self.linear = None
+        w = fused_adjoint_weight(p, adjoint_params, adjoint_options)
+        if w is not None:
+            aug_fn = self._linear_field(w)
 
         # ---- adjoint norm (adjoint.py:243-288) -------------------------------------------
         opts = dict(adjoint_options)
@@ -208,10 +224,52 @@ class _BackwardSolver:
         # solves run inside autograd's backward: never capture there (see AdaptiveEngine.prime)
         self.eng.capture_in_solve = False
 
+    def _linear_field(self, w):
+        """The augmented field of f = y W^T as one kernel: the raw slot (-g_t, +f, -g_y, -g_W) = (0, y W^T, -a W, -a^T y),
+        returned as one flat tensor (the flat-tensor branch of the engines' _call_fn).  The W product is skipped when
+        W is not an adjoint parameter.  The weight planes are filled by _prepare_linear at the start of every run()."""
+        lib, lay, n, dev, T = _lib.load(), self.lay, self.p.n, self.p.device, self.p.dtype
+        o_y, o_a = self.o_y, self.o_a
+        width = int(w.shape[0])
+        rows = n // width
+        o_w = lay.offsets[3] if self.params else None
+        nbytes = int(lib.tdq_linear_weights_bytes(width))
+        L = self.linear = dict(
+            weight=w, width=width, wt=torch.empty_like(w),
+            planes=torch.empty(nbytes, dtype=torch.uint8, device=dev),
+            planes_t=torch.empty(nbytes, dtype=torch.uint8, device=dev),
+            partials=(torch.empty(int(lib.tdq_linear_adjoint_partials_len(rows)), dtype=torch.float32, device=dev)
+                      if o_w is not None else None),
+            scales=(C.c_float * 3)(1.0, -1.0, -1.0))
+        pw, pwt = L["planes"].data_ptr(), L["planes_t"].data_ptr()
+        part = L["partials"].data_ptr() if o_w is not None else None
+
+        def linear_fn(t_, aug_flat):
+            out = torch.empty(lay.n, dtype=T, device=dev)
+            out[:o_y].zero_()                                     # vjp_t = -g_t = 0, and the padding after it
+            _lib.check(lib.tdq_linear_adjoint_field(
+                0, aug_flat[o_y:o_y + n].data_ptr(), aug_flat[o_a:o_a + n].data_ptr(), pw, pwt, width, rows,
+                out[o_y:o_y + n].data_ptr(), out[o_a:o_a + n].data_ptr(),
+                out[o_w:].data_ptr() if o_w is not None else None, L["scales"], part, _stream()))
+            return out
+        return linear_fn
+
+    def _prepare_linear(self):
+        """Split the weight (it is kept by reference and may have changed since the last backward pass) and its
+        transpose into the planes every evaluation of this run reads."""
+        L = self.linear
+        if L is None:
+            return
+        lib, st = _lib.load(), _stream()
+        L["wt"].copy_(L["weight"].detach().t())
+        _lib.check(lib.tdq_linear_prepare(0, L["weight"].data_ptr(), L["width"], L["planes"].data_ptr(), st))
+        _lib.check(lib.tdq_linear_prepare(0, L["wt"].data_ptr(), L["width"], L["planes_t"].data_ptr(), st))
+
     def prime(self, t, y_last):
         """Capture the backward step graph now (forward call, main thread) on stand-in data."""
         if self.fixed:
             return False
+        self._prepare_linear()
         lay, n = self.lay, self.p.n
         aug = torch.zeros(lay.n, dtype=self.p.dtype, device=self.p.device)
         aug[self.o_y:self.o_y + n] = y_last
@@ -224,6 +282,7 @@ class _BackwardSolver:
         p, lay, eng, n = self.p, self.lay, self.eng, self.p.n
         o_t, o_y, o_a = self.o_t, self.o_y, self.o_a
         dev, T = p.device, p.dtype
+        self._prepare_linear()
         aug = torch.zeros(lay.n, dtype=T, device=dev)
         aug[o_y:o_y + n] = y[-1]
         aug[o_a:o_a + n] = grad_sol[-1]
@@ -259,6 +318,22 @@ class _BackwardSolver:
         adj_y = aug[o_a:o_a + n].clone()
         adj_params = [aug[o:o + l].view(s).clone() for o, l, s in zip(lay.offsets[3:], lay.lens[3:], lay.shapes[3:])]
         return time_vjps, adj_y, adj_params
+
+
+def fused_adjoint_weight(p, adjoint_params, adjoint_options):
+    """The weight of func if the backward augmented field runs as one kernel (csrc/tdq_linear_adjoint.cu), else None:
+    func is exactly a LinearField on a float32 [..., 128] tensor state, the batch is not sharded, the adjoint parameters
+    are () or (weight,), and adjoint_options['fused_linear'] is True (the autograd backward is the default)."""
+    if p.is_tuple or p.shape is None or adjoint_options.get("fused_linear") is not True \
+            or adjoint_options.get("process_group") is not None:
+        return None
+    lib = _lib.load()
+    w = fusable(p.original_func, tuple(p.shape), p.dtype, p.device, lib)
+    if w is None or not lib.tdq_linear_adjoint_supported(0, int(w.shape[0])):
+        return None
+    if not (len(adjoint_params) == 0 or (len(adjoint_params) == 1 and adjoint_params[0] is w)):
+        return None
+    return w
 
 
 def _backward_key(p, adjoint_params, bargs):
@@ -339,6 +414,7 @@ class _AdjointFunction(torch.autograd.Function):
             except BaseException:
                 _cache_drop(ctx.bkey, "backward")         # a half-finished backward engine is never reused
                 raise
+            _LAST_STATS["fused_adjoint"] = bs.linear is not None
             if ctx.event_mode and time_vjps is not None:                 # adjoint.py:146-148
                 time_vjps = torch.cat([time_vjps[0].reshape(-1), torch.zeros_like(t_all[1:])])
         ctx.bsolver = None
