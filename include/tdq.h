@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define TDQ_ABI_VERSION 2
+#define TDQ_ABI_VERSION 3
 
 #define TDQ_MAX_STAGES 16            /* func evaluations per attempt, excluding f0 (dopri8: 13)   */
 #define TDQ_MAX_K      (TDQ_MAX_STAGES + 1) /* stage slots k_0 .. k_S                              */
@@ -477,12 +477,9 @@ int tdq_ctrl_set_exchange(void *ctrl_dev, const void *const *peer_ptrs, int32_t 
  *                           cleared.
  * tdq_rows_init_grid:       tdq_rows_init with per-row output times: t_grid is [B, n_out] float64, row r ascending in solver
  *                           time (t_sign applied), and row r starts at t_grid[r, 0], ends at t_grid[r, n_out - 1] and emits
- *                           solution[j, r, :] at t_grid[r, j] when the solve's attempts use tdq_rows_controller_grid
- *                           (or _controller_event_grid) and tdq_rows_fit_eval_grid in place of the launchers without
- *                           _grid, which have the same arguments.  Those read the table until the next init (its address
- *                           is kept in the control block, which tdq_ctrl_init and tdq_rows_init clear), so it must stay
- *                           alive and unchanged for the solve; with no table set they read the control block's t_out.
- *                           The launchers without _grid never read the table.
+ *                           solution[j, r, :] at t_grid[r, j].  Its address is kept in the control block, and every
+ *                           attempt launcher reads the table while one is set; tdq_ctrl_init and tdq_rows_init clear it.
+ *                           So it must stay alive and unchanged for the solve.
  * tdq_rows_sumsq:           out[r] = sum over row r of (x/scale)^2, or ((x - x2)/scale)^2 with x2; scale = atol + |y0|*rtol;
  *                           without x2 out[B + r] = number of non-finite y0 elements of row r (misc.py:55-58, :69).
  * tdq_rows_initial_h0 / _probe / _finish: misc.py:60-77 per row from tdq_rows_sumsq's sums; _set_first_step: options
@@ -538,10 +535,6 @@ int tdq_rows_controller(void *ctrl_dev, void *rows_dev, int32_t dtype, const dou
                         size_t row_len, void *stream);
 int tdq_rows_fit_eval(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, const void *y1,
                       const void *const *k, void *solution, size_t n_rows, size_t row_len, void *stream);
-int tdq_rows_controller_grid(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in, size_t n_rows,
-                             size_t row_len, void *stream);
-int tdq_rows_fit_eval_grid(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, const void *y1,
-                           const void *const *k, void *solution, size_t n_rows, size_t row_len, void *stream);
 
 /* ---- per-row events with independent step-size control (tdq_rows.cu) ---------------------------------------------------
  * Row r stops at its own event as the reference's odeint_event does for y0[r:r+1] alone (rk_common.py:252-262,
@@ -569,9 +562,6 @@ int tdq_rows_event_init(void *rows_dev, const double *ev_val, double *init_sign,
 int tdq_rows_controller_event(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in, const double *ev_val,
                               const double *init_sign, const double *sign0, int32_t *flag, size_t n_rows, size_t row_len,
                               int32_t K, void *stream);
-int tdq_rows_controller_event_grid(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in,
-                                   const double *ev_val, const double *init_sign, const double *sign0, int32_t *flag,
-                                   size_t n_rows, size_t row_len, int32_t K, void *stream);
 int tdq_rows_fit_store(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, const void *y1,
                        const void *const *k, const int32_t *flag, void *coeff, size_t n_rows, size_t row_len,
                        void *stream);

@@ -108,7 +108,7 @@ class _Field(torch.nn.Module):
 
 def test_cached_engine_reuse():
     """An nn.Module func (cached engine, graph + device loop): a second grid of the same shape, then a 1-D t, then the
-    grid again -- each result equals a fresh engine's."""
+    grid again, all on one engine -- each result equals a fresh engine's."""
     B, D, T = 8, 5, 4
     g = torch.Generator().manual_seed(30)
     rate = (10.0 ** (torch.rand(B, 1, generator=g, dtype=torch.float64) * 2 - 1)).to(DEV)
@@ -117,13 +117,14 @@ def test_cached_engine_reuse():
     L = dict(graph=True, device_loop=True)
     ta, tb = _times(B, T, 31).to(DEV), _times(B, T, 32).to(DEV)
     t1 = torch.tensor([0.0, 0.4, 0.9, 1.3], dtype=torch.float64, device=DEV)
+    M = importlib.import_module("torchdiffeq_b200.odeint")
     tdq.clear_cache()
     cached = [_run(m, y0, tt, options=L)[0].clone() for tt in (ta, tb, t1, ta)]
+    assert len(M._ENGINE_CACHE) == 1
     fresh = [_run(m, y0, tt, options=dict(L, cache=False))[0] for tt in (ta, tb, t1)]
     assert torch.equal(cached[0], fresh[0]) and torch.equal(cached[1], fresh[1]) and torch.equal(cached[2], fresh[2])
     assert torch.equal(cached[3], cached[0]) and not torch.equal(cached[0], cached[1])
-    # the per-row-grid engine itself: a 1-D solve after a grid solve reads the shared times again, then the grid again
-    M = importlib.import_module("torchdiffeq_b200.odeint")
+    # the engine itself: a 1-D solve after a grid solve reads the shared times again, then the grid again
     tdq.clear_cache()
     _run(m, y0, ta, options=L)
     (eng, _), = M._ENGINE_CACHE.values()
@@ -136,8 +137,7 @@ def test_cached_engine_reuse():
 
 
 def test_grid_is_scoped_to_its_solve():
-    """After a table solve, every other way into a solve (prime, a direct _begin) runs on the shared times, and a
-    captured attempt of the other kind is not replayed."""
+    """After a table solve, every other way into a solve (prime, a direct _begin) runs on the shared times."""
     B, D, T = 6, 3, 4
     g = torch.Generator().manual_seed(42)
     rate = (0.5 + torch.rand(B, 1, generator=g, dtype=torch.float64)).to(DEV)
@@ -154,9 +154,38 @@ def test_grid_is_scoped_to_its_solve():
         assert eng.grid is not None
         eng._begin(y0.reshape(-1), t1, 0.0)
         torch.cuda.synchronize()
+        # the captured attempt is dropped only because the solution's shape changed: T = 5 in the table, 4 here
         assert eng.grid is None and eng._graph is None
         assert torch.equal(_f_t0(eng), torch.zeros(B, dtype=torch.float64))
         assert torch.equal(eng.solve(y0.reshape(-1), t1, t_start=0.0).view(T, B, D), fresh)
+    torch.cuda.synchronize()
+
+
+def test_one_captured_attempt_serves_table_and_shared_times():
+    """With equal T, a cached engine (graph + device loop) replays the attempt it captured in a table solve for a 1-D
+    solve, and the other way round; every result, and the per-row counts, equal a fresh engine's bit for bit."""
+    B, D, T = 8, 5, 4
+    g = torch.Generator().manual_seed(44)
+    rate = (10.0 ** (torch.rand(B, 1, generator=g, dtype=torch.float64) * 2 - 1)).to(DEV)
+    y0 = torch.randn(B, D, generator=g, dtype=torch.float64).to(DEV)
+    m = _Field(rate)
+    L = dict(graph=True, device_loop=True)
+    ta = _times(B, T, 45).to(DEV)
+    t1 = torch.tensor([0.0, 0.4, 0.9, 1.3], dtype=torch.float64, device=DEV)
+    fresh = {"table": _run(m, y0, ta, options=dict(L, cache=False)),
+             "1-D": _run(m, y0, t1, options=dict(L, cache=False))}
+    M = importlib.import_module("torchdiffeq_b200.odeint")
+    for first, second in (("table", "1-D"), ("1-D", "table")):
+        tdq.clear_cache()
+        got = {first: _run(m, y0, ta if first == "table" else t1, options=L)}
+        (eng, _), = M._ENGINE_CACHE.values()
+        graph = eng._graph
+        assert graph is not None and eng._loop is not None
+        got[second] = _run(m, y0, ta if second == "table" else t1, options=L)
+        assert len(M._ENGINE_CACHE) == 1 and eng._graph is graph and eng._loop is not None
+        for kind in (first, second):
+            assert torch.equal(_bits(got[kind][0]), _bits(fresh[kind][0])), (first, kind)
+            assert torch.equal(got[kind][1], fresh[kind][1]) and torch.equal(got[kind][2], fresh[kind][2]), (first, kind)
     torch.cuda.synchronize()
 
 

@@ -1,6 +1,6 @@
-"""Per-row output times (tdq_rows_init_grid and the *_grid launchers) one launch at a time, on row state set by hand: the
-grid init's per-row start, the controller's cursor and emit range on each row's own table, the fit bitwise at each row's own
-x against the oracle, the launchers without _grid ignoring the table, and a plain tdq_rows_init clearing it."""
+"""Per-row output times (tdq_rows_init_grid) one launch at a time, on row state set by hand: the grid init's per-row
+start, the controller's cursor and emit range on each row's own table, the fit bitwise at each row's own x against the
+oracle, and a plain tdq_rows_init clearing the table, after which the same launchers read the control block's times."""
 import ctypes as C
 
 import pytest
@@ -59,7 +59,7 @@ def test_grid_init_per_row_start(dtype, t_sign):
     assert (_f(eng, _lib.ROWS_DONE, torch.int32).cpu() == 0).all()
 
 
-def test_controller_cursor_follows_each_rows_table():
+def test_controller_reads_each_rows_table_then_t_out():
     """Every row accepts the step [a_r, b_r]; the cursor, emit range, fit flag, done and the interval's step count follow the
     row's own times.  Then a plain init: the same launch reads the shared times."""
     B, D, n_out = 6, 4, 4
@@ -74,7 +74,7 @@ def test_controller_cursor_follows_each_rows_table():
     b = torch.tensor([0.25, 0.5, 0.8, 0.15, 0.2, 0.25], dtype=torch.float64)
     want_cur = [3, 1, 4, 2, 4, 1]
 
-    def launch(controller):
+    def launch():
         F = lambda w, d: _f(eng, w, d)
         F(_lib.ROWS_ATT_T0, torch.float64).copy_(a)
         F(_lib.ROWS_ATT_DT, torch.float64).copy_(b - a)
@@ -84,8 +84,8 @@ def test_controller_cursor_follows_each_rows_table():
         F(_lib.ROWS_CURSOR, torch.int32).fill_(1)
         F(_lib.ROWS_N_STEPS, torch.int64).fill_(3)
         eng.row_norm.zero_()                                              # ratio 0: every row accepts
-        _lib.check(controller(eng.ctrl.data_ptr(), eng.rows.data_ptr(), eng.dt_code, eng.row_norm.data_ptr(), B, D,
-                              _stream()))
+        _lib.check(eng.lib.tdq_rows_controller(eng.ctrl.data_ptr(), eng.rows.data_ptr(), eng.dt_code,
+                                               eng.row_norm.data_ptr(), B, D, _stream()))
         torch.cuda.synchronize()
         return {w: F(w, torch.int32).cpu().tolist() for w in (_lib.ROWS_CURSOR, _lib.ROWS_EMIT_LO, _lib.ROWS_EMIT_HI,
                                                                _lib.ROWS_FIT, _lib.ROWS_DONE)}, \
@@ -94,23 +94,21 @@ def test_controller_cursor_follows_each_rows_table():
     shared = torch.linspace(0.0, 1.0, n_out, dtype=torch.float64)
     want_shared = [int((shared <= float(b[r])).sum()) for r in range(B)]
     _init_grid(eng, grid)
-    got, _ = launch(eng.lib.tdq_rows_controller)                        # the shared-times launcher ignores the table
-    assert got[_lib.ROWS_CURSOR] == want_shared
-    got, steps = launch(eng.lib.tdq_rows_controller_grid)
+    got, steps = launch()
     assert got[_lib.ROWS_CURSOR] == want_cur
     assert got[_lib.ROWS_EMIT_LO] == [1] * B and got[_lib.ROWS_EMIT_HI] == want_cur
     assert got[_lib.ROWS_FIT] == [int(c > 1) for c in want_cur]
     assert got[_lib.ROWS_DONE] == [int(c >= n_out) for c in want_cur]
     assert steps == [0 if c > 1 else 4 for c in want_cur]
-    # a plain init clears the table: the table launcher then reads the control block's own times, linspace(0, 1, 4)
+    # a plain init clears the table: the same launcher then reads the control block's own times, linspace(0, 1, 4)
     _lib.check(eng.lib.tdq_rows_init(eng.ctrl.data_ptr(), eng.rows.data_ptr(), eng.dt_code, B, 0.0, _stream()))
-    got, _ = launch(eng.lib.tdq_rows_controller_grid)
+    got, _ = launch()
     assert got[_lib.ROWS_CURSOR] == want_shared
 
 
 @pytest.mark.parametrize("method", ["dopri5", "dopri8", "bosh3", "adaptive_heun"])
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
-def test_fit_eval_on_each_rows_times_bitwise(method, dtype):
+def test_fit_eval_reads_each_rows_table_bitwise(method, dtype):
     B, D, n_out = 5, 3, 5
     eng = _engine(method, dtype, B, D, n_out=n_out)
     grid = _grid(B, n_out, 3).to(DEV)
@@ -137,8 +135,8 @@ def test_fit_eval_on_each_rows_times_bitwise(method, dtype):
         F(_lib.ROWS_FIT_DT, torch.float64)[r] = t1 - t0
         F(_lib.ROWS_EMIT_LO, torch.int32)[r] = lo
         F(_lib.ROWS_EMIT_HI, torch.int32)[r] = hi
-    _lib.check(eng.lib.tdq_rows_fit_eval_grid(eng.ctrl.data_ptr(), eng.rows.data_ptr(), C.byref(eng.tab), eng.dt_code,
-                                              y1.data_ptr(), kp, eng.solution.data_ptr(), B, D, _stream()))
+    _lib.check(eng.lib.tdq_rows_fit_eval(eng.ctrl.data_ptr(), eng.rows.data_ptr(), C.byref(eng.tab), eng.dt_code,
+                                         y1.data_ptr(), kp, eng.solution.data_ptr(), B, D, _stream()))
     torch.cuda.synchronize()
     sol = eng.solution.cpu()
     yb, kb = [b.cpu() for b in eng.ybuf], [b.cpu() for b in eng.kbuf]

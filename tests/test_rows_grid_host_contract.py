@@ -1,7 +1,5 @@
 """CPU checks of per-row output times with independent rows: tdq_rows_init_grid's refusals before the device is touched
 (every pointer is fake), and the host validation of a [B, T] t."""
-import ctypes as C
-
 import pytest
 import torch
 
@@ -34,35 +32,6 @@ def test_init_grid_refuses_before_touching_the_device(lib):
         refused(L.tdq_rows_init_grid(P, P, 0, n_rows, P, 3, None), "n_rows out of range")
     assert L.tdq_rows_init_grid(P, P, 2, 4, P, 3, None) != 0
     assert L.tdq_last_error().decode() == "unsupported dtype 2"
-
-
-def test_grid_launchers_refuse_before_touching_the_device(lib):
-    """The per-row-table launchers check their arguments as the launchers without _grid do, naming themselves."""
-    L = lib.load()
-    P = 16
-    ks = lib.ptr_array([P] * 7)
-
-    def refused(rc, fn, msg):
-        assert rc != 0 and L.tdq_last_error().decode() == "%s: %s" % (fn, msg)
-
-    null, nrows, rlen = "null argument", "n_rows out of range", "row_len must be at least 1"
-    fn = "tdq_rows_controller_grid"
-    refused(L.tdq_rows_controller_grid(P, P, 0, None, 4, 8, None), fn, null)
-    refused(L.tdq_rows_controller_grid(P, P, 0, P, 0, 8, None), fn, nrows)
-    refused(L.tdq_rows_controller_grid(P, P, 0, P, 4, 0, None), fn, rlen)
-    fn = "tdq_rows_controller_event_grid"
-    refused(L.tdq_rows_controller_event_grid(P, P, 0, P, P, P, P, None, 4, 8, 1, None), fn, null)
-    refused(L.tdq_rows_controller_event_grid(P, P, 0, P, P, P, P, P, 4, 8, 0, None), fn, "K out of range")
-    fn = "tdq_rows_fit_eval_grid"
-    tab = C.byref(lib.tableau("dopri5"))
-    refused(L.tdq_rows_fit_eval_grid(P, P, tab, 0, P, ks, None, 4, 8, None), fn, null)
-    refused(L.tdq_rows_fit_eval_grid(P, P, tab, 0, P, lib.ptr_array([P] * 6 + [None]), P, 4, 8, None), fn,
-            "k_S is required")
-    refused(L.tdq_rows_fit_eval_grid(P, P, tab, 0, P, ks, P, 4, 0, None), fn, rlen)
-    for call in (lambda: L.tdq_rows_controller_grid(P, P, 5, P, 4, 8, None),
-                 lambda: L.tdq_rows_controller_event_grid(P, P, 5, P, P, P, P, P, 4, 8, 1, None),
-                 lambda: L.tdq_rows_fit_eval_grid(P, P, tab, 5, P, ks, P, 4, 8, None)):
-        assert call() != 0 and L.tdq_last_error().decode() == "unsupported dtype 5"
 
 
 def _rows(*rows, dtype=torch.float64):

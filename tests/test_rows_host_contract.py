@@ -70,6 +70,7 @@ def test_rows_launchers_refuse_before_touching_the_device(lib):
     refused(L.tdq_rows_prepare(P, P, 0, None, 0, None), "tdq_rows_prepare", nrows)
     refused(L.tdq_rows_controller(P, P, 0, None, 4, 8, None), "tdq_rows_controller", null)
     refused(L.tdq_rows_controller(P, P, 0, P, 0, 8, None), "tdq_rows_controller", nrows)
+    refused(L.tdq_rows_controller(P, P, 0, P, 4, 0, None), "tdq_rows_controller", rlen)
 
     fn, missing = "tdq_rows_combine", "missing stage slot for a non-zero tableau entry"
     refused(L.tdq_rows_combine(P, None, tab("dopri5"), 0, 2, P, ks(6), 4, 8, None), fn, null)
@@ -95,5 +96,6 @@ def test_rows_launchers_refuse_before_touching_the_device(lib):
             "missing stage slot for a non-zero mid-point weight")
     refused(L.tdq_rows_fit_eval(P, P, tab("dopri5"), 0, P, ks(6), P, 4, 0, None), fn, rlen)
     # an unsupported dtype is refused by every dtype-dispatching launcher after its argument checks
-    assert L.tdq_rows_controller(P, P, 5, P, 4, 8, None) != 0
-    assert L.tdq_last_error().decode() == "unsupported dtype 5"
+    for call in (lambda: L.tdq_rows_controller(P, P, 5, P, 4, 8, None),
+                 lambda: L.tdq_rows_fit_eval(P, P, tab("dopri5"), 5, P, ks(6), P, 4, 8, None)):
+        assert call() != 0 and L.tdq_last_error().decode() == "unsupported dtype 5"

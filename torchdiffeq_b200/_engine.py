@@ -1026,7 +1026,6 @@ class RowsEngine(AdaptiveEngine):
         self.ev_fn = None                # set by solve_until_event: the attempt then tests each row's event
         self.grid = None                 # per-row output times [B, T] of the solve in progress, or None
         self._next_grid = None           # what solve(grid=...) hands to the next _begin
-        self._graph_grid = False         # the captured attempt launches the per-row-table kernels
 
     def solve(self, y0_flat, t64, t_start=None, grid=None):
         """AdaptiveEngine.solve, or with `grid` (an ascending float64 [B, T] device tensor) per-row output times: row r
@@ -1046,13 +1045,8 @@ class RowsEngine(AdaptiveEngine):
 
     def _begin(self, y0_flat, t64, t_start=None, loop=False):
         """AdaptiveEngine._begin with the grid solve() was given, or none: every other way into a solve (prime, a direct
-        _begin) runs on the shared times.  The per-row-table and shared-times attempts launch different kernels, so a
-        captured attempt of the other kind is dropped."""
+        _begin) runs on the shared times."""
         self.grid = self._next_grid
-        if (self.grid is not None) != self._graph_grid:
-            self._drop_graph()
-            self._graph_grid = self.grid is not None
-            loop = False
         return super()._begin(y0_flat, t64, t_start, loop)
 
     def _rows_sumsq(self, x, x2, out):
@@ -1089,18 +1083,15 @@ class RowsEngine(AdaptiveEngine):
             self.rtol_vec.data_ptr() if self.rtol_vec is not None else None,
             self.atol_vec.data_ptr() if self.atol_vec is not None else None,
             B, D, self.row_partials.data_ptr(), self.row_norm.data_ptr(), st))
-        grid = self.grid is not None                 # the per-row-table kernels read each row's own times
         if self.ev_fn is None:
-            controller = lib.tdq_rows_controller_grid if grid else lib.tdq_rows_controller
-            self._launch(controller(ctrl, rows, dc, self.row_norm.data_ptr(), B, D, st))
+            self._launch(lib.tdq_rows_controller(ctrl, rows, dc, self.row_norm.data_ptr(), B, D, st))
         else:
             # each row's event value at its candidate (ATT_T1, y1), then the controller with the sign test inside it
             torch.mul(self.row_field(_lib.ROWS_ATT_T1, torch.float64), self.opt.t_sign, out=self.ev_t)
             self._ev_call(self.y1)
-            controller = lib.tdq_rows_controller_event_grid if grid else lib.tdq_rows_controller_event
-            self._launch(controller(ctrl, rows, dc, self.row_norm.data_ptr(), self.ev_val.data_ptr(),
-                                    self.ev_init.data_ptr(), self.ev_sign0.data_ptr(), self.ev_flag.data_ptr(), B, D,
-                                    self.K, st))
+            self._launch(lib.tdq_rows_controller_event(ctrl, rows, dc, self.row_norm.data_ptr(), self.ev_val.data_ptr(),
+                                                       self.ev_init.data_ptr(), self.ev_sign0.data_ptr(),
+                                                       self.ev_flag.data_ptr(), B, D, self.K, st))
         return k, kp, keep
 
     def _attempt_back(self, kp):
@@ -1109,9 +1100,9 @@ class RowsEngine(AdaptiveEngine):
                                                      self.dt_code, self.y1.data_ptr(), kp, self.ev_flag.data_ptr(),
                                                      self.ev_coeff.data_ptr(), self.B, self.D, _stream()))
             return
-        fit_eval = self.lib.tdq_rows_fit_eval_grid if self.grid is not None else self.lib.tdq_rows_fit_eval
-        self._launch(fit_eval(self.ctrl.data_ptr(), self.rows.data_ptr(), C.byref(self.tab), self.dt_code,
-                              self.y1.data_ptr(), kp, self.solution.data_ptr(), self.B, self.D, _stream()))
+        self._launch(self.lib.tdq_rows_fit_eval(self.ctrl.data_ptr(), self.rows.data_ptr(), C.byref(self.tab),
+                                                self.dt_code, self.y1.data_ptr(), kp, self.solution.data_ptr(), self.B,
+                                                self.D, _stream()))
 
     # ---- per-row events (rk_common.py:252-262, event_handling.py:5-35) ------------------------------------------------
     def _ev_call(self, y_flat):

@@ -18,7 +18,7 @@ TDQ_MAX_RANKS = 16
  ROWS_ACCEPT, ROWS_FIT, ROWS_DONE, ROWS_STATUS, ROWS_CURSOR, ROWS_EMIT_LO, ROWS_EMIT_HI, ROWS_N_STEPS, ROWS_N_ACCEPT,
  ROWS_N_REJECT, ROWS_T_FIRST, ROWS_T_PROBE, ROWS_T_STAGE) = range(24)
 ROWS_HEADER = 255
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 
 class IpcHandle(C.Structure):
@@ -150,12 +150,9 @@ _SIGNATURES = {
     "tdq_rows_combine_final": (C.c_int, [_vp, _vp, _ptab, _i32, _vp, _vp, _pp, _sz, _sz, _vp]),
     "tdq_rows_error_norm_commit": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _vp, _vp, _vp]),
     "tdq_rows_controller": (C.c_int, [_vp, _vp, _i32, _vp, _sz, _sz, _vp]),
-    "tdq_rows_controller_grid": (C.c_int, [_vp, _vp, _i32, _vp, _sz, _sz, _vp]),
     "tdq_rows_fit_eval": (C.c_int, [_vp, _vp, _ptab, _i32, _vp, _pp, _vp, _sz, _sz, _vp]),
-    "tdq_rows_fit_eval_grid": (C.c_int, [_vp, _vp, _ptab, _i32, _vp, _pp, _vp, _sz, _sz, _vp]),
     "tdq_rows_event_init": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _sz, _i32, _vp]),
     "tdq_rows_controller_event": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _i32, _vp]),
-    "tdq_rows_controller_event_grid": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _i32, _vp]),
     "tdq_rows_fit_store": (C.c_int, [_vp, _vp, _ptab, _i32, _vp, _pp, _vp, _vp, _sz, _sz, _vp]),
     "tdq_rows_event_bisect": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                         _sz, _sz, _i32, _vp]),

@@ -35,10 +35,9 @@ template <typename X> __device__ __forceinline__ X *fld(const Rows &R, int which
 }
 __device__ __forceinline__ int *hdr(const Rows &R) { return reinterpret_cast<int *>(R.base); }
 
-// Row r's output times in the per-row-table kernels (template parameter GRID, the tdq_rows_*_grid entry points): its own row
-// of the [B, n] table set by tdq_rows_init_grid (c.row_t), or the shared c.t_out when none is set.  The values are read as
-// they are stored, so a table whose rows all equal t_out gives the arithmetic of the shared one bit for bit.  The kernels
-// of the shared-times entry points (GRID = false) read c.t_out / c.n_out directly and compile as they did without tables.
+// Row r's output times: its own row of the [B, n] table set by tdq_rows_init_grid (c.row_t), or the shared c.t_out
+// when none is set.  The values are read as they are stored, so a table whose rows all equal t_out gives the arithmetic
+// of the shared one bit for bit.
 struct RowTimes {
     const double *t;
     int n;
@@ -323,7 +322,7 @@ template <typename T, int NK> struct RowQuartic {
     }
 };
 
-template <typename T, int NK, bool GRID>
+template <typename T, int NK>
 __global__ void __launch_bounds__(kThreads)
 k_rows_fit_eval(const TdqCtrl *__restrict__ c, Rows R, Geom g, const T *__restrict__ y1p, const T *__restrict__ kSp,
                 KPtrs kmid, T *__restrict__ solution, size_t n) {
@@ -334,13 +333,13 @@ k_rows_fit_eval(const TdqCtrl *__restrict__ c, Rows R, Geom g, const T *__restri
     const RowQuartic<T, NK> q(c, R, r, base, y1p, kSp, kmid);
     const int jlo = fld<int>(R, TDQ_ROWS_EMIT_LO)[r], jhi = fld<int>(R, TDQ_ROWS_EMIT_HI)[r];
     const double t0 = fld<double>(R, TDQ_ROWS_T0)[r], t1 = fld<double>(R, TDQ_ROWS_T1)[r];
-    const double *t_row = GRID ? row_times(*c, r).t : nullptr;
+    const double *t_row = row_times(*c, r).t;
     const int lane = threadIdx.x & 31;
     for (size_t i = lo + lane; i < hi; i += 32) {
         T e, d, cq, b, a;
         q.at(i, e, d, cq, b, a);
         for (int j = jlo; j < jhi; ++j) {
-            const T x = (T)(((GRID ? t_row : c->t_out)[j] - t0) / (t1 - t0));
+            const T x = (T)((t_row[j] - t0) / (t1 - t0));
             solution[(size_t)j * n + base + i] = tdq_eval_poly<T>(e, d, cq, b, a, x);
         }
     }
@@ -381,7 +380,7 @@ struct NoEvent {
 // whether the row's event fires in this attempt (rk_common.py:259): such a row is done, keeps the accepted step as
 // [T0, T1] and takes no next attempt, so neither a non-finite y1 nor max_num_steps can fail it (the reference tests the
 // sign before it would take that attempt).
-template <typename T, bool GRID = false, typename Event = NoEvent>
+template <typename T, typename Event = NoEvent>
 __device__ void row_control(const TdqCtrl &c, const Rows &R, int r, double sumsq, double n_bad, size_t D,
                             Event event = Event{}) {
     double ratio = tdq_rms<T>(sumsq, (double)D, c.ratio_f64);
@@ -409,21 +408,17 @@ __device__ void row_control(const TdqCtrl &c, const Rows &R, int r, double sumsq
     fld<int>(R, TDQ_ROWS_EMIT_LO)[r] = cur;
     int64_t *steps = fld<int64_t>(R, TDQ_ROWS_N_STEPS);
     steps[r] += 1;
+    const RowTimes times = row_times(c, r);
     if (accept) {
         const double t1 = fld<double>(R, TDQ_ROWS_T1)[r];
         const int c0 = cur;
-        if constexpr (GRID) {
-            const RowTimes times = row_times(c, r);
-            cur = tdq_cursor_after(times.t, times.n, cur, t1);
-        } else {
-            cur = tdq_cursor_after(c.t_out, c.n_out, cur, t1);
-        }
+        cur = tdq_cursor_after(times.t, times.n, cur, t1);
         if (cur != c0) steps[r] = 0;
         fld<int>(R, TDQ_ROWS_CURSOR)[r] = cur;
     }
     fld<int>(R, TDQ_ROWS_EMIT_HI)[r] = cur;
     fld<int>(R, TDQ_ROWS_FIT)[r] = (accept && cur > fld<int>(R, TDQ_ROWS_EMIT_LO)[r]) ? 1 : 0;
-    const bool done = cur >= (GRID ? row_times(c, r).n : c.n_out) || fired;
+    const bool done = cur >= times.n || fired;
     fld<int>(R, TDQ_ROWS_DONE)[r] = done ? 1 : 0;
     if (status[r] == TDQ_RUN_OK && !done) row_prepare<T>(c, R, r, false);
 }
@@ -501,7 +496,7 @@ __global__ void __launch_bounds__(kThreads) k_rows_init(const TdqCtrl *__restric
     row_init<T>(c, R, r, t_start, c->n_out);
 }
 
-// Row r starts at grid[r, 0]; the table is recorded in the control block for the per-row-table kernels.
+// Row r starts at grid[r, 0]; the table is recorded in the control block, where the controller and the fit read it.
 template <typename T>
 __global__ void __launch_bounds__(kThreads) k_rows_init_grid(TdqCtrl *c, Rows R, const double *__restrict__ grid,
                                                              int n_grid) {
@@ -592,7 +587,7 @@ __device__ __forceinline__ double ev_combined(const double *val, const double *i
     return m;
 }
 
-template <typename T, bool EVENT, bool GRID>
+template <typename T, bool EVENT>
 __global__ void __launch_bounds__(kThreads)
 k_rows_controller(TdqCtrl *c, Rows R, const double *norm_in, size_t D, RowEvents ev) {
     const int r = blockIdx.x * kThreads + threadIdx.x;
@@ -623,13 +618,13 @@ k_rows_controller(TdqCtrl *c, Rows R, const double *norm_in, size_t D, RowEvents
         } else {
             if (EVENT) {
                 // an accepted candidate whose combined sign differs from sign0 ends the row
-                row_control<T, GRID>(*c, R, r, norm_in[r], norm_in[R.B + r], D, [&](bool accept) {
+                row_control<T>(*c, R, r, norm_in[r], norm_in[R.B + r], D, [&](bool accept) {
                     const bool fired = accept && !(sign_of(ev_combined(ev.val, ev.init, ev.K, r)) == ev.sign0[r]);
                     ev.flag[r] = fired ? 1 : 0;
                     return fired;
                 });
             } else {
-                row_control<T, GRID>(*c, R, r, norm_in[r], norm_in[R.B + r], D);
+                row_control<T>(*c, R, r, norm_in[r], norm_in[R.B + r], D);
             }
             failed = fld<int>(R, TDQ_ROWS_STATUS)[r] != TDQ_RUN_OK;
             running = !fld<int>(R, TDQ_ROWS_DONE)[r];
@@ -767,7 +762,8 @@ int tdq_rows_init(void *ctrl_dev, void *rows_dev, int32_t dtype, size_t n_rows, 
     TDQ_DISPATCH_T(dtype, (k_rows_init<T><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
                                (const TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), t_start)));
     TDQ_CHECK_CUDA(cudaGetLastError());
-    // no per-row table in this solve: a table left by an earlier tdq_rows_init_grid is cleared
+    // no per-row table in this solve: clearing one left by an earlier tdq_rows_init_grid is what makes the controller
+    // and the fit read the control block's t_out
     TDQ_CHECK_CUDA(cudaMemsetAsync((char *)ctrl_dev + offsetof(TdqCtrl, row_t), 0,
                                    sizeof(TdqCtrl) - offsetof(TdqCtrl, row_t), (cudaStream_t)stream));
     return TDQ_OK;
@@ -922,29 +918,14 @@ int tdq_rows_combine_final(void *ctrl_dev, void *rows_dev, const tdq_tableau *ta
     return TDQ_OK;
 }
 
-static int rows_controller(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in, size_t n_rows,
-                           size_t row_len, bool grid, void *stream) {
-    TDQ_DISPATCH_T(dtype, tdq_dispatch(TdqBool{}, grid, [&](auto GRID) {
-        k_rows_controller<T, false, GRID><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
-            (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), norm_in, row_len, RowEvents{});
-        return 0;
-    }));
-    TDQ_CHECK_CUDA(cudaGetLastError());
-    return TDQ_OK;
-}
-
 int tdq_rows_controller(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in, size_t n_rows,
                         size_t row_len, void *stream) {
     TDQ_REQUIRE(ctrl_dev && rows_dev && norm_in, "null argument");
     TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
-    return rows_controller(ctrl_dev, rows_dev, dtype, norm_in, n_rows, row_len, false, stream);
-}
-
-int tdq_rows_controller_grid(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in, size_t n_rows,
-                             size_t row_len, void *stream) {
-    TDQ_REQUIRE(ctrl_dev && rows_dev && norm_in, "null argument");
-    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
-    return rows_controller(ctrl_dev, rows_dev, dtype, norm_in, n_rows, row_len, true, stream);
+    TDQ_DISPATCH_T(dtype, (k_rows_controller<T, false><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), norm_in, row_len, RowEvents{})));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
 }
 
 #define TDQ_ROWS_REQUIRE_K(K) TDQ_REQUIRE((K) >= 1 && (K) <= 65536, "K out of range")
@@ -960,35 +941,17 @@ int tdq_rows_event_init(void *rows_dev, const double *ev_val, double *init_sign,
     return TDQ_OK;
 }
 
-static int rows_controller_event(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in, const RowEvents &ev,
-                                 size_t n_rows, size_t row_len, bool grid, void *stream) {
-    TDQ_DISPATCH_T(dtype, tdq_dispatch(TdqBool{}, grid, [&](auto GRID) {
-        k_rows_controller<T, true, GRID><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
-            (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), norm_in, row_len, ev);
-        return 0;
-    }));
-    TDQ_CHECK_CUDA(cudaGetLastError());
-    return TDQ_OK;
-}
-
 int tdq_rows_controller_event(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in, const double *ev_val,
                               const double *init_sign, const double *sign0, int32_t *flag, size_t n_rows, size_t row_len,
                               int32_t K, void *stream) {
     TDQ_REQUIRE(ctrl_dev && rows_dev && norm_in && ev_val && init_sign && sign0 && flag, "null argument");
     TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
     TDQ_ROWS_REQUIRE_K(K);
-    return rows_controller_event(ctrl_dev, rows_dev, dtype, norm_in, RowEvents{ev_val, init_sign, sign0, flag, K}, n_rows,
-                                 row_len, false, stream);
-}
-
-int tdq_rows_controller_event_grid(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *norm_in,
-                                   const double *ev_val, const double *init_sign, const double *sign0, int32_t *flag,
-                                   size_t n_rows, size_t row_len, int32_t K, void *stream) {
-    TDQ_REQUIRE(ctrl_dev && rows_dev && norm_in && ev_val && init_sign && sign0 && flag, "null argument");
-    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
-    TDQ_ROWS_REQUIRE_K(K);
-    return rows_controller_event(ctrl_dev, rows_dev, dtype, norm_in, RowEvents{ev_val, init_sign, sign0, flag, K}, n_rows,
-                                 row_len, true, stream);
+    TDQ_DISPATCH_T(dtype, (k_rows_controller<T, true><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), norm_in, row_len,
+                               RowEvents{ev_val, init_sign, sign0, flag, K})));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
 }
 
 int tdq_rows_fit_store(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, const void *y1,
@@ -1037,39 +1000,30 @@ int tdq_rows_event_bisect(void *ctrl_dev, void *rows_dev, int32_t dtype, int32_t
     return TDQ_OK;
 }
 
-// Checks and launch of tdq_rows_fit_eval / _grid; the messages name the entry point (TDQ_REQUIRE's __func__).
-#define TDQ_ROWS_FIT_EVAL(GRID_FLAG)                                                                                     \
-    TDQ_REQUIRE(ctrl_dev && rows_dev && tab && y1 && k && solution, "null argument");                                   \
-    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);                                                                             \
-    TdqHostShape hs;                                                                                                     \
-    tdq_shape_from_tableau(tab, &hs);                                                                                    \
-    const int S = hs.n_stages, nk = hs.mid_nnz;                                                                          \
-    TDQ_REQUIRE(nk >= 1, "tableau has no mid-point weights");                                                           \
-    TDQ_REQUIRE(k[S] != nullptr, "k_S is required");                                                                     \
-    KPtrs kmid;                                                                                                          \
-    bool vec = true;                                                                                                     \
-    TDQ_REQUIRE(plan_kp(hs.mid_idx, nk, k, kmid, vec), "missing stage slot for a non-zero mid-point weight");            \
-    const Geom g = make_geom(n_rows, row_len);                                                                           \
-    const Rows R = make_rows(rows_dev, n_rows);                                                                          \
-    int rc = -1;                                                                                                         \
-    TDQ_DISPATCH_T(dtype, rc = tdq_dispatch(TdqRange<1, TDQ_MAX_K>{}, nk, [&](auto NK) {                                 \
-                       k_rows_fit_eval<T, NK, GRID_FLAG><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(        \
-                           (const TdqCtrl *)ctrl_dev, R, g, (const T *)y1, (const T *)k[S], kmid, (T *)solution,        \
-                           n_rows * row_len);                                                                            \
-                       return 0;                                                                                         \
-                   }));                                                                                                  \
-    TDQ_REQUIRE(rc == 0, "unsupported number of mid-point terms");                                                      \
-    TDQ_CHECK_CUDA(cudaGetLastError());                                                                                  \
-    return TDQ_OK
-
 int tdq_rows_fit_eval(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, const void *y1,
                       const void *const *k, void *solution, size_t n_rows, size_t row_len, void *stream) {
-    TDQ_ROWS_FIT_EVAL(false);
-}
-
-int tdq_rows_fit_eval_grid(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, const void *y1,
-                           const void *const *k, void *solution, size_t n_rows, size_t row_len, void *stream) {
-    TDQ_ROWS_FIT_EVAL(true);
+    TDQ_REQUIRE(ctrl_dev && rows_dev && tab && y1 && k && solution, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TdqHostShape hs;
+    tdq_shape_from_tableau(tab, &hs);
+    const int S = hs.n_stages, nk = hs.mid_nnz;
+    TDQ_REQUIRE(nk >= 1, "tableau has no mid-point weights");
+    TDQ_REQUIRE(k[S] != nullptr, "k_S is required");
+    KPtrs kmid;
+    bool vec = true;
+    TDQ_REQUIRE(plan_kp(hs.mid_idx, nk, k, kmid, vec), "missing stage slot for a non-zero mid-point weight");
+    const Geom g = make_geom(n_rows, row_len);
+    const Rows R = make_rows(rows_dev, n_rows);
+    int rc = -1;
+    TDQ_DISPATCH_T(dtype, rc = tdq_dispatch(TdqRange<1, TDQ_MAX_K>{}, nk, [&](auto NK) {
+                       k_rows_fit_eval<T, NK><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(
+                           (const TdqCtrl *)ctrl_dev, R, g, (const T *)y1, (const T *)k[S], kmid, (T *)solution,
+                           n_rows * row_len);
+                       return 0;
+                   }));
+    TDQ_REQUIRE(rc == 0, "unsupported number of mid-point terms");
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
 }
 
 }  // extern "C"

@@ -524,7 +524,7 @@ def _func_signature(func, explicit=False):
     return None
 
 
-def _cache_key(p, extra=()):
+def _cache_key(p):
     o = p.options
     if (o.get("cache", True) is False or p.callbacks or p.norm_fn is not None or p.rtol_vec is not None
             or p.atol_vec is not None):
@@ -542,7 +542,7 @@ def _cache_key(p, extra=()):
     shapes = tuple(tuple(s_) for s_ in p.layout.shapes) if p.is_tuple else tuple(p.shape)
     try:
         key = (fsig, p.method, p.dtype, str(p.device), p.is_tuple, shapes, p.rtol, p.atol,
-               p.t_sign, tuple(items), torch.is_autocast_enabled(), extra)
+               p.t_sign, tuple(items), torch.is_autocast_enabled())
         hash(key)
     except TypeError:
         return None
@@ -585,8 +585,7 @@ def last_stats():
 def _solve(p):
     """Run the normalised problem; returns the flat solution [len(t), n] and the engine."""
     if p.method in ADAPTIVE_METHODS:
-        row_grid = p.t_cpu.dim() == 2                   # per-row output times (independent rows): data, not part of the key
-        key = _cache_key(p, extra=("row_grid",) if row_grid else ())
+        key = _cache_key(p)
         hit = _cache_get(key)
         if hit is not None:
             eng = hit[0]
@@ -595,7 +594,7 @@ def _solve(p):
             _cache_put(key, (eng, p.original_func))     # the func reference keeps id(func) from being recycled
         t64 = p.t_cpu.to(torch.float64).to(p.device)                                   # solvers.py:31
         try:
-            if row_grid:
+            if p.t_cpu.dim() == 2:                      # per-row output times (independent rows): data, not in the key
                 sol = eng.solve(p.y0_flat, None, t_start=float(p.t_cpu[0, 0]), grid=t64)
             else:
                 sol = eng.solve(p.y0_flat, t64, t_start=float(p.t_cpu[0]))
