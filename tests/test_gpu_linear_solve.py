@@ -39,7 +39,7 @@ def _solve(W, y0, t, method="dopri5", cache=False, **opts):
 
 def _persistent(st):
     """a fused solve that ran as one launch: the start-up's ten launches at most, + 1, whatever the number of attempts"""
-    return bool(st["fused_attempt"]) and st["launches"] <= 11
+    return bool(st["fused_attempt"]) and st["launches"] <= 11 and st["driver"] == "persistent"
 
 
 def _same(a, b):
@@ -118,6 +118,7 @@ def test_other_modes_take_the_per_attempt_path(opts):
     else:
         st = _solve(W, y0, t, **opts)[1]
     assert st["launches"] > st["attempts"], st
+    assert st["driver"] == ("lockstep" if opts.get("run_ahead") == 0 else "capture"), st
 
 
 def _failure(W, y0, t, **opts):

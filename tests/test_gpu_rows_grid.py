@@ -152,10 +152,11 @@ def test_grid_is_scoped_to_its_solve():
     (eng, _), = M._ENGINE_CACHE.values()
     with torch.no_grad():
         assert eng.grid is not None
-        eng._begin(y0.reshape(-1), t1, 0.0)
+        driver = eng._begin(y0.reshape(-1), t1, 0.0)
         torch.cuda.synchronize()
         # the captured attempt is dropped only because the solution's shape changed: T = 5 in the table, 4 here
         assert eng.grid is None and eng._graph is None
+        assert driver == "capture"
         assert torch.equal(_f_t0(eng), torch.zeros(B, dtype=torch.float64))
         assert torch.equal(eng.solve(y0.reshape(-1), t1, t_start=0.0).view(T, B, D), fresh)
     torch.cuda.synchronize()
@@ -181,8 +182,10 @@ def test_one_captured_attempt_serves_table_and_shared_times():
         (eng, _), = M._ENGINE_CACHE.values()
         graph = eng._graph
         assert graph is not None and eng._loop is not None
+        assert eng.driver == "capture"
         got[second] = _run(m, y0, ta if second == "table" else t1, options=L)
         assert len(M._ENGINE_CACHE) == 1 and eng._graph is graph and eng._loop is not None
+        assert eng.driver == "loop"
         for kind in (first, second):
             assert torch.equal(_bits(got[kind][0]), _bits(fresh[kind][0])), (first, kind)
             assert torch.equal(got[kind][1], fresh[kind][1]) and torch.equal(got[kind][2], fresh[kind][2]), (first, kind)

@@ -863,6 +863,7 @@ def test_adjoint_many_parameter_tensors(norm, mode):
         (bs, _), = list(_BACKWARD_CACHE.values())[-1:]
         assert bs.eng.norm_fn is None and bs.eng.n_seg == (83 if norm == "default" else 3)
         assert bs.eng._graph is not None and bs.eng._loop is not None       # captured and looping on the device
+        assert bs.eng.driver == "loop"
 
 
 AD = ld("adams.pt")

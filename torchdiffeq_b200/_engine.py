@@ -173,6 +173,24 @@ def find_event(interp_fn, sign0, t0, t1, event_fn, tol):
     return event_t, interp_fn(event_t)
 
 
+def choose_driver(*, lockstep, fused_solve, device_loop, agree_fn, norm_fn, exchange, keep_interp, has_loop, has_graph,
+                  graph, graph_failed, capture_in_solve):
+    """The driver of one adaptive solve (AdaptiveEngine._run), from what the engine holds once its solution buffer has
+    the solve's shape.  fused_solve: a whole-attempt linear field with the norm folded in, never refused.  device_loop
+    and graph are options (True / False / 'auto'), the rest bools; agree_fn / norm_fn: host work between attempts."""
+    if lockstep:
+        return "lockstep"
+    if fused_solve and device_loop in (True, "auto") and not (agree_fn or norm_fn or exchange or keep_interp):
+        return "persistent"
+    if has_loop and not (agree_fn or norm_fn):
+        return "loop"
+    if has_graph:
+        return "replay"
+    if graph in (True, "auto") and not graph_failed and capture_in_solve:
+        return "capture"
+    return "eager"
+
+
 class AdaptiveEngine:
     """One adaptive explicit-RK solve on a flat state vector, all state on the device.
 
@@ -218,7 +236,6 @@ class AdaptiveEngine:
         if self.callbacks or (jump_t is not None and jump_t.numel() > 0):
             # both need the host between attempts: callbacks by definition, jump_t because f is re-evaluated on
             # the far side of the discontinuity after the step that lands on it (rk_common.py:346-351)
-            self.graph_opt = False
             self.run_ahead = 0
 
         segs = segs if segs is not None else [(0, self.n)]
@@ -294,7 +311,8 @@ class AdaptiveEngine:
         self._loop_handle = 0
         self._loop_failed = False
         self._solve_scratch = None       # tdq_linear_solve's barrier words and partials (engine-owned)
-        self._solve_refused = False      # the device refused its cooperative launch: attempts take the loop below
+        self._solve_refused = False      # the device refused its cooperative launch: no persistent solve again
+        self.driver = None               # the driver of the last solve (choose_driver), after any refusal fallback
         self._always_copy = False        # set when func is seen to reuse its output buffer (see _call_fn)
         self.linear = None               # set_linear(): every stage fused with a linear field (csrc/tdq_linear.cu)
         self.capture_in_solve = True     # False: only a prime()d graph is used (solves run inside autograd backward)
@@ -555,26 +573,27 @@ class AdaptiveEngine:
             raise SolverFailure("max_num_steps exceeded ({}>={})".format(m, m) + where)
         raise SolverFailure("solver failed with status %d" % s + where)
 
-    def _lockstep_mode(self):
-        return bool(self.callbacks) or self.run_ahead == 0
+    def _plan(self, priming=False):
+        """choose_driver on this engine.  priming: prime() captures for solves that may not (capture_in_solve off)."""
+        return choose_driver(
+            lockstep=self.run_ahead == 0, device_loop=self.device_loop, graph=self.graph_opt,
+            fused_solve=self.linear is not None and self.linear["fold"] and not self._solve_refused,
+            agree_fn=self.agree_fn is not None, norm_fn=self.norm_fn is not None, exchange=self.exchange is not None,
+            has_loop=self._loop is not None, has_graph=self._graph is not None, graph_failed=self._graph_failed,
+            capture_in_solve=self.capture_in_solve or priming, keep_interp=self.keep_interp)
 
-    def _use_loop(self):
-        """Run this solve inside the device-side while loop?  Needs the captured attempt and a body without
-        collectives launched by the host between attempts."""
-        return (self._loop is not None and not self._lockstep_mode() and self.agree_fn is None
-                and self.norm_fn is None)
-
-    def solve(self, y0_flat, t64, t_start=None):
+    def solve(self, y0_flat, t64, t_start=None, grid=None):
         """Integrate from t64[0] through t64[-1] (ascending float64 device tensor); returns
         solution [len(t), n] (solvers.py:28-35).  The returned tensor is owned by the engine and is
-        overwritten by the next solve() with the same number of output times."""
+        overwritten by the next solve() with the same number of output times.  grid: see RowsEngine.solve."""
         try:
-            if self._lockstep_mode():
-                for _ in self._lockstep(y0_flat, t64, t_start):
+            driver = self.driver = self._begin(y0_flat, t64, t_start, grid)
+            if driver == "lockstep":
+                for _ in self._lockstep_attempts():
                     pass
             else:
-                if self._begin(y0_flat, t64, t_start, loop=self._use_loop()) > 1:
-                    self._loop_run_ahead()
+                if self.solution.shape[0] > 1:
+                    self._run(driver)
                 self._read_counters()
         except BaseException:
             # attempts may still be queued: let them drain before anybody resets the mailbox, and do not let a
@@ -598,30 +617,33 @@ class AdaptiveEngine:
         attempt, then capture).  Used by odeint_adjoint to capture the backward step body during the
         FORWARD call: capturing inside autograd's backward is unsafe (a re-entrant engine call may run
         unrelated nodes of the outer graph on the legacy stream in the middle of the capture)."""
-        if self.graph_opt not in (True, "auto") or self._lockstep_mode():
+        self._solution_for(int(t64.numel()))
+        if self._plan(priming=True) != "capture":
             return False
-        n_out = self._begin(y0_flat, t64, t_start)
-        if n_out <= 1:
+        self._begin(y0_flat, t64, t_start)
+        if self.solution.shape[0] <= 1:
             return False
-        self._warm_attempt()
+        self._attempt()                  # a real attempt that doubles as the warm-up torch wants before capture
         self._capture()
         torch.cuda.current_stream().synchronize()
         return self._graph is not None
 
-    def _begin(self, y0_flat, t64, t_start=None, loop=False):
+    def _solution_for(self, n_out):
+        if self.solution is None or self.solution.shape[0] != n_out:    # a captured graph holds its address
+            self.solution = torch.empty(n_out, self.n, dtype=self.dtype, device=self.device)
+            self._drop_graph()
+            self._own_ptrs = None
+
+    def _begin(self, y0_flat, t64, t_start=None, grid=None):
         """Everything of a solve that precedes the first attempt (rk_common.py:166-241): the per-solve reset of the
-        engine and the control block, then `_start`.  Returns the number of output times."""
+        engine and the control block, then `_start`.  Returns the solve's driver (choose_driver)."""
         lib = self.lib
         self.nfe_total += self.nfe
         self.nfe, self.launches = 0, 0                  # per-solve counters (engines are reused)
         n_out = int(t64.numel())
         self.t_out = t64.contiguous()
-        if getattr(self, "solution", None) is None or self.solution.shape[0] != n_out:
-            # a captured graph holds this buffer's address: a new shape invalidates it
-            self.solution = torch.empty(n_out, self.n, dtype=self.dtype, device=self.device)
-            self._drop_graph()
-            self._own_ptrs = None
-            loop = False
+        self._solution_for(n_out)
+        driver = self._plan()
         self.solution[0].copy_(y0_flat)
         self.ybuf[0].copy_(y0_flat)
         st = _stream()
@@ -630,13 +652,14 @@ class AdaptiveEngine:
         mb.n_accept, mb.n_reject = 0, 0
         if t_start is None:
             t_start = float(t64[0])                                   # callers pass it whenever they hold t on the host
-        self.opt.loop_handle = self._loop_handle if loop else 0
+        # k_controller re-arms the loop through it (the persistent kernel does not read it; a refused launch may loop)
+        self.opt.loop_handle = self._loop_handle if driver in ("loop", "persistent") else 0
         _lib.check(lib.tdq_ctrl_init(self.ctrl.data_ptr(), C.byref(self.tab), C.byref(self.opt),
                                      self.t_out.data_ptr(), float(t_start), n_out, self.mbox_dev, st))
-        self._start(float(t_start), n_out)
-        return n_out
+        self._start(float(t_start), n_out, grid)
+        return driver
 
-    def _start(self, t_start, n_out):
+    def _start(self, t_start, n_out, grid=None):
         """The solve's start after the reset: the time grids, f0, the initial step and the first attempt's prepare."""
         lib = self.lib
         st = _stream()
@@ -706,9 +729,14 @@ class AdaptiveEngine:
         return issued, mb
 
     def _lockstep(self, y0_flat, t64, t_start=None):
-        """A lock-step solve: yields the mailbox once after the start and once after every attempt, until the solve is
-        done or the caller closes the generator after an attempt; it then synchronises and reads the counters."""
-        n_out = self._begin(y0_flat, t64, t_start)
+        """A lock-step solve (see _lockstep_attempts)."""
+        self.driver = self._begin(y0_flat, t64, t_start)
+        return self._lockstep_attempts()
+
+    def _lockstep_attempts(self):
+        """Yields the mailbox once after _begin and once after every attempt, until the solve is done or the caller
+        closes the generator after an attempt; it then synchronises and reads the counters."""
+        n_out = self.solution.shape[0]
         torch.cuda.current_stream().synchronize()          # first attempt's (t0, dt) and status are in the mailbox
         mb = self.mbox_host.contents
         self._raise_if_failed(mb)
@@ -795,33 +823,31 @@ class AdaptiveEngine:
         kw = dict(dtype=torch.float64, device=self.device)
         return torch.tensor(t0, **kw), torch.tensor(dt, **kw)
 
-    # ---- bounded run-ahead: no host sync, optional CUDA graph -----------------------------------
-    def _loop_run_ahead(self):
-        if self._linear_solve_ready() and self._linear_solve():
-            return
+    # ---- the drivers after _begin (lock step: _lockstep_attempts) ------------------------------
+    def _run(self, driver):
+        """Every attempt of a solve with more than one output time, by `driver` (choose_driver)."""
+        if driver == "persistent":
+            if self._linear_solve():
+                return
+            driver = self.driver = self._plan()            # refused: the same solve takes the per-attempt choice
+        if driver == "loop":
+            return self._launch_loop()
+        if driver == "replay":
+            return self._run_ahead(issued=0)
+        # capture or eager: attempt 1 runs eagerly, and doubles as the warm-up torch wants before a capture
+        self._attempt()
+        if driver == "capture":
+            self._capture()
+            if self._loop is not None:
+                # hand the rest of this solve to the loop (if the first attempt already finished it, the loop's single
+                # iteration is a no-op on the device)
+                _lib.check(self.lib.tdq_ctrl_set_loop(self.ctrl.data_ptr(), self._loop_handle, _stream()))
+                return self._launch_loop(first=1)
+        self._run_ahead(issued=1)
+
+    def _run_ahead(self, issued):
         D = max(1, self.run_ahead)
         mb = self.mbox_host.contents
-        issued = 0
-        use_graph = self.graph_opt in (True, "auto") and not self._graph_failed and self.capture_in_solve
-        if self._use_loop() and self.opt.loop_handle != 0:
-            # the whole adaptive loop is ONE graph launch: a conditional WHILE node around the captured attempt,
-            # re-armed by k_controller until the solve has finished or failed
-            self._launch_loop()
-            return
-        # attempt 1 runs eagerly: it is a real attempt and doubles as the warm-up torch wants before capture
-        if self._graph is None:
-            if use_graph:
-                self._warm_attempt()
-                self._capture()
-            else:
-                self._attempt()
-            issued += 1
-            if self._use_loop():
-                # hand the rest of this solve to the loop (if the first attempt already finished it, the loop's
-                # single iteration is a no-op on the device)
-                _lib.check(self.lib.tdq_ctrl_set_loop(self.ctrl.data_ptr(), self._loop_handle, _stream()))
-                self._launch_loop(first=1)
-                return
         while True:
             seen = mb.seq
             if mb.status != _lib.RUN_OK or mb.done:
@@ -829,38 +855,27 @@ class AdaptiveEngine:
             if issued - seen > D:
                 time.sleep(0)                              # the device is >D attempts behind: yield the GIL
                 continue
-            if self._graph is not None:
-                self._graph.replay()
-                self.nfe += self.S
-                self.launches += self._graph_launches
-            else:
-                self._attempt()
+            self._queue_attempt()
             issued += 1
         if self.agree_fn is not None:
             # every attempt holds a collective: all ranks must have queued the same number before anyone
             # waits for its stream (trailing attempts are no-ops on the device)
             target = self.agree_fn(issued)
             while issued < target:
-                if self._graph is not None:
-                    self._graph.replay()
-                    self.nfe += self.S
-                    self.launches += self._graph_launches
-                else:
-                    self._attempt()
+                self._queue_attempt()
                 issued += 1
         mb = self._wait_seq(issued)
         self._raise_if_failed(mb)
         torch.cuda.current_stream().synchronize()
 
-    persistent_linear = True             # RowsEngine: per-row control blocks, no persistent solve
-
-    def _linear_solve_ready(self):
-        """Can this solve's attempts run as ONE persistent launch (tdq_linear_solve)?  Whole-attempt linear field with the
-        norm folded in, and a solve the device loop would run: no host work between attempts and no stored interpolants."""
-        L = self.linear
-        return (L is not None and L["whole"] and L["fold"] and self.persistent_linear and not self._solve_refused
-                and self.device_loop in (True, "auto") and not self._lockstep_mode() and self.agree_fn is None
-                and self.norm_fn is None and self.exchange is None and not self.keep_interp)
+    def _queue_attempt(self):
+        """A replay of the captured attempt, or an eager attempt when there is none."""
+        if self._graph is not None:
+            self._graph.replay()
+            self.nfe += self.S
+            self.launches += self._graph_launches
+        else:
+            self._attempt()
 
     def _linear_solve(self):
         """Every attempt of the solve in one cooperative launch (csrc/tdq_attempt.cu k_linear_solve): the attempt, the
@@ -885,6 +900,7 @@ class AdaptiveEngine:
         return True
 
     def _launch_loop(self, first=0):
+        """The rest of the solve as ONE launch of the device-side WHILE loop; `first` attempts ran before it."""
         _lib.check(self.lib.tdq_loop_launch(self._loop, _stream()))
         torch.cuda.current_stream().synchronize()
         mb = self.mbox_host.contents
@@ -892,11 +908,6 @@ class AdaptiveEngine:
         self.nfe += self.S * ran
         self.launches += self._graph_launches * ran
         self._raise_if_failed(mb)
-
-    def _warm_attempt(self):
-        """The first attempt of a solve that is about to be captured: a real attempt that doubles as the
-        warm-up torch wants before capture (we are already on the solver stream, never the legacy one)."""
-        self._attempt()
 
     def _capture(self):
         """Capture one attempt.  A first capture that involves autograd (the adjoint's augmented dynamics)
@@ -998,8 +1009,6 @@ class RowsEngine(AdaptiveEngine):
     time; finished rows see copies of their last state.  Stage slots, capture, the device-side loop and the run-ahead and
     lock-step drivers are AdaptiveEngine's; only the launches differ."""
 
-    persistent_linear = False
-
     def __init__(self, fn, shape, dtype, device, method, **kw):
         shape = torch.Size(shape)
         self.B = int(shape[0])
@@ -1025,7 +1034,6 @@ class RowsEngine(AdaptiveEngine):
         self.row_n_accept = self.row_n_reject = None
         self.ev_fn = None                # set by solve_until_event: the attempt then tests each row's event
         self.grid = None                 # per-row output times [B, T] of the solve in progress, or None
-        self._next_grid = None           # what solve(grid=...) hands to the next _begin
 
     def solve(self, y0_flat, t64, t_start=None, grid=None):
         """AdaptiveEngine.solve, or with `grid` (an ascending float64 [B, T] device tensor) per-row output times: row r
@@ -1037,17 +1045,7 @@ class RowsEngine(AdaptiveEngine):
                                  % (self.B, self.device, grid.dtype, tuple(grid.shape), grid.device))
             grid = grid.contiguous()
             t64 = grid[0]
-        self._next_grid = grid
-        try:
-            return super().solve(y0_flat, t64, t_start)
-        finally:
-            self._next_grid = None
-
-    def _begin(self, y0_flat, t64, t_start=None, loop=False):
-        """AdaptiveEngine._begin with the grid solve() was given, or none: every other way into a solve (prime, a direct
-        _begin) runs on the shared times."""
-        self.grid = self._next_grid
-        return super()._begin(y0_flat, t64, t_start, loop)
+        return super().solve(y0_flat, t64, t_start, grid)
 
     def _rows_sumsq(self, x, x2, out):
         self._launch(self.lib.tdq_rows_sumsq(
@@ -1163,11 +1161,12 @@ class RowsEngine(AdaptiveEngine):
                 self._ev_call(self.ytmp)
         return self.ev_event_t, self.solution
 
-    def _start(self, t_start, n_out):
+    def _start(self, t_start, n_out, grid=None):
         """rk_common.py:213-241 for every row: f0 on the whole batch, then each row's initial step."""
         lib, st = self.lib, _stream()
         ctrl, rows, dc, B, D = self.ctrl.data_ptr(), self.rows.data_ptr(), self.dt_code, self.B, self.D
-        if self.grid is not None:                                   # each row from its own grid[r, 0]
+        self.grid = grid
+        if grid is not None:                                        # each row from its own grid[r, 0]
             self._launch(lib.tdq_rows_init_grid(ctrl, rows, dc, B, self.grid.data_ptr(), n_out, st))
         else:
             self._launch(lib.tdq_rows_init(ctrl, rows, dc, B, t_start, st))

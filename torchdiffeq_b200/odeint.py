@@ -833,7 +833,8 @@ def _odeint_backprop(p, func, y0, t, params, _stats):
 
 def _publish_stats(eng, _stats, add_launches):
     """last_stats() of the solve `eng` just ran.  `_stats` (private: solver counters for bench.py and the tests) gets
-    the same counters except the per-row ones; its launches are added to what it holds when add_launches is set."""
+    the same counters except the per-row ones, and the adaptive engine's driver; its launches are added to what it holds
+    when add_launches is set."""
     _LAST_STATS.clear()
     _LAST_STATS.update(nfe=eng.nfe, launches=getattr(eng, "launches", 0), attempts=getattr(eng, "n_attempts", None),
                        n_accept=getattr(eng, "n_accept", None), n_reject=getattr(eng, "n_reject", None),
@@ -841,7 +842,7 @@ def _publish_stats(eng, _stats, add_launches):
                        fused_attempt=bool((getattr(eng, "linear", None) or {}).get("whole")))
     if _stats is not None:
         launches = _stats.get("launches", 0) if add_launches else 0
-        _stats.update(_LAST_STATS, launches=launches + _LAST_STATS["launches"])
+        _stats.update(_LAST_STATS, launches=launches + _LAST_STATS["launches"], driver=getattr(eng, "driver", None))
     if getattr(eng, "row_n_accept", None) is not None:
         _LAST_STATS.update(row_n_accept=eng.row_n_accept, row_n_reject=eng.row_n_reject)
 
