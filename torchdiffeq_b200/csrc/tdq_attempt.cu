@@ -15,13 +15,14 @@
 // (tdq_tc.cuh tile_product) -- k_i, y1 and the error-sum prefix are BITWISE what tdq_linear_stage writes, (err/tol)^2 per
 // element bitwise what k_norm computes; only the order of the float64 sum over elements differs (tests/test_gpu_linear.py).
 //
-// Layout: one CTA of two warpgroups per SM, persistent; the weight planes (96 KB) sit in shared memory once per CTA.  A tile
-// is 32 state rows x 128 features; warpgroup h owns output features [64 h, 64 h + 64) of it and issues m64n32k16 products
-// (tdq_tc.cuh), so every 2 KB weight operand fetched from shared memory serves 32 rows (DESIGN.md section 3c).  The hi
-// weight plane of the warpgroup's features is in registers instead (32 per thread, loaded once per CTA): it is the A operand
-// of 24 of the 48 products of a stage, which then read only their 1 KB B operand from shared memory.  A thread
-// owns 16 elements of the tile in the accumulator layout of tdq_tc.cuh.  State per thread: k_0..k_3 in registers, y0 in
-// shared memory; once k_0..k_3 are known the remaining rows and the error estimate are running sums that each later k_j is
+// Layout: one CTA of two warpgroups per SM, persistent.  A tile is 32 state rows x 128 features; warpgroup h owns output
+// features [64 h, 64 h + 64) of it and issues m64n32k16 products (tdq_tc.cuh), so every 2 KB weight operand fetched from
+// shared memory serves 32 rows (DESIGN.md section 3c).  The hi and mid weight planes of the warpgroup's features are in
+// registers (64 per thread, loaded once per CTA from the global weight image): they are the A operand of 40 of the 48
+// products of a stage, which then read only their 1 KB B operand from shared memory.  Only the lo plane (32 KB) sits in
+// shared memory, for the 8 lo.hi products.  A thread owns 16 elements of the tile in the accumulator layout of tdq_tc.cuh.
+// State per thread: y0 and k_0..k_2 in shared memory (each thread reads back only what it wrote), read in the MMA windows;
+// the newest kept slot is taken from the registers that hold it anyway; once k_0..k_3 are known the remaining rows and the error estimate are running sums in registers that each later k_j is
 // folded into.  Per stage: newest term + split + st.shared of the warpgroup's feature half of the B planes,
 // fence.proxy.async, bar.sync (all 256 threads: the product needs both halves), 48 wgmma + commits per warpgroup; while they
 // run, the prefix of the next row's sum; then wgmma.wait and k_{i+1} = small + big.  The chain of a tile is serial by nature
@@ -45,10 +46,13 @@ using namespace tdq_tc;
 
 constexpr int AT_ROWS = 32;                    // state rows per tile = MMA N
 constexpr int AT_THREADS = 256;                // two warpgroups, one per half of the output features
+constexpr int AT_NR = 2;                       // weight planes held in registers (hi, mid); only lo is in shared memory
+constexpr int AT_W = W_BYTES - AT_NR * W_PLANE;   // the weight planes in shared memory (32 KB)
 constexpr int AT_STAGE = 3 * y_plane<AT_ROWS>();   // the B planes of a tile (24 KB)
 constexpr int AT_Y0 = AT_ROWS * LD * 4;        // a tile's y0 (float32) stays in shared memory: read once per stage
+constexpr int AT_MAX_KEEP = 4;                 // kept slots k_0 .. k_{KEEP-1}; the area holds AT_MAX_KEEP tiles of float32
 constexpr int AT_AUX = 2048;                   // flag, coefficient tables, reduction scratch
-constexpr int AT_SMEM = W_BYTES + AT_STAGE + AT_Y0 + AT_AUX + 128;
+constexpr int AT_SMEM = AT_W + AT_STAGE + AT_Y0 + AT_MAX_KEEP * AT_Y0 + AT_AUX + 128;
 constexpr int AT_MAX_S = 7;
 
 // explicit shared-space accesses with 32-bit addresses (a pointer derived from the aligned dynamic shared memory base is
@@ -72,6 +76,13 @@ __device__ __forceinline__ float lds_pinned_f32(uint32_t addr) {
     float v;
     asm volatile("ld.volatile.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
     return v;
+}
+
+// the row block's address formed once: the compiler would otherwise form it again inside each predicated store of the
+// partial tile, one 64-bit register pair per store
+__device__ __forceinline__ float *held(float *p) {
+    asm volatile("" : "+l"(p));
+    return p;
 }
 
 struct AttOut {
@@ -98,7 +109,7 @@ __device__ __forceinline__ uint8_t *at_smem() {
     extern __shared__ uint8_t smem_raw[];
     return reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
 }
-__device__ __forceinline__ uint8_t *at_aux(uint8_t *smem) { return smem + W_BYTES + AT_STAGE + AT_Y0; }
+__device__ __forceinline__ uint8_t *at_aux(uint8_t *smem) { return smem + AT_W + AT_STAGE + AT_Y0 + AT_MAX_KEEP * AT_Y0; }
 
 // This attempt's coefficients (prepare_tables) as float32, laid out by slot: the coefficient of k_j in row i at s_cr[8 i + j],
 // the error weight of k_j at s_ce[j] (j = 0..S), zero where the tableau has none.  Every index the tile loop uses is then a
@@ -143,19 +154,20 @@ __device__ __forceinline__ bool attempt_store(const TdqCtrl *c, int store_always
     return store;
 }
 
-// the hi weight plane of the warpgroup's features as the register A operand of every hi.* product (k-step ks: ahi[ks]);
-// the weight image is in shared memory and the block has synchronised since
-__device__ __forceinline__ void load_ahi(uint32_t (&ahi)[LD / 16][4], const uint8_t *smem) {
+// the hi and mid weight planes of the warpgroup's features as the register A operand of every hi.* and mid.* product
+// (plane p, k-step ks: afr[p][ks]), read from the global weight image (tdq_tc.cuh's layout, L2-resident after the first CTAs)
+__device__ __forceinline__ void load_afrag(AFrag (&afr)[AT_NR], const uint32_t *__restrict__ wt) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int h = warp >> 2, w = warp & 3;
-    const uint32_t wsm_h = smem_u32(smem) + h * 8 * SBO;
 #pragma unroll
-    for (int ks = 0; ks < LD / 16; ++ks) {
+    for (int p = 0; p < AT_NR; ++p) {
 #pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            const int f = 16 * w + (lane >> 2) + 8 * (r & 1), k = 16 * ks + 2 * (lane & 3) + 8 * (r >> 1);
-            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(ahi[ks][r])
-                         : "r"(wsm_h + (f >> 3) * SBO + (k >> 3) * LBO + (f & 7) * 16 + (k & 7) * 2));
+        for (int ks = 0; ks < LD / 16; ++ks) {
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int f = 64 * h + 16 * w + (lane >> 2) + 8 * (r & 1), k = 16 * ks + 2 * (lane & 3) + 8 * (r >> 1);
+                afr[p][ks][r] = __ldg(wt + (p * W_PLANE + (f >> 3) * SBO + (k >> 3) * LBO + (f & 7) * 16 + (k & 7) * 2) / 4);
+            }
         }
     }
 }
@@ -163,7 +175,7 @@ __device__ __forceinline__ void load_ahi(uint32_t (&ahi)[LD / 16][4], const uint
 // This CTA's tiles of one attempt (tiles blockIdx.x, blockIdx.x + gridDim.x, ...) through all S stages.  tid = threadIdx.x.
 // acc / nbad: this thread's share of the squared error norm (fold) and of the non-finite y1 count.
 template <int S, unsigned long long RM, unsigned EM>
-__device__ __forceinline__ void attempt_tiles(uint8_t *smem, const uint32_t (&ahi)[LD / 16][4], bool store, bool fold, int n_rows,
+__device__ __forceinline__ void attempt_tiles(uint8_t *smem, const AFrag (&afr)[AT_NR], bool store, bool fold, int n_rows,
                                               int tid, double &acc, int &nbad) {
     const int lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);                  // warp-uniform for the compiler as well
@@ -174,9 +186,10 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const uint32_t (&ah
     const uint32_t scoef = wsm + (uint32_t)(at_aux(smem) - smem) + AUX_CR;
     // the coefficient of k_j in row i (i = AT_MAX_S: the error weights); i and j are compile-time constants at every use
     auto coef = [scoef](int i, int j) { return lds_pinned_f32(scoef + 4 * (8 * i + j)); };
-    const uint32_t wsm_h = wsm + h * 8 * SBO;                             // the weight rows of features [64 h, 64 h + 64)
-    const uint32_t stage = wsm + W_BYTES;
+    const uint32_t wsm_h = wsm + h * 8 * SBO;                             // the lo weight rows of features [64 h, 64 h + 64)
+    const uint32_t stage = wsm + AT_W;
     const uint32_t sy0 = stage + AT_STAGE + tid * 4;                      // element e at sy0 + 1024 e: this thread's only
+    const uint32_t skept = sy0 + AT_Y0;                                   // k_j's element e at skept + AT_Y0 j + 1024 e: the same
     const uint64_t dw = make_desc(wsm_h), dy = make_desc(stage);          // every wgmma descriptor is one of these + offset
     const int toff = thread_offset(w, lane) + 64 * h;
 
@@ -191,9 +204,13 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const uint32_t (&ah
     //                   (sum over j <= i of k_j c_{i+1,j}: ascending j, so the newest term is always added last and the
     //                   value is bitwise the one a single ascending loop produces), the running sums, y1's bookkeeping
     //   then            wgmma.wait, k_{i+1} = small + big
-    // Registers: k_0 .. k_{KEEP-1} are kept; once they are all known the remaining rows (and the error estimate) become
-    // running sums that each later k_j is folded into as it arrives, so at most four state-sized arrays are live.
-    constexpr int KEEP = S < 4 ? S : 4;
+    // k_0 .. k_{KEEP-2} are kept in shared memory (each thread stores and reads back only its own elements, like y0: no
+    // barrier); they are read in the MMA windows only, where the newest slot k_i is still in KN and is taken from there
+    // (k_{KEEP-1} is never stored), so the window adds as little as possible to the operand traffic of the product in
+    // flight.  Once they are all known the remaining rows (and the error estimate)
+    // become running sums in registers that each later k_j is folded into as it arrives.
+    constexpr int KEEP = S < AT_MAX_KEEP ? S : AT_MAX_KEEP;
+    auto kept = [skept](int j, int e) { return skept + AT_Y0 * j + 1024 * e; };
     constexpr int NACC = S - KEEP;
     auto row_mask = [](int i) -> unsigned { return (unsigned)((RM >> (8 * i)) & 0xffull); };
     auto do_tile = [&](auto full_tag, const int t) {
@@ -201,7 +218,6 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const uint32_t (&ah
         const int row0 = t * AT_ROWS;
         const int rows_here = n_rows - row0;
         const size_t base = (size_t)row0 * LD + toff;
-        float K[KEEP][16];
         float A[NACC > 0 ? NACC : 1][16];                             // A[q - KEEP]: running sum of row q
         float AE[16], PRE[16], KN[16], Y1[16];
         {
@@ -226,9 +242,9 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const uint32_t (&ah
             const bool last = i == S - 1;
             const bool has_prefix = (mask & ((1u << i) - 1u)) != 0u, has_new = ((mask >> i) & 1u) != 0u;
             const float c_new = has_new ? coef(i, i) : 0.f;
-            if (i < KEEP) {
+            if (i < KEEP - 1) {
 #pragma unroll
-                for (int e = 0; e < 16; ++e) K[i < KEEP ? i : 0][e] = KN[e];
+                for (int e = 0; e < 16; ++e) sts_f32(kept(i, e), KN[e]);
             }
             // ---- critical path: y_i, split, planes ----
             {
@@ -251,7 +267,7 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const uint32_t (&ah
             fence_async_smem();
             __syncthreads();                                              // both feature halves of the B planes are stored
             TileAcc<AT_ROWS> tacc;
-            tile_product(dw, dy, tacc, ahi);
+            tile_product<AT_ROWS, AT_NR>(dw, dy, tacc, afr);
             // ---- MMA window ----
             if (i + 1 < KEEP && i + 1 < S) {
                 // prefix of the next row's sum over the slots known so far
@@ -263,7 +279,7 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const uint32_t (&ah
                         const float cj = coef(i + 1, j);
 #pragma unroll
                         for (int e = 0; e < 16; ++e) {
-                            const float p = K[j < KEEP ? j : 0][e] * cj;
+                            const float p = (j == i ? KN[e] : lds_f32(kept(j, e))) * cj;
                             PRE[e] = first ? p : PRE[e] + p;
                         }
                         first = false;
@@ -292,7 +308,7 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const uint32_t (&ah
 #pragma unroll
                         for (int j = 0; j <= i; ++j) {
                             if ((mq >> j) & 1u) {
-                                const float p = K[j < KEEP ? j : 0][e] * cq[qrow - KEEP][j];
+                                const float p = (j == i ? KN[e] : lds_f32(kept(j, e))) * cq[qrow - KEEP][j];
                                 a_ = first ? p : a_ + p;
                                 first = false;
                             }
@@ -304,7 +320,7 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const uint32_t (&ah
 #pragma unroll
                     for (int j = 0; j <= i; ++j) {
                         if ((EM >> j) & 1u) {
-                            const float p = K[j < KEEP ? j : 0][e] * ce[j];
+                            const float p = (j == i ? KN[e] : lds_f32(kept(j, e))) * ce[j];
                             e_ = first ? p : e_ + p;
                             first = false;
                         }
@@ -367,10 +383,10 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const uint32_t (&ah
             wgmma_wait();
             tile_result(tacc, KN);
             if (store) {
-                float *ko = reinterpret_cast<float *>(lds_u64(ssc + offsetof(Scalars, out.k) + 8 * (i + 1)));
+                float *ko = held(reinterpret_cast<float *>(lds_u64(ssc + offsetof(Scalars, out.k) + 8 * (i + 1))) + base);
 #pragma unroll
                 for (int e = 0; e < 16; ++e)
-                    if (FULL || elem_row<AT_ROWS>(e, lane) < rows_here) ko[base + elem_offset<AT_ROWS>(e)] = KN[e];
+                    if (FULL || elem_row<AT_ROWS>(e, lane) < rows_here) ko[elem_offset<AT_ROWS>(e)] = KN[e];
             }
             if (last) {
                 // ---- k_S: candidate commit, error ratio (misc.py:80-82 up to the mean) ----
@@ -458,15 +474,15 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
     const int tid = threadIdx.x;
     const bool fold = partials != nullptr;                                // squared error norm + candidate commit in here
     attempt_prologue<S, RM, EM>(c, y0, k0, out, fold, n_rows_sz, aux, tid);
-    load_weights(smem, wt, tid, AT_THREADS);
+    load_weights(smem, wt, tid, AT_THREADS, AT_NR);
     fence_async_smem();
+    AFrag afr[AT_NR];
+    load_afrag(afr, wt);
     __syncthreads();
     const bool store = attempt_store(c, store_always);
-    uint32_t ahi[LD / 16][4];
-    load_ahi(ahi, smem);
     double acc = 0.0;
     int nbad = 0;
-    attempt_tiles<S, RM, EM>(smem, ahi, store, fold, (int)n_rows_sz, tid, acc, nbad);
+    attempt_tiles<S, RM, EM>(smem, afr, store, fold, (int)n_rows_sz, tid, acc, nbad);
 
     // ---- per-CTA partial of the squared norm and of the non-finite count; the last CTA adds them in index order ----
     if (!fold) return;
@@ -494,8 +510,8 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
 }
 
 // ---- a whole fused solve in one launch ---------------------------------------------------------------------------------
-// k_linear_solve runs every attempt of a solve: the CTAs stay resident (cooperative launch), keep the weight image in shared
-// memory and the hi plane in registers, and meet at a grid barrier after each attempt.  There CTA 0 adds the partials and
+// k_linear_solve runs every attempt of a solve: the CTAs stay resident (cooperative launch), keep the lo weight plane in
+// shared memory and the hi and mid planes in registers, and meet at a grid barrier after each attempt.  There CTA 0 adds the partials and
 // runs the controller step on a shared-memory copy of the control block (tdq_ctrl_step.cuh, what k_controller runs), then
 // releases the others.  When an output time fell into the step, every CTA runs the fit (tdq_fit.cuh, k_fit_eval's body)
 // and they meet once more: the next attempt overwrites the pair the fit reads.
@@ -594,8 +610,8 @@ k_linear_solve(TdqCtrl *c, AttOut out, const uint32_t *__restrict__ wt, unsigned
         if (blockIdx.x == 0) solve_controller_step(c, smem, sx, cnt);
         return;
     }
-    // ---- once per launch: the weight image, the hi plane ----
-    load_weights(smem, wt, tid, AT_THREADS);
+    // ---- once per launch: the lo weight plane, the hi and mid planes ----
+    load_weights(smem, wt, tid, AT_THREADS, AT_NR);
     fence_async_smem();
     if (tid == 0) {
         sx->attempt = 0;
@@ -608,9 +624,9 @@ k_linear_solve(TdqCtrl *c, AttOut out, const uint32_t *__restrict__ wt, unsigned
         sx->block = blockIdx.x;
         sx->blocks = gridDim.x;
     }
+    AFrag afr[AT_NR];
+    load_afrag(afr, wt);
     __syncthreads();
-    uint32_t ahi[LD / 16][4];
-    load_ahi(ahi, smem);
     for (;;) {
         // ---- the attempt: same prologue, tiles and per-CTA partial as k_linear_attempt ----
         attempt_prologue<S, RM, EM>(c, nullptr, nullptr, out, true, n_rows_sz, aux, opaque_tid());
@@ -618,7 +634,7 @@ k_linear_solve(TdqCtrl *c, AttOut out, const uint32_t *__restrict__ wt, unsigned
         const bool store = attempt_store(c, 0);
         double acc = 0.0;
         int nbad = 0;
-        attempt_tiles<S, RM, EM>(smem, ahi, store, true, (int)n_rows_sz, opaque_tid(), acc, nbad);
+        attempt_tiles<S, RM, EM>(smem, afr, store, true, (int)n_rows_sz, opaque_tid(), acc, nbad);
         const unsigned a = (unsigned)sxv->attempt;
         double *p_sum = part + (a & 1u) * 2 * P, *p_bad = p_sum + P;
         cta_partial(acc, nbad, s_red, p_sum, p_bad);

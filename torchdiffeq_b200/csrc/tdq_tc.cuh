@@ -4,11 +4,12 @@
 // The product of one tile: K^T = W Y^T for N state rows (N = 16 in the stage kernels, 32 in the attempt kernel) and K = 128
 // input features, issued by one warpgroup over C = 32 / N m64 halves of the output features ("chains"; with N = 32 the two
 // warpgroups of a CTA take one half each).  A = the weight planes (K-major), B = the stage-value planes (MN-major), both in
-// shared memory without swizzle, except that the attempt kernel holds its warpgroup's hi weight plane in registers (the A
-// operand of the 24 hi.* products of a tile, loaded once per CTA: tile_product's `ahi`), so those products fetch only their
-// B operand from shared memory; the accumulators are registers, 16 per thread for either N.  Every kernel issues the same
-// sequence of products into each accumulator, so a row's result does not depend on which kernel computed it or where the
-// row sits in the tiling (tests/test_gpu_linear.py compares the attempt kernel with the stage kernel bitwise).
+// shared memory without swizzle, except that the attempt kernel holds its warpgroup's hi and mid weight planes in registers
+// (the A operand of the 40 hi.* and mid.* products of a tile, loaded once per CTA: tile_product's fragment table `afr`), so
+// those products fetch only their B operand from shared memory; the accumulators are registers, 16 per thread for either N.
+// Every kernel issues the same sequence of products into each accumulator, so a row's result does not depend on which
+// kernel computed it or where the row sits in the tiling (tests/test_gpu_linear.py compares the attempt kernel with the
+// stage kernel bitwise).
 #pragma once
 
 #include <cstdint>
@@ -148,12 +149,17 @@ template <int N> __device__ __forceinline__ void acc_fence(TileAcc<N> &a) {
     fence_hi(a);
 }
 
+// The weight planes as register A operands: afr[p][ks] = the m64k16 fragment (wgmma_rs32) of plane p, k-step ks, of the
+// warpgroup's output features.  With NR register planes, planes 0 .. NR-1 (hi, then mid) come from afr and plane p >= NR
+// from shared memory at dw + (p - NR) W_PLANE: only the planes not held in registers occupy shared memory.
+using AFrag = uint32_t[LD / 16][4];
+
 // weight plane PW x stage plane PY over k-steps [k0, k1) into d (d is overwritten at k0 when `fresh`); dw = the descriptor
-// of the weights of the warpgroup's first chain, dy = the descriptor of stage plane 0; with ahi (N = 32) the hi plane's A
-// operand of k-step ks is the register fragment ahi[ks]
-template <int N>
+// of the first shared weight plane of the warpgroup's first chain, dy = the descriptor of stage plane 0
+template <int N, int NR>
 __device__ __forceinline__ void plane_product(uint64_t dw, uint64_t dy, int pw, int py, int k0, int k1, bool fresh,
-                                              float (&d)[32 / N][N / 2], const uint32_t (*ahi)[4]) {
+                                              float (&d)[32 / N][N / 2], const AFrag *afr) {
+    static_assert(NR == 0 || N == 32, "register A operands are m64n32k16 fragments of one warpgroup's chain");
 #pragma unroll
     for (int ks = k0; ks < k1; ++ks) {
 #pragma unroll
@@ -161,12 +167,12 @@ __device__ __forceinline__ void plane_product(uint64_t dw, uint64_t dy, int pw, 
             const uint64_t db = desc_add(dy, py * y_plane<N>() + ks * 2 * LBO);
             const uint32_t acc = fresh && ks == k0 ? 0u : 1u;
             if constexpr (N == 32) {
-                if (pw == 0 && ahi != nullptr) {
-                    wgmma_rs32(d[c], ahi[ks], db, acc);
+                if (pw < NR) {
+                    wgmma_rs32(d[c], afr[pw][ks], db, acc);
                     continue;
                 }
             }
-            wgmma_n<N>(d[c], desc_add(dw, pw * W_PLANE + c * 8 * SBO + ks * 2 * LBO), db, acc);
+            wgmma_n<N>(d[c], desc_add(dw, (pw - NR) * W_PLANE + c * 8 * SBO + ks * 2 * LBO), db, acc);
         }
     }
 }
@@ -179,26 +185,27 @@ template <int N> __device__ __forceinline__ void add_part(TileAcc<N> &a) {
 }
 
 // cross term p of the list below into `small`
-template <int N>
-__device__ __forceinline__ void cross_term(uint64_t dw, uint64_t dy, int p, TileAcc<N> &a, const uint32_t (*ahi)[4]) {
+template <int N, int NR>
+__device__ __forceinline__ void cross_term(uint64_t dw, uint64_t dy, int p, TileAcc<N> &a, const AFrag *afr) {
     constexpr int PW[5] = {1, 2, 0, 1, 0}, PY[5] = {1, 0, 2, 0, 1};
-    plane_product<N>(dw, dy, PW[p], PY[p], 0, LD / 16, p == 0, a.small, ahi);
+    plane_product<N, NR>(dw, dy, PW[p], PY[p], 0, LD / 16, p == 0, a.small, afr);
 }
 // partial q (k-steps 2q, 2q + 1) of hi.hi into `part`, once the previous partial has been added to `big`
-template <int N>
-__device__ __forceinline__ void next_partial(uint64_t dw, uint64_t dy, int q, TileAcc<N> &a, const uint32_t (*ahi)[4]) {
+template <int N, int NR>
+__device__ __forceinline__ void next_partial(uint64_t dw, uint64_t dy, int q, TileAcc<N> &a, const AFrag *afr) {
     wgmma_wait<1>();                                      // the group holding partial q - 1 (only newer cross terms may run)
     fence_hi(a);
     add_part(a);
     fence_hi(a);
     wgmma_fence();
-    plane_product<N>(dw, dy, 0, 0, 2 * q, 2 * q + 2, true, a.part, ahi);
+    plane_product<N, NR>(dw, dy, 0, 0, 2 * q, 2 * q + 2, true, a.part, afr);
     wgmma_commit();
 }
-// Issue the product of one tile (dy = make_desc of the stage planes, dw = make_desc of the weight planes of the first chain,
-// both formed once per kernel; ahi = the hi weight plane as register fragments, N = 32 only, or nullptr to read it from
-// shared memory like the other planes); the caller waits (wgmma_wait) and then calls tile_result.  Weight plane PW x stage
-// plane PY: mid.mid, lo.hi, hi.lo, mid.hi, hi.mid -- the five cross terms >= 2^-16, ascending in magnitude -- into the small accumulator; hi.hi into the big one;
+// Issue the product of one tile (dy = make_desc of the stage planes, dw = make_desc of the first weight plane in shared
+// memory for the first chain, both formed once per kernel; afr = the first NR weight planes as register fragments, N = 32
+// only, or NR = 0 to read every plane from shared memory); the caller waits (wgmma_wait) and then calls tile_result.
+// Weight plane PW x stage plane PY: mid.mid, lo.hi, hi.lo, mid.hi, hi.mid -- the five cross terms >= 2^-16, ascending in
+// magnitude -- into the small accumulator; hi.hi into the big one;
 // k = small + big.  The three remaining cross terms (lo.lo, lo.mid, mid.lo) are below 2^-24 of a product, the rounding of a
 // float32 product itself, and are not computed.
 // The tensor cores round a float32 accumulation toward zero, which over the eight k-steps of hi.hi shrinks every k by about
@@ -209,22 +216,22 @@ __device__ __forceinline__ void next_partial(uint64_t dw, uint64_t dy, int q, Ti
 // Issue order: each wait for a hi.hi partial (which is needed on the CUDA cores before the next one can be issued into the
 // same accumulator) has a batch of cross terms queued behind it, so the tensor pipe does not drain while `big += part` runs.
 // Each accumulator still sees the same products and float32 additions in the same order.  Issued by the whole warpgroup.
-template <int N> __device__ __forceinline__ void tile_product(uint64_t dw, uint64_t dy, TileAcc<N> &a,
-                                                   const uint32_t (*ahi)[4] = nullptr) {
+template <int N, int NR = 0> __device__ __forceinline__ void tile_product(uint64_t dw, uint64_t dy, TileAcc<N> &a,
+                                                   const AFrag *afr = nullptr) {
     acc_fence(a);
     wgmma_fence();
-    plane_product<N>(dw, dy, 0, 0, 0, 2, true, a.big, ahi);
-    plane_product<N>(dw, dy, 0, 0, 2, 4, true, a.part, ahi);
+    plane_product<N, NR>(dw, dy, 0, 0, 0, 2, true, a.big, afr);
+    plane_product<N, NR>(dw, dy, 0, 0, 2, 4, true, a.part, afr);
     wgmma_commit();
-    cross_term(dw, dy, 0, a, ahi);
-    cross_term(dw, dy, 1, a, ahi);
+    cross_term<N, NR>(dw, dy, 0, a, afr);
+    cross_term<N, NR>(dw, dy, 1, a, afr);
     wgmma_commit();
-    next_partial(dw, dy, 2, a, ahi);
-    cross_term(dw, dy, 2, a, ahi);
-    cross_term(dw, dy, 3, a, ahi);
+    next_partial<N, NR>(dw, dy, 2, a, afr);
+    cross_term<N, NR>(dw, dy, 2, a, afr);
+    cross_term<N, NR>(dw, dy, 3, a, afr);
     wgmma_commit();
-    next_partial(dw, dy, 3, a, ahi);
-    cross_term(dw, dy, 4, a, ahi);
+    next_partial<N, NR>(dw, dy, 3, a, afr);
+    cross_term<N, NR>(dw, dy, 4, a, afr);
     wgmma_commit();
     acc_fence(a);
 }
@@ -237,12 +244,13 @@ template <int N> __device__ __forceinline__ void tile_result(TileAcc<N> &a, floa
     for (int e = 0; e < 16; ++e) k[e] = a.small[e / (N / 2)][e % (N / 2)] + a.big[e / (N / 2)][e % (N / 2)];
 }
 
-// the weight image (W_BYTES, 16-byte aligned) -> shared memory, by all `threads` threads of the block; the caller then
-// synchronises the block and fences the generic-proxy writes (fence_async_smem) before the first MMA
-__device__ __forceinline__ void load_weights(uint8_t *wsm, const uint32_t *wt, int tid, int threads) {
-    const uint4 *src = reinterpret_cast<const uint4 *>(wt);
+// the weight image (W_BYTES, 16-byte aligned), or its planes from `first` on, -> shared memory, by all `threads` threads of
+// the block; the caller then synchronises the block and fences the generic-proxy writes (fence_async_smem) before the
+// first MMA
+__device__ __forceinline__ void load_weights(uint8_t *wsm, const uint32_t *wt, int tid, int threads, int first = 0) {
+    const uint4 *src = reinterpret_cast<const uint4 *>(wt) + first * (W_PLANE / 16);
     uint4 *dst = reinterpret_cast<uint4 *>(wsm);
-    for (int i = tid; i < W_BYTES / 16; i += threads) dst[i] = __ldg(src + i);
+    for (int i = tid; i < (W_BYTES - first * W_PLANE) / 16; i += threads) dst[i] = __ldg(src + i);
 }
 
 }  // namespace tdq_tc
