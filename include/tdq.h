@@ -570,6 +570,70 @@ int tdq_rows_event_bisect(void *ctrl_dev, void *rows_dev, int32_t dtype, int32_t
                           const void *coeff, const void *y_start, void *y_mid, double *t_ev, double *event_t,
                           void *y_event, size_t n_rows, size_t row_len, int32_t K, void *stream);
 
+/* ---- gradients of independent-row solves: a per-row step tape and the reverse sweep (tdq_rows.cu) ---------------------
+ * The forward of a differentiable row solve runs in lock step and, after tdq_rows_controller, tdq_rows_tape_push records
+ * every row that accepted in that attempt (count[r] < N_ACCEPT[r]): one SLOT holding the pair the step started from
+ * (ybuf/kbuf[par_r ^ 1], D elements each) and its record (float64 T0, T1, FIT_DT; int32 EMIT_LO, EMIT_HI, step index).
+ * Slots are taken in any order; index[k * B + r] is the slot of row r's step k.  Slots live in caller-owned segments of
+ * seg_slots slots each (tdq_rows_tape_segment_bytes); seg is a device table of their base addresses, so a tape grows by
+ * adding segments without moving what it holds.  The caller keeps n_seg * seg_slots >= *used + B and n_steps > the number
+ * of attempts before every push; *used_host (pinned host memory) holds *used after each push, readable once a later
+ * attempt has reported through the mailbox.  count, used: zero before the solve.  fresh: [B] int32 scratch.
+ * The reverse sweep runs iteration iter = 0, 1, ... over the whole batch: row r works on its step count[r] - 1 - iter,
+ * and is idle once iter >= count[r].  An idle row's stage values are copies of y_start and its stage times t_first, where
+ * func has already been evaluated; its adjoints are not touched and its kbar rows are 0.
+ * tdq_rows_grad_gather:     the step's pair into y0 / k0, every stage time into t_stage (tdq_stage_time, bitwise the
+ *                           forward's), kbar_S = gk, the other kbar = 0, ybar0 = 0, ybar1 = gy.
+ * tdq_rows_grad_combine:    row in [0, S): stage[row] = y0 + sum_j fl_T(beta_row,j * T(dt_r)) k_j; row == S: y1 from the
+ *                           c_sol row (non-FSAL tableaus); row == -1: ymid from c_mid.  Bitwise the forward's values.
+ * tdq_rows_grad_dense:      for rows whose step emitted outputs [lo, hi): the adjoint of the quartic (interp.py:1-48) from
+ *                           grad_sol[j] into ybar0, ybar1, kbar_0, kbar_S and, through c_mid, kbar_j; with sbar, each
+ *                           output's time gradient G . p'(x) / (T1 - T0) as a float64 row sum in an order set by D alone
+ *                           (k_rows_norm's), added to sbar[r, j] and subtracted from shift[r] (needs y1, ymid, k_S).
+ * tdq_rows_grad_stage:      row in [0, S): after the VJP of stage row against kbar[row + 1], Ybar = gY (+ ybar1 for the
+ *                           last stage of an FSAL tableau): ybar0 += Ybar, kbar_j += fl_T(beta_row,j * T(dt_r)) Ybar, shift[r]
+ *                           += t_sign * gt[r]; row == S (non-FSAL): the same with Ybar = ybar1 through c_sol.  At row 0
+ *                           the hand-over: gy = ybar0, and kbar_0 goes to gk, or to gk_first for the row's first step.
+ * gY, gt may be NULL (func does not depend on y or t). */
+typedef struct tdq_rows_tape {
+    void *const *seg;            /* device table of n_seg segment base addresses                                   */
+    int64_t seg_slots;           /* slots per segment, a positive multiple of 256                                  */
+    int64_t n_seg;
+    int32_t *index;              /* [n_steps][B] int32                                                             */
+    int64_t n_steps;
+    int32_t *count;              /* [B] steps taped per row                                                        */
+    int32_t *fresh;              /* [B] scratch                                                                    */
+    int32_t *used;               /* device word: slots taken                                                       */
+    int32_t *used_host;          /* pinned host word (cudaHostAlloc): *used after each push, or NULL               */
+} tdq_rows_tape;
+typedef struct tdq_rows_sweep {
+    const void *y_start;         /* [B*D] the solve's y0                                                           */
+    const void *t_first;         /* [B] state dtype: func's time of f0 (TDQ_ROWS_T_FIRST)                          */
+    void *y0, *k0;               /* [B*D] the gathered pair                                                        */
+    void *stage[TDQ_MAX_STAGES]; /* [B*D] Y_i                                                                      */
+    const void *k[TDQ_MAX_K];    /* [B*D] k_j = f(t_{j-1}, Y_{j-1}), j = 1..S (k[0] unused: k0 is read)            */
+    void *y1, *ymid;             /* [B*D]                                                                          */
+    void *t_stage;               /* [S][B] state dtype: func's time of each stage                                  */
+    void *kbar[TDQ_MAX_K];       /* [B*D] adjoints of k_0 .. k_S                                                   */
+    void *ybar0, *ybar1, *gy, *gk, *gk_first;   /* [B*D]                                                           */
+    double *shift;               /* [B]                                                                            */
+    double *sbar;                /* [B][n_out] or NULL                                                             */
+    const void *grad_sol;        /* [n_out][B*D]                                                                   */
+    int32_t iter, n_out;
+} tdq_rows_sweep;
+size_t tdq_rows_tape_segment_bytes(int32_t dtype, size_t seg_slots, size_t row_len);
+int tdq_rows_tape_push(void *ctrl_dev, void *rows_dev, int32_t dtype, const tdq_rows_tape *tape, size_t n_rows,
+                       size_t row_len, void *stream);
+int tdq_rows_grad_gather(void *ctrl_dev, int32_t dtype, const tdq_rows_tape *tape, const tdq_rows_sweep *sw,
+                         size_t n_rows, size_t row_len, void *stream);
+int tdq_rows_grad_combine(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, const tdq_rows_tape *tape,
+                          const tdq_rows_sweep *sw, int32_t row, size_t n_rows, size_t row_len, void *stream);
+int tdq_rows_grad_dense(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, const tdq_rows_tape *tape,
+                        const tdq_rows_sweep *sw, size_t n_rows, size_t row_len, void *stream);
+int tdq_rows_grad_stage(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, const tdq_rows_tape *tape,
+                        const tdq_rows_sweep *sw, int32_t row, const void *gY, const void *gt, size_t n_rows,
+                        size_t row_len, void *stream);
+
 /* ---- adjoint augmented state (adjoint.py:72-105, misc.py:137-165) ------------------------- */
 /* dst[offset_i .. offset_i + len_i) = scale_i * src_i for i < n_src, one launch
  * (the torch.cat of _TupleFunc, the unary minus on adj_y and the *(-1) of _ReverseFunc).

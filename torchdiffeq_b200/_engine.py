@@ -728,9 +728,9 @@ class AdaptiveEngine:
             del f
         return issued, mb
 
-    def _lockstep(self, y0_flat, t64, t_start=None):
+    def _lockstep(self, y0_flat, t64, t_start=None, grid=None):
         """A lock-step solve (see _lockstep_attempts)."""
-        self.driver = self._begin(y0_flat, t64, t_start)
+        self.driver = self._begin(y0_flat, t64, t_start, grid)
         return self._lockstep_attempts()
 
     def _lockstep_attempts(self):
@@ -1034,18 +1034,37 @@ class RowsEngine(AdaptiveEngine):
         self.row_n_accept = self.row_n_reject = None
         self.ev_fn = None                # set by solve_until_event: the attempt then tests each row's event
         self.grid = None                 # per-row output times [B, T] of the solve in progress, or None
+        self.tape = None                 # the RowTape of a solve_taped in progress
 
     def solve(self, y0_flat, t64, t_start=None, grid=None):
         """AdaptiveEngine.solve, or with `grid` (an ascending float64 [B, T] device tensor) per-row output times: row r
         starts at grid[r, 0], ends at grid[r, T-1] and solution[j] holds row r at grid[r, j].  t64 is then not read: the
         control block gets row 0's times, so its n_out is T.  The engine keeps the grid alive until the next solve."""
+        t64, grid = self._check_grid(t64, grid)
+        return super().solve(y0_flat, t64, t_start, grid)
+
+    def _check_grid(self, t64, grid):
         if grid is not None:
             if grid.dim() != 2 or grid.shape[0] != self.B or grid.dtype != torch.float64 or grid.device != self.device:
                 raise ValueError("grid must be a float64 [%d, T] tensor on %s, got %s %s on %s"
                                  % (self.B, self.device, grid.dtype, tuple(grid.shape), grid.device))
             grid = grid.contiguous()
             t64 = grid[0]
-        return super().solve(y0_flat, t64, t_start, grid)
+        return t64, grid
+
+    def solve_taped(self, y0_flat, t64, t_start=None, grid=None):
+        """A lock-step solve (what solve computes, bit for bit) that tapes every accepted row-step for the reverse sweep of
+        backprop.rows_backward.  Returns (solution, RowTape); the tape keeps this engine, whose control block and row
+        buffer the sweep reads."""
+        t64, grid = self._check_grid(t64, grid)
+        tape = self.tape = RowTape(self)
+        try:
+            for _ in self._lockstep(y0_flat, t64, t_start, grid):
+                pass
+        finally:
+            self.tape = None
+        tape.check()
+        return self.solution, tape
 
     def _rows_sumsq(self, x, x2, out):
         self._launch(self.lib.tdq_rows_sumsq(
@@ -1093,6 +1112,8 @@ class RowsEngine(AdaptiveEngine):
         return k, kp, keep
 
     def _attempt_back(self, kp):
+        if self.tape is not None:
+            self.tape.push()
         if self.ev_fn is not None:                  # the interpolant of a row's event step, kept for the bisection
             self._launch(self.lib.tdq_rows_fit_store(self.ctrl.data_ptr(), self.rows.data_ptr(), C.byref(self.tab),
                                                      self.dt_code, self.y1.data_ptr(), kp, self.ev_flag.data_ptr(),
@@ -1208,3 +1229,88 @@ class RowsEngine(AdaptiveEngine):
         self.row_n_reject = self.row_field(_lib.ROWS_N_REJECT, torch.int64).cpu()
         self.n_accept, self.n_reject = int(self.row_n_accept.sum()), int(self.row_n_reject.sum())
         self.n_attempts = int((self.row_n_accept + self.row_n_reject).max())   # loop iterations that did work
+
+
+class RowTape:
+    """The accepted steps of a differentiable independent-row solve (RowsEngine.solve_taped), on the device.
+
+    After every lock-step attempt tdq_rows_tape_push gives each row that accepted one slot: the (y0, k_0) pair its step
+    started from and the step's T0, T1, dt, output range and index.  Slots live in segments of seg_slots slots (at least
+    one attempt's worth), added as the solve goes, so the finished tape holds 2 D elements per accepted row-step, rounded
+    up to whole segments.  Before each push the host makes room for B more slots from the slot count the previous push left
+    in pinned memory; the lock-step driver has waited for the attempt's report by then, so this reads no device memory.
+    index[k, r] is the slot of row r's step k, count[r] the number of steps row r took."""
+
+    def __init__(self, eng):
+        self.eng, self.B, self.D = eng, eng.B, eng.D
+        dev, i32 = eng.device, dict(dtype=torch.int32, device=eng.device)
+        self.seg_slots = (max(self.B, 256) + 255) // 256 * 256
+        self.seg_bytes = int(eng.lib.tdq_rows_tape_segment_bytes(eng.dt_code, self.seg_slots, self.D))
+        self.segs = []
+        self.seg_table = torch.zeros(16, dtype=torch.int64, device=dev)
+        self.index = torch.full((16, self.B), -1, **i32)
+        self.count = torch.zeros(self.B, **i32)
+        self.fresh = torch.zeros(self.B, **i32)
+        self.used = torch.zeros(1, **i32)
+        self.used_host = torch.zeros(1, dtype=torch.int32, pin_memory=True)
+        self.n_push = 0
+        self.st = _lib.RowsTape()
+
+    @property
+    def capacity(self):
+        return len(self.segs) * self.seg_slots
+
+    @property
+    def nbytes(self):
+        return len(self.segs) * self.seg_bytes + self.index.numel() * 4
+
+    def _sync_struct(self):
+        st = self.st
+        st.seg, st.seg_slots, st.n_seg = self.seg_table.data_ptr(), self.seg_slots, len(self.segs)
+        st.index, st.n_steps = self.index.data_ptr(), self.index.shape[0]
+        st.count, st.fresh, st.used = self.count.data_ptr(), self.fresh.data_ptr(), self.used.data_ptr()
+        st.used_host = self.used_host.data_ptr()
+
+    def _reserve(self):
+        """Room for one more attempt: B free slots and a row of the index table for step n_push."""
+        dev = self.eng.device
+        while self.capacity < int(self.used_host[0]) + self.B:
+            if len(self.segs) == self.seg_table.numel():
+                self.seg_table = torch.cat([self.seg_table, torch.zeros_like(self.seg_table)])
+            seg = torch.empty(self.seg_bytes, dtype=torch.uint8, device=dev)
+            self.seg_table[len(self.segs)].fill_(seg.data_ptr())         # a fill kernel: no host-device copy
+            self.segs.append(seg)
+        if self.index.shape[0] <= self.n_push:
+            self.index = torch.cat([self.index, torch.full_like(self.index, -1)])
+
+    def push(self):
+        self._reserve()
+        self._sync_struct()
+        e = self.eng
+        e._launch(e.lib.tdq_rows_tape_push(e.ctrl.data_ptr(), e.rows.data_ptr(), e.dt_code, C.byref(self.st), self.B, self.D,
+                                           _stream()))
+        self.n_push += 1
+
+    def check(self):
+        """After the solve's final synchronisation: every accepted row-step found a slot; the segments past the last slot
+        taken (the reserve for an attempt that did not come) are released, so the tape holds ceil(slots / seg_slots)
+        segments."""
+        used = int(self.used_host[0])
+        if used > self.capacity:
+            raise _lib.TdqError("row tape overflow: %d slots taken, %d reserved" % (used, self.capacity))
+        del self.segs[(used + self.seg_slots - 1) // self.seg_slots:]
+        self._sync_struct()
+
+    def slots(self):
+        """Device views of the segments: (y [capacity, D], k [capacity, D], rec_t [capacity, 3] float64, rec_i [capacity, 3]
+        int32), for tests and inspection."""
+        dt, D, ss = self.eng.dtype, self.D, self.seg_slots
+        es = torch.empty((), dtype=dt).element_size()
+        parts = [[], [], [], []]
+        for seg in self.segs:
+            o1, o2, o3 = ss * D * es, 2 * ss * D * es, 2 * ss * D * es + 24 * ss
+            parts[0].append(seg[:o1].view(dt).view(ss, D))
+            parts[1].append(seg[o1:o2].view(dt).view(ss, D))
+            parts[2].append(seg[o2:o3].view(torch.float64).view(ss, 3))
+            parts[3].append(seg[o3:o3 + 12 * ss].view(torch.int32).view(ss, 3))
+        return tuple(torch.cat(p_) for p_ in parts)

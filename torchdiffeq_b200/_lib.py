@@ -62,6 +62,28 @@ class Mailbox(C.Structure):
     ]
 
 
+class RowsTape(C.Structure):
+    """tdq_rows_tape (include/tdq.h): the step tape of a differentiable independent-row solve."""
+    _fields_ = [
+        ("seg", C.c_void_p), ("seg_slots", C.c_int64), ("n_seg", C.c_int64),
+        ("index", C.c_void_p), ("n_steps", C.c_int64),
+        ("count", C.c_void_p), ("fresh", C.c_void_p), ("used", C.c_void_p), ("used_host", C.c_void_p),
+    ]
+
+
+class RowsSweep(C.Structure):
+    """tdq_rows_sweep (include/tdq.h): the buffers of one reverse iteration over an independent-row solve."""
+    _fields_ = [
+        ("y_start", C.c_void_p), ("t_first", C.c_void_p), ("y0", C.c_void_p), ("k0", C.c_void_p),
+        ("stage", C.c_void_p * TDQ_MAX_STAGES), ("k", C.c_void_p * TDQ_MAX_K),
+        ("y1", C.c_void_p), ("ymid", C.c_void_p), ("t_stage", C.c_void_p),
+        ("kbar", C.c_void_p * TDQ_MAX_K),
+        ("ybar0", C.c_void_p), ("ybar1", C.c_void_p), ("gy", C.c_void_p), ("gk", C.c_void_p), ("gk_first", C.c_void_p),
+        ("shift", C.c_void_p), ("sbar", C.c_void_p), ("grad_sol", C.c_void_p),
+        ("iter", C.c_int32), ("n_out", C.c_int32),
+    ]
+
+
 class TdqError(RuntimeError):
     pass
 
@@ -156,6 +178,13 @@ _SIGNATURES = {
     "tdq_rows_fit_store": (C.c_int, [_vp, _vp, _ptab, _i32, _vp, _pp, _vp, _vp, _sz, _sz, _vp]),
     "tdq_rows_event_bisect": (C.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                         _sz, _sz, _i32, _vp]),
+    "tdq_rows_tape_segment_bytes": (_sz, [_i32, _sz, _sz]),
+    "tdq_rows_tape_push": (C.c_int, [_vp, _vp, _i32, C.POINTER(RowsTape), _sz, _sz, _vp]),
+    "tdq_rows_grad_gather": (C.c_int, [_vp, _i32, C.POINTER(RowsTape), C.POINTER(RowsSweep), _sz, _sz, _vp]),
+    "tdq_rows_grad_combine": (C.c_int, [_vp, _ptab, _i32, C.POINTER(RowsTape), C.POINTER(RowsSweep), _i32, _sz, _sz, _vp]),
+    "tdq_rows_grad_dense": (C.c_int, [_vp, _ptab, _i32, C.POINTER(RowsTape), C.POINTER(RowsSweep), _sz, _sz, _vp]),
+    "tdq_rows_grad_stage": (C.c_int, [_vp, _ptab, _i32, C.POINTER(RowsTape), C.POINTER(RowsSweep), _i32, _vp, _vp, _sz,
+                                      _sz, _vp]),
     "tdq_xchg_create": (C.c_int, [_pp, C.POINTER(IpcHandle)]),
     "tdq_xchg_open": (C.c_int, [C.POINTER(IpcHandle), _pp]),
     "tdq_xchg_close": (C.c_int, [_vp]),

@@ -23,10 +23,12 @@ well and the grid constructor is differentiated by autograd itself.  One documen
 step size comes from _select_initial_step, whose value depends differentiably on y0 and t[0] (misc.py:36-77); that
 dependence -- a derivative of the discretisation error, not of the solution -- is not propagated here.
 """
+import ctypes as C
+
 import torch
 
 from . import _lib
-from ._engine import on_solver_stream
+from ._engine import _stream, on_solver_stream
 from ._fixed import stage_times
 
 
@@ -285,6 +287,87 @@ def adaptive_backward(p, tab, tape, t, grad_sol, params, need_t):
     return tbar, y0bar, sa.pbar
 
 
+def rows_backward(p, tape, t, grad_sol, params, need_t):
+    """Reverse sweep over the taped steps of an independent-row solve (options={'independent_rows': True,
+    'differentiable': True}): adaptive_backward for every row at once.  Iteration j takes row r's step count[r] - 1 - j
+    (rows with fewer steps are idle and contribute exactly 0); the per-element and per-row work is libtdq's row-segmented
+    kernels (tdq_rows_grad_*), func's VJPs run on the whole batch with its [B, 1, ...] time tensor.  Works in the engine's
+    raw time (func's own t = t_sign * s), so the coefficients are the forward's signed ones.  Returns (t_bar or None,
+    y0_bar, [param_bar]): t_bar has t's shape, a [B, T] table's rows or, for a 1-D t, the sum over rows."""
+    eng = tape.eng
+    lib, dc, dev, T, B, D, S = eng.lib, eng.dt_code, eng.device, eng.dtype, eng.B, eng.D, eng.S
+    n, sign, fsal = B * D, p.t_sign, eng.fsal
+    tshape = eng.t_first.shape
+
+    def F(t_, y_):
+        out = p.fn(t_, y_).reshape(-1)
+        return out if out.dtype == T else out.to(T)
+    sa = StepAdjoint(F, params, need_t)
+    buf = lambda: torch.zeros(n, dtype=T, device=dev)
+    y_start = p.y0_flat.to(T).contiguous()
+    stage = [buf() for _ in range(S)]
+    ks = [None] * (S + 1)
+    kbar = [buf() for _ in range(S + 1)]
+    t_stage = torch.zeros(S, B, dtype=T, device=dev)
+    keep = dict(y0=buf(), k0=buf(), y1=buf(), ymid=buf(), ybar0=buf(), ybar1=buf(), gy=buf(), gk=buf(), gk_first=buf(),
+                shift=torch.zeros(B, dtype=torch.float64, device=dev))
+    n_out = grad_sol.shape[0]
+    sbar = torch.zeros(B, n_out, dtype=torch.float64, device=dev) if need_t else None
+    sw = _lib.RowsSweep()
+    for name, x in keep.items():
+        setattr(sw, name, x.data_ptr())
+    sw.y_start, sw.t_first, sw.t_stage = y_start.data_ptr(), eng.t_first.data_ptr(), t_stage.data_ptr()
+    sw.sbar = sbar.data_ptr() if sbar is not None else None
+    sw.grad_sol, sw.n_out = grad_sol.data_ptr(), n_out
+    for i in range(S):
+        sw.stage[i] = stage[i].data_ptr()
+    for j in range(S + 1):
+        sw.kbar[j] = kbar[j].data_ptr()
+    tab, tp, st = C.byref(eng.tab), C.byref(tape.st), _stream()
+    ctrl = eng.ctrl.data_ptr()
+    y1 = stage[S - 1] if fsal else keep["y1"]
+    for it in range(int(tape.count.max()) if B else 0):
+        sw.iter = it
+        _lib.check(lib.tdq_rows_grad_gather(ctrl, dc, tp, C.byref(sw), B, D, st))
+        # the step's stages, bitwise the forward's; k_S only feeds the output times' gradient (p'(x) needs f1)
+        for i in range(S):
+            _lib.check(lib.tdq_rows_grad_combine(ctrl, tab, dc, tp, C.byref(sw), i, B, D, st))
+            if i < S - 1 or need_t:
+                ks[i + 1] = F(t_stage[i].view(tshape), stage[i]).contiguous()
+                sw.k[i + 1] = ks[i + 1].data_ptr()
+        if need_t:
+            if not fsal:
+                _lib.check(lib.tdq_rows_grad_combine(ctrl, tab, dc, tp, C.byref(sw), S, B, D, st))
+            _lib.check(lib.tdq_rows_grad_combine(ctrl, tab, dc, tp, C.byref(sw), -1, B, D, st))
+        _lib.check(lib.tdq_rows_grad_dense(ctrl, tab, dc, tp, C.byref(sw), B, D, st))
+        if not fsal:                                                          # y1 = y0 + sum_j c_sol_j dt k_j
+            _lib.check(lib.tdq_rows_grad_stage(ctrl, tab, dc, tp, C.byref(sw), S, None, None, B, D, st))
+        for i in reversed(range(S)):
+            gY, gt = sa.vjp(t_stage[i].view(tshape), stage[i], kbar[i + 1])
+            gY = gY.to(T).contiguous() if gY is not None else None
+            gt = gt.to(T).contiguous() if gt is not None else None
+            _lib.check(lib.tdq_rows_grad_stage(ctrl, tab, dc, tp, C.byref(sw), i, gY.data_ptr() if gY is not None else None,
+                                               gt.data_ptr() if gt is not None else None, B, D, st))
+            del gY, gt
+        ks = [None] * (S + 1)
+        for j in range(1, S + 1):
+            sw.k[j] = None
+    # each row's first k_0 = f(t_first, y0) (rk_common.py:214): one VJP for the whole batch
+    gyk, gt = sa.vjp(eng.t_first, y_start, keep["gk_first"])
+    y0bar = keep["gy"] + grad_sol[0]                                            # solution[0] = y0 (solvers.py:30)
+    if gyk is not None:
+        y0bar = y0bar + gyk
+    tbar = None
+    if need_t:
+        shift = keep["shift"]
+        if gt is not None:
+            shift = shift + sign * gt.reshape(B).double()
+        sbar[:, 0] += shift
+        tbar = sbar if t.dim() == 2 else sbar.sum(dim=0)
+        tbar = (tbar * sign).to(t.dtype).to(t.device)
+    return tbar, y0bar, sa.pbar
+
+
 def fixed_backward(p, method, tape, grid, t_cpu, grad_sol, params, need_t):
     """Reverse sweep over the steps of a fixed-grid solve (solvers.py:102-128, linear interpolation :175-181).
     grid / t_cpu: ascending CPU tensors.  Returns (grid_bar, t_out_bar) as float64 device tensors (or None), y0_bar,
@@ -386,7 +469,10 @@ class _BackpropFunction(torch.autograd.Function):
         t, *params = ctx.saved_tensors
         grad_sol = grad_sol.contiguous()
         with on_solver_stream(p.device) as ss:
-            if ctx.aux["kind"] == "adaptive":
+            if ctx.aux["kind"] == "rows":
+                with torch.no_grad():
+                    tbar, y0bar, pbar = rows_backward(p, ctx.aux["tape"], t, grad_sol, params, ctx.need_t)
+            elif ctx.aux["kind"] == "adaptive":
                 with torch.no_grad():
                     tbar, y0bar, pbar = adaptive_backward(p, ctx.aux["tab"], ctx.aux["tape"], t, grad_sol, params,
                                                           ctx.need_t)

@@ -730,6 +730,286 @@ k_rows_event_bisect(const TdqCtrl *__restrict__ c, Rows R, Geom g, BisectArgs a,
         out[i] = tdq_eval_poly<T>(cf[i], cf[n + i], cf[2 * n + i], cf[3 * n + i], cf[4 * n + i], x);
 }
 
+// ---- the step tape of a differentiable solve (include/tdq.h, "gradients of independent-row solves") -------------------------
+// A segment holds seg_slots slots as [y pairs][k pairs][float64 T0, T1, FIT_DT per slot][int32 EMIT_LO, EMIT_HI, step].
+inline size_t tape_segment_bytes(size_t es, size_t seg_slots, size_t D) { return seg_slots * (2 * D * es + 24 + 12); }
+
+template <typename T> struct TapeSlot {
+    T *y, *k;
+    double *rt;                           // T0, T1, FIT_DT
+    int *ri;                              // EMIT_LO, EMIT_HI, step index
+};
+template <typename T> __device__ __forceinline__ TapeSlot<T> tape_slot(const tdq_rows_tape &tp, size_t D, long long slot) {
+    const size_t ss = (size_t)tp.seg_slots, o = (size_t)(slot % tp.seg_slots);
+    unsigned char *b = reinterpret_cast<unsigned char *>(tp.seg[slot / tp.seg_slots]);
+    T *y = reinterpret_cast<T *>(b);
+    double *rt = reinterpret_cast<double *>(b + 2 * ss * D * sizeof(T));
+    int *ri = reinterpret_cast<int *>(rt + 3 * ss);
+    return TapeSlot<T>{y + o * D, y + (ss + o) * D, rt + 3 * o, ri + 3 * o};
+}
+
+// One thread per row: a row that accepted in this attempt takes a slot and writes its record and index entry.  ACCEPT is
+// not read: a done row keeps the value of its last attempt.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_rows_tape_claim(Rows R, tdq_rows_tape tp, size_t D) {
+    const int r = blockIdx.x * kThreads + threadIdx.x;
+    if (r >= R.B) return;
+    const int n = tp.count[r];
+    int fresh = -1;
+    if ((int64_t)n < fld<int64_t>(R, TDQ_ROWS_N_ACCEPT)[r]) {
+        const int slot = atomicAdd(tp.used, 1);
+        // past the capacity the slot is dropped; the caller sees *used beyond it and fails the solve
+        if ((int64_t)slot < tp.n_seg * tp.seg_slots && (int64_t)n < tp.n_steps) {
+            const TapeSlot<T> s = tape_slot<T>(tp, D, slot);
+            s.rt[0] = fld<double>(R, TDQ_ROWS_T0)[r];
+            s.rt[1] = fld<double>(R, TDQ_ROWS_T1)[r];
+            s.rt[2] = fld<double>(R, TDQ_ROWS_FIT_DT)[r];
+            s.ri[0] = fld<int>(R, TDQ_ROWS_EMIT_LO)[r];
+            s.ri[1] = fld<int>(R, TDQ_ROWS_EMIT_HI)[r];
+            s.ri[2] = n;
+            tp.index[(size_t)n * R.B + r] = slot;
+            fresh = slot;
+        }
+        tp.count[r] = n + 1;
+    }
+    tp.fresh[r] = fresh;
+}
+
+// Per unit: the claimed slot gets the pair the step started from, bit for bit.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_rows_tape_copy(const TdqCtrl *__restrict__ c, Rows R, Geom g, tdq_rows_tape tp,
+                                                             int *used_host) {
+    if (used_host && blockIdx.x == 0 && threadIdx.x == 0) {
+        *reinterpret_cast<volatile int *>(used_host) = *tp.used;
+        __threadfence_system();
+    }
+    size_t u, lo, hi;
+    int r;
+    if (!unit_of(g, u, r, lo, hi)) return;
+    const int slot = tp.fresh[r];
+    if (slot < 0) return;
+    const int par = fld<int>(R, TDQ_ROWS_PAR)[r] ^ 1;
+    const size_t base = (size_t)r * g.D;
+    const T *y0 = reinterpret_cast<const T *>(c->ybuf[par]) + base, *k0 = reinterpret_cast<const T *>(c->kbuf[par]) + base;
+    const TapeSlot<T> s = tape_slot<T>(tp, g.D, slot);
+    for (size_t i = lo + (threadIdx.x & 31); i < hi; i += 32) {
+        s.y[i] = y0[i];
+        s.k[i] = k0[i];
+    }
+}
+
+// ---- the reverse sweep ------------------------------------------------------------------------------------------------------
+// Row r's step in iteration s.iter, or -1 (idle).
+__device__ __forceinline__ int sweep_slot(const tdq_rows_tape &tp, const tdq_rows_sweep &s, int B, int r) {
+    const int step = tp.count[r] - 1 - s.iter;
+    return step >= 0 ? tp.index[(size_t)step * B + r] : -1;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_rows_grad_gather(const TdqCtrl *__restrict__ c, Geom g, int B, tdq_rows_tape tp,
+                                                               tdq_rows_sweep s) {
+    size_t u, lo, hi;
+    int r;
+    if (!unit_of(g, u, r, lo, hi)) return;
+    const int slot = sweep_slot(tp, s, B, r), S = c->n_stages, lane = threadIdx.x & 31;
+    const size_t base = (size_t)r * g.D;
+    T *ts = reinterpret_cast<T *>(s.t_stage);
+    if (slot < 0) {
+        if (lane == 0 && lo == 0)
+            for (int i = 0; i < S; ++i) ts[(size_t)i * B + r] = reinterpret_cast<const T *>(s.t_first)[r];
+        for (size_t i = lo + lane; i < hi; i += 32)
+            for (int j = 0; j <= S; ++j) reinterpret_cast<T *>(s.kbar[j])[base + i] = (T)0;
+        return;
+    }
+    const TapeSlot<T> p = tape_slot<T>(tp, g.D, slot);
+    if (lane == 0 && lo == 0) {                                           // rk_common.py:72-78, as row_prepare forms them
+        const T t0T = (T)p.rt[0], t1T = (T)p.rt[1], dtT = (T)p.rt[2], sgn = (T)c->t_sign;
+        for (int i = 0; i < S; ++i) ts[(size_t)i * B + r] = tdq_stage_time<T>((T)c->alpha[i], t0T, dtT, t1T, sgn);
+    }
+    T *y0 = reinterpret_cast<T *>(s.y0) + base, *k0 = reinterpret_cast<T *>(s.k0) + base;
+    T *yb0 = reinterpret_cast<T *>(s.ybar0) + base, *yb1 = reinterpret_cast<T *>(s.ybar1) + base;
+    const T *gy = reinterpret_cast<const T *>(s.gy) + base, *gk = reinterpret_cast<const T *>(s.gk) + base;
+    for (size_t i = lo + lane; i < hi; i += 32) {
+        y0[i] = p.y[i];
+        k0[i] = p.k[i];
+        yb0[i] = (T)0;
+        yb1[i] = gy[i];
+        for (int j = 0; j < S; ++j) reinterpret_cast<T *>(s.kbar[j])[base + i] = (T)0;
+        reinterpret_cast<T *>(s.kbar[S])[base + i] = gk[i];
+    }
+}
+
+// out = y0 + sum_m k_m * fl_T(w_m * T(dt_r)) for an active row (k_rows_combine's arithmetic, the forward's terms), y_start
+// for an idle one.  coefs: the compacted row of the control block (beta row, c_sol row or c_mid).
+template <typename T, int NK>
+__global__ void __launch_bounds__(kThreads)
+k_rows_grad_combine(const TdqCtrl *__restrict__ c, Geom g, int B, tdq_rows_tape tp, tdq_rows_sweep s, int row, KPtrs kp,
+                    T *__restrict__ out) {
+    size_t u, lo, hi;
+    int r;
+    if (!unit_of(g, u, r, lo, hi)) return;
+    const int slot = sweep_slot(tp, s, B, r), lane = threadIdx.x & 31;
+    const size_t base = (size_t)r * g.D;
+    T *o = out + base;
+    if (slot < 0) {
+        const T *ys = reinterpret_cast<const T *>(s.y_start) + base;
+        for (size_t i = lo + lane; i < hi; i += 32) o[i] = ys[i];
+        return;
+    }
+    const T dtT = (T)tape_slot<T>(tp, g.D, slot).rt[2], sgn = (T)c->t_sign;
+    const double *w = row >= 0 ? c->beta[row] : c->c_mid;
+    T cf[NK];
+    const T *k[NK];
+#pragma unroll
+    for (int m = 0; m < NK; ++m) {
+        cf[m] = tdq_coef<T>(sgn, (T)w[m], dtT);
+        k[m] = reinterpret_cast<const T *>(kp.p[m] ? kp.p[m] : s.k0) + base;
+    }
+    const T *y0 = reinterpret_cast<const T *>(s.y0) + base;
+    for (size_t i = lo + lane; i < hi; i += 32) o[i] = tdq_combine<T, NK>(y0[i], TdqTerms<T>{k, i}, cf);
+}
+
+// The adjoint of the quartic for the outputs [lo, hi) of an active row's step.  With p(x) = e + d x + c x^2 + b x^3 + a x^4
+// and the sums E, D1, C, B3, A of G_j x_j^p over the step's outputs:
+//   ybar0 += E + 18 B3 - 8 A - 11 C + M,  ybar1 += -8 A + 14 B3 - 5 C,  M = 16 A - 32 B3 + 16 C  (ymid's adjoint),
+//   kbar_0 += sdt (-2 A + 5 B3 - 4 C + D1),  kbar_S += sdt (2 A - 3 B3 + C),  kbar_j += fl_T(c_mid_j * T(dt)) M.
+template <typename T, int NM>
+__global__ void __launch_bounds__(kThreads)
+k_rows_grad_dense(const TdqCtrl *__restrict__ c, Geom g, int B, tdq_rows_tape tp, tdq_rows_sweep s, KPtrsMut km) {
+    using A = Ar<T>;
+    size_t u, lo, hi;
+    int r;
+    if (!unit_of(g, u, r, lo, hi)) return;
+    const int slot = sweep_slot(tp, s, B, r);
+    if (slot < 0) return;
+    const TapeSlot<T> p = tape_slot<T>(tp, g.D, slot);
+    const int jlo = p.ri[0], jhi = p.ri[1];
+    if (jhi <= jlo) return;
+    const double t0 = p.rt[0], t1 = p.rt[1];
+    const T dtT = (T)p.rt[2], sgn = (T)c->t_sign, sdt = A::mul(sgn, dtT);
+    const int S = c->n_stages;
+    T mf[NM];
+    T *kmid[NM];
+    const size_t base = (size_t)r * g.D, n = (size_t)B * g.D;
+#pragma unroll
+    for (int m = 0; m < NM; ++m) {
+        mf[m] = tdq_coef<T>(sgn, (T)c->c_mid[m], dtT);
+        kmid[m] = reinterpret_cast<T *>(km.p[m]) + base;
+    }
+    const double *t_row = row_times(*c, r).t;
+    const T *G = reinterpret_cast<const T *>(s.grad_sol) + base;
+    T *yb0 = reinterpret_cast<T *>(s.ybar0) + base, *yb1 = reinterpret_cast<T *>(s.ybar1) + base;
+    T *kb0 = reinterpret_cast<T *>(s.kbar[0]) + base, *kbS = reinterpret_cast<T *>(s.kbar[S]) + base;
+    for (size_t i = lo + (threadIdx.x & 31); i < hi; i += 32) {
+        T E = (T)0, D1 = (T)0, C = (T)0, B3 = (T)0, A4 = (T)0;
+        for (int j = jlo; j < jhi; ++j) {
+            const T x = (T)((t_row[j] - t0) / (t1 - t0));                 // k_rows_fit_eval's x
+            const T gv = G[(size_t)j * n + i];
+            const T x2 = A::mul(x, x), x3 = A::mul(x2, x), x4 = A::mul(x3, x);
+            E = A::add(E, gv);
+            D1 = A::add(D1, A::mul(x, gv));
+            C = A::add(C, A::mul(x2, gv));
+            B3 = A::add(B3, A::mul(x3, gv));
+            A4 = A::add(A4, A::mul(x4, gv));
+        }
+        const T M = A::add(A::sub(A::mul((T)16, A4), A::mul((T)32, B3)), A::mul((T)16, C));
+        yb0[i] = A::add(yb0[i], A::add(A::sub(A::sub(A::add(E, A::mul((T)18, B3)), A::mul((T)8, A4)), A::mul((T)11, C)), M));
+        yb1[i] = A::add(yb1[i], A::sub(A::sub(A::mul((T)14, B3), A::mul((T)8, A4)), A::mul((T)5, C)));
+        kb0[i] = A::add(kb0[i], A::mul(sdt, A::add(A::sub(A::add(A::mul((T)-2, A4), A::mul((T)5, B3)), A::mul((T)4, C)), D1)));
+        kbS[i] = A::add(kbS[i], A::mul(sdt, A::add(A::sub(A::mul((T)2, A4), A::mul((T)3, B3)), C)));
+#pragma unroll
+        for (int m = 0; m < NM; ++m) kmid[m][i] = A::add(kmid[m][i], A::mul(mf[m], M));
+    }
+}
+
+// One warp per row: each output's time gradient G_j . p'(x_j) / (T1 - T0), summed in float64 chunk by chunk in
+// k_rows_norm's order (lane-sequential, the shuffle tree, chunks in index order), so it depends on D alone.
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+k_rows_grad_time(const TdqCtrl *__restrict__ c, Geom g, int B, tdq_rows_tape tp, tdq_rows_sweep s, const T *__restrict__ y1p) {
+    using A = Ar<T>;
+    const int r = blockIdx.x * kWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (r >= B) return;
+    const int slot = sweep_slot(tp, s, B, r);
+    if (slot < 0) return;
+    const TapeSlot<T> p = tape_slot<T>(tp, g.D, slot);
+    const int jlo = p.ri[0], jhi = p.ri[1];
+    if (jhi <= jlo) return;
+    const double t0 = p.rt[0], t1 = p.rt[1];
+    const T sdt = A::mul((T)c->t_sign, (T)p.rt[2]), two_sdt = A::mul((T)2, sdt);
+    const size_t base = (size_t)r * g.D, n = (size_t)B * g.D;
+    const T *y0 = reinterpret_cast<const T *>(s.y0) + base, *f0 = reinterpret_cast<const T *>(s.k0) + base;
+    const T *y1 = y1p + base, *f1 = reinterpret_cast<const T *>(s.k[c->n_stages]) + base;
+    const T *ym = reinterpret_cast<const T *>(s.ymid) + base;
+    const T *G = reinterpret_cast<const T *>(s.grad_sol) + base;
+    const double *t_row = row_times(*c, r).t;
+    for (int j = jlo; j < jhi; ++j) {
+        const T x = (T)((t_row[j] - t0) / (t1 - t0));
+        const T x2 = A::mul((T)2, x), x3 = A::mul((T)3, A::mul(x, x)), x4 = A::mul((T)4, A::mul(A::mul(x, x), x));
+        double total = 0.0;
+        for (size_t lo = 0; lo < g.D; lo += kChunk) {
+            const size_t hi = lo + kChunk < g.D ? lo + kChunk : g.D;
+            double acc = 0.0;
+            for (size_t i = lo + lane; i < hi; i += 32) {
+                T e, d, cq, b, a;
+                tdq_quartic<T>(y0[i], y1[i], f0[i], f1[i], ym[i], sdt, two_sdt, e, d, cq, b, a);
+                const T dp = A::add(A::add(A::add(d, A::mul(x2, cq)), A::mul(x3, b)), A::mul(x4, a));
+                acc += (double)G[(size_t)j * n + i] * (double)dp;
+            }
+            total += warp_sum(acc);
+        }
+        if (lane == 0) {
+            const double xb = total / (t1 - t0);
+            s.sbar[(size_t)r * s.n_out + j] += xb;
+            s.shift[r] -= xb;
+        }
+    }
+}
+
+// The adjoint of Y_row = y0 + sum_j w_j k_j for an active row: Ybar = gY (+ ybar1), ybar0 += Ybar, kbar_j += w_j Ybar; the
+// time gradient of the stage into shift; at row 0 the hand-over to the row's previous step.
+template <typename T, int NK>
+__global__ void __launch_bounds__(kThreads)
+k_rows_grad_stage(const TdqCtrl *__restrict__ c, Geom g, int B, tdq_rows_tape tp, tdq_rows_sweep s, int row, KPtrsMut kb,
+                  const T *__restrict__ gY, const T *__restrict__ gt, bool add_ybar1) {
+    using A = Ar<T>;
+    size_t u, lo, hi;
+    int r;
+    if (!unit_of(g, u, r, lo, hi)) return;
+    const int slot = sweep_slot(tp, s, B, r), lane = threadIdx.x & 31;
+    if (slot < 0) return;
+    const TapeSlot<T> p = tape_slot<T>(tp, g.D, slot);
+    const T dtT = (T)p.rt[2], sgn = (T)c->t_sign;
+    if (gt && lane == 0 && lo == 0) s.shift[r] += c->t_sign * (double)gt[r];   // d/ds of func's time sgn * s
+    T cf[NK];
+    T *k[NK];
+    const size_t base = (size_t)r * g.D;
+#pragma unroll
+    for (int m = 0; m < NK; ++m) {
+        cf[m] = tdq_coef<T>(sgn, (T)c->beta[row][m], dtT);
+        k[m] = reinterpret_cast<T *>(kb.p[m]) + base;
+    }
+    T *yb0 = reinterpret_cast<T *>(s.ybar0) + base;
+    const T *yb1 = reinterpret_cast<const T *>(s.ybar1) + base, *gYr = gY ? gY + base : nullptr;
+    const bool handover = row == 0;
+    const bool first = p.ri[2] == 0;
+    T *kb0 = reinterpret_cast<T *>(s.kbar[0]) + base, *gy = reinterpret_cast<T *>(s.gy) + base;
+    T *gk = reinterpret_cast<T *>(first ? s.gk_first : s.gk) + base, *gk_zero = reinterpret_cast<T *>(s.gk) + base;
+    for (size_t i = lo + lane; i < hi; i += 32) {
+        T yb = gYr ? gYr[i] : (T)0;
+        if (add_ybar1) yb = A::add(yb, yb1[i]);
+        const T y0n = A::add(yb0[i], yb);
+        yb0[i] = y0n;
+#pragma unroll
+        for (int m = 0; m < NK; ++m) k[m][i] = A::add(k[m][i], A::mul(cf[m], yb));
+        if (handover) {
+            gy[i] = y0n;
+            gk[i] = kb0[i];
+            if (first) gk_zero[i] = (T)0;
+        }
+    }
+}
+
 // ---- host helpers -----------------------------------------------------------------------------------------------------------
 bool plan_kp(const int *idx, int nnz, const void *const *k, KPtrs &kp, bool &vec) {
     return tdq_plan_terms(idx, nnz, k, kp.p, vec) == TDQ_PLAN_OK;
@@ -1022,6 +1302,156 @@ int tdq_rows_fit_eval(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, in
                        return 0;
                    }));
     TDQ_REQUIRE(rc == 0, "unsupported number of mid-point terms");
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+// ---- gradients of independent-row solves ------------------------------------------------------------------------------------
+size_t tdq_rows_tape_segment_bytes(int32_t dtype, size_t seg_slots, size_t row_len) {
+    const size_t es = dtype == TDQ_F32 ? 4 : (dtype == TDQ_F64 ? 8 : 0);
+    if (es == 0) return 0;
+    return tape_segment_bytes(es, seg_slots, row_len);
+}
+
+#define TDQ_ROWS_REQUIRE_TAPE(tp)                                                                                  \
+    TDQ_REQUIRE((tp) && (tp)->seg && (tp)->index && (tp)->count && (tp)->fresh && (tp)->used, "null argument"); \
+    TDQ_REQUIRE((tp)->seg_slots >= 256 && (tp)->seg_slots % 256 == 0, "seg_slots must be a positive multiple of 256"); \
+    TDQ_REQUIRE((tp)->n_seg >= 1 && (tp)->n_steps >= 1, "empty tape")
+
+int tdq_rows_tape_push(void *ctrl_dev, void *rows_dev, int32_t dtype, const tdq_rows_tape *tape, size_t n_rows,
+                       size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev, "null argument");
+    TDQ_ROWS_REQUIRE_TAPE(tape);
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    int *used_host = nullptr;
+    if (tape->used_host) TDQ_CHECK_CUDA(cudaHostGetDevicePointer((void **)&used_host, tape->used_host, 0));
+    const Geom g = make_geom(n_rows, row_len);
+    const Rows R = make_rows(rows_dev, n_rows);
+    cudaStream_t st = (cudaStream_t)stream;
+    TDQ_DISPATCH_T(dtype, (k_rows_tape_claim<T><<<row_blocks(n_rows), kThreads, 0, st>>>(R, *tape, row_len),
+                           k_rows_tape_copy<T><<<unit_blocks(g), kThreads, 0, st>>>((const TdqCtrl *)ctrl_dev, R, g, *tape,
+                                                                                      used_host)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+#define TDQ_ROWS_REQUIRE_SWEEP(sw)                                                                                 \
+    TDQ_REQUIRE((sw) && (sw)->y_start && (sw)->t_first && (sw)->y0 && (sw)->k0 && (sw)->t_stage && (sw)->ybar0 &&  \
+                    (sw)->ybar1 && (sw)->gy && (sw)->gk && (sw)->gk_first && (sw)->shift && (sw)->grad_sol,     \
+                "null argument");                                                                            \
+    TDQ_REQUIRE((sw)->iter >= 0 && (sw)->n_out >= 1, "iter / n_out out of range")
+
+int tdq_rows_grad_gather(void *ctrl_dev, int32_t dtype, const tdq_rows_tape *tape, const tdq_rows_sweep *sw,
+                         size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev, "null argument");
+    TDQ_ROWS_REQUIRE_TAPE(tape);
+    TDQ_ROWS_REQUIRE_SWEEP(sw);
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    const Geom g = make_geom(n_rows, row_len);
+    TDQ_DISPATCH_T(dtype, (k_rows_grad_gather<T><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(
+                               (const TdqCtrl *)ctrl_dev, g, (int)n_rows, *tape, *sw)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_grad_combine(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, const tdq_rows_tape *tape,
+                          const tdq_rows_sweep *sw, int32_t row, size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && tab, "null argument");
+    TDQ_ROWS_REQUIRE_TAPE(tape);
+    TDQ_ROWS_REQUIRE_SWEEP(sw);
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TdqHostShape hs;
+    tdq_shape_from_tableau(tab, &hs);
+    const int S = hs.n_stages;
+    TDQ_REQUIRE(row >= -1 && row <= S && !(row == S && hs.fsal), "row out of range");
+    const int nk = row >= 0 ? hs.row_nnz[row] : hs.mid_nnz;
+    const int *idx = row >= 0 ? hs.row_idx[row] : hs.mid_idx;
+    void *out = row < 0 ? sw->ymid : (row == S ? sw->y1 : sw->stage[row]);
+    TDQ_REQUIRE(out != nullptr, "null argument");
+    TDQ_REQUIRE(nk >= 1, "empty tableau row");
+    KPtrs kp;
+    bool vec = true;
+    TDQ_REQUIRE(plan_kp(idx, nk, sw->k, kp, vec), "missing stage slot for a non-zero tableau entry");
+    const Geom g = make_geom(n_rows, row_len);
+    int rc = -1;
+    TDQ_DISPATCH_T(dtype, rc = tdq_dispatch(TdqRange<1, TDQ_MAX_K>{}, nk, [&](auto NK) {
+                       k_rows_grad_combine<T, NK><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(
+                           (const TdqCtrl *)ctrl_dev, g, (int)n_rows, *tape, *sw, row, kp, (T *)out);
+                       return 0;
+                   }));
+    TDQ_REQUIRE(rc == 0, "unsupported number of stage terms");
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+// The adjoint pointers kbar[idx[m]] of a compacted coefficient row.
+static bool plan_kbar(const tdq_rows_sweep *sw, const int *idx, int nk, KPtrsMut &kb) {
+    for (int m = 0; m < TDQ_MAX_K; ++m) kb.p[m] = nullptr;
+    for (int m = 0; m < nk; ++m) {
+        kb.p[m] = sw->kbar[idx[m]];
+        if (!kb.p[m]) return false;
+    }
+    return true;
+}
+
+int tdq_rows_grad_dense(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, const tdq_rows_tape *tape,
+                        const tdq_rows_sweep *sw, size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && tab, "null argument");
+    TDQ_ROWS_REQUIRE_TAPE(tape);
+    TDQ_ROWS_REQUIRE_SWEEP(sw);
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TdqHostShape hs;
+    tdq_shape_from_tableau(tab, &hs);
+    const int S = hs.n_stages, nm = hs.mid_nnz;
+    TDQ_REQUIRE(nm >= 1, "tableau has no mid-point weights");
+    TDQ_REQUIRE(sw->kbar[0] && sw->kbar[S], "null argument");
+    KPtrsMut km;
+    TDQ_REQUIRE(plan_kbar(sw, hs.mid_idx, nm, km), "missing adjoint slot for a non-zero mid-point weight");
+    const void *y1 = hs.fsal ? sw->stage[S - 1] : sw->y1;
+    if (sw->sbar) TDQ_REQUIRE(y1 && sw->ymid && sw->k[S], "the time gradient needs y1, ymid and k_S");
+    const Geom g = make_geom(n_rows, row_len);
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = -1;
+    TDQ_DISPATCH_T(dtype, rc = tdq_dispatch(TdqRange<1, TDQ_MAX_K>{}, nm, [&](auto NM) {
+                       // the time dots read the quartic's inputs only: they go first, in the same stream
+                       if (sw->sbar)
+                           k_rows_grad_time<T><<<tdq_grid(n_rows, kWarps, 0), kThreads, 0, st>>>(
+                               (const TdqCtrl *)ctrl_dev, g, (int)n_rows, *tape, *sw, (const T *)y1);
+                       k_rows_grad_dense<T, NM><<<unit_blocks(g), kThreads, 0, st>>>((const TdqCtrl *)ctrl_dev, g,
+                                                                                    (int)n_rows, *tape, *sw, km);
+                       return 0;
+                   }));
+    TDQ_REQUIRE(rc == 0, "unsupported number of mid-point terms");
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_grad_stage(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, const tdq_rows_tape *tape,
+                        const tdq_rows_sweep *sw, int32_t row, const void *gY, const void *gt, size_t n_rows,
+                        size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && tab, "null argument");
+    TDQ_ROWS_REQUIRE_TAPE(tape);
+    TDQ_ROWS_REQUIRE_SWEEP(sw);
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TdqHostShape hs;
+    tdq_shape_from_tableau(tab, &hs);
+    const int S = hs.n_stages;
+    TDQ_REQUIRE(row >= 0 && row <= S && !(row == S && hs.fsal), "row out of range");
+    TDQ_REQUIRE(row < S || (gY == nullptr && gt == nullptr), "the c_sol row takes no VJP");
+    const int nk = hs.row_nnz[row];
+    TDQ_REQUIRE(nk >= 1, "empty tableau row");
+    KPtrsMut kb;
+    TDQ_REQUIRE(plan_kbar(sw, hs.row_idx[row], nk, kb), "missing adjoint slot for a non-zero tableau entry");
+    const bool add_ybar1 = row == S || (hs.fsal && row == S - 1);
+    const Geom g = make_geom(n_rows, row_len);
+    int rc = -1;
+    TDQ_DISPATCH_T(dtype, rc = tdq_dispatch(TdqRange<1, TDQ_MAX_K>{}, nk, [&](auto NK) {
+                       k_rows_grad_stage<T, NK><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(
+                           (const TdqCtrl *)ctrl_dev, g, (int)n_rows, *tape, *sw, row, kb, (const T *)gY, (const T *)gt,
+                           add_ybar1);
+                       return 0;
+                   }));
+    TDQ_REQUIRE(rc == 0, "unsupported number of stage terms");
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
 }

@@ -35,7 +35,7 @@ _FIXED_OPTIONS = {"step_size", "grid_constructor", "interp", "perturb", "norm"}
 _ADAMS_OPTIONS = _FIXED_OPTIONS | {"max_iters", "max_order"}
 _IMPLICIT_OPTIONS = _FIXED_OPTIONS | {"max_iters"}                                  # rk_common.py:382-388
 _OUR_OPTIONS = {"graph", "run_ahead", "process_group", "cache", "exchange", "device_loop", "fused_linear", "fused_attempt",
-                 "independent_rows"}
+                 "independent_rows", "differentiable"}
 
 
 def _rms_norm(tensor):
@@ -388,7 +388,11 @@ def _check_independent_rows(func, y0, t, method, options, event_fn):
     if torch.is_grad_enabled():
         from .backprop import discover_params
         if y0.requires_grad or (isinstance(t, torch.Tensor) and t.requires_grad) or discover_params(func):
-            no("gradients (odeint under autograd with anything requiring grad); run it under torch.no_grad()")
+            if not options.get("differentiable"):
+                no("gradients (odeint under autograd with anything requiring grad) without options['differentiable']: "
+                   "pass options={'independent_rows': True, 'differentiable': True}, or run it under torch.no_grad()")
+            if event_fn is not None:
+                no("gradients through per-row events (event_fn / odeint_event under autograd)")
     if y0.dim() < 1 or y0.shape[0] < 1:
         raise ValueError("options['independent_rows'] needs y0 of shape [B, ...] with B >= 1, got %s" % (tuple(y0.shape),))
     if event_fn is None:
@@ -797,6 +801,15 @@ def _odeint_backprop(p, func, y0, t, params, _stats):
     holder = {}
 
     def run():
+        if p.options.get("independent_rows"):     # options['differentiable'] (_check_independent_rows)
+            eng = _make_adaptive_engine(p, lockstep=True)
+            t64 = p.t_cpu.to(torch.float64).to(p.device)
+            if p.t_cpu.dim() == 2:
+                sol, tape = eng.solve_taped(p.y0_flat, None, t_start=float(p.t_cpu[0, 0]), grid=t64)
+            else:
+                sol, tape = eng.solve_taped(p.y0_flat, t64, t_start=float(p.t_cpu[0]))
+            holder["eng"] = eng
+            return sol.clone(), {"kind": "rows", "tape": tape}
         if p.method in ADAPTIVE_METHODS:
             eng = _make_adaptive_engine(p, lockstep=True)
             t64 = p.t_cpu.to(torch.float64).to(p.device)
@@ -878,6 +891,11 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
     ignored.  event_t has shape [B] and the solution [2, B, ...].  The bisection tolerance is atol; with a per-element atol
     tensor row r uses the smallest of its own elements (the reference refuses a tensor atol there).  last_stats() adds
     event_calls and bisect_iters (the largest per-row bisection count).
+
+    Independent rows under autograd need options={'independent_rows': True, 'differentiable': True} (NotImplementedError
+    otherwise): row r's gradients w.r.t. y0[r] and t (or t[r]) are those of odeint(func, y0[r:r+1], t_r) differentiated
+    as above, a 1-D t and func's parameters get the sums over rows.  The solve then runs in lock step and keeps 2 D
+    elements per accepted row-step for the backward pass.  Not with event_fn / odeint_event or odeint_adjoint.
     """
     row_ev0 = row_event_fn = None
     if options and options.get("independent_rows"):
