@@ -634,6 +634,25 @@ int tdq_rows_grad_stage(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, c
                         const tdq_rows_sweep *sw, int32_t row, const void *gY, const void *gt, size_t n_rows,
                         size_t row_len, void *stream);
 
+/* ---- gradients through per-row events (tdq_rows.cu) -------------------------------------------------------------------
+ * A taped event solve runs with the per-row output table row_t [B][row_n] = (t0_r, inf, ...): no step emits, and each row's
+ * event step is its last taped slot.
+ * tdq_rows_tape_event:      after the last bisection launch, one thread per row with count[r] > 0: the row's last slot
+ *                           gets the emit range [1, 2) and row_t[r][1] = event_t[r] * t_sign (the ascending solver time the
+ *                           bisection evaluated the quartic at), so tdq_rows_grad_dense applies the quartic's adjoint at the
+ *                           event time.  Rows done at t0 (count 0) are not touched.
+ * tdq_rows_event_reroute:   the backward of the implicit-function rerouting (the reference's ImplicitFnGradientRerouting)
+ *                           for every row in one launch, one warp per row:
+ *                             out = gs + dc_dy . (-(grad_t + <gs, f>) / (dc_dt + <dc_dy, f> + 1e-12))
+ *                           gs = grad_state, f = func(event_t, state_t), dc_dy = the combined event function's gradient in
+ *                           y ([B*D], state dtype); dc_dt, grad_t: float64 [B].  Both dots are float64 sums in
+ *                           k_rows_norm's order (lane-sequential per 1024-element chunk, the shuffle tree, chunks in order),
+ *                           so a row's result depends on its own data and D alone.  out may alias grad_state. */
+int tdq_rows_tape_event(void *ctrl_dev, int32_t dtype, const tdq_rows_tape *tape, const double *event_t, double *row_t,
+                        size_t row_n, size_t n_rows, size_t row_len, void *stream);
+int tdq_rows_event_reroute(int32_t dtype, const void *grad_state, const void *f, const void *dc_dy, const double *dc_dt,
+                           const double *grad_t, void *out, size_t n_rows, size_t row_len, void *stream);
+
 /* ---- adjoint augmented state (adjoint.py:72-105, misc.py:137-165) ------------------------- */
 /* dst[offset_i .. offset_i + len_i) = scale_i * src_i for i < n_src, one launch
  * (the torch.cat of _TupleFunc, the unary minus on adj_y and the *(-1) of _ReverseFunc).

@@ -1143,6 +1143,28 @@ class RowsEngine(AdaptiveEngine):
         with the usual drivers (run-ahead, graph capture, device-side loop, lock step); the bisection is max(nitrs) + 1
         launches with one ev call between two of them and no synchronisation.  Returns (event_t float64 [B] in the
         caller's time, solution [2, n]); both are engine buffers."""
+        t64, grid = self._event_begin(t_start, ev, ev0, t_starts)
+        self.solve(y0_flat, t64, t_start, grid=grid)
+        return self._event_bisect(tol)
+
+    def solve_until_event_taped(self, y0_flat, t_start, ev, ev0, tol, t_starts=None):
+        """solve_until_event with the stepping phase in lock step and taped as solve_taped tapes it, for the reverse sweep of
+        backprop.rows_backward; bit for bit what solve_until_event computes.  It always runs on a per-row table
+        (t0_r, inf) (t_starts, or t_start for every row), whose rows give the shared start's arithmetic bit for bit.  After
+        the bisection tdq_rows_tape_event makes each row's event step (its last slot) emit output 1 and writes the row's
+        event time into column 1 of the table.  Returns (event_t, solution, RowTape)."""
+        if t_starts is None:
+            t_starts = torch.full((self.B,), float(t_start), dtype=torch.float64, device=self.device)
+        t64, grid = self._event_begin(t_start, ev, ev0, t_starts)
+        _, tape = self.solve_taped(y0_flat, t64, t_start, grid=grid)
+        event_t, sol = self._event_bisect(tol)
+        self._launch(self.lib.tdq_rows_tape_event(self.ctrl.data_ptr(), self.dt_code, C.byref(tape.st),
+                                                  event_t.data_ptr(), self.grid.data_ptr(), self.grid.shape[1], self.B,
+                                                  self.D, _stream()))
+        return event_t, sol, tape
+
+    def _event_begin(self, t_start, ev, ev0, t_starts):
+        """The event state of a solve_until_event; returns the output times (t64, grid) its stepping phase runs on."""
         B, dev = self.B, self.device
         K = int(ev0.numel()) // B
         f64 = dict(dtype=torch.float64, device=dev)
@@ -1164,7 +1186,11 @@ class RowsEngine(AdaptiveEngine):
         # the cursor never completes a row: output times [t0, inf], one row of them per row with per-row starts
         t64 = torch.tensor([t_start, float("inf")], **f64)
         grid = None if t_starts is None else torch.stack([t_starts, torch.full_like(t_starts, float("inf"))], dim=1)
-        self.solve(y0_flat, t64, t_start, grid=grid)
+        return t64, grid
+
+    def _event_bisect(self, tol):
+        """The bisection of a solve_until_event whose stepping phase has ended."""
+        B = self.B
         # nitrs from each row's last step, on the host as the reference computes it (one copy of 2 B doubles)
         o0, o1 = self.lib.tdq_rows_offset(_lib.ROWS_T0, B), self.lib.tdq_rows_offset(_lib.ROWS_T1, B)
         tt = self.rows[o0:o1 + 8 * B].view(torch.float64).cpu()
@@ -1177,7 +1203,7 @@ class RowsEngine(AdaptiveEngine):
                 ctrl, rows, dc, it, self.ev_val.data_ptr(), self.ev_init.data_ptr(), self.ev_sign0.data_ptr(),
                 self.ev_nitrs.data_ptr(), self.ev_lo.data_ptr(), self.ev_hi.data_ptr(), self.ev_coeff.data_ptr(),
                 self.solution[0].data_ptr(), self.ytmp.data_ptr(), self.ev_t.data_ptr(), self.ev_event_t.data_ptr(),
-                self.solution[1].data_ptr(), B, self.D, K, st))
+                self.solution[1].data_ptr(), B, self.D, self.K, st))
             if it < self.bisect_iters:
                 self._ev_call(self.ytmp)
         return self.ev_event_t, self.solution

@@ -185,6 +185,8 @@ _SIGNATURES = {
     "tdq_rows_grad_dense": (C.c_int, [_vp, _ptab, _i32, C.POINTER(RowsTape), C.POINTER(RowsSweep), _sz, _sz, _vp]),
     "tdq_rows_grad_stage": (C.c_int, [_vp, _ptab, _i32, C.POINTER(RowsTape), C.POINTER(RowsSweep), _i32, _vp, _vp, _sz,
                                       _sz, _vp]),
+    "tdq_rows_tape_event": (C.c_int, [_vp, _i32, C.POINTER(RowsTape), _vp, _vp, _sz, _sz, _sz, _vp]),
+    "tdq_rows_event_reroute": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _vp]),
     "tdq_xchg_create": (C.c_int, [_pp, C.POINTER(IpcHandle)]),
     "tdq_xchg_open": (C.c_int, [C.POINTER(IpcHandle), _pp]),
     "tdq_xchg_close": (C.c_int, [_vp]),

@@ -443,6 +443,9 @@ def odeint_adjoint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=No
     """adjoint.py:156-223, same signature and defaults."""
     if options and options.get("independent_rows"):
         raise NotImplementedError("options['independent_rows'] does not support odeint_adjoint")
+    if options and "event_gradient" in options:
+        from .odeint import check_event_gradient
+        check_event_gradient(options, rows=False)
     if adjoint_params is None and not isinstance(func, nn.Module):                     # adjoint.py:161-164
         raise ValueError('func must be an instance of nn.Module to specify the adjoint parameters; alternatively they '
                          'can be specified explicitly via the `adjoint_params` argument. If there are no parameters '

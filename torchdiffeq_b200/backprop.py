@@ -287,13 +287,17 @@ def adaptive_backward(p, tab, tape, t, grad_sol, params, need_t):
     return tbar, y0bar, sa.pbar
 
 
-def rows_backward(p, tape, t, grad_sol, params, need_t):
+def rows_backward(p, tape, t, grad_sol, params, need_t, event=False):
     """Reverse sweep over the taped steps of an independent-row solve (options={'independent_rows': True,
     'differentiable': True}): adaptive_backward for every row at once.  Iteration j takes row r's step count[r] - 1 - j
     (rows with fewer steps are idle and contribute exactly 0); the per-element and per-row work is libtdq's row-segmented
     kernels (tdq_rows_grad_*), func's VJPs run on the whole batch with its [B, 1, ...] time tensor.  Works in the engine's
     raw time (func's own t = t_sign * s), so the coefficients are the forward's signed ones.  Returns (t_bar or None,
-    y0_bar, [param_bar]): t_bar has t's shape, a [B, T] table's rows or, for a 1-D t, the sum over rows."""
+    y0_bar, [param_bar]): t_bar has t's shape, a [B, T] table's rows or, for a 1-D t, the sum over rows.
+
+    event: the tape of RowsEngine.solve_until_event_taped, whose solution[1] is each row's quartic at its detached event
+    time (rk_common.py:263, event_handling.py:20): that output time gets no gradient, nor does t[1] or t[:, 1], while the
+    quartic's dependence on T0 and T1 (and so on t0) stays in the shift; a row done at t0 returned y0 itself."""
     eng = tape.eng
     lib, dc, dev, T, B, D, S = eng.lib, eng.dt_code, eng.device, eng.dtype, eng.B, eng.D, eng.S
     n, sign, fsal = B * D, p.t_sign, eng.fsal
@@ -357,11 +361,16 @@ def rows_backward(p, tape, t, grad_sol, params, need_t):
     y0bar = keep["gy"] + grad_sol[0]                                            # solution[0] = y0 (solvers.py:30)
     if gyk is not None:
         y0bar = y0bar + gyk
+    if event:                                                                   # rows done at t0: solution[1] = y0
+        g1 = grad_sol[1].view(B, D)
+        y0bar = y0bar + torch.where((tape.count == 0)[:, None], g1, torch.zeros_like(g1)).view(-1)
     tbar = None
     if need_t:
         shift = keep["shift"]
         if gt is not None:
             shift = shift + sign * gt.reshape(B).double()
+        if event:
+            sbar[:, 1] = 0.0
         sbar[:, 0] += shift
         tbar = sbar if t.dim() == 2 else sbar.sum(dim=0)
         tbar = (tbar * sign).to(t.dtype).to(t.device)
@@ -469,9 +478,10 @@ class _BackpropFunction(torch.autograd.Function):
         t, *params = ctx.saved_tensors
         grad_sol = grad_sol.contiguous()
         with on_solver_stream(p.device) as ss:
-            if ctx.aux["kind"] == "rows":
+            if ctx.aux["kind"] in ("rows", "rows_event"):
                 with torch.no_grad():
-                    tbar, y0bar, pbar = rows_backward(p, ctx.aux["tape"], t, grad_sol, params, ctx.need_t)
+                    tbar, y0bar, pbar = rows_backward(p, ctx.aux["tape"], t, grad_sol, params, ctx.need_t,
+                                                      event=ctx.aux["kind"] == "rows_event")
             elif ctx.aux["kind"] == "adaptive":
                 with torch.no_grad():
                     tbar, y0bar, pbar = adaptive_backward(p, ctx.aux["tab"], ctx.aux["tape"], t, grad_sol, params,

@@ -1010,6 +1010,52 @@ k_rows_grad_stage(const TdqCtrl *__restrict__ c, Geom g, int B, tdq_rows_tape tp
     }
 }
 
+// ---- gradients through per-row events ----------------------------------------------------------------------------------------
+// One thread per row: the event step (the row's last slot) gets the single output 1, at the time the bisection ended on.
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+k_rows_tape_event(const TdqCtrl *__restrict__ c, tdq_rows_tape tp, int B, size_t D, const double *__restrict__ event_t,
+                  double *__restrict__ row_t, size_t row_n) {
+    const int r = blockIdx.x * kThreads + threadIdx.x;
+    if (r >= B) return;
+    const int n = tp.count[r];
+    if (n <= 0) return;                                                   // done at t0: no step
+    const TapeSlot<T> s = tape_slot<T>(tp, D, tp.index[(size_t)(n - 1) * B + r]);
+    s.ri[0] = 1;
+    s.ri[1] = 2;
+    row_t[(size_t)r * row_n + 1] = event_t[r] * c->t_sign;               // exact: t_sign is +-1
+}
+
+// One warp per row: the two float64 dots <gs, f> and <dc_dy, f> in k_rows_norm's order, then
+// out = gs + dc_dy * T(-(grad_t + <gs, f>) / (dc_dt + <dc_dy, f> + 1e-12)), in the reference's order of operations.
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+k_rows_event_reroute(int B, size_t D, const T *__restrict__ gs, const T *__restrict__ f, const T *__restrict__ dc,
+                     const double *__restrict__ dc_dt, const double *__restrict__ grad_t, T *out) {
+    using A = Ar<T>;
+    const int r = blockIdx.x * kWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (r >= B) return;
+    const size_t base = (size_t)r * D;
+    const T *g = gs + base, *fr = f + base, *d = dc + base;
+    double tg = 0.0, tc = 0.0;
+    for (size_t lo = 0; lo < D; lo += kChunk) {
+        const size_t hi = lo + kChunk < D ? lo + kChunk : D;
+        double ag = 0.0, ac = 0.0;
+        for (size_t i = lo + lane; i < hi; i += 32) {
+            const double fv = (double)fr[i];
+            ag += (double)g[i] * fv;
+            ac += (double)d[i] * fv;
+        }
+        tg += warp_sum(ag);
+        tc += warp_sum(ac);
+    }
+    tg = __shfl_sync(0xffffffffu, tg, 0);
+    tc = __shfl_sync(0xffffffffu, tc, 0);
+    const T scale = (T)(-(grad_t[r] + tg) / (dc_dt[r] + tc + 1e-12));
+    T *o = out + base;
+    for (size_t i = lane; i < D; i += 32) o[i] = A::add(g[i], A::mul(d[i], scale));
+}
+
 // ---- host helpers -----------------------------------------------------------------------------------------------------------
 bool plan_kp(const int *idx, int nnz, const void *const *k, KPtrs &kp, bool &vec) {
     return tdq_plan_terms(idx, nnz, k, kp.p, vec) == TDQ_PLAN_OK;
@@ -1452,6 +1498,30 @@ int tdq_rows_grad_stage(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, c
                        return 0;
                    }));
     TDQ_REQUIRE(rc == 0, "unsupported number of stage terms");
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+// ---- gradients through per-row events ---------------------------------------------------------------------------------------
+int tdq_rows_tape_event(void *ctrl_dev, int32_t dtype, const tdq_rows_tape *tape, const double *event_t, double *row_t,
+                        size_t row_n, size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && event_t && row_t, "null argument");
+    TDQ_ROWS_REQUIRE_TAPE(tape);
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_REQUIRE(row_n >= 2, "row_n must be at least 2 (the event time is column 1)");
+    TDQ_DISPATCH_T(dtype, (k_rows_tape_event<T><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (const TdqCtrl *)ctrl_dev, *tape, (int)n_rows, row_len, event_t, row_t, row_n)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_event_reroute(int32_t dtype, const void *grad_state, const void *f, const void *dc_dy, const double *dc_dt,
+                           const double *grad_t, void *out, size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(grad_state && f && dc_dy && dc_dt && grad_t && out, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_DISPATCH_T(dtype, (k_rows_event_reroute<T><<<tdq_grid(n_rows, kWarps, 0), kThreads, 0, (cudaStream_t)stream>>>(
+                               (int)n_rows, row_len, (const T *)grad_state, (const T *)f, (const T *)dc_dy, dc_dt, grad_t,
+                               (T *)out)));
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
 }

@@ -14,7 +14,7 @@ import warnings
 import torch
 
 from . import _lib
-from ._engine import AdaptiveEngine, Layout, RowsEngine, on_solver_stream
+from ._engine import _DTYPES, AdaptiveEngine, Layout, RowsEngine, on_solver_stream
 from ._adams import ADAMS_METHODS
 from ._fixed import FIXED_METHODS, choose_grid_constructor, make_engine, signed_grid_constructor
 from ._implicit import IMPLICIT_METHODS
@@ -35,7 +35,7 @@ _FIXED_OPTIONS = {"step_size", "grid_constructor", "interp", "perturb", "norm"}
 _ADAMS_OPTIONS = _FIXED_OPTIONS | {"max_iters", "max_order"}
 _IMPLICIT_OPTIONS = _FIXED_OPTIONS | {"max_iters"}                                  # rk_common.py:382-388
 _OUR_OPTIONS = {"graph", "run_ahead", "process_group", "cache", "exchange", "device_loop", "fused_linear", "fused_attempt",
-                 "independent_rows", "differentiable"}
+                 "independent_rows", "differentiable", "event_gradient"}
 
 
 def _rms_norm(tensor):
@@ -370,6 +370,18 @@ def _make_fixed_engine(p, *, graph=None, interp=None):
                        sharded=o.get("process_group") is not None)
 
 
+def check_event_gradient(options, rows=True):
+    """options['event_gradient']: 'discrete' (gradients of the discrete solve up to each row's event, the reference's
+    odeint differentiated through its event step) is the only value, and only independent rows implement it."""
+    v = options.get("event_gradient")
+    if not (isinstance(v, str) and v == "discrete"):
+        raise ValueError("options['event_gradient'] must be 'discrete', got %r" % (v,))
+    if not rows:
+        raise NotImplementedError("options['event_gradient'] is implemented for options={'independent_rows': True, "
+                                  "'differentiable': True} only; a shared-batch event solve gets its gradients from "
+                                  "odeint_adjoint")
+
+
 def _check_independent_rows(func, y0, t, method, options, event_fn):
     """What options={'independent_rows': True} does not cover raises NotImplementedError before any work."""
     def no(what):
@@ -391,8 +403,10 @@ def _check_independent_rows(func, y0, t, method, options, event_fn):
             if not options.get("differentiable"):
                 no("gradients (odeint under autograd with anything requiring grad) without options['differentiable']: "
                    "pass options={'independent_rows': True, 'differentiable': True}, or run it under torch.no_grad()")
-            if event_fn is not None:
-                no("gradients through per-row events (event_fn / odeint_event under autograd)")
+            if event_fn is not None and options.get("event_gradient") is None:
+                no("gradients through per-row events (event_fn / odeint_event under autograd) without "
+                   "options['event_gradient']: pass options={'independent_rows': True, 'differentiable': True, "
+                   "'event_gradient': 'discrete'}, or run it under torch.no_grad()")
     if y0.dim() < 1 or y0.shape[0] < 1:
         raise ValueError("options['independent_rows'] needs y0 of shape [B, ...] with B >= 1, got %s" % (tuple(y0.shape),))
     if event_fn is None:
@@ -422,14 +436,15 @@ def _check_independent_rows(func, y0, t, method, options, event_fn):
     return v
 
 
-def _solve_rows_event(p, event_fn, ev0):
+def _solve_rows_event(p, event_fn, ev0, taped=False):
     """Every row until its own event (options={'independent_rows': True}); returns (event_t float64 [B] in the caller's
-    time, solution [2, n], engine).  The captured attempt runs event_fn's Python once, so graph='auto' captures only when
-    func and event_fn are both nn.Modules.  Event engines are not cached."""
+    time, solution [2, n], engine, RowTape or None).  The captured attempt runs event_fn's Python once, so graph='auto'
+    captures only when func and event_fn are both nn.Modules.  taped: the lock-step solve that tapes every row-step for
+    the reverse sweep (RowsEngine.solve_until_event_taped).  Event engines are not cached."""
     graph = p.options.get("graph", "auto")
     if graph == "auto" and not isinstance(event_fn, torch.nn.Module):
         graph = False
-    eng = _make_adaptive_engine(p, graph=graph)
+    eng = _make_adaptive_engine(p, graph=graph, lockstep=taped)
     B, shape = p.shape[0], p.shape
     # the bisection tolerance: atol, or with a per-element atol the smallest of the row's own elements
     if p.atol_vec is not None:
@@ -438,9 +453,12 @@ def _solve_rows_event(p, event_fn, ev0):
         tol = torch.full((B,), float(p.atol), dtype=torch.float64)
     t0 = p.t_cpu[..., 0]                                  # [B]: each row's own start (per-row times), or one start
     t_starts = t0.to(torch.float64).to(p.device) if t0.dim() == 1 else None
-    event_t, sol = eng.solve_until_event(p.y0_flat, float(t0.view(-1)[0]), lambda t_, y_: event_fn(t_, y_.view(shape)),
-                                         ev0, tol, t_starts=t_starts)
-    return event_t, sol, eng
+    ev = lambda t_, y_: event_fn(t_, y_.view(shape))
+    if taped:
+        event_t, sol, tape = eng.solve_until_event_taped(p.y0_flat, float(t0.view(-1)[0]), ev, ev0, tol, t_starts=t_starts)
+        return event_t, sol, eng, tape
+    event_t, sol = eng.solve_until_event(p.y0_flat, float(t0.view(-1)[0]), ev, ev0, tol, t_starts=t_starts)
+    return event_t, sol, eng, None
 
 
 # ---- engine cache -------------------------------------------------------------------------------
@@ -725,9 +743,10 @@ def odeint_event(func, y0, t0, *, event_fn, reverse_time=False, odeint_interface
     else:
         t = torch.cat([t0.reshape(-1), t0.reshape(-1).detach() + 1.0])
     if rows:
-        # one event time per row: the implicit-function rerouting below assumes one scalar event time, and this mode
-        # refuses gradients anyway
-        return odeint_interface(func, y0, t, event_fn=event_fn, **kwargs)
+        event_t, solution = odeint_interface(func, y0, t, event_fn=event_fn, **kwargs)
+        if not solution.requires_grad:                 # no_grad, or nothing to differentiate: nothing to reroute
+            return event_t, solution
+        return _reroute_rows(func, y0, t, event_fn, reverse_time, event_t, solution)
     event_t, solution = odeint_interface(func, y0, t, event_fn=event_fn, **kwargs)
     p = normalise(func, y0, t, 0.0, 0.0, kwargs.get("method"), None, event_fn)        # flat func / event_fn, :172
     sign_ = p.t_sign
@@ -747,6 +766,64 @@ def odeint_event(func, y0, t0, *, event_fn, reverse_time=False, odeint_interface
     else:
         solution = torch.cat([solution[:-1], state_t.view(p.shape)[None]], dim=0)
     return event_t, solution
+
+
+class _RowsImplicitFnGradientRerouting(torch.autograd.Function):
+    """_ImplicitFnGradientRerouting for every row of an independent-row event solve at once: row r's event time solves its
+    own combined event function c_r(t, y_r) = 0.  The backward makes one whole-batch call of func, one VJP of the combined
+    event functions, and tdq_rows_event_reroute for the per-row formula.  Works in the solver's ascending time: fn(s, y)
+    and c_fn(s, y) take s as a float64 [B] tensor."""
+
+    @staticmethod
+    def forward(ctx, fn, c_fn, event_t, state_t):
+        ctx.fn, ctx.c_fn = fn, c_fn
+        ctx.save_for_backward(event_t, state_t)
+        return event_t.detach(), state_t.detach()
+
+    @staticmethod
+    def backward(ctx, grad_t, grad_state):
+        event_t, state_t = ctx.saved_tensors
+        B, dt = state_t.shape[0], state_t.dtype
+        y = state_t.detach()
+        s = event_t.detach().to(torch.float64)
+        with torch.no_grad():
+            f = ctx.fn(s, y).reshape(B, -1).to(dt).contiguous()
+        dcdt = dstate = None
+        with torch.enable_grad():
+            s_req, y_req = s.clone().requires_grad_(True), y.clone().requires_grad_(True)
+            c = ctx.c_fn(s_req, y_req)
+            if c.requires_grad:
+                dcdt, dstate = torch.autograd.grad(c, (s_req, y_req), torch.ones_like(c), allow_unused=True)
+        zeros = lambda: torch.zeros(B, dtype=torch.float64, device=y.device)
+        dcdt = dcdt.to(torch.float64).contiguous() if dcdt is not None else zeros()
+        dstate = dstate.reshape(B, -1).to(dt).contiguous() if dstate is not None else torch.zeros_like(f)
+        gt = grad_t.to(torch.float64).reshape(B).contiguous() if grad_t is not None else zeros()
+        gs = grad_state.reshape(B, -1).to(dt).contiguous() if grad_state is not None else torch.zeros_like(f)
+        out = torch.empty_like(gs)
+        lib = _lib.load()
+        _lib.check(lib.tdq_rows_event_reroute(_DTYPES[dt], gs.data_ptr(), f.data_ptr(), dstate.data_ptr(),
+                                              dcdt.data_ptr(), gt.data_ptr(), out.data_ptr(), B, f.shape[1],
+                                              torch.cuda.current_stream().cuda_stream))
+        return None, None, None, out.view_as(state_t)
+
+
+def _reroute_rows(func, y0, t, event_fn, reverse_time, event_t, solution):
+    """odeint_event's rerouting (odeint.py:175-194 of the reference) row by row, with reverse time handled as there: the
+    event time goes to solver time before the rerouting and back after it."""
+    B = y0.shape[0]
+    sign = -1.0 if reverse_time else 1.0
+    tshape = (B,) + (1,) * (y0.dim() - 1)
+    t0 = (t[:, 0] if t.dim() == 2 else t[0].expand(B)).detach().to(device=y0.device, dtype=torch.float64)
+    with torch.no_grad():                                                              # event_handling.py:28-29
+        init_sign = torch.sign(event_fn(t0.view(tshape), y0.detach())).reshape(B, -1)
+
+    def fn(s, y):                                                                      # the ascending-time dynamics
+        return func((s * sign).to(y.dtype).view(tshape), y) * sign
+
+    def c_fn(s, y):                   # amin, not min(dim): its gradient splits over ties as the reference's torch.min does
+        return torch.amin(event_fn((s * sign).view(tshape), y).reshape(B, -1) * init_sign, dim=1)
+    s_t, state_t = _RowsImplicitFnGradientRerouting.apply(fn, c_fn, event_t * sign, solution[-1])
+    return s_t * sign, torch.cat([solution[:-1], state_t[None]], dim=0)
 
 
 def _as_flat(p, f):
@@ -844,6 +921,31 @@ def _odeint_backprop(p, func, y0, t, params, _stats):
     return _unflatten(p, sol)
 
 
+def _odeint_rows_event_backprop(p, y0, t, params, event_fn, ev0, _stats):
+    """odeint(event_fn=...) with independent rows under autograd (options['event_gradient'] = 'discrete'): row r is the
+    reference's odeint(func, y0[r:r+1], t_r, event_fn=ev_r) differentiated through its discrete solve up to the event step
+    and the quartic of that step at the detached event time (rk_common.py:252-264, event_handling.py:5-20).  Returns
+    (event_t [B], solution [2, B, ...]); event_t is detached except at rows done at t0, where it is t0 itself."""
+    from .backprop import _BackpropFunction
+    holder = {}
+
+    def run():
+        event_t, sol, eng, tape = _solve_rows_event(p, event_fn, ev0, taped=True)
+        holder["event_t"], holder["eng"] = event_t.clone(), eng
+        return sol.clone(), {"kind": "rows_event", "tape": tape}
+    with on_solver_stream(p.device) as ss:
+        sol = _BackpropFunction.apply(p, run, t, y0.reshape(-1), *params)
+        event_t = holder["event_t"].to(device=t.device, dtype=t.dtype)
+        ss.publish(sol, event_t)
+    eng = holder["eng"]
+    _publish_stats(eng, _stats, add_launches=False)
+    _LAST_STATS.update(event_calls=eng.n_ev, bisect_iters=eng.bisect_iters)
+    # a row done at t0 returns (t0, y0) (rk_common.py:254-255): the same value, now with t0's gradient
+    done = (eng.row_n_accept == 0).to(t.device)
+    t0 = t[:, 0] if t.dim() == 2 else t[0].expand(p.shape[0])
+    return torch.where(done, t0, event_t), _unflatten(p, sol)
+
+
 def _publish_stats(eng, _stats, add_launches):
     """last_stats() of the solve `eng` just ran.  `_stats` (private: solver counters for bench.py and the tests) gets
     the same counters except the per-row ones, and the adaptive engine's driver; its launches are added to what it holds
@@ -895,9 +997,18 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
     Independent rows under autograd need options={'independent_rows': True, 'differentiable': True} (NotImplementedError
     otherwise): row r's gradients w.r.t. y0[r] and t (or t[r]) are those of odeint(func, y0[r:r+1], t_r) differentiated
     as above, a 1-D t and func's parameters get the sums over rows.  The solve then runs in lock step and keeps 2 D
-    elements per accepted row-step for the backward pass.  Not with event_fn / odeint_event or odeint_adjoint.
+    elements per accepted row-step for the backward pass.  Not with odeint_adjoint.
+
+    event_fn / odeint_event with independent rows under autograd also need options['event_gradient'] = 'discrete' (the
+    only value; NotImplementedError without independent rows, whose shared-batch event solve takes odeint_adjoint's
+    gradients): row r's gradients are those of the reference's odeint(func, y0[r:r+1], t_r, event_fn=ev_r), the discrete
+    solve up to the row's event step and that step's interpolant at the detached event time; t[1] (or t[:, 1]) gets none,
+    and neither do event_fn's parameters.  event_t is detached, except at rows done at t0, where it is t0.  odeint_event
+    then gives every row's event time its implicit-function gradient, as the reference's odeint_event does for one.
     """
     row_ev0 = row_event_fn = None
+    if options and "event_gradient" in options:
+        check_event_gradient(options, rows=bool(options.get("independent_rows")))
     if options and options.get("independent_rows"):
         row_ev0 = _check_independent_rows(func, y0, t, method, options, event_fn)
         if row_ev0 is not None:
@@ -920,6 +1031,8 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
                                           event_fn=event_fn)
                 raise NotImplementedError("gradients through odeint(event_fn=...) need an nn.Module func (they are "
                                           "computed by odeint_adjoint)")
+            if row_event_fn is not None:
+                return _odeint_rows_event_backprop(p, y0, t, params, row_event_fn, row_ev0, _stats)
             return _odeint_backprop(p, func, y0, t, params, _stats)
     with torch.no_grad(), on_solver_stream(p.device) as ss:
         if p.event_fn is not None:
@@ -928,7 +1041,7 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
             event_t = torch.tensor(float(event_t) * p.t_sign, dtype=t.dtype, device=t.device)  # odeint.py:98-100
             return event_t, _unflatten(p, sol)                                                   # :105-108
         if row_event_fn is not None:
-            row_event_t, sol, eng = _solve_rows_event(p, row_event_fn, row_ev0)
+            row_event_t, sol, eng, _ = _solve_rows_event(p, row_event_fn, row_ev0)
             row_event_t = row_event_t.to(device=t.device, dtype=t.dtype, copy=True)
             ss.publish(row_event_t, sol)
         else:
