@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define TDQ_ABI_VERSION 3
+#define TDQ_ABI_VERSION 4
 
 #define TDQ_MAX_STAGES 16            /* func evaluations per attempt, excluding f0 (dopri8: 13)   */
 #define TDQ_MAX_K      (TDQ_MAX_STAGES + 1) /* stage slots k_0 .. k_S                              */
@@ -108,6 +108,7 @@ typedef struct {
     volatile double next_t0, next_dt; /* the same for the attempt prepared next (callback_step)     */
     volatile int32_t on_jump_t;       /* the accepted attempt ended on a jump_t point: the host must */
                                       /* re-evaluate f at taux[2] = next(T(t1)) (rk_common.py:346-351) */
+    volatile int32_t on_step_t;       /* the accepted attempt ended on a step_t point (not a jump_t one) */
     volatile int32_t par;             /* which pair of the pointer table holds the accepted state now */
 } tdq_mailbox;
 

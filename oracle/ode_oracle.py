@@ -188,6 +188,43 @@ def interp_eval(coeffs, t0, t1, t):
 
 
 # ------------------------------------------------------------------------------------------------
+# step_t / jump_t (rk_common.py:293-308, :343-351)
+# ------------------------------------------------------------------------------------------------
+def clip_step(a0, dt, step_t, jump_t, next_step, next_jump):
+    """rk_common.py:293-308: the attempt from a0 with step dt, ended on the next step_t point, or on the next jump_t point
+    (which wins), when that point lies strictly inside (a0, a0 + dt).  step_t / jump_t: sorted float64 tensors (possibly
+    empty), next_step / next_jump: the cursors into them.  Returns (a1, dt, on_step_t, on_jump_t); the clipped dt is
+    a1 - a0."""
+    a1 = a0 + dt
+    on_step_t = False
+    if len(step_t):
+        nxt = step_t[next_step]
+        on_step_t = bool(a0 < nxt < a0 + dt)
+        if on_step_t:
+            a1 = nxt
+            dt = a1 - a0
+    on_jump_t = False
+    if len(jump_t):
+        nxt = jump_t[next_jump]
+        on_jump_t = bool(a0 < nxt < a0 + dt)
+        if on_jump_t:
+            on_step_t = False
+            a1 = nxt
+            dt = a1 - a0
+    return a1, dt, on_step_t, on_jump_t
+
+
+def advance_cursors(step_t, jump_t, next_step, next_jump, on_step_t, on_jump_t):
+    """rk_common.py:343-348: after an accepted attempt the cursor of the point it ended on moves on, and sticks at the
+    last point."""
+    if on_step_t and next_step != len(step_t) - 1:
+        next_step += 1
+    if on_jump_t and next_jump != len(jump_t) - 1:
+        next_jump += 1
+    return next_step, next_jump
+
+
+# ------------------------------------------------------------------------------------------------
 # adaptive driver
 # ------------------------------------------------------------------------------------------------
 def odeint_adaptive(func, y0, t, method="dopri5", rtol=1e-7, atol=1e-9, norm=rms, min_step=0.,
@@ -237,7 +274,7 @@ def odeint_adaptive(func, y0, t, method="dopri5", rtol=1e-7, atol=1e-9, norm=rms
     next_jump = min(bisect.bisect(jump_t.tolist(), t[0]), len(jump_t) - 1)   # :241
     st = {"y": y0, "f": f0, "t_lo": t[0], "t_hi": t[0], "dt": dt, "coeffs": [y0] * 5, "next_step": next_step,
           "next_jump": next_jump}
-    stats = {"n_accept": 0, "n_reject": 0, "dts": [], "accepted": []}
+    stats = {"n_accept": 0, "n_reject": 0, "dts": [], "accepted": [], "ends": [], "clipped": [], "jumped": []}
 
     def attempt():
         """rk_common.py:266-361."""
@@ -247,24 +284,9 @@ def odeint_adaptive(func, y0, t, method="dopri5", rtol=1e-7, atol=1e-9, norm=rms
         dt = dt.clamp(min_step, max_step)
         y, f = st["y"], st["f"]
         a0 = st["t_hi"]
-        a1 = a0 + dt
         assert a0 + dt > a0, 'underflow in dt {}'.format(dt.item())
         assert torch.isfinite(y).all(), 'non-finite values in state `y`: {}'.format(y)
-        on_step_t = False
-        if len(step_t):
-            nxt = step_t[st["next_step"]]
-            on_step_t = bool(a0 < nxt < a0 + dt)
-            if on_step_t:
-                a1 = nxt
-                dt = a1 - a0
-        on_jump_t = False
-        if len(jump_t):                                             # :302-308
-            nxt = jump_t[st["next_jump"]]
-            on_jump_t = bool(a0 < nxt < a0 + dt)
-            if on_jump_t:
-                on_step_t = False
-                a1 = nxt
-                dt = a1 - a0
+        a1, dt, on_step_t, on_jump_t = clip_step(a0, dt, step_t, jump_t, st["next_step"], st["next_jump"])
         y1, f1, err, ks = rk_attempt(func, y, f, a0, dt, a1, ct)
         ratio = error_ratio(err, rtol, atol, y, y1, norm)
         accept = bool(ratio <= 1)
@@ -274,13 +296,14 @@ def odeint_adaptive(func, y0, t, method="dopri5", rtol=1e-7, atol=1e-9, norm=rms
             accept = True
         stats["dts"].append(float(dt))
         stats["accepted"].append(accept)
+        stats["ends"].append(float(a1))
+        stats["clipped"].append(on_step_t or on_jump_t)
+        stats["jumped"].append(on_jump_t)
         if accept:
             st["coeffs"] = interp_fit(y, y1, ks, dt, ct)
-            if on_step_t and st["next_step"] != len(step_t) - 1:
-                st["next_step"] += 1
+            st["next_step"], st["next_jump"] = advance_cursors(step_t, jump_t, st["next_step"], st["next_jump"],
+                                                               on_step_t, on_jump_t)
             if on_jump_t:                                           # :346-351
-                if st["next_jump"] != len(jump_t) - 1:
-                    st["next_jump"] += 1
                 f1 = func(_next(a1.to(T)), y1)
             st["y"], st["f"], st["t_lo"], st["t_hi"] = y1, f1, a0, a1
             stats["n_accept"] += 1

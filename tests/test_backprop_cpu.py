@@ -27,8 +27,10 @@ def _problem(f, y0, t):
     return p
 
 
-def _tape_adaptive(p, method, y0, rtol, atol):
-    """Accepted steps of the oracle's solve, re-stepped with the sweep's own stage formulas."""
+def _tape_adaptive(p, method, y0, rtol, atol, **options):
+    """Accepted steps of the oracle's solve, re-stepped with the sweep's own stage formulas.  options: the oracle's
+    step-control keywords (first_step, step_t, jump_t in true time).  Each step's end and clip flag are the oracle's,
+    as the engine tapes the device's."""
     tab = B.adaptive_tableau(method)
     T = p.dtype
     f_user = lambda tt, yy: p.fn(tt, yy)
@@ -36,19 +38,19 @@ def _tape_adaptive(p, method, y0, rtol, atol):
     t_true = p.t_cpu * p.t_sign
     with torch.no_grad():
         O.odeint_adaptive(lambda tt, yy: f_user(tt, yy.reshape(-1)).view(yy.shape), y0.detach(), t_true, method,
-                          rtol=rtol, atol=atol, record=rec)
+                          rtol=rtol, atol=atol, record=rec, **options)
     F = lambda s_, y_: (p.fn(s_ * p.t_sign, y_).reshape(-1) * p.t_sign)
     sa = B.StepAdjoint(F, (), False)
     s = float(p.t_cpu[0])
     y = y0.detach().reshape(-1).clone()
     with torch.no_grad():
         k = F(torch.tensor(s, dtype=torch.float64).to(T), y)
-    tape, cursor, first = [], 1, True
+    tape, cursor, first, jumped = [], 1, True, None
     s_out = p.t_cpu.double()
-    for dt, acc in zip(rec["dts"], rec["accepted"]):
+    for dt, acc, s1, clipped, jump in zip(rec["dts"], rec["accepted"], rec["ends"], rec["clipped"], rec["jumped"]):
         if not acc:
             continue
-        dtT, t0T, t1T = B._T(dt, T), B._T(s, T), B._T(s + dt, T)
+        dtT, t0T, t1T = B._T(dt, T), B._T(s, T), B._T(s1, T)
         times = [B._prev(t1T) if a == 1.0 else t0T + B._T(a, T) * dtT for a in tab.alpha]
         coefs = [[float(B._T(b, T) * dtT) for b in row] for row in tab.beta]
         Ys, ks = sa.stages(times, y, k, coefs)
@@ -57,12 +59,17 @@ def _tape_adaptive(p, method, y0, rtol, atol):
         else:
             y1 = y + sum(kk * float(dtT * B._T(c, T)) for kk, c in zip(ks, tab.c_sol) if c != 0.0)
         hi = cursor
-        while hi < len(s_out) and not (float(s_out[hi]) > s + dt):
+        while hi < len(s_out) and not (float(s_out[hi]) > s1):
             hi += 1
         # the engine's tape holds RAW func outputs (the reverse-time sign lives in its coefficients)
-        tape.append(dict(t0=s, dt=dt, y0=y, k0=k * p.t_sign, out_lo=cursor, out_hi=hi, first=first, jumped_into=None))
+        tape.append(dict(t0=s, dt=dt, t1=s1, clipped=clipped, y0=y, k0=k * p.t_sign, out_lo=cursor, out_hi=hi,
+                         first=first, jumped_into=jumped))
         cursor, first = hi, False
-        y, k, s = y1, ks[-1], s + dt
+        y, k, s = y1, ks[-1], s1
+        jumped = True if jump else None
+        if jump:                                            # f on the far side of the discontinuity (rk_common.py:346-351)
+            with torch.no_grad():
+                k = F(B._next(t1T), y)
     assert cursor == len(s_out)
     return tab, tape
 

@@ -768,9 +768,10 @@ class AdaptiveEngine:
 
     # ---- taped solve for the differentiable (non-adjoint) odeint (torchdiffeq_b200/backprop.py) ------------------
     def solve_taped(self, y0_flat, t64, t_start=None):
-        """Lock-step solve that records every ACCEPTED step: start time, step size, the (y0, k_0) pair it started from
-        (clones: 2 n elements per step), the output rows it produced and whether it followed a jump_t re-evaluation.
-        Returns (solution, tape)."""
+        """Lock-step solve that records every ACCEPTED step: start time, step size, end time as the device has it, whether
+        the step was clipped to a step_t / jump_t point (the device's decision, not a comparison of values), the (y0, k_0)
+        pair it started from (clones: 2 n elements per step), the output rows it produced and whether it followed a
+        jump_t re-evaluation.  Returns (solution, tape)."""
         steps = self._lockstep(y0_flat, t64, t_start)
         next(steps)
         tape, cursor, first, jumped = [], 1, True, None
@@ -778,7 +779,8 @@ class AdaptiveEngine:
             if mb.accept:
                 prev = (mb.par ^ 1) & 1                                     # the pair the accepted step started from
                 k0 = self.kbuf[prev]
-                tape.append(dict(t0=float(mb.att_t0), dt=float(mb.att_dt), y0=self.ybuf[prev].clone(), k0=k0.clone(),
+                tape.append(dict(t0=float(mb.att_t0), dt=float(mb.att_dt), t1=float(mb.t1),
+                                 clipped=bool(mb.on_jump_t or mb.on_step_t), y0=self.ybuf[prev].clone(), k0=k0.clone(),
                                  out_lo=cursor, out_hi=int(mb.out_cursor), first=first, jumped_into=jumped))
                 cursor, first = int(mb.out_cursor), False
                 jumped = True if mb.on_jump_t else None

@@ -18,7 +18,7 @@ TDQ_MAX_RANKS = 16
  ROWS_ACCEPT, ROWS_FIT, ROWS_DONE, ROWS_STATUS, ROWS_CURSOR, ROWS_EMIT_LO, ROWS_EMIT_HI, ROWS_N_STEPS, ROWS_N_ACCEPT,
  ROWS_N_REJECT, ROWS_T_FIRST, ROWS_T_PROBE, ROWS_T_STAGE) = range(24)
 ROWS_HEADER = 255
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 
 class IpcHandle(C.Structure):
@@ -58,7 +58,7 @@ class Mailbox(C.Structure):
         ("t0", C.c_double), ("t1", C.c_double), ("dt", C.c_double),
         ("ratio", C.c_double), ("att_t0", C.c_double), ("att_dt", C.c_double),
         ("next_t0", C.c_double), ("next_dt", C.c_double),
-        ("on_jump_t", C.c_int32), ("par", C.c_int32),
+        ("on_jump_t", C.c_int32), ("on_step_t", C.c_int32), ("par", C.c_int32),
     ]
 
 

@@ -165,12 +165,20 @@ class _BackwardSolver:
                 def _cb(t0, y_flat, dt, _cb_=cb):
                     tq, yq, aq, pq = views_of(y_flat)
                     state = (tq, *yq, *aq, *pq) if p.is_tuple else (tq, yq, aq, *pq)
-                    return _cb_(t0 * self.bsign, state, dt)               # misc.py:330-331
+                    # misc.py:330-331 on the reference's backward interval, which is always decreasing: -s whatever
+                    # the forward's direction (the true time for a forward-time solve)
+                    return _cb_(-t0, state, dt)
                 callbacks[name] = _cb
 
         # The backward solve always runs against the forward time direction (adjoint.py:136
         # t[i-1:i+1].flip(0)).  The engine integrates ascending s = bsign * t, bsign = -p.t_sign.
         self.bsign = -p.t_sign
+        # step_t / jump_t in the backward engine's time.  The reference solves each interval on its normalised (ascending)
+        # forward times flipped, a decreasing t, so misc.py:292-293 negates the points every time: -v.  For a forward-time
+        # solve that is bsign * v, the true points; for a reverse-time one the reference's backward mirrors them.
+        for name in ("step_t", "jump_t"):
+            if isinstance(opts.get(name), torch.Tensor):
+                opts[name] = -opts[name]
         self.fixed = adjoint_method in FIXED_METHODS or adjoint_method in IMPLICIT_METHODS
         if self.fixed:
             # fixed-grid backward (adjoint.py:134-138 with a FixedGridODESolver): the grid of every interval comes from

@@ -181,9 +181,20 @@ def _next(t):
     return torch.nextafter(t, t + 1)
 
 
+def _dot_weighted(g, ks, w, T):
+    """g . sum_j T(w_j) k_j in float64 (None when g is None): the adjoint of dt in a term dt * sum_j w_j k_j."""
+    if g is None:
+        return None
+    v = sum(ks[j] * float(_T(c, T)) for j, c in enumerate(w) if c != 0.0)
+    return torch.dot(g.double(), v.double()) if isinstance(v, torch.Tensor) else None
+
+
 def adaptive_backward(p, tab, tape, t, grad_sol, params, need_t):
     """Reverse sweep over the taped accepted steps of an adaptive solve.  Times on the tape are the engine's ascending
-    s = sign * t.  Returns (t_bar or None, y0_bar, [param_bar])."""
+    s = sign * t; every step records its start t0, its step size dt, its end t1 as the solver had it, and whether it was
+    clipped to a step_t / jump_t point (a step without t1 / clipped ends at t0 + dt and is not clipped, as every step of a
+    solve without step_t / jump_t).  The step_t / jump_t values themselves get no gradient.  Returns (t_bar or None,
+    y0_bar, [param_bar])."""
     dev, T, sign = p.device, p.dtype, p.t_sign
 
     def F(s_, y_):                                        # reference-sense dynamics in ascending time (misc.py:158-165)
@@ -202,7 +213,11 @@ def adaptive_backward(p, tab, tape, t, grad_sol, params, need_t):
     shift = None         # adjoint of a common shift of all step times (= d/d s[0])
     for st in reversed(tape):
         s0, dt = st["t0"], st["dt"]
-        s1 = s0 + dt
+        s1 = st.get("t1", s0 + dt)
+        # A clipped step ends on a step_t / jump_t point: s1 is a constant and dt = s1 - s0 (rk_common.py:293-308), so
+        # moving s0 changes dt as well.  Its s0-derivative is then the one at fixed dt minus dt's adjoint, `dtbar`.
+        clip = need_t and st.get("clipped", False)
+        own, dtbar = None, None          # this step's contributions to the shift, and to dt's adjoint
         dtT, t0T, t1T = _T(dt, T, dev), _T(s0, T, dev), _T(s1, T, dev)
         y0, k0 = st["y0"], st["k0"]
         if sign != 1.0:
@@ -242,7 +257,9 @@ def adaptive_backward(p, tab, tape, t, grad_sol, params, need_t):
                     dp = d + (2 * x) * c + (3 * x * x) * b + (4 * x ** 3) * a
                     xbar = torch.dot(G.double(), dp.double())
                     sbar[j] += xbar / (s1 - s0)
-                    shift = _acc(shift, -xbar / (s1 - s0))
+                    own = _acc(own, -xbar / (s1 - s0))
+                    if clip:
+                        dtbar = _acc(dtbar, -x * xbar / (s1 - s0))
             ybar0 = _acc(_acc(_acc(_acc(ybar0, eb), bb, 18.0), ab, -8.0), cb, -11.0)
             ybar1 = _acc(_acc(_acc(ybar1, ab, -8.0), bb, 14.0), cb, -5.0)
             kbar[0] = _acc(_acc(_acc(_acc(kbar[0], ab, -2 * dtf), bb, 5 * dtf), cb, -4 * dtf), db, dtf)
@@ -252,6 +269,12 @@ def adaptive_backward(p, tab, tape, t, grad_sol, params, need_t):
             for j, cm in enumerate(cmid):
                 if cm != 0.0:
                     kbar[j] = _acc(kbar[j], ymb, cm)
+            if clip:                                      # the dt f terms of a, b, c, d and dt c_mid in y_mid
+                dp_dt = None
+                for gb, w0, w1 in ((ab, -2.0, 2.0), (bb, 5.0, -3.0), (cb, -4.0, 1.0), (db, 1.0, 0.0)):
+                    if gb is not None:
+                        dp_dt = _acc(dp_dt, torch.dot(gb.double(), (w0 * f0 + w1 * f1).double()))
+                dtbar = _acc(_acc(dtbar, dp_dt), _dot_weighted(ymb, ks, tab.c_mid, T))
         # ---- y1 (rk_common.py:83-87) and the stages ---------------------------------------------------------------
         Ybar_last = None
         if tab.fsal:
@@ -261,24 +284,36 @@ def adaptive_backward(p, tab, tape, t, grad_sol, params, need_t):
             for j, cs in enumerate(csol):
                 if cs != 0.0:
                     kbar[j] = _acc(kbar[j], ybar1, cs)
-        ybar0, kbar0, tsum, _ = sa.sweep(times, Ys, coefs, kbar, ybar0, Ybar_last)
-        shift = _acc(shift, tsum.double() if tsum is not None else None)
+            if clip:
+                dtbar = _acc(dtbar, _dot_weighted(ybar1, ks, tab.c_sol, T))
+        ybar0, kbar0, tsum, per_stage = sa.sweep(times, Ys, coefs, kbar, ybar0, Ybar_last)
+        own = _acc(own, tsum.double() if tsum is not None else None)
+        if clip:
+            for i, (Yb, tb) in enumerate(per_stage):                  # t_i = t0 + alpha_i dt, or prev(t1) for alpha = 1
+                dtbar = _acc(dtbar, _dot_weighted(Yb, ks, tab.beta[i], T))
+                if tb is not None:
+                    dtbar = _acc(dtbar, tb.double(), float(tab.alpha[i]))
         # ---- where this step's k_0 came from ----------------------------------------------------------------------
         if st["first"]:                                   # k_0 = f(t[0], y0) (rk_common.py:214)
             if kbar0 is not None:
                 gyk, tb = sa.vjp(_dev(t0T, dev), y0, kbar0)
                 ybar0 = _acc(ybar0, gyk)
-                shift = _acc(shift, tb.double() if tb is not None else None)
+                own = _acc(own, tb.double() if tb is not None else None)
             gk = None
         elif st["jumped_into"] is not None:               # re-evaluated after a discontinuity at next(t0) (rk_common.py:346-351)
             if kbar0 is not None:
                 gyk, tb = sa.vjp(_dev(_next(t0T), dev), y0, kbar0)
                 ybar0 = _acc(ybar0, gyk)
-                shift = _acc(shift, tb.double() if tb is not None else None)
+                own = _acc(own, tb.double() if tb is not None else None)
             gk = None
         else:
             gk = kbar0
         gy = ybar0
+        if clip:
+            # the steps after this one start from the constant s1 and do not move with s0: their shift is dropped
+            shift = _acc(own, dtbar, -1.0)
+        else:
+            shift = _acc(shift, own)
     y0bar = _acc(gy, grad_sol[0])                                     # solution[0] = y0 (solvers.py:30)
     tbar = None
     if need_t:

@@ -123,7 +123,9 @@ __device__ __forceinline__ double block_norm_from_sums(const TdqCtrl &c, const d
 
 // final_only: nobody polls between attempts (the device-side loop, the persistent linear solve), so only the attempt that
 // ends the solve reports (saves the system-scope fence and the stores over PCIe on every other attempt)
-__device__ __forceinline__ void write_mailbox(TdqCtrl &c, bool final_only, double fin_t0, double fin_dt, int jumped = 0) {
+// jumped / stepped: the accepted attempt ended on a jump_t / step_t point (0 for a rejected one)
+__device__ __forceinline__ void write_mailbox(TdqCtrl &c, bool final_only, double fin_t0, double fin_dt, int jumped = 0,
+                                              int stepped = 0) {
     c.seq += 1;
     tdq_mailbox *m = c.mbox;
     if (!m) return;
@@ -143,6 +145,7 @@ __device__ __forceinline__ void write_mailbox(TdqCtrl &c, bool final_only, doubl
     m->next_t0 = c.att_t0;
     m->next_dt = c.att_dt;
     m->on_jump_t = jumped;
+    m->on_step_t = stepped;
     m->par = c.par;
     __threadfence_system();
     m->seq = c.seq;                  // kernel completion flushes this last store; no second fence needed
@@ -231,8 +234,9 @@ __device__ __forceinline__ void controller(TdqCtrl &c, const double *norm_in, in
     }
     const double fin_t0 = c.att_t0, fin_dt = c.att_dt;
     const int jumped = (accept && c.on_jump_t) ? 1 : 0;
+    const int stepped = (accept && c.on_step_t) ? 1 : 0;
     prepare_scalar<T>(c);                 // the tables of the next attempt are filled by the whole block (k_controller)
-    write_mailbox(c, final_only, fin_t0, fin_dt, jumped);
+    write_mailbox(c, final_only, fin_t0, fin_dt, jumped, stepped);
 }
 
 // The control block is ~10 KB of scalars that one thread reads and writes hundreds of times; from global memory every access

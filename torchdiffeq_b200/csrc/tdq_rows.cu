@@ -461,6 +461,7 @@ __device__ void rows_finish(TdqCtrl *c, const Rows &R, bool running, bool failed
         m->accept = 0;
         m->done = c->done;
         m->on_jump_t = 0;
+        m->on_step_t = 0;
         m->par = 0;
         __threadfence_system();
         if (attempt) m->seq = c->seq;
