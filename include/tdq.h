@@ -506,7 +506,8 @@ typedef enum {
     TDQ_ROWS_N_STEPS, TDQ_ROWS_N_ACCEPT, TDQ_ROWS_N_REJECT,                /* int64 (N_STEPS: attempts in this interval) */
     TDQ_ROWS_T_FIRST, TDQ_ROWS_T_PROBE, TDQ_ROWS_T_STAGE,                  /* state dtype; T_STAGE + i for stage i       */
     TDQ_ROWS_N_FIELDS = TDQ_ROWS_T_STAGE + TDQ_MAX_STAGES,
-    TDQ_ROWS_HEADER = 255       /* int32 words: [3] = the smallest failing row of the attempt that ended the solve, or -1 */
+    TDQ_ROWS_HEADER = 255       /* int32 words: [3] = the smallest failing row of the attempt that ended the solve, or -1; */
+                                /* [4..7] row compaction: threshold, running rows, listed rows, paused (see below)        */
 } tdq_rows_field;
 size_t tdq_rows_size(size_t n_rows);
 size_t tdq_rows_offset(int32_t field, size_t n_rows);                     /* (size_t)-1 for an unknown field             */
@@ -653,6 +654,37 @@ int tdq_rows_tape_event(void *ctrl_dev, int32_t dtype, const tdq_rows_tape *tape
                         size_t row_n, size_t n_rows, size_t row_len, void *stream);
 int tdq_rows_event_reroute(int32_t dtype, const void *grad_state, const void *f, const void *dc_dy, const double *dc_dt,
                            const double *grad_t, void *out, size_t n_rows, size_t row_len, void *stream);
+
+/* ---- row compaction: func evaluated on the rows still running (tdq_rows.cu) ---------------------------------------------
+ * Replaces the whole-batch func call of an attempt (and the per-row event call of its stepping phase) by a call on the B'
+ * rows listed in idx: gather the stage value and its time, func on [B', D], scatter the result into a full-size stage slot.
+ * The solver kernels keep working on all B rows.  Header words of the row buffer (TDQ_ROWS_HEADER): [4] threshold,
+ * [5] rows running after the last per-row launch, [6] rows listed by the last tdq_rows_compact, [7] paused.
+ * tdq_rows_set_compact_threshold: after tdq_rows_init / _init_grid, before tdq_rows_prepare; words 4..7 are 0 in a zeroed
+ *                           buffer, and a threshold of 0 leaves words 5..7 unwritten.  With
+ *                           threshold > 0 the end of tdq_rows_prepare / _controller / _controller_event halts the solve
+ *                           without done (a pause: the mailbox's status is OK, done 0) when 0 < running rows <= threshold,
+ *                           and every mailbox report also writes the running count into out_cursor.  Queued attempts are
+ *                           then no-ops, as after the end, and the device-side loop exits.  threshold 0 changes nothing.
+ *                           0 <= threshold < n_rows.
+ * tdq_rows_compact:         idx[0, n) = the rows whose DONE flag is 0, ascending (n = their count, at most n_compact:
+ *                           the caller picks n_compact >= n from the running count); idx[n, n_compact) repeat idx[n - 1]
+ *                           (0 when n = 0).  Deterministic, one block, O(n_rows).  Records n as the listed count, sets the
+ *                           threshold (0 <= threshold < n_compact) and resumes a paused solve.
+ * tdq_rows_gather:          dst row c = src row idx[c] for c < n_compact ([n_compact, row_len] from [n_rows, row_len]), and
+ *                           t_dst[c] = t_src[idx[c]] when both are given (same dtype).  Serves the stage value with its time
+ *                           field, y1 for the event call, and (dtype float64, row_len 1) the event times.
+ * tdq_rows_scatter:         dst row idx[c] = src row c for c < the listed count of rows_dev's header (padding rows and rows
+ *                           not listed are not written).  Event values: dtype float64, row_len K.
+ * Gather and scatter take one warp per unit of at most 1024 elements of a row, 128-bit accesses where both rows start at the
+ * same vector phase, scalar code at row edges; an index outside [0, n_rows) copies nothing. */
+int tdq_rows_set_compact_threshold(void *rows_dev, size_t n_rows, int32_t threshold, void *stream);
+int tdq_rows_compact(void *ctrl_dev, void *rows_dev, int64_t *idx, size_t n_rows, size_t n_compact, int32_t threshold,
+                     void *stream);
+int tdq_rows_gather(int32_t dtype, const int64_t *idx, size_t n_compact, const void *src, const void *t_src, void *dst,
+                    void *t_dst, size_t n_rows, size_t row_len, void *stream);
+int tdq_rows_scatter(void *rows_dev, int32_t dtype, const int64_t *idx, size_t n_compact, const void *src, void *dst,
+                     size_t n_rows, size_t row_len, void *stream);
 
 /* ---- adjoint augmented state (adjoint.py:72-105, misc.py:137-165) ------------------------- */
 /* dst[offset_i .. offset_i + len_i) = scale_i * src_i for i < n_src, one launch

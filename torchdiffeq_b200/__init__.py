@@ -7,8 +7,9 @@ from .odeint import odeint, odeint_event, odeint_dense, clear_cache, set_cache_s
 from .adjoint import odeint_adjoint, find_parameters
 from .fields import LinearField
 from ._engine import SolverFailure
+from ._compact import active_rows
 from ._lib import TdqError
 
 __version__ = "0.2.0"
 __all__ = ["odeint", "odeint_adjoint", "odeint_event", "odeint_dense", "find_parameters", "clear_cache", "set_cache_size", "last_stats",
-           "LinearField", "SolverFailure", "TdqError"]
+           "active_rows", "LinearField", "SolverFailure", "TdqError"]

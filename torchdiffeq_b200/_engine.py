@@ -31,7 +31,7 @@ import time
 
 import torch
 
-from . import _lib
+from . import _compact, _lib
 
 _DTYPES = {torch.float32: _lib.TDQ_F32, torch.float64: _lib.TDQ_F64}
 
@@ -827,15 +827,17 @@ class AdaptiveEngine:
 
     # ---- the drivers after _begin (lock step: _lockstep_attempts) ------------------------------
     def _run(self, driver):
-        """Every attempt of a solve with more than one output time, by `driver` (choose_driver)."""
+        """Every attempt of a solve with more than one output time, by `driver` (choose_driver), or the attempts up to the
+        next pause of a compacting row solve (RowsEngine._run): `base`, the attempts already reported, is 0 otherwise."""
+        base = int(self.mbox_host.contents.seq)
         if driver == "persistent":
             if self._linear_solve():
                 return
             driver = self.driver = self._plan()            # refused: the same solve takes the per-attempt choice
         if driver == "loop":
-            return self._launch_loop()
+            return self._launch_loop(first=base)
         if driver == "replay":
-            return self._run_ahead(issued=0)
+            return self._run_ahead(issued=base)
         # capture or eager: attempt 1 runs eagerly, and doubles as the warm-up torch wants before a capture
         self._attempt()
         if driver == "capture":
@@ -844,15 +846,19 @@ class AdaptiveEngine:
                 # hand the rest of this solve to the loop (if the first attempt already finished it, the loop's single
                 # iteration is a no-op on the device)
                 _lib.check(self.lib.tdq_ctrl_set_loop(self.ctrl.data_ptr(), self._loop_handle, _stream()))
-                return self._launch_loop(first=1)
-        self._run_ahead(issued=1)
+                return self._launch_loop(first=base + 1)
+        self._run_ahead(issued=base + 1)
+
+    def _halted(self, mb):
+        """The device stopped the solve: it failed or is done (RowsEngine: or paused for a compaction)."""
+        return mb.status != _lib.RUN_OK or mb.done
 
     def _run_ahead(self, issued):
         D = max(1, self.run_ahead)
         mb = self.mbox_host.contents
         while True:
             seen = mb.seq
-            if mb.status != _lib.RUN_OK or mb.done:
+            if self._halted(mb):
                 break
             if issued - seen > D:
                 time.sleep(0)                              # the device is >D attempts behind: yield the GIL
@@ -1009,13 +1015,22 @@ class RowsEngine(AdaptiveEngine):
     row-wise func: its own initial step, error ratio, accept/reject, step size, max_num_steps count and interpolant
     (csrc/tdq_rows.cu).  func is still called on the whole batch, with t a tensor of shape [B, 1, ...] holding each row's
     time; finished rows see copies of their last state.  Stage slots, capture, the device-side loop and the run-ahead and
-    lock-step drivers are AdaptiveEngine's; only the launches differ."""
+    lock-step drivers are AdaptiveEngine's; only the launches differ.
 
-    def __init__(self, fn, shape, dtype, device, method, **kw):
+    compact_fn (options['compact_rows']): func(t, y) with y of shape [B', *rest].  Whenever the running rows fall to the
+    next batch size of _compact.bucket_sizes, the device pauses the solve and the host compacts: tdq_rows_compact lists the
+    running rows, and from then on each stage's func call gets only those rows (tdq_rows_gather), its result going to
+    their rows of an engine-owned full-size slot (tdq_rows_scatter).  Every solver kernel still works on all B rows.  Each
+    batch size keeps its own captured attempt and device-side loop, across solves."""
+
+    def __init__(self, fn, shape, dtype, device, method, compact_fn=None, **kw):
         shape = torch.Size(shape)
         self.B = int(shape[0])
         self.D = int(shape[1:].numel())
         self.row_shape = shape[1:]
+        self.compact_fn = compact_fn
+        self.size = self.B               # the batch size func sees now
+        self._graphs = {}                # batch size -> its captured attempt, while another size is in use
         super().__init__(fn, self.B * self.D, dtype, device, method, **kw)
         lib, B = self.lib, self.B
         self.rows = torch.zeros(lib.tdq_rows_size(B), dtype=torch.uint8, device=device)
@@ -1037,6 +1052,13 @@ class RowsEngine(AdaptiveEngine):
         self.ev_fn = None                # set by solve_until_event: the attempt then tests each row's event
         self.grid = None                 # per-row output times [B, T] of the solve in progress, or None
         self.tape = None                 # the RowTape of a solve_taped in progress
+        self.compactions = self.func_rows = 0     # per solve: batch shrinks, and rows summed over func calls
+        self._nfe_mark = 0
+        self.threshold = 0
+        if compact_fn is not None:
+            self.sizes = _compact.bucket_sizes(B)
+            self._idx = {B: torch.arange(B, dtype=torch.int64, device=device)}   # per size: the static index list
+            self._cbuf = {}              # per size: compact (y, t, event t) buffers
 
     def solve(self, y0_flat, t64, t_start=None, grid=None):
         """AdaptiveEngine.solve, or with `grid` (an ascending float64 [B, T] device tensor) per-row output times: row r
@@ -1068,6 +1090,111 @@ class RowsEngine(AdaptiveEngine):
         tape.check()
         return self.solution, tape
 
+    # ---- row compaction (compact_fn) ----------------------------------------------------------------------------------
+    def _begin(self, y0_flat, t64, t_start=None, grid=None):
+        self._use_size(self.B)
+        self.compactions = self.func_rows = self._nfe_mark = 0
+        self.mbox_host.contents.out_cursor = 0          # the running count a compacting solve reports there
+        return super()._begin(y0_flat, t64, t_start, grid)
+
+    def _use_size(self, size):
+        """Make `size` the batch size func sees: its captured attempt and loop become the engine's current ones."""
+        if size == self.size:
+            return
+        self._flush_rows()
+        self._graphs[self.size] = (self._graph, self._graph_keep, self._loop, self._loop_handle, self._graph_launches)
+        (self._graph, self._graph_keep, self._loop, self._loop_handle,
+         self._graph_launches) = self._graphs.pop(size, (None, None, None, 0, 0))
+        self.size = size
+
+    def _drop_graph(self):
+        for _g, _keep, loop, _h, _n in getattr(self, "_graphs", {}).values():
+            if loop is not None:
+                try:
+                    self.lib.tdq_loop_destroy(loop)
+                except Exception:
+                    pass
+        if getattr(self, "_graphs", None):
+            self._graphs.clear()
+        super()._drop_graph()
+
+    def _flush_rows(self):
+        """func_rows: every func call since the last flush saw self.size rows."""
+        self.func_rows += (self.nfe - self._nfe_mark) * self.size
+        self._nfe_mark = self.nfe
+
+    def _paused(self, mb):
+        """The device paused the solve for a compaction (tdq_rows.cu rows_finish): running rows in (0, threshold]."""
+        return (self.threshold > 0 and mb.status == _lib.RUN_OK and not mb.done
+                and 0 < int(mb.out_cursor) <= self.threshold)
+
+    def _compact_rows(self, mb):
+        """List the running rows for the smallest batch size that holds them, and resume the solve."""
+        size, self.threshold = _compact.pick(self.sizes, int(mb.out_cursor))
+        if size not in self._idx:
+            kw = dict(dtype=self.dtype, device=self.device)
+            self._idx[size] = torch.zeros(size, dtype=torch.int64, device=self.device)
+            self._cbuf[size] = (torch.zeros(size * self.D, **kw), torch.zeros(size, **kw),
+                                torch.zeros(size, dtype=torch.float64, device=self.device))
+        self._launch(self.lib.tdq_rows_compact(self.ctrl.data_ptr(), self.rows.data_ptr(), self._idx[size].data_ptr(),
+                                               self.B, size, self.threshold, _stream()))
+        self._use_size(size)
+        self.compactions += 1
+
+    def _run(self, driver):
+        """AdaptiveEngine._run, segment by segment between the pauses of a compacting solve: after each pause the host
+        compacts and choose_driver picks the next segment's driver from what the new batch size holds."""
+        if self.compact_fn is None:
+            return super()._run(driver)
+        mb = self.mbox_host.contents
+        torch.cuda.current_stream().synchronize()       # tdq_rows_prepare may have paused already (rows done at t0)
+        while True:
+            if self._paused(mb):
+                self._compact_rows(mb)
+                driver = self.driver = self._plan()
+                # the controller reports through, and re-arms, the loop of the size in use (none outside the loop driver)
+                _lib.check(self.lib.tdq_ctrl_set_loop(self.ctrl.data_ptr(), self._loop_handle if driver == "loop" else 0,
+                                                      _stream()))
+            super()._run(driver)
+            if not self._paused(mb):
+                return
+
+    def _halted(self, mb):
+        return super()._halted(mb) or self._paused(mb)
+
+    def _lockstep_attempt(self, issued, mb):
+        if self._paused(mb):
+            self._compact_rows(mb)
+        return super()._lockstep_attempt(issued, mb)
+
+    def _call_fn(self, t, y, slot, taken=(), dst=None):
+        if self.compact_fn is None:
+            return super()._call_fn(t, y, slot, taken, dst)
+        with _compact.rows(self._idx[self.B]):
+            return super()._call_fn(t, y, slot, taken, dst)
+
+    def _stage_fn(self, t, y, slot, taken):
+        """func on stage value y with per-row times t; returns (the full-size result, what a capture must keep)."""
+        if self.size == self.B:
+            f = self._call_fn(t, y, slot, taken=taken)
+            return f, f
+        lib, st, size = self.lib, _stream(), self.size
+        idx, (yc, tc, _) = self._idx[size], self._cbuf[size]
+        self._launch(lib.tdq_rows_gather(self.dt_code, idx.data_ptr(), size, y.data_ptr(), t.data_ptr(), yc.data_ptr(),
+                                         tc.data_ptr(), self.B, self.D, st))
+        self.nfe += 1
+        with _compact.rows(idx):
+            f = self.compact_fn(tc.view(size, *([1] * len(self.row_shape))), yc.view(size, *self.row_shape))
+        if not isinstance(f, torch.Tensor):
+            raise ValueError("with options['compact_rows'] func must return a tensor")
+        if f.numel() != size * self.D:
+            raise ValueError("func returned %d elements for a compacted batch of %d rows of %d" % (f.numel(), size, self.D))
+        f = f.to(self.dtype).reshape(-1).contiguous()
+        out = self._slot(slot)
+        self._launch(lib.tdq_rows_scatter(self.rows.data_ptr(), self.dt_code, idx.data_ptr(), size, f.data_ptr(),
+                                          out.data_ptr(), self.B, self.D, st))
+        return out, f
+
     def _rows_sumsq(self, x, x2, out):
         self._launch(self.lib.tdq_rows_sumsq(
             self.ctrl.data_ptr(), self.rows.data_ptr(), self.dt_code, x.data_ptr(),
@@ -1090,8 +1217,8 @@ class RowsEngine(AdaptiveEngine):
             else:
                 out = self.ytmp
                 self._launch(lib.tdq_rows_combine(ctrl, rows, tab, dc, i, out.data_ptr(), _lib.ptr_array(k), B, D, st))
-            f = self._call_fn(self.t_stage[i], out, i + 1, taken=k)
-            keep.append(f)
+            f, kept = self._stage_fn(self.t_stage[i], out, i + 1, taken=k)
+            keep.append(kept)
             k[i + 1] = f.data_ptr()
         if not self.fsal:
             self._launch(lib.tdq_rows_combine_final(ctrl, rows, tab, dc, self.y1.data_ptr(), self.errp.data_ptr(),
@@ -1107,7 +1234,7 @@ class RowsEngine(AdaptiveEngine):
         else:
             # each row's event value at its candidate (ATT_T1, y1), then the controller with the sign test inside it
             torch.mul(self.row_field(_lib.ROWS_ATT_T1, torch.float64), self.opt.t_sign, out=self.ev_t)
-            self._ev_call(self.y1)
+            keep.append(self._ev_call(self.y1))
             self._launch(lib.tdq_rows_controller_event(ctrl, rows, dc, self.row_norm.data_ptr(), self.ev_val.data_ptr(),
                                                        self.ev_init.data_ptr(), self.ev_sign0.data_ptr(),
                                                        self.ev_flag.data_ptr(), B, D, self.K, st))
@@ -1126,15 +1253,37 @@ class RowsEngine(AdaptiveEngine):
                                                 self.D, _stream()))
 
     # ---- per-row events (rk_common.py:252-262, event_handling.py:5-35) ------------------------------------------------
-    def _ev_call(self, y_flat):
+    def _ev_call(self, y_flat, stepping=True):
         """ev on the whole batch at the times in ev_t; its values, widened to float64 [B, K], into ev_val.  Values of rows
-        that did not accept in this attempt, or are done, are ignored by the kernels."""
+        that did not accept in this attempt, or are done, are ignored by the kernels.  stepping: a call of the stepping
+        phase, which a compacting solve makes on the rows func sees (the bisection's calls take the whole batch)."""
         self.n_ev += 1
-        v = self.ev_fn(self.ev_t_view, y_flat.view(self.B, *self.row_shape))
-        if not isinstance(v, torch.Tensor) or v.dim() == 0 or v.shape[0] != self.B or v.numel() != self.B * self.K:
+        if self.compact_fn is None or not stepping:
+            v = self.ev_fn(self.ev_t_view, y_flat.view(self.B, *self.row_shape))
+            B = self.B
+        elif self.size == self.B:
+            with _compact.rows(self._idx[self.B]):
+                v = self.ev_fn(self.ev_t_view, y_flat.view(self.B, *self.row_shape))
+            B = self.B
+        else:
+            lib, st, B = self.lib, _stream(), self.size
+            idx, (yc, _, ec) = self._idx[B], self._cbuf[B]
+            self._launch(lib.tdq_rows_gather(self.dt_code, idx.data_ptr(), B, y_flat.data_ptr(), None, yc.data_ptr(), None,
+                                             self.B, self.D, st))
+            self._launch(lib.tdq_rows_gather(_lib.TDQ_F64, idx.data_ptr(), B, self.ev_t.data_ptr(), None, ec.data_ptr(),
+                                             None, self.B, 1, st))
+            with _compact.rows(idx):
+                v = self.ev_fn(ec.view(B, *([1] * len(self.row_shape))), yc.view(B, *self.row_shape))
+        if not isinstance(v, torch.Tensor) or v.dim() == 0 or v.shape[0] != B or v.numel() != B * self.K:
             raise ValueError("event_fn returned %s; with independent rows it must keep the shape of its first result, "
-                             "[B, K...] with B = %d and K = %d" % (tuple(getattr(v, "shape", ())), self.B, self.K))
-        self.ev_val.copy_(v.reshape(self.B, self.K))
+                             "[B, K...] with B = %d and K = %d" % (tuple(getattr(v, "shape", ())), B, self.K))
+        if B == self.B:
+            self.ev_val.copy_(v.reshape(self.B, self.K))
+            return v
+        v = v.reshape(B, self.K).to(torch.float64).contiguous()
+        self._launch(self.lib.tdq_rows_scatter(self.rows.data_ptr(), _lib.TDQ_F64, idx.data_ptr(), B, v.data_ptr(),
+                                               self.ev_val.data_ptr(), self.B, self.K, _stream()))
+        return v
 
     def solve_until_event(self, y0_flat, t_start, ev, ev0, tol, t_starts=None):
         """Row r integrates from t_start (or t_starts[r], a float64 [B] device tensor in ascending solver time) until the
@@ -1207,7 +1356,7 @@ class RowsEngine(AdaptiveEngine):
                 self.solution[0].data_ptr(), self.ytmp.data_ptr(), self.ev_t.data_ptr(), self.ev_event_t.data_ptr(),
                 self.solution[1].data_ptr(), B, self.D, self.K, st))
             if it < self.bisect_iters:
-                self._ev_call(self.ytmp)
+                self._ev_call(self.ytmp, stepping=False)
         return self.ev_event_t, self.solution
 
     def _start(self, t_start, n_out, grid=None):
@@ -1238,6 +1387,9 @@ class RowsEngine(AdaptiveEngine):
         if self.ev_fn is not None:                                  # rows done at t0 take no attempt
             self._launch(lib.tdq_rows_event_init(rows, self.ev_val.data_ptr(), self.ev_init.data_ptr(),
                                                  self.ev_sign0.data_ptr(), self.ev_flag.data_ptr(), B, self.K, st))
+        if self.compact_fn is not None:                             # the first pause: at the next smaller batch size
+            self.threshold = _compact.pick(self.sizes, B)[1]
+            self._launch(lib.tdq_rows_set_compact_threshold(rows, B, self.threshold, st))
         self._launch(lib.tdq_rows_prepare(ctrl, rows, dc, d[0].data_ptr() if n_out > 1 else None, B, st))
 
     def row_field(self, which, dtype):
@@ -1253,6 +1405,7 @@ class RowsEngine(AdaptiveEngine):
         self._raise_status(mb.status, float(self.row_field(_lib.ROWS_ATT_DT, torch.float64)[r]), y, " (row %d)" % r)
 
     def _read_counters(self):
+        self._flush_rows()
         self.row_n_accept = self.row_field(_lib.ROWS_N_ACCEPT, torch.int64).cpu()
         self.row_n_reject = self.row_field(_lib.ROWS_N_REJECT, torch.int64).cpu()
         self.n_accept, self.n_reject = int(self.row_n_accept.sum()), int(self.row_n_reject.sum())

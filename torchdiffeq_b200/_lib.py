@@ -187,6 +187,10 @@ _SIGNATURES = {
                                       _sz, _vp]),
     "tdq_rows_tape_event": (C.c_int, [_vp, _i32, C.POINTER(RowsTape), _vp, _vp, _sz, _sz, _sz, _vp]),
     "tdq_rows_event_reroute": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _vp]),
+    "tdq_rows_set_compact_threshold": (C.c_int, [_vp, _sz, _i32, _vp]),
+    "tdq_rows_compact": (C.c_int, [_vp, _vp, _vp, _sz, _sz, _i32, _vp]),
+    "tdq_rows_gather": (C.c_int, [_i32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _sz, _vp]),
+    "tdq_rows_scatter": (C.c_int, [_vp, _i32, _vp, _sz, _vp, _vp, _sz, _sz, _vp]),
     "tdq_xchg_create": (C.c_int, [_pp, C.POINTER(IpcHandle)]),
     "tdq_xchg_open": (C.c_int, [C.POINTER(IpcHandle), _pp]),
     "tdq_xchg_close": (C.c_int, [_vp]),

@@ -21,7 +21,11 @@ namespace {
 
 constexpr int kThreads = 256, kWarps = kThreads / 32;
 constexpr size_t kChunk = 1024;          // elements per unit
-constexpr size_t kHdr = 256;             // header bytes: int32 words [0] ticket, [1] active, [2] failing-row minimum, [3] result
+// header bytes: int32 words [0] ticket, [1] active, [2] failing-row minimum, [3] result, and for row compaction
+// [4] threshold (0, as in a zeroed buffer: never pause, and words 5-7 are not written), [5] rows running after the last
+// per-row launch, [6] rows listed by the last tdq_rows_compact, [7] paused
+constexpr size_t kHdr = 256;
+enum { kHdrThreshold = 4, kHdrRunning = 5, kHdrListed = 6, kHdrPaused = 7 };
 
 struct Rows {
     unsigned char *base;
@@ -425,6 +429,8 @@ __device__ void row_control(const TdqCtrl &c, const Rows &R, int r, double sumsq
 
 // End of a per-row launch: every block adds its count of rows still running and its smallest failing row; the last block
 // ends the solve when no row runs or some row failed, reports through the mailbox and keeps or ends the device-side loop.
+// With a compaction threshold set (header word kHdrThreshold > 0) it also halts, without done, when 0 < running <=
+// threshold: the solve pauses until tdq_rows_compact resumes it, and the mailbox's out_cursor carries the running count.
 __device__ void rows_finish(TdqCtrl *c, const Rows &R, bool running, bool failed, int r, bool attempt) {
     __shared__ int s_fail;
     __shared__ bool is_last;
@@ -442,7 +448,8 @@ __device__ void rows_finish(TdqCtrl *c, const Rows &R, bool running, bool failed
     __syncthreads();
     if (!is_last || threadIdx.x != 0) return;
     __threadfence();
-    const int total = atomicAdd(&h[1], 0), fail = atomicAdd(&h[2], 0);
+    const int total = atomicAdd(&h[1], 0), fail = atomicAdd(&h[2], 0), threshold = h[kHdrThreshold];
+    if (threshold > 0) h[kHdrRunning] = total;
     if (fail != INT_MAX) {
         c->status = fld<int>(R, TDQ_ROWS_STATUS)[fail];
         c->halt = 1;
@@ -450,6 +457,9 @@ __device__ void rows_finish(TdqCtrl *c, const Rows &R, bool running, bool failed
     } else if (total == 0) {
         c->done = 1;
         c->halt = 1;
+    } else if (total <= threshold) {
+        c->halt = 1;
+        h[kHdrPaused] = 1;
     }
     h[0] = 0;
     h[1] = 0;
@@ -463,6 +473,7 @@ __device__ void rows_finish(TdqCtrl *c, const Rows &R, bool running, bool failed
         m->on_jump_t = 0;
         m->on_step_t = 0;
         m->par = 0;
+        if (threshold > 0) m->out_cursor = total;
         __threadfence_system();
         if (attempt) m->seq = c->seq;
     }
@@ -1057,6 +1068,92 @@ k_rows_event_reroute(int B, size_t D, const T *__restrict__ gs, const T *__restr
     for (size_t i = lane; i < D; i += 32) o[i] = A::add(g[i], A::mul(d[i], scale));
 }
 
+// ---- row compaction: func sees only the rows still running ------------------------------------------------------------------
+// One block walks the DONE flags in tiles of kCompactThreads rows: a ballot and a scan of the warp counts place each running
+// row after the running rows of earlier tiles, so the list is ascending and depends on the flags alone.
+constexpr int kCompactThreads = 1024;
+__global__ void __launch_bounds__(kCompactThreads)
+k_rows_compact(TdqCtrl *c, Rows R, int64_t *__restrict__ idx, int n_compact, int threshold) {
+    __shared__ int s_warp[kCompactThreads / 32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int *done = fld<int>(R, TDQ_ROWS_DONE);
+    int base = 0;                                                       // running rows of the tiles before this one
+    for (int t0 = 0; t0 < R.B; t0 += kCompactThreads) {
+        const int r = t0 + threadIdx.x;
+        const bool run = r < R.B && !done[r];
+        const unsigned ball = __ballot_sync(0xffffffffu, run);
+        if (lane == 0) s_warp[w] = __popc(ball);
+        __syncthreads();
+        if (w == 0) {                                                   // inclusive scan of the warp counts
+            int v = s_warp[lane];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int x = __shfl_up_sync(0xffffffffu, v, o);
+                if (lane >= o) v += x;
+            }
+            s_warp[lane] = v;
+        }
+        __syncthreads();
+        const int pos = base + (w ? s_warp[w - 1] : 0) + __popc(ball & ((1u << lane) - 1u));
+        if (run && pos < n_compact) idx[pos] = r;
+        base += s_warp[kCompactThreads / 32 - 1];
+        __syncthreads();                                                // s_warp is rewritten by the next tile
+    }
+    const int listed = base < n_compact ? base : n_compact;
+    const int64_t pad = listed > 0 ? idx[listed - 1] : 0;              // written before the last __syncthreads
+    for (int p = listed + threadIdx.x; p < n_compact; p += kCompactThreads) idx[p] = pad;
+    if (threadIdx.x == 0) {
+        int *h = hdr(R);
+        h[kHdrThreshold] = threshold;
+        h[kHdrRunning] = base;
+        h[kHdrListed] = listed;
+        if (h[kHdrPaused]) {                                            // resume a paused solve
+            h[kHdrPaused] = 0;
+            c->halt = 0;
+        }
+    }
+}
+
+__global__ void k_rows_set_threshold(Rows R, int threshold) { hdr(R)[kHdrThreshold] = threshold; }
+
+// Unit c of a compact batch of g.units / g.nch rows copies between compact row c and full row idx[c].  Vector accesses
+// where both rows start at the same phase of a 16-byte vector (and both bases are aligned: `vec`), scalar code otherwise.
+template <typename T, bool GATHER>
+__device__ __forceinline__ void row_copy(const Geom &g, const int64_t *idx, const T *src, T *dst, size_t n_rows, bool vec,
+                                         int listed) {
+    size_t u, lo, hi;
+    int cr;
+    if (!unit_of(g, u, cr, lo, hi) || cr >= listed) return;
+    const int64_t r = idx[cr];
+    if (r < 0 || (size_t)r >= n_rows) return;
+    const size_t full = (size_t)r * g.D, compact = (size_t)cr * g.D;
+    const size_t sb = GATHER ? full : compact, db = GATHER ? compact : full;
+    const bool v = vec && sb % Vec<T>::N == db % Vec<T>::N;
+    const T *s = src + sb;
+    T *d = dst + db;
+    row_span<T>(db, lo, hi, v, [&](size_t i) { st_vec<T>(d + i, ld_stream<T>(s + i)); }, [&](size_t i) { d[i] = s[i]; });
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+k_rows_gather(Geom g, const int64_t *__restrict__ idx, const T *__restrict__ src, const T *__restrict__ t_src,
+              T *__restrict__ dst, T *__restrict__ t_dst, size_t n_rows, bool vec) {
+    row_copy<T, true>(g, idx, src, dst, n_rows, vec, INT_MAX);
+    size_t u, lo, hi;
+    int cr;
+    if (t_dst && unit_of(g, u, cr, lo, hi) && lo == 0 && (threadIdx.x & 31) == 0) {
+        const int64_t r = idx[cr];
+        if (r >= 0 && (size_t)r < n_rows) t_dst[cr] = t_src[r];
+    }
+}
+
+// min blocks 1: without it ptxas holds the float instance to 32 registers and spills 4 bytes
+template <typename T>
+__global__ void __launch_bounds__(kThreads, 1)
+k_rows_scatter(Rows R, Geom g, const int64_t *__restrict__ idx, const T *__restrict__ src, T *__restrict__ dst, bool vec) {
+    row_copy<T, false>(g, idx, src, dst, (size_t)R.B, vec, hdr(R)[kHdrListed]);
+}
+
 // ---- host helpers -----------------------------------------------------------------------------------------------------------
 bool plan_kp(const int *idx, int nnz, const void *const *k, KPtrs &kp, bool &vec) {
     return tdq_plan_terms(idx, nnz, k, kp.p, vec) == TDQ_PLAN_OK;
@@ -1256,6 +1353,55 @@ int tdq_rows_controller(void *ctrl_dev, void *rows_dev, int32_t dtype, const dou
 }
 
 #define TDQ_ROWS_REQUIRE_K(K) TDQ_REQUIRE((K) >= 1 && (K) <= 65536, "K out of range")
+
+int tdq_rows_set_compact_threshold(void *rows_dev, size_t n_rows, int32_t threshold, void *stream) {
+    TDQ_REQUIRE(rows_dev, "null argument");
+    TDQ_REQUIRE(n_rows >= 1 && n_rows <= (size_t)INT_MAX, "n_rows out of range");
+    TDQ_REQUIRE(threshold >= 0 && (size_t)threshold < n_rows, "threshold out of range");
+    k_rows_set_threshold<<<1, 1, 0, (cudaStream_t)stream>>>(make_rows(rows_dev, n_rows), threshold);
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_compact(void *ctrl_dev, void *rows_dev, int64_t *idx, size_t n_rows, size_t n_compact, int32_t threshold,
+                     void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && idx, "null argument");
+    TDQ_REQUIRE(n_rows >= 1 && n_rows <= (size_t)INT_MAX, "n_rows out of range");
+    TDQ_REQUIRE(n_compact >= 1 && n_compact <= n_rows, "n_compact out of range");
+    TDQ_REQUIRE(threshold >= 0 && (size_t)threshold < n_compact, "threshold out of range");
+    k_rows_compact<<<1, kCompactThreads, 0, (cudaStream_t)stream>>>((TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), idx,
+                                                                     (int)n_compact, threshold);
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+static bool rows_copy_vec(const void *a, const void *b) { return tdq_aligned16(a) && tdq_aligned16(b); }
+
+int tdq_rows_gather(int32_t dtype, const int64_t *idx, size_t n_compact, const void *src, const void *t_src, void *dst,
+                    void *t_dst, size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(idx && src && dst, "null argument");
+    TDQ_REQUIRE((t_src == nullptr) == (t_dst == nullptr), "t_src and t_dst go together");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_REQUIRE(n_compact >= 1 && n_compact <= n_rows, "n_compact out of range");
+    const Geom g = make_geom(n_compact, row_len);
+    TDQ_DISPATCH_T(dtype, (k_rows_gather<T><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(
+                               g, idx, (const T *)src, (const T *)t_src, (T *)dst, (T *)t_dst, n_rows,
+                               rows_copy_vec(src, dst))));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_scatter(void *rows_dev, int32_t dtype, const int64_t *idx, size_t n_compact, const void *src, void *dst,
+                     size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(rows_dev && idx && src && dst, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_REQUIRE(n_compact >= 1 && n_compact <= n_rows, "n_compact out of range");
+    const Geom g = make_geom(n_compact, row_len);
+    TDQ_DISPATCH_T(dtype, (k_rows_scatter<T><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(
+                               make_rows(rows_dev, n_rows), g, idx, (const T *)src, (T *)dst, rows_copy_vec(src, dst))));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
 
 int tdq_rows_event_init(void *rows_dev, const double *ev_val, double *init_sign, double *sign0, int32_t *flag,
                         size_t n_rows, int32_t K, void *stream) {

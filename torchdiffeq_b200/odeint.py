@@ -35,7 +35,7 @@ _FIXED_OPTIONS = {"step_size", "grid_constructor", "interp", "perturb", "norm"}
 _ADAMS_OPTIONS = _FIXED_OPTIONS | {"max_iters", "max_order"}
 _IMPLICIT_OPTIONS = _FIXED_OPTIONS | {"max_iters"}                                  # rk_common.py:382-388
 _OUR_OPTIONS = {"graph", "run_ahead", "process_group", "cache", "exchange", "device_loop", "fused_linear", "fused_attempt",
-                 "independent_rows", "differentiable", "event_gradient"}
+                 "independent_rows", "differentiable", "event_gradient", "compact_rows"}
 
 
 def _rms_norm(tensor):
@@ -319,7 +319,8 @@ def _make_adaptive_engine(p, lockstep=False, keep_interp=False, graph=None, repl
         control["run_ahead"], graph = 0, False
     tol = dict(rtol=p.rtol, atol=p.atol, rtol_vec=p.rtol_vec, atol_vec=p.atol_vec, t_sign=p.t_sign)
     if o.get("independent_rows"):
-        return RowsEngine(p.fn, p.shape, p.dtype, p.device, p.method, graph=graph, **tol, **control)
+        return RowsEngine(p.fn, p.shape, p.dtype, p.device, p.method, graph=graph,
+                          compact_fn=p.original_func if o.get("compact_rows") else None, **tol, **control)
     step_t, jump_t = step_jump_times(o.get("step_t"), o.get("jump_t"), float(p.t_cpu[0]), p.device)
     reduce_fn, n_global, seg_counts_global, agree_fn, exchange = None, None, None, None, None
     pg = o.get("process_group")
@@ -382,6 +383,16 @@ def check_event_gradient(options, rows=True):
                                   "odeint_adjoint")
 
 
+def check_compact_rows(options):
+    """options['compact_rows']: a bool, meaningful only with options['independent_rows']."""
+    v = options.get("compact_rows")
+    if not isinstance(v, bool):
+        raise ValueError("options['compact_rows'] must be a bool, got %r" % (v,))
+    if v and not options.get("independent_rows"):
+        raise ValueError("options['compact_rows'] needs options['independent_rows'] = True: it evaluates func on the rows "
+                         "still running, which only independent rows have")
+
+
 def _check_independent_rows(func, y0, t, method, options, event_fn):
     """What options={'independent_rows': True} does not cover raises NotImplementedError before any work."""
     def no(what):
@@ -403,6 +414,9 @@ def _check_independent_rows(func, y0, t, method, options, event_fn):
             if not options.get("differentiable"):
                 no("gradients (odeint under autograd with anything requiring grad) without options['differentiable']: "
                    "pass options={'independent_rows': True, 'differentiable': True}, or run it under torch.no_grad()")
+            if options.get("compact_rows"):
+                no("options['compact_rows'] under autograd: the differentiable solve and its reverse sweep evaluate func "
+                   "on the whole batch; drop compact_rows, or run the solve under torch.no_grad()")
             if event_fn is not None and options.get("event_gradient") is None:
                 no("gradients through per-row events (event_fn / odeint_event under autograd) without "
                    "options['event_gradient']: pass options={'independent_rows': True, 'differentiable': True, "
@@ -445,7 +459,7 @@ def _solve_rows_event(p, event_fn, ev0, taped=False):
     if graph == "auto" and not isinstance(event_fn, torch.nn.Module):
         graph = False
     eng = _make_adaptive_engine(p, graph=graph, lockstep=taped)
-    B, shape = p.shape[0], p.shape
+    B = p.shape[0]
     # the bisection tolerance: atol, or with a per-element atol the smallest of the row's own elements
     if p.atol_vec is not None:
         tol = p.atol_vec.view(B, -1).min(dim=1).values.cpu()
@@ -453,7 +467,7 @@ def _solve_rows_event(p, event_fn, ev0, taped=False):
         tol = torch.full((B,), float(p.atol), dtype=torch.float64)
     t0 = p.t_cpu[..., 0]                                  # [B]: each row's own start (per-row times), or one start
     t_starts = t0.to(torch.float64).to(p.device) if t0.dim() == 1 else None
-    ev = lambda t_, y_: event_fn(t_, y_.view(shape))
+    ev = event_fn                                         # the engine passes y as [B', *rest] (B' < B when compacting)
     if taped:
         event_t, sol, tape = eng.solve_until_event_taped(p.y0_flat, float(t0.view(-1)[0]), ev, ev0, tol, t_starts=t_starts)
         return event_t, sol, eng, tape
@@ -600,7 +614,8 @@ _LAST_STATS = {}
 
 
 def last_stats():
-    """{'nfe', 'n_accept', 'n_reject', 'attempts', 'launches'} of the most recent odeint call in this process."""
+    """{'nfe', 'n_accept', 'n_reject', 'attempts', 'launches'} of the most recent odeint call in this process (independent
+    rows add row_n_accept, row_n_reject, compactions and func_rows)."""
     return dict(_LAST_STATS)
 
 
@@ -959,7 +974,8 @@ def _publish_stats(eng, _stats, add_launches):
         launches = _stats.get("launches", 0) if add_launches else 0
         _stats.update(_LAST_STATS, launches=launches + _LAST_STATS["launches"], driver=getattr(eng, "driver", None))
     if getattr(eng, "row_n_accept", None) is not None:
-        _LAST_STATS.update(row_n_accept=eng.row_n_accept, row_n_reject=eng.row_n_reject)
+        _LAST_STATS.update(row_n_accept=eng.row_n_accept, row_n_reject=eng.row_n_reject, compactions=eng.compactions,
+                           func_rows=eng.func_rows)
 
 
 def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, event_fn=None, _stats=None):
@@ -999,6 +1015,18 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
     as above, a 1-D t and func's parameters get the sums over rows.  The solve then runs in lock step and keeps 2 D
     elements per accepted row-step for the backward pass.  Not with odeint_adjoint.
 
+    options['compact_rows'] = True (a bool; ValueError without independent_rows) calls func only on the rows still
+    running: whenever they fall to the next of the batch sizes ceil(B / 2^k), the running rows are listed in ascending order
+    and padded to the smallest such size that holds them, and every later func call gets y of shape [B', *rest] and t of
+    shape [B', 1, ...] for those rows (rows that end between two compactions stay, masked as before).  The per-row
+    event_fn calls of the stepping phase get the same rows; the bisection still evaluates the whole batch.  A func or
+    event_fn with per-row data picks its rows through torchdiffeq_b200.active_rows().  Results, row_n_accept /
+    row_n_reject, event_t and failures (with the original row) are bit for bit those of the solve without the option for a
+    func whose output for a row depends only on that row's inputs; a func whose arithmetic depends on the batch size (a
+    matmul, whose library kernel may change with the row count) agrees to rounding.  last_stats() adds compactions and
+    func_rows (rows summed over func calls; without the option func_rows = nfe * B).  Not under autograd
+    (NotImplementedError): the differentiable solve evaluates the whole batch.
+
     event_fn / odeint_event with independent rows under autograd also need options['event_gradient'] = 'discrete' (the
     only value; NotImplementedError without independent rows, whose shared-batch event solve takes odeint_adjoint's
     gradients): row r's gradients are those of the reference's odeint(func, y0[r:r+1], t_r, event_fn=ev_r), the discrete
@@ -1007,6 +1035,8 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
     then gives every row's event time its implicit-function gradient, as the reference's odeint_event does for one.
     """
     row_ev0 = row_event_fn = None
+    if options and "compact_rows" in options:
+        check_compact_rows(options)
     if options and "event_gradient" in options:
         check_event_gradient(options, rows=bool(options.get("independent_rows")))
     if options and options.get("independent_rows"):
