@@ -693,6 +693,68 @@ int tdq_rows_scatter(void *rows_dev, int32_t dtype, const int64_t *idx, size_t n
 int tdq_pack_segments(int32_t dtype, void *dst, const void *const *src, const int64_t *offsets,
                       const int64_t *lens, const double *scales, int32_t n_src, void *stream);
 
+/* ---- odeint_adjoint for independent rows (tdq_rows.cu) -------------------------------------------------------------------
+ * The backward solve runs the augmented state of every row as one row of aug_len elements, [vjp_t | pad | y | adj_y] with
+ * vjp_t at 0, y at o_y and adj_y at o_a (row_len = D elements each), under per-row step control.  Its error ratio is the
+ * reference's seminorm, max(|vjp_t|, rms(y), rms(adj_y)) over the row's own elements (adjoint.py:267-271): a max over
+ * SEGMENTS of the row, given by a small table that is the same for every row.  Scalar tolerances only.
+ * tdq_rows_seg_sumsq / _seg_error_norm_commit: tdq_rows_sumsq / tdq_rows_error_norm_commit with one sum per row and segment,
+ *                           out[s * B + r], and non-finite counts out[(n_seg + s) * B + r] (out: 2 n_seg B doubles).  Segment
+ *                           s of row r is summed in exactly the order tdq_rows_sumsq sums a row of len[s] elements, so each
+ *                           sum equals that kernel's on the sliced segment bit for bit.  The commit copies only segment
+ *                           elements into ybuf / kbuf[par ^ 1]; elements outside every segment are never written.
+ *                           partials: tdq_rows_seg_partials_len(B, segs) doubles, zeroed once.
+ * tdq_rows_seg_initial_h0 / _finish, _seg_prepare, _seg_controller: tdq_rows_initial_h0 / _finish, tdq_rows_prepare and
+ *                           tdq_rows_controller reading the segmented sums: d0, d1, d2 and the ratio are max_s of
+ *                           sqrt(sum_s / len_s) (NaN if any is NaN), the non-finite count is summed over segments.
+ * tdq_rows_adjoint_pack:    row r of out [B, aug_len] = (-vjp_t[r], 0 in the pad, f[r], -vjp_y[r]) from func's result f and
+ *                           the VJPs [B, row_len] / [B] (NULL: zeros); the raw stage slot of one evaluation.
+ * tdq_rows_adjoint_handover: per row, when y_next is given: y <- y_next[r], adj_y += g_next[r]; when f is given: dot =
+ *                           <f[r], g_cur[r]> as a float64 sum in k_rows_norm's order, vjp_t -= T(dot), tgrad[r] = dot.
+ * The parameter quadrature, after tdq_rows_seg_controller of every attempt (parameters are not part of the row state):
+ * tdq_rows_adjoint_weights: one thread per row.  A row accepted in this attempt when N_ACCEPT[r] > seen[r] (seen: int64
+ *                           [B], zero before each solve; set to N_ACCEPT); flag[r] says so.  w [n_k][B] (state dtype) =
+ *                           fl_T(t_sign * fl_T(T(omega_j) * T(FIT_DT))) for such a row, 0 for every other row (rejected, done,
+ *                           or an attempt after the end).  omega_j = b_j, except for a row whose accepted step emits its last
+ *                           output and ends its solve (FIT and DONE): there omega_j(x) are the weights of the step's quartic
+ *                           increment at that output (x as tdq_rows_fit_eval forms it), whose value the reference reads.
+ *                           b: device float64 [2][n_k], the c_sol row then c_mid (n_k = S + 1).  t_point [B]: func's time at
+ *                           the accepted step's start (T0), or at the row's current point (T1), t_sign applied.
+ * tdq_rows_adjoint_scale:   cot[j][r] = w[j][r] * adj_j[r] for flagged rows and 0 otherwise, where adj_0 is the adj_y of
+ *                           the pair the step started from (ybuf[par ^ 1]) and adj_j (j >= 1) = adj[j], [B, row_len]; y_point
+ *                           [B, row_len] = the y of that pair (flagged) or of the current pair.  adj, cot: DEVICE arrays of
+ *                           n_k pointers; cot[j] NULL skips stage j. */
+#define TDQ_ROWS_MAX_SEGS 4
+typedef struct tdq_rows_segs {
+    int32_t n_seg;                               /* 1 .. TDQ_ROWS_MAX_SEGS                                          */
+    int32_t offset[TDQ_ROWS_MAX_SEGS];           /* within a row; segments lie inside [0, row_len)                  */
+    int32_t len[TDQ_ROWS_MAX_SEGS];              /* >= 1                                                            */
+} tdq_rows_segs;
+size_t tdq_rows_seg_partials_len(size_t n_rows, const tdq_rows_segs *segs);   /* 0 for a malformed table            */
+int tdq_rows_seg_sumsq(void *ctrl_dev, void *rows_dev, int32_t dtype, const tdq_rows_segs *segs, const void *x,
+                       const void *x2, size_t n_rows, size_t row_len, double *partials, double *out, void *stream);
+int tdq_rows_seg_error_norm_commit(void *ctrl_dev, void *rows_dev, int32_t dtype, const tdq_rows_segs *segs,
+                                   const void *err_pre, const void *k_last, const void *y1, size_t n_rows, size_t row_len,
+                                   double *partials, double *out, void *stream);
+int tdq_rows_seg_initial_h0(void *ctrl_dev, void *rows_dev, int32_t dtype, const tdq_rows_segs *segs,
+                            const double *d0_sumsq, const double *d1_sumsq, size_t n_rows, size_t row_len, void *stream);
+int tdq_rows_seg_initial_finish(void *ctrl_dev, void *rows_dev, int32_t dtype, const tdq_rows_segs *segs,
+                                const double *d2_sumsq, size_t n_rows, size_t row_len, void *stream);
+int tdq_rows_seg_prepare(void *ctrl_dev, void *rows_dev, int32_t dtype, const tdq_rows_segs *segs,
+                         const double *y0_nonfinite_dev, size_t n_rows, size_t row_len, void *stream);
+int tdq_rows_seg_controller(void *ctrl_dev, void *rows_dev, int32_t dtype, const tdq_rows_segs *segs, const double *norm_in,
+                            size_t n_rows, size_t row_len, void *stream);
+int tdq_rows_adjoint_pack(int32_t dtype, const void *f, const void *vjp_y, const void *vjp_t, void *out, size_t n_rows,
+                          size_t row_len, size_t o_y, size_t o_a, size_t aug_len, void *stream);
+int tdq_rows_adjoint_handover(int32_t dtype, void *aug, const void *y_next, const void *g_next, const void *f,
+                              const void *g_cur, double *tgrad, size_t n_rows, size_t row_len, size_t o_y, size_t o_a,
+                              size_t aug_len, void *stream);
+int tdq_rows_adjoint_weights(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *b, int32_t n_k, int64_t *seen,
+                             int32_t *flag, void *w, void *t_point, size_t n_rows, void *stream);
+int tdq_rows_adjoint_scale(void *ctrl_dev, void *rows_dev, int32_t dtype, const int32_t *flag, const void *w, int32_t n_k,
+                           const void *const *adj, void *const *cot, void *y_point, size_t n_rows, size_t row_len,
+                           size_t o_y, size_t o_a, size_t aug_len, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -612,7 +612,7 @@ class AdaptiveEngine:
         self.n_accept, self.n_reject = int(mb.n_accept), int(mb.n_reject)
         self.n_attempts = self.n_accept + self.n_reject
 
-    def prime(self, y0_flat, t64, t_start=None):
+    def prime(self, y0_flat, t64, t_start=None, grid=None):
         """Warm up and capture the attempt graph ahead of time on representative inputs (one eager
         attempt, then capture).  Used by odeint_adjoint to capture the backward step body during the
         FORWARD call: capturing inside autograd's backward is unsafe (a re-entrant engine call may run
@@ -620,7 +620,7 @@ class AdaptiveEngine:
         self._solution_for(int(t64.numel()))
         if self._plan(priming=True) != "capture":
             return False
-        self._begin(y0_flat, t64, t_start)
+        self._begin(y0_flat, t64, t_start, grid)
         if self.solution.shape[0] <= 1:
             return False
         self._attempt()                  # a real attempt that doubles as the warm-up torch wants before capture
@@ -1021,9 +1021,13 @@ class RowsEngine(AdaptiveEngine):
     next batch size of _compact.bucket_sizes, the device pauses the solve and the host compacts: tdq_rows_compact lists the
     running rows, and from then on each stage's func call gets only those rows (tdq_rows_gather), its result going to
     their rows of an engine-owned full-size slot (tdq_rows_scatter).  Every solver kernel still works on all B rows.  Each
-    batch size keeps its own captured attempt and device-side loop, across solves."""
+    batch size keeps its own captured attempt and device-side loop, across solves.
 
-    def __init__(self, fn, shape, dtype, device, method, compact_fn=None, **kw):
+    row_segs (odeint_adjoint's backward): [(offset, len), ...] within a row.  Each row's error ratio and initial-step norms
+    are then the max over these segments of each one's RMS (the seminorm), elements outside them enter no norm, and the
+    candidate commit writes only segment elements.  Scalar tolerances only."""
+
+    def __init__(self, fn, shape, dtype, device, method, compact_fn=None, row_segs=None, **kw):
         shape = torch.Size(shape)
         self.B = int(shape[0])
         self.D = int(shape[1:].numel())
@@ -1045,14 +1049,28 @@ class RowsEngine(AdaptiveEngine):
         self.t_probe = field(_lib.ROWS_T_PROBE, dtype, es).view(tshape)
         self.t_stage = [field(_lib.ROWS_T_STAGE + i, dtype, es).view(tshape) for i in range(self.S)]
         f64 = dict(dtype=torch.float64, device=device)
-        self.row_partials = torch.zeros(lib.tdq_rows_partials_len(B, self.D), **f64)
-        self.row_norm = torch.zeros(2 * B, **f64)                   # sums of squares, then non-finite counts
-        self.row_dsum = [torch.zeros(2 * B, **f64) for _ in range(3)]
+        self.row_segs, n_seg = None, 1
+        if row_segs is not None:
+            if self.rtol_vec is not None or len(row_segs) > _lib.TDQ_ROWS_MAX_SEGS:
+                raise _lib.TdqError("row segments take scalar tolerances and at most %d segments" % _lib.TDQ_ROWS_MAX_SEGS)
+            sg = self.row_segs = _lib.RowsSegs()
+            sg.n_seg = n_seg = len(row_segs)
+            for i, (o, l) in enumerate(row_segs):
+                sg.offset[i], sg.len[i] = int(o), int(l)
+            n_part = lib.tdq_rows_seg_partials_len(B, C.byref(sg))
+            if n_part == 0:
+                raise _lib.TdqError("row segments %s do not fit rows of %d elements" % (list(row_segs), self.D))
+        else:
+            n_part = lib.tdq_rows_partials_len(B, self.D)
+        self.row_partials = torch.zeros(n_part, **f64)
+        self.row_norm = torch.zeros(2 * n_seg * B, **f64)           # sums of squares, then non-finite counts
+        self.row_dsum = [torch.zeros(2 * n_seg * B, **f64) for _ in range(3)]
         self.row_n_accept = self.row_n_reject = None
         self.ev_fn = None                # set by solve_until_event: the attempt then tests each row's event
         self.grid = None                 # per-row output times [B, T] of the solve in progress, or None
         self.tape = None                 # the RowTape of a solve_taped in progress
         self.compactions = self.func_rows = 0     # per solve: batch shrinks, and rows summed over func calls
+        self.after_control = None        # row_segs: called after every attempt's controller (odeint_adjoint's parameter pass)
         self._nfe_mark = 0
         self.threshold = 0
         if compact_fn is not None:
@@ -1075,6 +1093,10 @@ class RowsEngine(AdaptiveEngine):
             grid = grid.contiguous()
             t64 = grid[0]
         return t64, grid
+
+    def prime(self, y0_flat, t64, t_start=None, grid=None):
+        t64, grid = self._check_grid(t64, grid)
+        return super().prime(y0_flat, t64, t_start, grid)
 
     def solve_taped(self, y0_flat, t64, t_start=None, grid=None):
         """A lock-step solve (what solve computes, bit for bit) that tapes every accepted row-step for the reverse sweep of
@@ -1196,6 +1218,12 @@ class RowsEngine(AdaptiveEngine):
         return out, f
 
     def _rows_sumsq(self, x, x2, out):
+        if self.row_segs is not None:
+            self._launch(self.lib.tdq_rows_seg_sumsq(
+                self.ctrl.data_ptr(), self.rows.data_ptr(), self.dt_code, C.byref(self.row_segs), x.data_ptr(),
+                x2.data_ptr() if x2 is not None else None, self.B, self.D, self.row_partials.data_ptr(), out.data_ptr(),
+                _stream()))
+            return
         self._launch(self.lib.tdq_rows_sumsq(
             self.ctrl.data_ptr(), self.rows.data_ptr(), self.dt_code, x.data_ptr(),
             x2.data_ptr() if x2 is not None else None,
@@ -1224,6 +1252,15 @@ class RowsEngine(AdaptiveEngine):
             self._launch(lib.tdq_rows_combine_final(ctrl, rows, tab, dc, self.y1.data_ptr(), self.errp.data_ptr(),
                                                     _lib.ptr_array(k), B, D, st))
         kp = _lib.ptr_array(k)
+        if self.row_segs is not None:
+            sg = C.byref(self.row_segs)
+            self._launch(lib.tdq_rows_seg_error_norm_commit(ctrl, rows, dc, sg, self.errp.data_ptr(), k[S],
+                                                            self.y1.data_ptr(), B, D, self.row_partials.data_ptr(),
+                                                            self.row_norm.data_ptr(), st))
+            self._launch(lib.tdq_rows_seg_controller(ctrl, rows, dc, sg, self.row_norm.data_ptr(), B, D, st))
+            if self.after_control is not None:
+                keep.append(self.after_control())
+            return k, kp, keep
         self._launch(lib.tdq_rows_error_norm_commit(
             ctrl, rows, dc, self.errp.data_ptr(), k[S], self.y1.data_ptr(),
             self.rtol_vec.data_ptr() if self.rtol_vec is not None else None,
@@ -1376,12 +1413,20 @@ class RowsEngine(AdaptiveEngine):
         self._rows_sumsq(self.ybuf[0], None, d[0])                 # also counts each row's non-finite y0 elements
         if self.first_step is None:                                 # misc.py:36-77, row by row
             self._rows_sumsq(self.kbuf[0], None, d[1])
-            self._launch(lib.tdq_rows_initial_h0(ctrl, rows, dc, d[0].data_ptr(), d[1].data_ptr(), B, D, st))
+            if self.row_segs is not None:
+                self._launch(lib.tdq_rows_seg_initial_h0(ctrl, rows, dc, C.byref(self.row_segs), d[0].data_ptr(),
+                                                         d[1].data_ptr(), B, D, st))
+            else:
+                self._launch(lib.tdq_rows_initial_h0(ctrl, rows, dc, d[0].data_ptr(), d[1].data_ptr(), B, D, st))
             self._launch(lib.tdq_rows_initial_probe(ctrl, rows, dc, self.ytmp.data_ptr(), B, D, st))
             f1 = self._call_fn(self.t_probe, self.ytmp, 1)
             self._rows_sumsq(f1, self.kbuf[0], d[2])
             del f1
-            self._launch(lib.tdq_rows_initial_finish(ctrl, rows, dc, d[2].data_ptr(), B, D, st))
+            if self.row_segs is not None:
+                self._launch(lib.tdq_rows_seg_initial_finish(ctrl, rows, dc, C.byref(self.row_segs), d[2].data_ptr(),
+                                                             B, D, st))
+            else:
+                self._launch(lib.tdq_rows_initial_finish(ctrl, rows, dc, d[2].data_ptr(), B, D, st))
         else:
             self._launch(lib.tdq_rows_set_first_step(rows, B, float(self.first_step), st))
         if self.ev_fn is not None:                                  # rows done at t0 take no attempt
@@ -1390,7 +1435,11 @@ class RowsEngine(AdaptiveEngine):
         if self.compact_fn is not None:                             # the first pause: at the next smaller batch size
             self.threshold = _compact.pick(self.sizes, B)[1]
             self._launch(lib.tdq_rows_set_compact_threshold(rows, B, self.threshold, st))
-        self._launch(lib.tdq_rows_prepare(ctrl, rows, dc, d[0].data_ptr() if n_out > 1 else None, B, st))
+        y0_bad = d[0].data_ptr() if n_out > 1 else None
+        if self.row_segs is not None:
+            self._launch(lib.tdq_rows_seg_prepare(ctrl, rows, dc, C.byref(self.row_segs), y0_bad, B, D, st))
+        else:
+            self._launch(lib.tdq_rows_prepare(ctrl, rows, dc, y0_bad, B, st))
 
     def row_field(self, which, dtype):
         return self._field(which, dtype, torch.empty((), dtype=dtype).element_size())

@@ -84,6 +84,14 @@ class RowsSweep(C.Structure):
     ]
 
 
+TDQ_ROWS_MAX_SEGS = 4
+
+
+class RowsSegs(C.Structure):
+    """tdq_rows_segs (include/tdq.h): the segments of every row for the seminorm of odeint_adjoint's row solve."""
+    _fields_ = [("n_seg", C.c_int32), ("offset", C.c_int32 * TDQ_ROWS_MAX_SEGS), ("len", C.c_int32 * TDQ_ROWS_MAX_SEGS)]
+
+
 class TdqError(RuntimeError):
     pass
 
@@ -191,6 +199,18 @@ _SIGNATURES = {
     "tdq_rows_compact": (C.c_int, [_vp, _vp, _vp, _sz, _sz, _i32, _vp]),
     "tdq_rows_gather": (C.c_int, [_i32, _vp, _sz, _vp, _vp, _vp, _vp, _sz, _sz, _vp]),
     "tdq_rows_scatter": (C.c_int, [_vp, _i32, _vp, _sz, _vp, _vp, _sz, _sz, _vp]),
+    "tdq_rows_seg_partials_len": (_sz, [_sz, C.POINTER(RowsSegs)]),
+    "tdq_rows_seg_sumsq": (C.c_int, [_vp, _vp, _i32, C.POINTER(RowsSegs), _vp, _vp, _sz, _sz, _vp, _vp, _vp]),
+    "tdq_rows_seg_error_norm_commit": (C.c_int, [_vp, _vp, _i32, C.POINTER(RowsSegs), _vp, _vp, _vp, _sz, _sz, _vp, _vp,
+                                                 _vp]),
+    "tdq_rows_seg_initial_h0": (C.c_int, [_vp, _vp, _i32, C.POINTER(RowsSegs), _vp, _vp, _sz, _sz, _vp]),
+    "tdq_rows_seg_initial_finish": (C.c_int, [_vp, _vp, _i32, C.POINTER(RowsSegs), _vp, _sz, _sz, _vp]),
+    "tdq_rows_seg_prepare": (C.c_int, [_vp, _vp, _i32, C.POINTER(RowsSegs), _vp, _sz, _sz, _vp]),
+    "tdq_rows_seg_controller": (C.c_int, [_vp, _vp, _i32, C.POINTER(RowsSegs), _vp, _sz, _sz, _vp]),
+    "tdq_rows_adjoint_pack": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _sz, _sz, _sz, _sz, _sz, _vp]),
+    "tdq_rows_adjoint_handover": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _sz, _sz, _sz, _vp]),
+    "tdq_rows_adjoint_weights": (C.c_int, [_vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "tdq_rows_adjoint_scale": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _sz, _sz, _sz, _sz, _sz, _vp]),
     "tdq_xchg_create": (C.c_int, [_pp, C.POINTER(IpcHandle)]),
     "tdq_xchg_open": (C.c_int, [C.POINTER(IpcHandle), _pp]),
     "tdq_xchg_close": (C.c_int, [_vp]),

@@ -33,9 +33,11 @@ from ._engine import Layout, _stream, on_solver_stream
 from ._fixed import FIXED_METHODS, signed_grid_constructor
 from ._implicit import IMPLICIT_METHODS
 from .fields import fusable
+from ._rows_adjoint import RowsBackwardSolver
 from .odeint import (ADAPTIVE_METHODS, _ADJOINT_CALLBACK_NAMES, _CALLBACK_NAMES, _LAST_STATS, _cache_drop, _cache_get,
-                     _cache_key, _cache_put, _make_adaptive_engine, _make_fixed_engine, _mixed_norm, _rms_norm, _solve,
-                     _solve_event, _unflatten, fixed_grid, normalise, Problem, valid_callbacks)
+                     _cache_key, _cache_put, _check_independent_rows, _make_adaptive_engine, _make_fixed_engine,
+                     _mixed_norm, _rms_norm, _solve, _solve_event, _unflatten, check_compact_rows, fixed_grid, normalise,
+                     Problem, valid_callbacks)
 
 
 def find_parameters(module):
@@ -389,7 +391,7 @@ class _AdjointFunction(torch.autograd.Function):
                     if hit is not None:
                         bs = hit[0]
                     else:
-                        bs = _BackwardSolver(p, adjoint_params, *ctx.bargs)
+                        bs = _backward_solver(p, adjoint_params, ctx.bargs)
                         bs.prime(t, sol[-1])
                         _cache_put(bkey, (bs, p.original_func), "backward")
                     ctx.bsolver = bs
@@ -416,17 +418,69 @@ class _AdjointFunction(torch.autograd.Function):
         with torch.no_grad():
             bs = ctx.bsolver
             if bs is None:
-                bs = _BackwardSolver(p, adjoint_params, *ctx.bargs)
+                bs = _backward_solver(p, adjoint_params, ctx.bargs)
             try:
                 time_vjps, adj_y, adj_params = bs.run(t, y, grad_sol)
             except BaseException:
                 _cache_drop(ctx.bkey, "backward")         # a half-finished backward engine is never reused
                 raise
             _LAST_STATS["fused_adjoint"] = bs.linear is not None
+            if isinstance(bs, RowsBackwardSolver):
+                _LAST_STATS.update(adjoint_row_n_accept=bs.row_n_accept, adjoint_row_n_reject=bs.row_n_reject)
             if ctx.event_mode and time_vjps is not None:                 # adjoint.py:146-148
                 time_vjps = torch.cat([time_vjps[0].reshape(-1), torch.zeros_like(t_all[1:])])
         ctx.bsolver = None
         return (None, None, None, None, None, None, time_vjps, adj_y, *adj_params)
+
+
+def _backward_solver(p, adjoint_params, bargs):
+    cls = RowsBackwardSolver if p.options.get("independent_rows") else _BackwardSolver
+    return cls(p, adjoint_params, *bargs)
+
+
+def _is_scalar(tol):
+    return isinstance(tol, (int, float)) or (isinstance(tol, torch.Tensor) and tol.ndim == 0)
+
+
+def _check_rows_adjoint(func, y0, t, rtol, atol, method, options, event_fn, adjoint_rtol, adjoint_atol, adjoint_method,
+                        adjoint_options):
+    """What odeint_adjoint with options={'independent_rows': True} does not cover raises before any user code runs."""
+    def no(what):
+        raise NotImplementedError("odeint_adjoint with options['independent_rows'] does not support %s" % what)
+    if options.get("differentiable"):
+        no("options['differentiable']: that selects the gradients of the discrete solve, which odeint gives; "
+           "odeint_adjoint gives the continuous adjoint, and the two do not mix")
+    if adjoint_options is None or not (isinstance(adjoint_options.get("norm"), str)
+                                       and adjoint_options["norm"] == "seminorm"):
+        no("the default or a custom adjoint norm: pass adjoint_options={'norm': 'seminorm', ...}.  Each row's backward "
+           "solve implements the seminorm only, since the default norm would need every row's own parameter gradients")
+    if "independent_rows" in adjoint_options and adjoint_options["independent_rows"] is not True:
+        raise ValueError("adjoint_options['independent_rows'] must be True when options['independent_rows'] is: the "
+                         "backward solve is per row whenever the forward is")
+    if not isinstance(y0, torch.Tensor):
+        no("tuple states")
+    if event_fn is not None:
+        no("event_fn / odeint_event (use odeint with options['event_gradient'])")
+    for where, o in (("options", options), ("adjoint_options", adjoint_options)):
+        for name in ("step_t", "jump_t", "process_group"):
+            if o.get(name) is not None:
+                no("%s['%s']" % (where, name))
+        if o.get("compact_rows"):
+            no("%s['compact_rows']" % where)
+    if adjoint_options.get("fused_linear"):
+        no("adjoint_options['fused_linear']")
+    if any(getattr(func, name, None) is not None for name in _CALLBACK_NAMES + _ADJOINT_CALLBACK_NAMES):
+        no("callbacks")
+    am = adjoint_method if adjoint_method is not None else (method if method is not None else "dopri5")
+    if am not in ADAPTIVE_METHODS:
+        no("adjoint_method %r: it is implemented for the adaptive methods %s" % (am, ", ".join(ADAPTIVE_METHODS)))
+    for name, tol in (("rtol", rtol), ("atol", atol), ("adjoint_rtol", adjoint_rtol), ("adjoint_atol", adjoint_atol)):
+        if tol is not None and not _is_scalar(tol):
+            no("tuple or tensor tolerances (%s)" % name)
+    if "compact_rows" in options:
+        check_compact_rows(options)
+    with torch.no_grad():                     # the forward's own checks; its gradient rule is odeint's, not this one
+        _check_independent_rows(func, y0, t, method, options, None)
 
 
 def _adj_tol(tol, lay, device):
@@ -448,9 +502,17 @@ def _adj_tol(tol, lay, device):
 def odeint_adjoint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, event_fn=None,
                    adjoint_rtol=None, adjoint_atol=None, adjoint_method=None, adjoint_options=None,
                    adjoint_params=None):
-    """adjoint.py:156-223, same signature and defaults."""
+    """adjoint.py:156-223, same signature and defaults.
+
+    With options={'independent_rows': True} (y0 of shape [B, *rest], t 1-D or [B, T]) the forward is odeint's row solve and
+    row r's gradients are those of the reference's odeint_adjoint(func_r, y0[r:r+1], t or t[r]) on its own: y0[r]'s, t's
+    (t[r]'s, or summed over rows for a 1-D t) and the parameters' (summed over rows), each row's backward solve under its
+    own step control.  It needs adjoint_options={'norm': 'seminorm', ...}: the per-row backward implements the seminorm
+    only.  last_stats() then adds adjoint_row_n_accept / adjoint_row_n_reject (int64 [B], summed over the intervals)."""
     if options and options.get("independent_rows"):
-        raise NotImplementedError("options['independent_rows'] does not support odeint_adjoint")
+        _check_rows_adjoint(func, y0, t, rtol, atol, method, options, event_fn,
+                            rtol if adjoint_rtol is None else adjoint_rtol, atol if adjoint_atol is None else adjoint_atol,
+                            adjoint_method, adjoint_options)
     if options and "event_gradient" in options:
         from .odeint import check_event_gradient
         check_event_gradient(options, rows=False)

@@ -92,9 +92,7 @@ __device__ __forceinline__ double block_norm_from_sums(const TdqCtrl &c, const d
     for (int s = threadIdx.x; s < n_seg; s += THREADS) {
         const double cnt = counts ? (double)counts[s] : (double)c.n_global;
         if (cnt <= 0.0) continue;
-        const double r = tdq_rms<T>(sums[s], cnt, c.ratio_f64);
-        if (r != r) nan = 1;
-        if (r > best) best = r;
+        tdq_norm_max(tdq_rms<T>(sums[s], cnt, c.ratio_f64), best, nan);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {

@@ -219,9 +219,41 @@ struct RowNormArgs {
     double *out;                          // [2B]: sums, then non-finite counts
 };
 
-template <typename T, int MODE, bool VTOL>
+// Row segments (tdq_rows_segs): segment s of every row is its elements [off[s], off[s] + len[s]).  A segmented row is cut
+// into units segment by segment, chunk by chunk, so segment s is summed exactly as an unsegmented row of len[s] elements:
+// its sum depends on len[s] alone.  first[s]: the row's unit index where segment s starts (first[n] units per row).
+struct RowSegs {
+    int n;
+    int off[TDQ_ROWS_MAX_SEGS], len[TDQ_ROWS_MAX_SEGS], first[TDQ_ROWS_MAX_SEGS + 1];
+};
+
+// Every loop over a segment table below is unrolled to TDQ_ROWS_MAX_SEGS, so each table entry is read at a constant index
+// and the table stays in the kernel's parameters (a dynamic index would copy it to the stack).
+
+// The norm of row r from per-segment sums sums[s * B + r]: max over segments of the RMS (block_norm_from_sums' arithmetic).
+template <typename T>
+__device__ __forceinline__ double row_seg_norm(const TdqCtrl &c, const double *sums, const RowSegs &sg, int B, int r) {
+    double best = 0.0;
+    int nan = 0;
+#pragma unroll
+    for (int s = 0; s < TDQ_ROWS_MAX_SEGS; ++s)
+        if (s < sg.n) tdq_norm_max(tdq_rms<T>(sums[(size_t)s * B + r], (double)sg.len[s], c.ratio_f64), best, nan);
+    return nan ? CUDART_NAN : best;
+}
+
+// Row r's non-finite count from per-segment counts bad[s * B + r].
+__device__ __forceinline__ double row_seg_bad(const double *bad, const RowSegs &sg, int B, int r) {
+    double b = 0.0;
+#pragma unroll
+    for (int s = 0; s < TDQ_ROWS_MAX_SEGS; ++s)
+        if (s < sg.n) b += bad[(size_t)s * B + r];
+    return b;
+}
+
+// SEG: the sums are per (row, segment), out[s * B + r] and counts out[(n + s) * B + r]; without, per row as before.
+template <typename T, int MODE, bool VTOL, bool SEG>
 __global__ void __launch_bounds__(kThreads)
-k_rows_norm(const TdqCtrl *__restrict__ c, Rows R, Geom g, RowNormArgs a) {
+k_rows_norm(const TdqCtrl *__restrict__ c, Rows R, Geom g, RowNormArgs a, RowSegs sg) {
     if (c->halt) return;
     using A = Ar<T>;
     using Q = typename std::conditional<VTOL, double, T>::type;
@@ -229,6 +261,29 @@ k_rows_norm(const TdqCtrl *__restrict__ c, Rows R, Geom g, RowNormArgs a) {
     int r;
     const bool have = unit_of(g, u, r, lo, hi);
     const int lane = threadIdx.x & 31;
+    int s = 0;
+    size_t nch = g.nch, first = 0;
+    if (SEG && have) {
+        const int j = (int)(u % g.nch);
+        int off = 0, len = 0, f0 = 0, f1 = 0;
+#pragma unroll
+        for (int q = 0; q < TDQ_ROWS_MAX_SEGS; ++q) {
+            if (q < sg.n && j >= sg.first[q]) {
+                s = q;
+                off = sg.off[q];
+                len = sg.len[q];
+                f0 = sg.first[q];
+                f1 = sg.first[q + 1];
+            }
+        }
+        first = (size_t)f0;
+        nch = (size_t)(f1 - f0);
+        lo = (size_t)off + ((size_t)j - first) * kChunk;
+        const size_t end = (size_t)off + (size_t)len;
+        hi = lo + kChunk < end ? lo + kChunk : end;
+    }
+    const size_t o_sum = SEG ? (size_t)s * R.B + r : (size_t)r;
+    const size_t o_bad = SEG ? (size_t)(sg.n + s) * R.B + r : (size_t)R.B + r;
     double acc = 0.0, bad = 0.0;
     if (have && !(MODE == 0 && fld<int>(R, TDQ_ROWS_DONE)[r])) {
         const int par = fld<int>(R, TDQ_ROWS_PAR)[r];
@@ -266,30 +321,31 @@ k_rows_norm(const TdqCtrl *__restrict__ c, Rows R, Geom g, RowNormArgs a) {
     acc = warp_sum(acc);
     bad = warp_sum(bad);
     if (have && lane == 0) {
-        if (g.nch == 1) {
-            a.out[r] = acc;
-            a.out[R.B + r] = bad;
+        if (nch == 1) {
+            a.out[o_sum] = acc;
+            a.out[o_bad] = bad;
         } else {
             a.partials[2 + u] = acc;
             a.partials[2 + g.units + u] = bad;
         }
     }
-    if (g.nch == 1 || !have) return;
-    // rows of several units: the last unit of a row to finish adds that row's unit partials in index order (a ticket per
-    // row, so the serial sums of different rows run in different warps)
+    if (nch == 1 || !have) return;
+    // rows (segments) of several units: the last unit of a row to finish adds that row's unit partials in index order (a
+    // ticket per row and segment, so the serial sums of different rows run in different warps)
     if (lane == 0) {
-        unsigned int *ticket = reinterpret_cast<unsigned int *>(a.partials + 2 + 2 * g.units) + r;
+        unsigned int *ticket = reinterpret_cast<unsigned int *>(a.partials + 2 + 2 * g.units) +
+                               (SEG ? (size_t)r * sg.n + s : (size_t)r);
         __threadfence();
-        if (atomicAdd(ticket, 1u) == (unsigned)g.nch - 1) {
+        if (atomicAdd(ticket, 1u) == (unsigned)nch - 1) {
             __threadfence();
-            double s = 0.0, b = 0.0;
-            const double *ps = a.partials + 2 + (size_t)r * g.nch, *pb = ps + g.units;
-            for (size_t ch = 0; ch < g.nch; ++ch) {
-                s += __ldcg(ps + ch);
+            double sum = 0.0, b = 0.0;
+            const double *ps = a.partials + 2 + (size_t)r * g.nch + first, *pb = ps + g.units;
+            for (size_t ch = 0; ch < nch; ++ch) {
+                sum += __ldcg(ps + ch);
                 b += __ldcg(pb + ch);
             }
-            a.out[r] = s;
-            a.out[R.B + r] = b;
+            a.out[o_sum] = sum;
+            a.out[o_bad] = b;
             *ticket = 0;                                                  // self-reset for the next launch
         }
     }
@@ -385,10 +441,8 @@ struct NoEvent {
 // [T0, T1] and takes no next attempt, so neither a non-finite y1 nor max_num_steps can fail it (the reference tests the
 // sign before it would take that attempt).
 template <typename T, typename Event = NoEvent>
-__device__ void row_control(const TdqCtrl &c, const Rows &R, int r, double sumsq, double n_bad, size_t D,
-                            Event event = Event{}) {
-    double ratio = tdq_rms<T>(sumsq, (double)D, c.ratio_f64);
-    if (n_bad > 0.0) ratio = CUDART_NAN;                                   // a non-finite y1 poisons err/tol
+__device__ void row_control(const TdqCtrl &c, const Rows &R, int r, double ratio, double n_bad, Event event = Event{}) {
+    if (n_bad > 0.0) ratio = CUDART_NAN;                                  // a non-finite y1 poisons err/tol
     fld<double>(R, TDQ_ROWS_RATIO)[r] = ratio;
     const double dt = fld<double>(R, TDQ_ROWS_ATT_DT)[r];
     const bool accept = tdq_accept(ratio, dt, c.min_step, c.max_step);     // :324-330
@@ -522,12 +576,18 @@ __global__ void __launch_bounds__(kThreads) k_rows_init_grid(TdqCtrl *c, Rows R,
     row_init<T>(c, R, r, grid[(size_t)r * n_grid], n_grid);
 }
 
-template <typename T>
+// The norm of row r from k_rows_norm's sums: the RMS over the row, or with SEG the max over its segments.
+template <typename T, bool SEG>
+__device__ __forceinline__ double row_norm_of(const TdqCtrl &c, const double *sums, size_t D, const RowSegs &sg, int B, int r) {
+    return SEG ? row_seg_norm<T>(c, sums, sg, B, r) : tdq_rms<T>(sums[r], (double)D, c.ratio_f64);
+}
+
+template <typename T, bool SEG>
 __global__ void __launch_bounds__(kThreads)
-k_rows_h0(const TdqCtrl *__restrict__ c, Rows R, const double *s0, const double *s1, size_t D) {
+k_rows_h0(const TdqCtrl *__restrict__ c, Rows R, const double *s0, const double *s1, size_t D, RowSegs sg) {
     const int r = blockIdx.x * kThreads + threadIdx.x;
     if (r >= R.B) return;
-    const double d0 = tdq_rms<T>(s0[r], (double)D, c->ratio_f64), d1 = tdq_rms<T>(s1[r], (double)D, c->ratio_f64);
+    const double d0 = row_norm_of<T, SEG>(*c, s0, D, sg, R.B, r), d1 = row_norm_of<T, SEG>(*c, s1, D, sg, R.B, r);
     const double h0 = tdq_initial_h0<T>(c->ratio_f64 != 0, d0, d1);
     fld<double>(R, TDQ_ROWS_H0)[r] = h0;
     fld<double>(R, TDQ_ROWS_D1)[r] = d1;
@@ -548,11 +608,12 @@ __global__ void __launch_bounds__(kThreads) k_rows_probe(const TdqCtrl *__restri
     for (size_t i = lo + (threadIdx.x & 31); i < hi; i += 32) out[base + i] = tdq_probe<T>(y0[i], h, f0[i]);
 }
 
-template <typename T>
-__global__ void __launch_bounds__(kThreads) k_rows_finish(const TdqCtrl *__restrict__ c, Rows R, const double *s2, size_t D) {
+template <typename T, bool SEG>
+__global__ void __launch_bounds__(kThreads)
+k_rows_finish(const TdqCtrl *__restrict__ c, Rows R, const double *s2, size_t D, RowSegs sg) {
     const int r = blockIdx.x * kThreads + threadIdx.x;
     if (r >= R.B) return;
-    const double nd = tdq_rms<T>(s2[r], (double)D, c->ratio_f64);
+    const double nd = row_norm_of<T, SEG>(*c, s2, D, sg, R.B, r);
     fld<double>(R, TDQ_ROWS_DT)[r] = tdq_initial_finish<T>(c->ratio_f64 != 0, c->order, fld<double>(R, TDQ_ROWS_D1)[r],
                                                            fld<double>(R, TDQ_ROWS_H0)[r], nd);
 }
@@ -562,12 +623,13 @@ __global__ void k_rows_first_step(Rows R, double dt) {
     if (r < R.B) fld<double>(R, TDQ_ROWS_DT)[r] = dt;
 }
 
-template <typename T>
-__global__ void __launch_bounds__(kThreads) k_rows_prepare(TdqCtrl *c, Rows R, const double *y0_bad) {
+template <typename T, bool SEG>
+__global__ void __launch_bounds__(kThreads) k_rows_prepare(TdqCtrl *c, Rows R, const double *y0_bad, RowSegs sg) {
     const int r = blockIdx.x * kThreads + threadIdx.x;
     bool running = false, failed = false;
     if (!c->halt && r < R.B && !fld<int>(R, TDQ_ROWS_DONE)[r]) {
-        row_prepare<T>(*c, R, r, y0_bad != nullptr && y0_bad[R.B + r] > 0.0);
+        const double nb = y0_bad == nullptr ? 0.0 : (SEG ? row_seg_bad(y0_bad + (size_t)sg.n * R.B, sg, R.B, r) : y0_bad[R.B + r]);
+        row_prepare<T>(*c, R, r, nb > 0.0);
         failed = fld<int>(R, TDQ_ROWS_STATUS)[r] != TDQ_RUN_OK;
         running = true;
     }
@@ -599,9 +661,9 @@ __device__ __forceinline__ double ev_combined(const double *val, const double *i
     return m;
 }
 
-template <typename T, bool EVENT>
+template <typename T, bool EVENT, bool SEG>
 __global__ void __launch_bounds__(kThreads)
-k_rows_controller(TdqCtrl *c, Rows R, const double *norm_in, size_t D, RowEvents ev) {
+k_rows_controller(TdqCtrl *c, Rows R, const double *norm_in, size_t D, RowEvents ev, RowSegs sg) {
     const int r = blockIdx.x * kThreads + threadIdx.x;
     if (c->halt) {
         // attempts issued after the end are no-ops; the mailbox still ticks so that a host running ahead can account for
@@ -628,15 +690,17 @@ k_rows_controller(TdqCtrl *c, Rows R, const double *norm_in, size_t D, RowEvents
             fld<int>(R, TDQ_ROWS_FIT)[r] = 0;
             if (EVENT) ev.flag[r] = 0;
         } else {
+            const double ratio = row_norm_of<T, SEG>(*c, norm_in, D, sg, R.B, r);
+            const double n_bad = SEG ? row_seg_bad(norm_in + (size_t)sg.n * R.B, sg, R.B, r) : norm_in[R.B + r];
             if (EVENT) {
                 // an accepted candidate whose combined sign differs from sign0 ends the row
-                row_control<T>(*c, R, r, norm_in[r], norm_in[R.B + r], D, [&](bool accept) {
+                row_control<T>(*c, R, r, ratio, n_bad, [&](bool accept) {
                     const bool fired = accept && !(sign_of(ev_combined(ev.val, ev.init, ev.K, r)) == ev.sign0[r]);
                     ev.flag[r] = fired ? 1 : 0;
                     return fired;
                 });
             } else {
-                row_control<T>(*c, R, r, norm_in[r], norm_in[R.B + r], D);
+                row_control<T>(*c, R, r, ratio, n_bad);
             }
             failed = fld<int>(R, TDQ_ROWS_STATUS)[r] != TDQ_RUN_OK;
             running = !fld<int>(R, TDQ_ROWS_DONE)[r];
@@ -1155,6 +1219,127 @@ k_rows_scatter(Rows R, Geom g, const int64_t *__restrict__ idx, const T *__restr
 }
 
 // ---- host helpers -----------------------------------------------------------------------------------------------------------
+// ---- odeint_adjoint for independent rows: the augmented row [vjp_t | pad | y | adj_y] (adjoint.py:72-105, :124-141) ---------
+// Row r of the raw stage slot from one evaluation: (-g_t, 0 in the pad, +f, -g_y), the signs of the shared adjoint's pack.
+// A unit of the W-wide row takes its elements lane by lane; gt / gy NULL write 0.
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+k_rows_adjoint_pack(Geom g, size_t D, size_t o_y, size_t o_a, const T *__restrict__ f, const T *__restrict__ gy,
+                    const T *__restrict__ gt, T *__restrict__ out) {
+    size_t u, lo, hi;
+    int r;
+    if (!unit_of(g, u, r, lo, hi)) return;
+    const size_t rd = (size_t)r * D;
+    T *o = out + (size_t)r * g.D;
+    for (size_t i = lo + (threadIdx.x & 31); i < hi; i += 32) {
+        T v = (T)0;
+        if (i == 0) v = gt ? -gt[r] : (T)0;
+        else if (i >= o_a) v = gy ? -gy[rd + i - o_a] : (T)0;
+        else if (i >= o_y) v = f[rd + i - o_y];
+        o[i] = v;
+    }
+}
+
+// One warp per row at the hand-over between two output intervals: y <- y_next and adj_y += g_next (adjoint.py:140-141) when
+// y_next is given; when f is given, dot = <f, g_cur> as a float64 sum in k_rows_norm's order, vjp_t -= T(dot) and
+// tgrad[r] = dot (adjoint.py:127-133).
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+k_rows_adjoint_handover(int B, size_t D, size_t W, size_t o_y, size_t o_a, T *__restrict__ aug, const T *__restrict__ y_next,
+                        const T *__restrict__ g_next, const T *__restrict__ f, const T *__restrict__ g_cur,
+                        double *__restrict__ tgrad) {
+    using A = Ar<T>;
+    const int r = blockIdx.x * kWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (r >= B) return;
+    const size_t rd = (size_t)r * D;
+    T *row = aug + (size_t)r * W;
+    if (y_next) {
+        for (size_t i = lane; i < D; i += 32) {
+            row[o_y + i] = y_next[rd + i];
+            row[o_a + i] = A::add(row[o_a + i], g_next[rd + i]);
+        }
+    }
+    if (f) {
+        double total = 0.0;
+        for (size_t lo = 0; lo < D; lo += kChunk) {
+            const size_t hi = lo + kChunk < D ? lo + kChunk : D;
+            double acc = 0.0;
+            for (size_t i = lo + lane; i < hi; i += 32) acc += (double)f[rd + i] * (double)g_cur[rd + i];
+            total += warp_sum(acc);
+        }
+        if (lane == 0) {
+            row[0] = A::sub(row[0], (T)total);
+            tgrad[r] = total;
+        }
+    }
+}
+
+// The parameter quadrature (adjoint.py:95-105 integrated over the row's accepted steps): after the controller, one thread
+// per row.  A row accepted in this attempt when its N_ACCEPT passed seen[r]; only such a row gets weights, w[j][r] =
+// fl_T(t_sign * fl_T(T(omega_j) * T(dt))) with dt its accepted step (FIT_DT), formed as the row combines form theirs; every
+// other row, done or rejected, gets 0.  omega_j = b_j (c_sol), except on the step that ends the row's solve: the reference
+// reads the augmented state at the output time from that step's interpolant (rk_common.py:363-369, interp.py), so the
+// parameter part gets the quartic's increment at x, which is linear in the stages (y0 cancels):
+//   omega_j(x) = x [j=0] + x^2 ([j=S] - 4[j=0] - 5 b_j + 16 m_j) + x^3 (5[j=0] - 3[j=S] + 14 b_j - 32 m_j)
+//              + x^4 (2[j=S] - 2[j=0] - 8 b_j + 16 m_j)                       (m = c_mid; omega_j(1) = b_j)
+// t_point[r]: func's time at the attempt's start (accepted) or at the row's current point.
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+k_rows_adjoint_weights(const TdqCtrl *__restrict__ c, Rows R, const double *__restrict__ b, int n_k, int64_t *__restrict__ seen,
+                       int *__restrict__ flag, T *__restrict__ w, T *__restrict__ t_point) {
+    const int r = blockIdx.x * kThreads + threadIdx.x;
+    if (r >= R.B) return;
+    const int64_t na = fld<int64_t>(R, TDQ_ROWS_N_ACCEPT)[r];
+    const bool acc = na > seen[r];                  // halt is no test: the attempt that ends the solve sets it
+    seen[r] = na;
+    flag[r] = acc ? 1 : 0;
+    const T sgn = (T)c->t_sign, dtT = (T)fld<double>(R, TDQ_ROWS_FIT_DT)[r];
+    const double t0 = fld<double>(R, TDQ_ROWS_T0)[r], t1 = fld<double>(R, TDQ_ROWS_T1)[r];
+    const bool last = acc && fld<int>(R, TDQ_ROWS_FIT)[r] && fld<int>(R, TDQ_ROWS_DONE)[r];
+    double x = 1.0;
+    if (last) x = (double)(T)((row_times(*c, r).t[fld<int>(R, TDQ_ROWS_EMIT_HI)[r] - 1] - t0) / (t1 - t0));
+    const double x2 = x * x, x3 = x2 * x, x4 = x3 * x;
+    const int S = n_k - 1;
+    for (int j = 0; j < n_k; ++j) {
+        double om = b[j];
+        if (last) {
+            const double bj = b[j], mj = b[n_k + j], e0 = j == 0 ? 1.0 : 0.0, eS = j == S ? 1.0 : 0.0;
+            om = x * e0 + x2 * (eS - 4.0 * e0 - 5.0 * bj + 16.0 * mj) + x3 * (5.0 * e0 - 3.0 * eS + 14.0 * bj - 32.0 * mj) +
+                 x4 * (2.0 * eS - 2.0 * e0 - 8.0 * bj + 16.0 * mj);
+        }
+        w[(size_t)j * R.B + r] = acc ? tdq_coef<T>(sgn, (T)om, dtT) : (T)0;
+    }
+    t_point[r] = Ar<T>::mul(sgn, (T)(acc ? t0 : t1));
+}
+
+// Units of a D-element row: cot[j] = w[j][r] * adj_j for a row flagged by k_rows_adjoint_weights, 0 for the others (so a
+// rejected attempt contributes exactly 0).  adj_0 is the adj_y of the pair the accepted step started from (ybuf[par ^ 1]);
+// adj[j], j >= 1, the kept adj_y of the stage value k_j was evaluated at.  y_point: the y of that pair (flagged) or of
+// the row's current pair (others), where func is evaluated again for k_0's parameter VJP.
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+k_rows_adjoint_scale(const TdqCtrl *__restrict__ c, Rows R, Geom g, size_t W, size_t o_y, size_t o_a,
+                     const int *__restrict__ flag, const T *__restrict__ w, int n_k, const void *const *__restrict__ adj,
+                     void *const *__restrict__ cot, T *__restrict__ y_point) {
+    using A = Ar<T>;
+    size_t u, lo, hi;
+    int r;
+    if (!unit_of(g, u, r, lo, hi)) return;
+    const bool acc = flag[r] != 0;
+    const int par = fld<int>(R, TDQ_ROWS_PAR)[r];
+    const T *row = reinterpret_cast<const T *>(c->ybuf[acc ? par ^ 1 : par]) + (size_t)r * W;
+    const size_t base = (size_t)r * g.D;
+    const int lane = threadIdx.x & 31;
+    for (size_t i = lo + lane; i < hi; i += 32) y_point[base + i] = row[o_y + i];
+    for (int j = 0; j < n_k; ++j) {
+        T *out = reinterpret_cast<T *>(cot[j]);
+        if (out == nullptr) continue;
+        const T wj = w[(size_t)j * R.B + r];
+        const T *a = j == 0 ? row + o_a : reinterpret_cast<const T *>(adj[j]) + base;
+        for (size_t i = lo + lane; i < hi; i += 32) out[base + i] = acc ? A::mul(wj, a[i]) : (T)0;
+    }
+}
+
 bool plan_kp(const int *idx, int nnz, const void *const *k, KPtrs &kp, bool &vec) {
     return tdq_plan_terms(idx, nnz, k, kp.p, vec) == TDQ_PLAN_OK;
 }
@@ -1204,16 +1389,45 @@ int tdq_rows_init_grid(void *ctrl_dev, void *rows_dev, int32_t dtype, size_t n_r
     return TDQ_OK;
 }
 
+// The device form of a segment table, or false when it is malformed for rows of row_len elements.
+static bool make_segs(const tdq_rows_segs *s, size_t row_len, RowSegs &sg) {
+    if (s == nullptr || s->n_seg < 1 || s->n_seg > TDQ_ROWS_MAX_SEGS) return false;
+    sg = RowSegs{};
+    sg.n = s->n_seg;
+    for (int i = 0; i < sg.n; ++i) {
+        if (s->offset[i] < 0 || s->len[i] < 1 || (size_t)s->offset[i] + (size_t)s->len[i] > row_len) return false;
+        sg.off[i] = s->offset[i];
+        sg.len[i] = s->len[i];
+        sg.first[i + 1] = sg.first[i] + (int)(((size_t)s->len[i] + kChunk - 1) / kChunk);
+    }
+    return true;
+}
+
+// Units of a segmented row: one per chunk of each segment.
+static Geom seg_geom(size_t B, size_t row_len, const RowSegs &sg) {
+    Geom g;
+    g.D = row_len;
+    g.nch = (size_t)sg.first[sg.n];
+    g.units = B * g.nch;
+    return g;
+}
+
+// sg == NULL: one sum per row.  Segmented launches take scalar tolerances only.
 static int rows_norm(int mode, void *ctrl_dev, void *rows_dev, int32_t dtype, RowNormArgs &a, size_t n_rows,
-                     size_t row_len, cudaStream_t st) {
-    const Geom g = make_geom(n_rows, row_len);
+                     size_t row_len, const RowSegs *sg, cudaStream_t st) {
+    const Geom g = sg ? seg_geom(n_rows, row_len, *sg) : make_geom(n_rows, row_len);
     const Rows R = make_rows(rows_dev, n_rows);
     const TdqCtrl *c = (const TdqCtrl *)ctrl_dev;
     const bool vt = a.rtol_v != nullptr;
+    const RowSegs s = sg ? *sg : RowSegs{};
     TDQ_DISPATCH_T(dtype, tdq_dispatch(TdqBool{}, vt, [&](auto VT) {
-        if (mode == 0) k_rows_norm<T, 0, VT><<<unit_blocks(g), kThreads, 0, st>>>(c, R, g, a);
-        else if (mode == 1) k_rows_norm<T, 1, VT><<<unit_blocks(g), kThreads, 0, st>>>(c, R, g, a);
-        else k_rows_norm<T, 2, VT><<<unit_blocks(g), kThreads, 0, st>>>(c, R, g, a);
+        if (sg) {
+            if (mode == 0) k_rows_norm<T, 0, false, true><<<unit_blocks(g), kThreads, 0, st>>>(c, R, g, a, s);
+            else if (mode == 1) k_rows_norm<T, 1, false, true><<<unit_blocks(g), kThreads, 0, st>>>(c, R, g, a, s);
+            else k_rows_norm<T, 2, false, true><<<unit_blocks(g), kThreads, 0, st>>>(c, R, g, a, s);
+        } else if (mode == 0) k_rows_norm<T, 0, VT, false><<<unit_blocks(g), kThreads, 0, st>>>(c, R, g, a, s);
+        else if (mode == 1) k_rows_norm<T, 1, VT, false><<<unit_blocks(g), kThreads, 0, st>>>(c, R, g, a, s);
+        else k_rows_norm<T, 2, VT, false><<<unit_blocks(g), kThreads, 0, st>>>(c, R, g, a, s);
         return 0;
     }));
     TDQ_CHECK_CUDA(cudaGetLastError());
@@ -1226,7 +1440,7 @@ int tdq_rows_sumsq(void *ctrl_dev, void *rows_dev, int32_t dtype, const void *x,
     TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
     TDQ_REQUIRE((rtol_vec == nullptr) == (atol_vec == nullptr), "rtol_vec and atol_vec go together");
     RowNormArgs a{x, x2, nullptr, rtol_vec, atol_vec, partials, out};
-    return rows_norm(x2 ? 2 : 1, ctrl_dev, rows_dev, dtype, a, n_rows, row_len, (cudaStream_t)stream);
+    return rows_norm(x2 ? 2 : 1, ctrl_dev, rows_dev, dtype, a, n_rows, row_len, nullptr, (cudaStream_t)stream);
 }
 
 int tdq_rows_error_norm_commit(void *ctrl_dev, void *rows_dev, int32_t dtype, const void *err_pre, const void *k_last,
@@ -1236,15 +1450,16 @@ int tdq_rows_error_norm_commit(void *ctrl_dev, void *rows_dev, int32_t dtype, co
     TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
     TDQ_REQUIRE((rtol_vec == nullptr) == (atol_vec == nullptr), "rtol_vec and atol_vec go together");
     RowNormArgs a{err_pre, k_last, y1, rtol_vec, atol_vec, partials, out};
-    return rows_norm(0, ctrl_dev, rows_dev, dtype, a, n_rows, row_len, (cudaStream_t)stream);
+    return rows_norm(0, ctrl_dev, rows_dev, dtype, a, n_rows, row_len, nullptr, (cudaStream_t)stream);
 }
 
 int tdq_rows_initial_h0(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *d0_sumsq, const double *d1_sumsq,
                         size_t n_rows, size_t row_len, void *stream) {
     TDQ_REQUIRE(ctrl_dev && rows_dev && d0_sumsq && d1_sumsq, "null argument");
     TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
-    TDQ_DISPATCH_T(dtype, (k_rows_h0<T><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
-                               (const TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), d0_sumsq, d1_sumsq, row_len)));
+    TDQ_DISPATCH_T(dtype, (k_rows_h0<T, false><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (const TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), d0_sumsq, d1_sumsq, row_len,
+                               RowSegs{})));
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
 }
@@ -1264,8 +1479,8 @@ int tdq_rows_initial_finish(void *ctrl_dev, void *rows_dev, int32_t dtype, const
                             size_t row_len, void *stream) {
     TDQ_REQUIRE(ctrl_dev && rows_dev && d2_sumsq, "null argument");
     TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
-    TDQ_DISPATCH_T(dtype, (k_rows_finish<T><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
-                               (const TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), d2_sumsq, row_len)));
+    TDQ_DISPATCH_T(dtype, (k_rows_finish<T, false><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (const TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), d2_sumsq, row_len, RowSegs{})));
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
 }
@@ -1282,8 +1497,8 @@ int tdq_rows_prepare(void *ctrl_dev, void *rows_dev, int32_t dtype, const double
                      void *stream) {
     TDQ_REQUIRE(ctrl_dev && rows_dev, "null argument");
     TDQ_REQUIRE(n_rows >= 1 && n_rows <= (size_t)INT_MAX, "n_rows out of range");
-    TDQ_DISPATCH_T(dtype, (k_rows_prepare<T><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
-                               (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), y0_nonfinite_dev)));
+    TDQ_DISPATCH_T(dtype, (k_rows_prepare<T, false><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), y0_nonfinite_dev, RowSegs{})));
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
 }
@@ -1346,8 +1561,9 @@ int tdq_rows_controller(void *ctrl_dev, void *rows_dev, int32_t dtype, const dou
                         size_t row_len, void *stream) {
     TDQ_REQUIRE(ctrl_dev && rows_dev && norm_in, "null argument");
     TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
-    TDQ_DISPATCH_T(dtype, (k_rows_controller<T, false><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
-                               (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), norm_in, row_len, RowEvents{})));
+    TDQ_DISPATCH_T(dtype, (k_rows_controller<T, false, false><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), norm_in, row_len, RowEvents{},
+                               RowSegs{})));
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
 }
@@ -1420,9 +1636,9 @@ int tdq_rows_controller_event(void *ctrl_dev, void *rows_dev, int32_t dtype, con
     TDQ_REQUIRE(ctrl_dev && rows_dev && norm_in && ev_val && init_sign && sign0 && flag, "null argument");
     TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
     TDQ_ROWS_REQUIRE_K(K);
-    TDQ_DISPATCH_T(dtype, (k_rows_controller<T, true><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+    TDQ_DISPATCH_T(dtype, (k_rows_controller<T, true, false><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
                                (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), norm_in, row_len,
-                               RowEvents{ev_val, init_sign, sign0, flag, K})));
+                               RowEvents{ev_val, init_sign, sign0, flag, K}, RowSegs{})));
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
 }
@@ -1669,6 +1885,152 @@ int tdq_rows_event_reroute(int32_t dtype, const void *grad_state, const void *f,
     TDQ_DISPATCH_T(dtype, (k_rows_event_reroute<T><<<tdq_grid(n_rows, kWarps, 0), kThreads, 0, (cudaStream_t)stream>>>(
                                (int)n_rows, row_len, (const T *)grad_state, (const T *)f, (const T *)dc_dy, dc_dt, grad_t,
                                (T *)out)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+// ---- segmented row norms: odeint_adjoint's seminorm per row (adjoint.py:267-271) ---------------------------------------------
+#define TDQ_ROWS_REQUIRE_SEGS(segs, row_len, sg)                                                                    \
+    RowSegs sg;                                                                                                     \
+    TDQ_REQUIRE(make_segs((segs), (row_len), sg), "segment table out of range")
+
+size_t tdq_rows_seg_partials_len(size_t n_rows, const tdq_rows_segs *segs) {
+    RowSegs sg;
+    if (!make_segs(segs, SIZE_MAX, sg)) return 0;
+    bool several = false;
+    for (int s = 0; s < sg.n; ++s) several |= sg.first[s + 1] - sg.first[s] > 1;
+    const size_t units = n_rows * (size_t)sg.first[sg.n];
+    return 2 + (several ? 2 * units + (n_rows * sg.n + 1) / 2 : 0);
+}
+
+// tdq_rows_sumsq per segment (misc.py:55-58, :69 under the seminorm): replaces the one sum over the row.
+int tdq_rows_seg_sumsq(void *ctrl_dev, void *rows_dev, int32_t dtype, const tdq_rows_segs *segs, const void *x,
+                       const void *x2, size_t n_rows, size_t row_len, double *partials, double *out, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && segs && x && partials && out, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_ROWS_REQUIRE_SEGS(segs, row_len, sg);
+    RowNormArgs a{x, x2, nullptr, nullptr, nullptr, partials, out};
+    return rows_norm(x2 ? 2 : 1, ctrl_dev, rows_dev, dtype, a, n_rows, row_len, &sg, (cudaStream_t)stream);
+}
+
+// tdq_rows_error_norm_commit per segment (rk_common.py:338-352, misc.py:80-82): only segment elements are committed.
+int tdq_rows_seg_error_norm_commit(void *ctrl_dev, void *rows_dev, int32_t dtype, const tdq_rows_segs *segs,
+                                   const void *err_pre, const void *k_last, const void *y1, size_t n_rows, size_t row_len,
+                                   double *partials, double *out, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && segs && err_pre && k_last && y1 && partials && out, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_ROWS_REQUIRE_SEGS(segs, row_len, sg);
+    RowNormArgs a{err_pre, k_last, y1, nullptr, nullptr, partials, out};
+    return rows_norm(0, ctrl_dev, rows_dev, dtype, a, n_rows, row_len, &sg, (cudaStream_t)stream);
+}
+
+// tdq_rows_initial_h0 / _finish (misc.py:60-77) with d0, d1, d2 the max over segments of each segment's RMS.
+int tdq_rows_seg_initial_h0(void *ctrl_dev, void *rows_dev, int32_t dtype, const tdq_rows_segs *segs,
+                            const double *d0_sumsq, const double *d1_sumsq, size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && segs && d0_sumsq && d1_sumsq, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_ROWS_REQUIRE_SEGS(segs, row_len, sg);
+    TDQ_DISPATCH_T(dtype, (k_rows_h0<T, true><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (const TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), d0_sumsq, d1_sumsq, row_len, sg)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_rows_seg_initial_finish(void *ctrl_dev, void *rows_dev, int32_t dtype, const tdq_rows_segs *segs,
+                                const double *d2_sumsq, size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && segs && d2_sumsq, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_ROWS_REQUIRE_SEGS(segs, row_len, sg);
+    TDQ_DISPATCH_T(dtype, (k_rows_finish<T, true><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (const TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), d2_sumsq, row_len, sg)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+// tdq_rows_prepare (rk_common.py:246-247, :269-287) with the non-finite count summed over segments.
+int tdq_rows_seg_prepare(void *ctrl_dev, void *rows_dev, int32_t dtype, const tdq_rows_segs *segs,
+                         const double *y0_nonfinite_dev, size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && segs, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_ROWS_REQUIRE_SEGS(segs, row_len, sg);
+    TDQ_DISPATCH_T(dtype, (k_rows_prepare<T, true><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), y0_nonfinite_dev, sg)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+// tdq_rows_controller (rk_common.py:323-361, misc.py:85-95) with the row's ratio the max over segments of each RMS.
+int tdq_rows_seg_controller(void *ctrl_dev, void *rows_dev, int32_t dtype, const tdq_rows_segs *segs, const double *norm_in,
+                            size_t n_rows, size_t row_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && segs && norm_in, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_ROWS_REQUIRE_SEGS(segs, row_len, sg);
+    TDQ_DISPATCH_T(dtype, (k_rows_controller<T, false, true><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), norm_in, row_len, RowEvents{}, sg)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+#define TDQ_ROWS_REQUIRE_AUG(row_len, o_y, o_a, aug_len)                                                             \
+    TDQ_REQUIRE((o_y) >= 1 && (o_a) >= (o_y) + (row_len) && (aug_len) >= (o_a) + (row_len), "augmented layout out of range")
+
+// The augmented field's raw slot (adjoint.py:100-113 under the shared adjoint's signs), replacing its torch.cat.
+int tdq_rows_adjoint_pack(int32_t dtype, const void *f, const void *vjp_y, const void *vjp_t, void *out, size_t n_rows,
+                          size_t row_len, size_t o_y, size_t o_a, size_t aug_len, void *stream) {
+    TDQ_REQUIRE(f && out, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_ROWS_REQUIRE_AUG(row_len, o_y, o_a, aug_len);
+    const Geom g = make_geom(n_rows, aug_len);
+    TDQ_DISPATCH_T(dtype, (k_rows_adjoint_pack<T><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(
+                               g, row_len, o_y, o_a, (const T *)f, (const T *)vjp_y, (const T *)vjp_t, (T *)out)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+// adjoint.py:127-133 and :140-141 for every row in one launch.
+int tdq_rows_adjoint_handover(int32_t dtype, void *aug, const void *y_next, const void *g_next, const void *f,
+                              const void *g_cur, double *tgrad, size_t n_rows, size_t row_len, size_t o_y, size_t o_a,
+                              size_t aug_len, void *stream) {
+    TDQ_REQUIRE(aug, "null argument");
+    TDQ_REQUIRE((y_next == nullptr) == (g_next == nullptr), "y_next and g_next go together");
+    TDQ_REQUIRE((f == nullptr) == (g_cur == nullptr) && (f == nullptr) == (tgrad == nullptr), "f, g_cur and tgrad go together");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_ROWS_REQUIRE_AUG(row_len, o_y, o_a, aug_len);
+    TDQ_DISPATCH_T(dtype, (k_rows_adjoint_handover<T><<<tdq_grid(n_rows, kWarps, 0), kThreads, 0, (cudaStream_t)stream>>>(
+                               (int)n_rows, row_len, aug_len, o_y, o_a, (T *)aug, (const T *)y_next, (const T *)g_next,
+                               (const T *)f, (const T *)g_cur, tgrad)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+// The weights of the parameter quadrature: the reference's adj_params increments h * sum_i b_i k_i^theta of each row's
+// accepted steps (adjoint.py:95-105 through rk_common.py:83-87), masked per row, and on the step that ends the row's solve
+// the increment of its interpolant at the output time (rk_common.py:363-369).
+int tdq_rows_adjoint_weights(void *ctrl_dev, void *rows_dev, int32_t dtype, const double *b, int32_t n_k, int64_t *seen,
+                             int32_t *flag, void *w, void *t_point, size_t n_rows, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && b && seen && flag && w && t_point, "null argument");
+    TDQ_REQUIRE(n_rows >= 1 && n_rows <= (size_t)INT_MAX, "n_rows out of range");
+    TDQ_REQUIRE(n_k >= 1 && n_k <= TDQ_MAX_K, "n_k out of range");
+    TDQ_DISPATCH_T(dtype, (k_rows_adjoint_weights<T><<<row_blocks(n_rows), kThreads, 0, (cudaStream_t)stream>>>(
+                               (const TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), b, n_k, seen, flag, (T *)w,
+                               (T *)t_point)));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+// The cotangents of the parameter VJPs (the reference's grad of f against -adj_y per stage, adjoint.py:95-96) and k_0's
+// evaluation point.
+int tdq_rows_adjoint_scale(void *ctrl_dev, void *rows_dev, int32_t dtype, const int32_t *flag, const void *w, int32_t n_k,
+                           const void *const *adj, void *const *cot, void *y_point, size_t n_rows, size_t row_len,
+                           size_t o_y, size_t o_a, size_t aug_len, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && flag && w && adj && cot && y_point, "null argument");
+    TDQ_ROWS_REQUIRE_SHAPE(n_rows, row_len);
+    TDQ_ROWS_REQUIRE_AUG(row_len, o_y, o_a, aug_len);
+    TDQ_REQUIRE(n_k >= 1 && n_k <= TDQ_MAX_K, "n_k out of range");
+    const Geom g = make_geom(n_rows, row_len);
+    TDQ_DISPATCH_T(dtype, (k_rows_adjoint_scale<T><<<unit_blocks(g), kThreads, 0, (cudaStream_t)stream>>>(
+                               (const TdqCtrl *)ctrl_dev, make_rows(rows_dev, n_rows), g, aug_len, o_y, o_a, flag,
+                               (const T *)w, n_k, adj, cot, (T *)y_point)));
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;
 }

@@ -164,6 +164,14 @@ template <typename T> __device__ __forceinline__ double tdq_rms(double sumsq, do
     return r;
 }
 
+// One segment's RMS r folded into a max-of-RMS norm (misc.py:30-33 _mixed_norm, adjoint.py:247-250 and :267-271): the
+// running maximum, and a flag that makes the norm NaN once any segment's RMS is NaN.  max is order independent, so any
+// order of segments gives the same value.
+__device__ __forceinline__ void tdq_norm_max(double r, double &best, int &nan) {
+    if (r != r) nan = 1;
+    if (r > best) best = r;
+}
+
 // misc.py:85-95 _optimal_step_size (float64), then the clamp of rk_common.py:359.
 __device__ __forceinline__ double tdq_next_dt(double ratio, double dt, double safety, double ifactor, double dfactor,
                                               int order, double min_step, double max_step) {

@@ -1013,7 +1013,8 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
     Independent rows under autograd need options={'independent_rows': True, 'differentiable': True} (NotImplementedError
     otherwise): row r's gradients w.r.t. y0[r] and t (or t[r]) are those of odeint(func, y0[r:r+1], t_r) differentiated
     as above, a 1-D t and func's parameters get the sums over rows.  The solve then runs in lock step and keeps 2 D
-    elements per accepted row-step for the backward pass.  Not with odeint_adjoint.
+    elements per accepted row-step for the backward pass.  odeint_adjoint with independent rows gives each row's continuous
+    adjoint instead (its own docstring); 'differentiable' does not go with it.
 
     options['compact_rows'] = True (a bool; ValueError without independent_rows) calls func only on the rows still
     running: whenever they fall to the next of the batch sizes ceil(B / 2^k), the running rows are listed in ascending order
