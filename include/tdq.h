@@ -372,6 +372,27 @@ int tdq_linear_attempt(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, vo
                        const void *y0, const void *k0, const void *planes, int32_t width, size_t n, double *partials,
                        double *norm_out, const int64_t *seg_counts_dev, int32_t store_always, void *stream);
 
+/* ---- A WHOLE attempt of an independent-row solve of a linear vector field in one launch (tdq_attempt.cu) ------------------
+ * For the per-row state of tdq_rows_init (B = n_rows rows of width = 128 elements, see "independent step-size control per
+ * batch row" below): what S x (tdq_rows_combine / tdq_rows_combine_final + tdq_linear_apply) + tdq_rows_error_norm_commit do
+ * in 2 S + 1 launches, for every row with its own step.  Row r's coefficients are fl_T(t_sign * fl_T(w * T(ATT_DT[r]))), its
+ * (y0, k_0) is ybuf/kbuf[PAR[r]] and its candidate (y1, k_S) goes to ybuf/kbuf[PAR[r] ^ 1].  k_i, y1, the error prefix and the
+ * commit are bitwise what those launches write; norm_out[r] = row r's sum of ((err_pre + k_S e_S) / (atol + rtol
+ * max(|y0|,|y1|)))^2, added in tdq_rows_error_norm_commit's order (bitwise its value), norm_out[B + r] = its number of
+ * non-finite y1 elements.  A done row writes nothing but 0 and 0 into norm_out; a tile of 32 rows that are all done is not
+ * loaded.  k_out[i] (i = 1..S), y1_out and err_out receive row r's k_i, y1 and error prefix ONLY when the row runs and its
+ * candidate step can emit an output (its t_out[CURSOR[r]] <= ATT_T1[r]), when the control block keeps every step
+ * (always_fit) or when store_always != 0 (event solves: the event function reads y1, tdq_rows_fit_store the stages);
+ * otherwise their rows are not written.  Scalar tolerances only.  No-op after halt.  The row controller is the caller's next
+ * launch: tdq_rows_controller(ctrl, rows, dtype, norm_out, n_rows, width) or tdq_rows_controller_event.
+ * tdq_linear_rows_attempt_supported: 1 for float32, width 128 and the FSAL tableaus dopri5 / bosh3 (as
+ * tdq_linear_attempt_supported).  Null pointers, n_rows 0 and an unsupported dtype, width or tableau are refused before the
+ * device is touched. */
+int tdq_linear_rows_attempt_supported(const tdq_tableau *tab, int32_t dtype, int32_t width);
+int tdq_linear_rows_attempt(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, void *const *k_out,
+                            void *y1_out, void *err_out, const void *planes, int32_t width, size_t n_rows,
+                            double *norm_out, int32_t store_always, void *stream);
+
 /* ---- A WHOLE fused solve in one launch (tdq_attempt.cu) ---------------------------------------------------------------------
  * Every attempt of a solve whose attempts tdq_linear_attempt can run with the norm folded in (partials given, scalar tolerances,
  * one segment), with the controller step and the lazy interpolant fit in between: what the loop

@@ -995,6 +995,14 @@ class AdaptiveEngine:
         self._launch(self.lib.tdq_set_first_step(self.ctrl.data_ptr(), dt, _stream()))
 
 
+def rows_linear_attempt_ok(*, whole_attempt, supported, width, row_len, vector_tol, row_segs, compact):
+    """Whether an independent-row solve of a LinearField runs each attempt as one tdq_linear_rows_attempt launch: the
+    whole-attempt kernel takes the method (supported) and rows of exactly one field width, with scalar tolerances.  Not for
+    odeint_adjoint's backward (row_segs: a seminorm over segments of a longer row) nor row compaction (func sees fewer
+    rows than the kernels)."""
+    return bool(whole_attempt and supported and row_len == width and not vector_tol and row_segs is None and not compact)
+
+
 def bisect_iterations(lo, hi, tol):
     """event_handling.py:13 per row: ceil(log((hi - lo) / tol) / log 2) in float64 on the CPU, as the reference computes
     it.  The vectorised log may differ from the scalar one the reference runs on a 0-dim tensor in the last bit, which
@@ -1025,7 +1033,11 @@ class RowsEngine(AdaptiveEngine):
 
     row_segs (odeint_adjoint's backward): [(offset, len), ...] within a row.  Each row's error ratio and initial-step norms
     are then the max over these segments of each one's RMS (the seminorm), elements outside them enter no norm, and the
-    candidate commit writes only segment elements.  Scalar tolerances only."""
+    candidate commit writes only segment elements.  Scalar tolerances only.
+
+    set_linear (func a LinearField on rows of 128 float32 elements, dopri5 / bosh3): every attempt's stages, field
+    evaluations, error norms and commits are one tdq_linear_rows_attempt launch (csrc/tdq_attempt.cu), and f0 and the
+    initial-step probe are tdq_linear_apply, so the whole solve uses the tensor-core product."""
 
     def __init__(self, fn, shape, dtype, device, method, compact_fn=None, row_segs=None, **kw):
         shape = torch.Size(shape)
@@ -1077,6 +1089,22 @@ class RowsEngine(AdaptiveEngine):
             self.sizes = _compact.bucket_sizes(B)
             self._idx = {B: torch.arange(B, dtype=torch.int64, device=device)}   # per size: the static index list
             self._cbuf = {}              # per size: compact (y, t, event t) buffers
+
+    def set_linear(self, weight, whole_attempt=True):
+        """Run every attempt as one tdq_linear_rows_attempt launch with func = y @ weight^T (rows_linear_attempt_ok).
+        Returns False (and changes nothing) where the generic row path runs instead; there is no per-stage fused row path."""
+        width = int(weight.shape[0])
+        if not rows_linear_attempt_ok(
+                whole_attempt=whole_attempt, width=width, row_len=self.D, vector_tol=self.rtol_vec is not None,
+                row_segs=self.row_segs, compact=self.compact_fn is not None,
+                supported=self.lib.tdq_linear_rows_attempt_supported(C.byref(self.tab), self.dt_code, width)):
+            return False
+        planes = torch.empty(int(self.lib.tdq_linear_weights_bytes(width)), dtype=torch.uint8, device=self.device)
+        # fold=False: the row attempt hands its per-row sums to the row controller, there is no persistent row solve
+        self.linear = dict(weight=weight, width=width, planes=planes, whole=True, fold=False,
+                           k=[torch.zeros(self.n, dtype=self.dtype, device=self.device) for _ in range(self.S)])
+        self._drop_graph()
+        return True
 
     def solve(self, y0_flat, t64, t_start=None, grid=None):
         """AdaptiveEngine.solve, or with `grid` (an ascending float64 [B, T] device tensor) per-row output times: row r
@@ -1237,7 +1265,18 @@ class RowsEngine(AdaptiveEngine):
         S, B, D = self.S, self.B, self.D
         k = [None] * (S + 1)             # k[0] = NULL: each row's k_0 (and y0) comes from its half of the pointer table
         keep = []
-        for i in range(S):
+        if self.linear is not None:
+            # the whole attempt of every row in one wgmma launch (csrc/tdq_attempt.cu k_linear_rows_attempt): stages, error
+            # sums and commits; a row's stages, y1 and error prefix reach memory only when its step can emit an output, or
+            # always in an event solve (the event function reads y1, tdq_rows_fit_store the stages)
+            L = self.linear
+            for i in range(S):
+                k[i + 1] = L["k"][i].data_ptr()
+            self._launch(lib.tdq_linear_rows_attempt(ctrl, rows, tab, dc, _lib.ptr_array(k), self.y1.data_ptr(),
+                                                     self.errp.data_ptr(), L["planes"].data_ptr(), L["width"], B,
+                                                     self.row_norm.data_ptr(), 0 if self.ev_fn is None else 1, st))
+            self.nfe += S
+        for i in range(S if self.linear is None else 0):
             if i == S - 1 and self.fsal:
                 out = self.y1
                 self._launch(lib.tdq_rows_combine_final(ctrl, rows, tab, dc, out.data_ptr(), self.errp.data_ptr(),
@@ -1261,11 +1300,12 @@ class RowsEngine(AdaptiveEngine):
             if self.after_control is not None:
                 keep.append(self.after_control())
             return k, kp, keep
-        self._launch(lib.tdq_rows_error_norm_commit(
-            ctrl, rows, dc, self.errp.data_ptr(), k[S], self.y1.data_ptr(),
-            self.rtol_vec.data_ptr() if self.rtol_vec is not None else None,
-            self.atol_vec.data_ptr() if self.atol_vec is not None else None,
-            B, D, self.row_partials.data_ptr(), self.row_norm.data_ptr(), st))
+        if self.linear is None:
+            self._launch(lib.tdq_rows_error_norm_commit(
+                ctrl, rows, dc, self.errp.data_ptr(), k[S], self.y1.data_ptr(),
+                self.rtol_vec.data_ptr() if self.rtol_vec is not None else None,
+                self.atol_vec.data_ptr() if self.atol_vec is not None else None,
+                B, D, self.row_partials.data_ptr(), self.row_norm.data_ptr(), st))
         if self.ev_fn is None:
             self._launch(lib.tdq_rows_controller(ctrl, rows, dc, self.row_norm.data_ptr(), B, D, st))
         else:
@@ -1405,7 +1445,10 @@ class RowsEngine(AdaptiveEngine):
             self._launch(lib.tdq_rows_init_grid(ctrl, rows, dc, B, self.grid.data_ptr(), n_out, st))
         else:
             self._launch(lib.tdq_rows_init(ctrl, rows, dc, B, t_start, st))
-        f0 = self._call_fn(self.t_first, self.ybuf[0], 0, dst=self.kbuf[0])
+        if self.linear is not None:                                   # the weight may have changed since the last solve
+            L = self.linear
+            self._launch(lib.tdq_linear_prepare(dc, L["weight"].data_ptr(), L["width"], L["planes"].data_ptr(), st))
+        f0 = self._eval(self.t_first, self.ybuf[0], 0, dst=self.kbuf[0])
         if f0.data_ptr() != self.kbuf[0].data_ptr():
             self.kbuf[0].copy_(f0)
         del f0
@@ -1419,7 +1462,7 @@ class RowsEngine(AdaptiveEngine):
             else:
                 self._launch(lib.tdq_rows_initial_h0(ctrl, rows, dc, d[0].data_ptr(), d[1].data_ptr(), B, D, st))
             self._launch(lib.tdq_rows_initial_probe(ctrl, rows, dc, self.ytmp.data_ptr(), B, D, st))
-            f1 = self._call_fn(self.t_probe, self.ytmp, 1)
+            f1 = self._eval(self.t_probe, self.ytmp, 1)
             self._rows_sumsq(f1, self.kbuf[0], d[2])
             del f1
             if self.row_segs is not None:

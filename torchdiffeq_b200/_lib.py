@@ -155,6 +155,8 @@ _SIGNATURES = {
                                            _vp]),
     "tdq_linear_attempt_supported": (C.c_int, [_ptab, _i32, _i32]),
     "tdq_linear_attempt": (C.c_int, [_vp, _ptab, _i32, _pp, _vp, _vp, _vp, _vp, _vp, _i32, _sz, _vp, _vp, _vp, _i32, _vp]),
+    "tdq_linear_rows_attempt_supported": (C.c_int, [_ptab, _i32, _i32]),
+    "tdq_linear_rows_attempt": (C.c_int, [_vp, _vp, _ptab, _i32, _pp, _vp, _vp, _vp, _i32, _sz, _vp, _i32, _vp]),
     "tdq_linear_solve_scratch_len": (_sz, []),
     "tdq_linear_solve": (C.c_int, [_vp, _ptab, _i32, _pp, _vp, _vp, _vp, _i32, _sz, _vp, _sz, _vp, _vp, _vp]),
     "tdq_fixed_emit_cubic": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _sz, _vp]),

@@ -32,10 +32,16 @@
 //
 // Stage derivatives, y1 and the error prefix are written to HBM only for attempts that can contain an output time (the
 // lazy interpolant fit needs them, tdq_interp.cu) or when the caller keeps every step (dense output, events).
+//
+// k_linear_rows_attempt runs the same tile code for an independent-row solve (tdq_rows.cu), where every row has its own
+// step: the coefficients come from a per-tile [row][slot] table formed from each row's dt, each row reads its pair and
+// commits its candidate by its own parity, each row's squared error sum is reduced inside the tile in k_rows_norm's order,
+// and a tile whose rows are all done is skipped.
 #include "tdq_shape.cuh"
 #include "tdq_tc.cuh"
 #include "tdq_ctrl_step.cuh"
 #include "tdq_fit.cuh"
+#include "tdq_step.cuh"
 
 #include <cstddef>
 #include <type_traits>
@@ -62,6 +68,15 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
     float v;
     asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
     return v;
+}
+
+__device__ __forceinline__ int lds_s32(uint32_t addr) {
+    int v;
+    asm volatile("ld.shared.s32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void atoms_add_s32(uint32_t addr, int v) {
+    asm volatile("red.shared.add.s32 [%0], %1;" :: "r"(addr), "r"(v) : "memory");
 }
 
 __device__ __forceinline__ uint64_t lds_u64(uint32_t addr) {
@@ -103,13 +118,38 @@ constexpr int AUX_CR = 64;                     // float s_cr[AT_MAX_S][8], s_ce[
 constexpr int AUX_SC = 320;                    // Scalars
 constexpr int AUX_RED = 512;                   // double [2][32]: reduction scratch
 constexpr int AUX_SOLVE = 1024;                // k_linear_solve's words (SolveAux)
+constexpr int AUX_ROWS = AUX_SOLVE;            // k_linear_rows_attempt's words (RowPtrs): that kernel runs no solve
 static_assert(AUX_SC + sizeof(Scalars) <= AUX_RED, "aux layout");
+
+// ---- independent rows (k_linear_rows_attempt) ----
+// What a row attempt reads of the row buffer (tdq_rows.cu, include/tdq.h TDQ_ROWS_*): field pointers of B entries each.
+struct RowArgs {
+    const TdqCtrl *c;
+    const int *done, *par, *cursor;
+    const double *att_dt, *att_t1;
+    double *norm_out;                          // [2 B]: squared error sums, then non-finite y1 counts
+    int store_always;
+};
+struct RowPtrs {                               // the pointer table's two pairs, in the aux area at AUX_ROWS
+    float *yb[2], *kb[2];
+};
+static_assert(AUX_ROWS + sizeof(RowPtrs) <= AT_AUX, "aux layout");
+// Per-tile row table after the aux area: row rr of the tile at RT_STRIDE rr, its coefficients at slot 8 i + j (i = AT_MAX_S:
+// the error weights, as s_cr / s_ce), then its flags (bit 0 running, bit 1 stages stored), parity and non-finite y1 count.
+// 68 words per row: the four rows a warp reads at once (2 (lane & 3)) fall into four different bank octets.
+constexpr int RT_FLAG = 64, RT_PAR = 65, RT_BAD = 66;
+constexpr int RT_STRIDE = 68 * 4;
+constexpr int RT_BYTES = AT_ROWS * RT_STRIDE;
+constexpr int SQ_BYTES = AT_ROWS * LD * 4;     // the tile's (err/tol)^2 in the state layout, for the per-row sums
+constexpr int RW_SMEM = AT_SMEM + RT_BYTES + SQ_BYTES;
 
 __device__ __forceinline__ uint8_t *at_smem() {
     extern __shared__ uint8_t smem_raw[];
     return reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
 }
 __device__ __forceinline__ uint8_t *at_aux(uint8_t *smem) { return smem + AT_W + AT_STAGE + AT_Y0 + AT_MAX_KEEP * AT_Y0; }
+constexpr int RT_OFF = AT_W + AT_STAGE + AT_Y0 + AT_MAX_KEEP * AT_Y0 + AT_AUX;   // the row table (k_linear_rows_attempt)
+constexpr int SQ_OFF = RT_OFF + RT_BYTES;
 
 // This attempt's coefficients (prepare_tables) as float32, laid out by slot: the coefficient of k_j in row i at s_cr[8 i + j],
 // the error weight of k_j at s_ce[j] (j = 0..S), zero where the tableau has none.  Every index the tile loop uses is then a
@@ -154,6 +194,74 @@ __device__ __forceinline__ bool attempt_store(const TdqCtrl *c, int store_always
     return store;
 }
 
+// Rows: the table of tile rows [row0, row0 + 32) -- each row's coefficients fl_T(t_sign * fl_T(w * T(dt_r))) as k_rows_combine,
+// k_rows_combine_final and k_rows_norm form them (tdq_coef), its flags and parity -- and zero norm entries for the rows of
+// the tile that do not run.  A row runs when it exists and is not done; its stages are stored when its candidate step can
+// emit an output (`!(t_out[cursor] > ATT_T1)` on the row's own times, as the controller tests it), the control block keeps
+// every step, or store_always.  Returns, block-wide, whether any row of the tile runs.  The caller has synchronised the
+// block since the previous tile's last read of the table.
+template <int S, unsigned long long RM, unsigned EM>
+__device__ __forceinline__ bool rows_tile_setup(uint8_t *smem, const RowArgs &ra, int row0, int n_rows, int tid) {
+    const TdqCtrl *c = ra.c;
+    const int rr = tid & 31, r = row0 + rr, i = tid >> 5;                 // i = AT_MAX_S: the error weights
+    const bool in = r < n_rows;
+    const float dtT = in ? (float)ra.att_dt[r] : 0.f, sgn = (float)c->t_sign;
+    float *row = reinterpret_cast<float *>(smem + RT_OFF + rr * RT_STRIDE);
+    const unsigned mask = i < S ? (unsigned)((RM >> (8 * i)) & 0xffull) : 0u;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const unsigned below = (1u << j) - 1u;
+        float v = 0.f;
+        if ((mask >> j) & 1u) v = tdq_coef<float>(sgn, (float)c->beta[i][__popc(mask & below)], dtT);
+        if (i == AT_MAX_S && (j == S || ((EM >> j) & 1u)))
+            v = tdq_coef<float>(sgn, (float)c->c_err[j == S ? __popc(EM) : __popc(EM & below)], dtT);
+        row[8 * i + j] = v;
+    }
+    int run = 0;
+    if (tid < AT_ROWS) {
+        int *w = reinterpret_cast<int *>(row);
+        run = in && !ra.done[r];
+        bool keep = false;
+        if (run) {
+            keep = ra.store_always != 0 || c->always_fit != 0;
+            if (!keep) {
+                const RowTimes times = row_times(*c, r);
+                const int cur = ra.cursor[r];
+                keep = cur < times.n && !(times.t[cur] > ra.att_t1[r]);
+            }
+        }
+        w[RT_FLAG] = (run ? 1 : 0) | (keep ? 2 : 0);
+        w[RT_PAR] = in ? ra.par[r] : 0;
+        w[RT_BAD] = 0;
+        if (in && !run) {
+            ra.norm_out[r] = 0.0;
+            ra.norm_out[n_rows + r] = 0.0;
+        }
+    }
+    return __syncthreads_or(run) != 0;
+}
+
+// Rows: each running row's squared error sum from the tile's (err/tol)^2 in shared memory, in k_rows_norm's order for
+// D = 128 (lane l adds elements l, l + 32, l + 64, l + 96, then warp_sum), and its non-finite y1 count; warp w takes tile
+// rows 4 w .. 4 w + 3.  The caller has synchronised the block after the last (err/tol)^2 store.
+__device__ __forceinline__ void rows_tile_norm(uint8_t *smem, const RowArgs &ra, int row0, int n_rows, int tid) {
+    const int lane = tid & 31, warp = tid >> 5;
+    const uint32_t rt = smem_u32(smem) + RT_OFF, sq = smem_u32(smem) + SQ_OFF;
+#pragma unroll
+    for (int q = 0; q < AT_ROWS / (AT_THREADS / 32); ++q) {
+        const int rr = (AT_ROWS / (AT_THREADS / 32)) * warp + q;
+        if (!(lds_s32(rt + rr * RT_STRIDE + 4 * RT_FLAG) & 1)) continue;
+        double a = 0.0;
+#pragma unroll
+        for (int m = 0; m < LD / 32; ++m) a += (double)lds_f32(sq + 4 * (rr * LD + lane + 32 * m));
+        a = warp_sum(a);
+        if (lane == 0) {
+            ra.norm_out[row0 + rr] = a;
+            ra.norm_out[n_rows + row0 + rr] = (double)lds_s32(rt + rr * RT_STRIDE + 4 * RT_BAD);
+        }
+    }
+}
+
 // the hi and mid weight planes of the warpgroup's features as the register A operand of every hi.* and mid.* product
 // (plane p, k-step ks: afr[p][ks]), read from the global weight image (tdq_tc.cuh's layout, L2-resident after the first CTAs)
 __device__ __forceinline__ void load_afrag(AFrag (&afr)[AT_NR], const uint32_t *__restrict__ wt) {
@@ -174,9 +282,11 @@ __device__ __forceinline__ void load_afrag(AFrag (&afr)[AT_NR], const uint32_t *
 
 // This CTA's tiles of one attempt (tiles blockIdx.x, blockIdx.x + gridDim.x, ...) through all S stages.  tid = threadIdx.x.
 // acc / nbad: this thread's share of the squared error norm (fold) and of the non-finite y1 count.
-template <int S, unsigned long long RM, unsigned EM>
+// ROWS (k_linear_rows_attempt, ra given): every coefficient, predicate, pair and commit is the element's own row's (the
+// row table, rows_tile_setup), store and fold are not read, and each running row's sums go to ra->norm_out.
+template <int S, unsigned long long RM, unsigned EM, bool ROWS = false>
 __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const AFrag (&afr)[AT_NR], bool store, bool fold, int n_rows,
-                                              int tid, double &acc, int &nbad) {
+                                              int tid, double &acc, int &nbad, const RowArgs *ra = nullptr) {
     const int lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);                  // warp-uniform for the compiler as well
     // h = the warpgroup's half of the output features; w = warp inside the warpgroup
@@ -186,6 +296,17 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const AFrag (&afr)[
     const uint32_t scoef = wsm + (uint32_t)(at_aux(smem) - smem) + AUX_CR;
     // the coefficient of k_j in row i (i = AT_MAX_S: the error weights); i and j are compile-time constants at every use
     auto coef = [scoef](int i, int j) { return lds_pinned_f32(scoef + 4 * (8 * i + j)); };
+    // ROWS: the table entries of element e's row.  The thread's 8 rows are 2 (lane & 3) + a constant of e (elem_row), so
+    // every address is one base register plus an immediate.
+    const uint32_t rtab = ROWS ? wsm + RT_OFF + 2 * (lane & 3) * RT_STRIDE : 0u;
+    const uint32_t srp = wsm + (uint32_t)(at_aux(smem) - smem) + AUX_ROWS;
+    auto rrow = [](int e) { return (uint32_t)((8 * ((e >> 2) & 3) + (e & 1)) * RT_STRIDE); };
+    auto rcoef = [rtab, rrow](int i, int j, int e) { return lds_pinned_f32(rtab + rrow(e) + 4 * (8 * i + j)); };
+    auto rflag = [rtab, rrow](int e) { return lds_s32(rtab + rrow(e) + 4 * RT_FLAG); };
+    auto rpar = [rtab, rrow](int e) { return lds_s32(rtab + rrow(e) + 4 * RT_PAR); };
+    auto rpair = [srp](bool k, int p) {                                    // ybuf[p] / kbuf[p]
+        return reinterpret_cast<float *>(lds_u64(srp + offsetof(RowPtrs, yb) + (k ? 16 : 0) + 8 * p));
+    };
     const uint32_t wsm_h = wsm + h * 8 * SBO;                             // the lo weight rows of features [64 h, 64 h + 64)
     const uint32_t stage = wsm + AT_W;
     const uint32_t sy0 = stage + AT_STAGE + tid * 4;                      // element e at sy0 + 1024 e: this thread's only
@@ -220,7 +341,23 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const AFrag (&afr)[
         const size_t base = (size_t)row0 * LD + toff;
         float A[NACC > 0 ? NACC : 1][16];                             // A[q - KEEP]: running sum of row q
         float AE[16], PRE[16], KN[16], Y1[16];
-        {
+        if constexpr (ROWS) {
+            // each running row's pair ybuf / kbuf[PAR[r]]
+            float Y0[16];
+#pragma unroll
+            for (int e = 0; e < 16; ++e) {
+                Y0[e] = 0.f;
+                KN[e] = 0.f;
+                if (rflag(e) & 1) {
+                    const int p = rpar(e);
+                    const size_t o = base + elem_offset<AT_ROWS>(e);
+                    Y0[e] = __ldcs(rpair(false, p) + o);
+                    KN[e] = __ldcs(rpair(true, p) + o);
+                }
+            }
+#pragma unroll
+            for (int e = 0; e < 16; ++e) sts_f32(sy0 + e * 1024, Y0[e]);
+        } else {
             const float *y0 = reinterpret_cast<const float *>(lds_u64(ssc + offsetof(Scalars, y0)));
             const float *k0 = reinterpret_cast<const float *>(lds_u64(ssc + offsetof(Scalars, k0)));
             float Y0[16];
@@ -241,7 +378,7 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const AFrag (&afr)[
             const unsigned mask = row_mask(i);
             const bool last = i == S - 1;
             const bool has_prefix = (mask & ((1u << i) - 1u)) != 0u, has_new = ((mask >> i) & 1u) != 0u;
-            const float c_new = has_new ? coef(i, i) : 0.f;
+            const float c_new = (has_new && !ROWS) ? coef(i, i) : 0.f;
             if (i < KEEP - 1) {
 #pragma unroll
                 for (int e = 0; e < 16; ++e) sts_f32(kept(i, e), KN[e]);
@@ -252,10 +389,11 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const AFrag (&afr)[
 #pragma unroll
                 for (int e = 0; e < 16; ++e) {
                     const float pre = i < KEEP ? PRE[e] : A[i >= KEEP ? i - KEEP : 0][e];
+                    const float cn = ROWS && has_new ? rcoef(i, i, e) : c_new;
                     float sum;
-                    if (has_prefix && has_new) sum = pre + KN[e] * c_new;
+                    if (has_prefix && has_new) sum = pre + KN[e] * cn;
                     else if (has_prefix) sum = pre;
-                    else sum = KN[e] * c_new;
+                    else sum = KN[e] * cn;
                     yv[e] = lds_f32(sy0 + e * 1024) + sum;
                     if (last) Y1[e] = yv[e];
                 }
@@ -276,10 +414,10 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const AFrag (&afr)[
 #pragma unroll
                 for (int j = 0; j <= i; ++j) {
                     if ((mn >> j) & 1u) {
-                        const float cj = coef(i + 1, j);
+                        const float cj = ROWS ? 0.f : coef(i + 1, j);
 #pragma unroll
                         for (int e = 0; e < 16; ++e) {
-                            const float p = (j == i ? KN[e] : lds_f32(kept(j, e))) * cj;
+                            const float p = (j == i ? KN[e] : lds_f32(kept(j, e))) * (ROWS ? rcoef(i + 1, j, e) : cj);
                             PRE[e] = first ? p : PRE[e] + p;
                         }
                         first = false;
@@ -290,9 +428,10 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const AFrag (&afr)[
             if (i == KEEP - 1) {
                 // every kept slot is known: the remaining rows and the error estimate become running sums (element by element,
                 // so that the kept slots die as the sums are born); their coefficients are loaded once, before the element loop
+                // (ROWS: the element's own row's, loaded at the product)
                 float cq[NACC > 0 ? NACC : 1][KEEP], ce[KEEP];
 #pragma unroll
-                for (int j = 0; j < KEEP; ++j) {
+                for (int j = 0; j < KEEP && !ROWS; ++j) {
 #pragma unroll
                     for (int qrow = KEEP; qrow < S; ++qrow)
                         if ((row_mask(qrow) >> j) & 1u) cq[qrow - KEEP][j] = coef(qrow, j);
@@ -308,7 +447,8 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const AFrag (&afr)[
 #pragma unroll
                         for (int j = 0; j <= i; ++j) {
                             if ((mq >> j) & 1u) {
-                                const float p = (j == i ? KN[e] : lds_f32(kept(j, e))) * cq[qrow - KEEP][j];
+                                const float p = (j == i ? KN[e] : lds_f32(kept(j, e))) *
+                                                (ROWS ? rcoef(qrow, j, e) : cq[qrow - KEEP][j]);
                                 a_ = first ? p : a_ + p;
                                 first = false;
                             }
@@ -320,7 +460,7 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const AFrag (&afr)[
 #pragma unroll
                     for (int j = 0; j <= i; ++j) {
                         if ((EM >> j) & 1u) {
-                            const float p = (j == i ? KN[e] : lds_f32(kept(j, e))) * ce[j];
+                            const float p = (j == i ? KN[e] : lds_f32(kept(j, e))) * (ROWS ? rcoef(AT_MAX_S, j, e) : ce[j]);
                             e_ = first ? p : e_ + p;
                             first = false;
                         }
@@ -337,21 +477,21 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const AFrag (&afr)[
                 for (int qrow = i + 1; qrow < S; ++qrow) {
                     const unsigned mq = row_mask(qrow);
                     if ((mq >> i) & 1u) {
-                        const float cj = coef(qrow, i);
+                        const float cj = ROWS ? 0.f : coef(qrow, i);
                         const bool started = (mq & ((1u << i) - 1u)) != 0u;
 #pragma unroll
                         for (int e = 0; e < 16; ++e) {
-                            const float p = KN[e] * cj;
+                            const float p = KN[e] * (ROWS ? rcoef(qrow, i, e) : cj);
                             A[qrow - KEEP][e] = started ? A[qrow - KEEP][e] + p : p;
                         }
                     }
                 }
                 if ((EM >> i) & 1u) {
-                    const float cj = coef(AT_MAX_S, i);
+                    const float cj = ROWS ? 0.f : coef(AT_MAX_S, i);
                     const bool started = (EM & ((1u << i) - 1u)) != 0u;
 #pragma unroll
                     for (int e = 0; e < 16; ++e) {
-                        const float p = KN[e] * cj;
+                        const float p = KN[e] * (ROWS ? rcoef(AT_MAX_S, i, e) : cj);
                         AE[e] = started ? AE[e] + p : p;
                     }
                 }
@@ -362,12 +502,24 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const AFrag (&afr)[
             if (last) {
                 // y1: non-finite count, candidate commit, (optional) y1 and the error prefix; tol = atol + rtol * max(|y0|, |y1|)
                 // (misc.py:81) replaces y1 in its registers
-                float *ycand = reinterpret_cast<float *>(lds_u64(ssc + offsetof(Scalars, ycand)));
+                // (ROWS: a running row's count in its table entry, its commit to ybuf[PAR[r] ^ 1], k_rows_norm MODE 0's)
+                [[maybe_unused]] float *ycand = ROWS ? nullptr : reinterpret_cast<float *>(lds_u64(ssc + offsetof(Scalars, ycand)));
                 const float rtolT = lds_f32(ssc + offsetof(Scalars, rtol)), atolT = lds_f32(ssc + offsetof(Scalars, atol));
 #pragma unroll
                 for (int e = 0; e < 16; ++e) {
                     const float y1v = Y1[e];
-                    if (FULL || elem_row<AT_ROWS>(e, lane) < rows_here) {
+                    if constexpr (ROWS) {
+                        const int fl = rflag(e);
+                        if (fl & 1) {
+                            if (!isfinite(y1v)) atoms_add_s32(rtab + rrow(e) + 4 * RT_BAD, 1);
+                            const size_t o = base + elem_offset<AT_ROWS>(e);
+                            rpair(false, rpar(e) ^ 1)[o] = y1v;
+                            if (fl & 2) {
+                                reinterpret_cast<float *>(lds_u64(ssc + offsetof(Scalars, out.y1)))[o] = y1v;
+                                reinterpret_cast<float *>(lds_u64(ssc + offsetof(Scalars, out.err)))[o] = AE[e];
+                            }
+                        }
+                    } else if (FULL || elem_row<AT_ROWS>(e, lane) < rows_here) {
                         if (!isfinite(y1v)) nbad += 1;
                         const size_t o = base + elem_offset<AT_ROWS>(e);
                         if (ycand) ycand[o] = y1v;
@@ -382,13 +534,31 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const AFrag (&afr)[
             }
             wgmma_wait();
             tile_result(tacc, KN);
-            if (store) {
+            if constexpr (ROWS) {
+                float *ko = held(reinterpret_cast<float *>(lds_u64(ssc + offsetof(Scalars, out.k) + 8 * (i + 1))) + base);
+#pragma unroll
+                for (int e = 0; e < 16; ++e)
+                    if (rflag(e) & 2) ko[elem_offset<AT_ROWS>(e)] = KN[e];
+            } else if (store) {
                 float *ko = held(reinterpret_cast<float *>(lds_u64(ssc + offsetof(Scalars, out.k) + 8 * (i + 1))) + base);
 #pragma unroll
                 for (int e = 0; e < 16; ++e)
                     if (FULL || elem_row<AT_ROWS>(e, lane) < rows_here) ko[elem_offset<AT_ROWS>(e)] = KN[e];
             }
-            if (last) {
+            if (ROWS && last) {
+                // ---- k_S: a running row's commit to kbuf[PAR[r] ^ 1], its (err/tol)^2 into the tile's staging area ----
+                const uint32_t sq = wsm + SQ_OFF + 4 * toff;                  // element e at sq + 4 elem_offset(e)
+#pragma unroll
+                for (int e = 0; e < 16; ++e) {
+                    if (rflag(e) & 1) {
+                        rpair(true, rpar(e) ^ 1)[base + elem_offset<AT_ROWS>(e)] = KN[e];
+                        const float num = Ar<float>::add(AE[e], Ar<float>::mul(KN[e], rcoef(AT_MAX_S, S, e)));
+                        const float q = Ar<float>::div(num, Y1[e]);
+                        sts_f32(sq + 4 * elem_offset<AT_ROWS>(e), Ar<float>::mul(q, q));
+                    }
+                }
+            }
+            if (!ROWS && last) {
                 // ---- k_S: candidate commit, error ratio (misc.py:80-82 up to the mean) ----
                 float *kcand = reinterpret_cast<float *>(lds_u64(ssc + offsetof(Scalars, kcand)));
                 const float ecS = coef(AT_MAX_S, S);
@@ -408,20 +578,30 @@ __device__ __forceinline__ void attempt_tiles(uint8_t *smem, const AFrag (&afr)[
     };
 #pragma unroll 1
     for (int t = (int)blockIdx.x; t < tiles; t += (int)gridDim.x) {
-        {   // the next tile's y0 / k_0 rows of this warp towards L2: lane = row (the warp's 16 features of a row are 64
-            // contiguous bytes)
-            const int tn = t + (int)gridDim.x;
-            const long long prow = (long long)tn * AT_ROWS + lane;
-            if (tn < tiles && prow < (long long)n_rows) {
-                const float *y0 = reinterpret_cast<const float *>(lds_u64(ssc + offsetof(Scalars, y0)));
-                const float *k0 = reinterpret_cast<const float *>(lds_u64(ssc + offsetof(Scalars, k0)));
-                const size_t o = (size_t)prow * LD + 64 * h + 16 * w;
-                asm volatile("prefetch.global.L2 [%0];" :: "l"(y0 + o));
-                asm volatile("prefetch.global.L2 [%0];" :: "l"(k0 + o));
+        if constexpr (ROWS) {
+            // every element takes the predicated copy; a tile whose rows are all done costs its table and nothing else
+            __syncthreads();                                              // the previous tile's table and sums are read
+            if (rows_tile_setup<S, RM, EM>(smem, *ra, t * AT_ROWS, n_rows, tid)) {
+                do_tile(std::false_type{}, t);
+                __syncthreads();                                          // every (err/tol)^2 of the tile is stored
+                rows_tile_norm(smem, *ra, t * AT_ROWS, n_rows, tid);
             }
+        } else {
+            {   // the next tile's y0 / k_0 rows of this warp towards L2: lane = row (the warp's 16 features of a row are 64
+                // contiguous bytes)
+                const int tn = t + (int)gridDim.x;
+                const long long prow = (long long)tn * AT_ROWS + lane;
+                if (tn < tiles && prow < (long long)n_rows) {
+                    const float *y0 = reinterpret_cast<const float *>(lds_u64(ssc + offsetof(Scalars, y0)));
+                    const float *k0 = reinterpret_cast<const float *>(lds_u64(ssc + offsetof(Scalars, k0)));
+                    const size_t o = (size_t)prow * LD + 64 * h + 16 * w;
+                    asm volatile("prefetch.global.L2 [%0];" :: "l"(y0 + o));
+                    asm volatile("prefetch.global.L2 [%0];" :: "l"(k0 + o));
+                }
+            }
+            if (n_rows - t * AT_ROWS >= AT_ROWS) do_tile(std::true_type{}, t);
+            else do_tile(std::false_type{}, t);
         }
-        if (n_rows - t * AT_ROWS >= AT_ROWS) do_tile(std::true_type{}, t);
-        else do_tile(std::false_type{}, t);
     }
 }
 
@@ -507,6 +687,42 @@ k_linear_attempt(TdqCtrl *c, const float *y0, const float *k0, AttOut out, const
             *ticket = 0;                                                  // self-reset for the next launch
         }
     }
+}
+
+// ---- a whole attempt of an independent-row solve -----------------------------------------------------------------------
+// What S x (k_rows_combine[_final] + the field) + k_rows_norm MODE 0 do for every row, in one launch: the tile code above
+// with each row's own coefficients, pair and commit, and each running row's squared error sum and non-finite y1 count in
+// ra.norm_out (done rows: 0 and 0).  The row controller is the caller's next launch.
+template <int S, unsigned long long RM, unsigned EM>
+__global__ void __launch_bounds__(AT_THREADS, 1)
+k_linear_rows_attempt(TdqCtrl *c, RowArgs ra, AttOut out, const uint32_t *__restrict__ wt, size_t n_rows_sz) {
+    if (c->halt) return;                                  // an attempt issued after the end of the solve is a no-op
+    uint8_t *smem = at_smem();
+    uint8_t *aux = at_aux(smem);
+    const int tid = threadIdx.x;
+    if (tid == 0) {
+        Scalars sc;
+        sc.y0 = sc.k0 = nullptr;
+        sc.ycand = sc.kcand = nullptr;
+        sc.out = out;
+        sc.rtol = (float)c->rtol;
+        sc.atol = (float)c->atol;
+        *reinterpret_cast<Scalars *>(aux + AUX_SC) = sc;
+        RowPtrs rp;
+        for (int p = 0; p < 2; ++p) {
+            rp.yb[p] = tdq_detach(reinterpret_cast<float *>(c->ybuf[p]), n_rows_sz);
+            rp.kb[p] = tdq_detach(reinterpret_cast<float *>(c->kbuf[p]), n_rows_sz);
+        }
+        *reinterpret_cast<RowPtrs *>(aux + AUX_ROWS) = rp;
+    }
+    load_weights(smem, wt, tid, AT_THREADS, AT_NR);
+    fence_async_smem();
+    AFrag afr[AT_NR];
+    load_afrag(afr, wt);
+    __syncthreads();
+    double acc = 0.0;
+    int nbad = 0;
+    attempt_tiles<S, RM, EM, true>(smem, afr, true, true, (int)n_rows_sz, tid, acc, nbad, &ra);
 }
 
 // ---- a whole fused solve in one launch ---------------------------------------------------------------------------------
@@ -703,6 +919,14 @@ int launch_attempt(TdqCtrl *c, const float *y0, const float *k0, const AttOut &o
     return 0;
 }
 
+template <int S, unsigned long long RM, unsigned EM>
+int launch_rows_attempt(TdqCtrl *c, const RowArgs &ra, const AttOut &out, const uint32_t *wt, size_t n_rows, cudaStream_t st) {
+    auto kern = k_linear_rows_attempt<S, RM, EM>;
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, RW_SMEM) != cudaSuccess) return -2;
+    kern<<<tdq_grid(n_rows, AT_ROWS, 1), AT_THREADS, RW_SMEM, st>>>(c, ra, out, wt, n_rows);
+    return 0;
+}
+
 // Cooperative launch: every CTA must be resident at once for the grid barrier, or the launch is refused (-3).
 template <int S, unsigned long long RM, unsigned EM, int NK>
 int launch_solve(TdqCtrl *c, const AttOut &out, const uint32_t *wt, unsigned *bar, double *part, const int64_t *cnt,
@@ -798,6 +1022,50 @@ int tdq_linear_attempt(void *ctrl_dev, const tdq_tableau *tab, int32_t dtype, vo
     else if (S == 3 && rm == RM_BOSH3 && em == 0x07u)
         rc = launch_attempt<3, RM_BOSH3, 0x07u>(c, (const float *)y0, (const float *)k0, out, wt, partials, norm_out, store_always, n_rows, st);
     TDQ_REQUIRE(rc != -1, "no whole-attempt kernel for this tableau (tdq_linear_attempt_supported)");
+    TDQ_REQUIRE(rc == 0, "launch configuration failed");
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+int tdq_linear_rows_attempt_supported(const tdq_tableau *tab, int32_t dtype, int32_t width) {
+    return tdq_linear_attempt_supported(tab, dtype, width);
+}
+
+int tdq_linear_rows_attempt(void *ctrl_dev, void *rows_dev, const tdq_tableau *tab, int32_t dtype, void *const *k_out,
+                            void *y1_out, void *err_out, const void *planes, int32_t width, size_t n_rows,
+                            double *norm_out, int32_t store_always, void *stream) {
+    TDQ_REQUIRE(ctrl_dev && rows_dev && tab && k_out && y1_out && err_out && planes && norm_out, "null argument");
+    TDQ_REQUIRE(dtype == TDQ_F32 && width == LD, "the fused linear field is float32, width 128");
+    TDQ_REQUIRE(n_rows > 0 && n_rows < ((size_t)1 << 31) - 64, "n_rows out of range");
+    TDQ_REQUIRE(tdq_linear_attempt_supported(tab, dtype, width),
+                "no whole-attempt kernel for this tableau (tdq_linear_rows_attempt_supported)");
+    TdqHostShape hs;
+    tdq_shape_from_tableau(tab, &hs);
+    const int S = hs.n_stages;
+    AttOut out;
+    memset(&out, 0, sizeof(out));
+    for (int i = 1; i <= S; ++i) {
+        TDQ_REQUIRE(k_out[i] != nullptr, "missing stage slot");
+        out.k[i] = (float *)k_out[i];
+    }
+    out.y1 = (float *)y1_out;
+    out.err = (float *)err_out;
+    unsigned char *rb = (unsigned char *)rows_dev;
+    RowArgs ra;
+    ra.c = (const TdqCtrl *)ctrl_dev;
+    ra.done = (const int *)(rb + tdq_rows_offset(TDQ_ROWS_DONE, n_rows));
+    ra.par = (const int *)(rb + tdq_rows_offset(TDQ_ROWS_PAR, n_rows));
+    ra.cursor = (const int *)(rb + tdq_rows_offset(TDQ_ROWS_CURSOR, n_rows));
+    ra.att_dt = (const double *)(rb + tdq_rows_offset(TDQ_ROWS_ATT_DT, n_rows));
+    ra.att_t1 = (const double *)(rb + tdq_rows_offset(TDQ_ROWS_ATT_T1, n_rows));
+    ra.norm_out = norm_out;
+    ra.store_always = store_always;
+    TdqCtrl *c = (TdqCtrl *)ctrl_dev;
+    const uint32_t *wt = (const uint32_t *)planes;
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc;
+    if (S == 6) rc = launch_rows_attempt<6, RM_DOPRI5, 0x3du>(c, ra, out, wt, n_rows, st);
+    else rc = launch_rows_attempt<3, RM_BOSH3, 0x07u>(c, ra, out, wt, n_rows, st);
     TDQ_REQUIRE(rc == 0, "launch configuration failed");
     TDQ_CHECK_CUDA(cudaGetLastError());
     return TDQ_OK;

@@ -157,6 +157,18 @@ __device__ __forceinline__ P *tdq_detach(P *p, size_t n) {
     return reinterpret_cast<P *>(reinterpret_cast<uintptr_t>(p) + (n >> 63));
 }
 
+// Row r's output times in an independent-row solve: its own row of the [B, n] table set by tdq_rows_init_grid (c.row_t),
+// or the shared c.t_out when none is set.  The values are read as they are stored, so a table whose rows all equal t_out
+// gives the arithmetic of the shared one bit for bit.
+struct RowTimes {
+    const double *t;
+    int n;
+};
+__device__ __forceinline__ RowTimes row_times(const TdqCtrl &c, int r) {
+    if (c.row_t == nullptr) return RowTimes{c.t_out, c.n_out};
+    return RowTimes{c.row_t + (size_t)r * c.row_n, c.row_n};
+}
+
 // Stage-slot pointer bundle passed by value.
 struct KPtrs {
     const void *p[TDQ_MAX_K];

@@ -39,18 +39,6 @@ template <typename X> __device__ __forceinline__ X *fld(const Rows &R, int which
 }
 __device__ __forceinline__ int *hdr(const Rows &R) { return reinterpret_cast<int *>(R.base); }
 
-// Row r's output times: its own row of the [B, n] table set by tdq_rows_init_grid (c.row_t), or the shared c.t_out
-// when none is set.  The values are read as they are stored, so a table whose rows all equal t_out gives the arithmetic
-// of the shared one bit for bit.
-struct RowTimes {
-    const double *t;
-    int n;
-};
-__device__ __forceinline__ RowTimes row_times(const TdqCtrl &c, int r) {
-    if (c.row_t == nullptr) return RowTimes{c.t_out, c.n_out};
-    return RowTimes{c.row_t + (size_t)r * c.row_n, c.row_n};
-}
-
 struct Geom {
     size_t D;
     size_t nch;                           // units per row

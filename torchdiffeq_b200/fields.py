@@ -7,7 +7,10 @@ Runge-Kutta stage -- the combination `y_i = y0 + sum_j coef_ij k_j` (rk_common.p
 (rk_common.py:80) -- is ONE hand-written wgmma kernel (csrc/tdq_linear.cu): `y_i` never goes to memory, the float32
 product runs on the tensor cores as a split-bfloat16 emulation (3 planes per operand, 6 products) with float32-grade accuracy.  Everything else about the solve (error
 norm, controller, dense output, the device-side loop) is unchanged; `forward` itself is only called for f(t0, y0), the
-initial step size and `jump_t` restarts.  `options={'fused_linear': False}` keeps the generic path (func as a torch call)."""
+initial step size and `jump_t` restarts.  With `options={'independent_rows': True}` (dopri5 / bosh3, `[B, 128]` rows, scalar
+tolerances) every attempt of every row is one kernel with each row's own step (csrc/tdq_attempt.cu k_linear_rows_attempt);
+the taped row solves of `differentiable` / `event_gradient` and `compact_rows` keep the generic row path.
+`options={'fused_linear': False}` keeps the generic path (func as a torch call)."""
 import torch
 
 

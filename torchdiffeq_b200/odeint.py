@@ -309,9 +309,11 @@ def step_jump_times(step_t, jump_t, t0, device):
     return (st.to(device) if step_t is not None else None), (jt.to(device) if jump_t is not None else None)
 
 
-def _make_adaptive_engine(p, lockstep=False, keep_interp=False, graph=None, replicated=(), post_fn=None):
+def _make_adaptive_engine(p, lockstep=False, keep_interp=False, graph=None, replicated=(), post_fn=None, row_tape=False):
     """The adaptive engine of a Problem: method, tolerances, step control, norm, callbacks and state come from `p`.
-    lockstep: the reference's exact call sequence (run_ahead=0, no graph).  graph: instead of options['graph']."""
+    lockstep: the reference's exact call sequence (run_ahead=0, no graph).  graph: instead of options['graph'].
+    row_tape: the engine of a taped independent-row solve, whose reverse sweep recomputes every stage through func and
+    so needs func's arithmetic in the forward too: its attempts are never fused with a LinearField."""
     o = p.options
     control = _step_control(p.method, o)
     graph = _resolve_graph(o.get("graph", "auto") if graph is None else graph, p.original_func)
@@ -319,8 +321,15 @@ def _make_adaptive_engine(p, lockstep=False, keep_interp=False, graph=None, repl
         control["run_ahead"], graph = 0, False
     tol = dict(rtol=p.rtol, atol=p.atol, rtol_vec=p.rtol_vec, atol_vec=p.atol_vec, t_sign=p.t_sign)
     if o.get("independent_rows"):
-        return RowsEngine(p.fn, p.shape, p.dtype, p.device, p.method, graph=graph,
-                          compact_fn=p.original_func if o.get("compact_rows") else None, **tol, **control)
+        eng = RowsEngine(p.fn, p.shape, p.dtype, p.device, p.method, graph=graph,
+                         compact_fn=p.original_func if o.get("compact_rows") else None, **tol, **control)
+        if not row_tape and o.get("fused_linear", True):
+            # a LinearField on [B, 128] float32 rows: each attempt of every row is one wgmma launch (RowsEngine.set_linear)
+            from .fields import fusable
+            w = fusable(p.original_func, tuple(p.shape), p.dtype, p.device, eng.lib)
+            if w is not None:
+                eng.set_linear(w, whole_attempt=o.get("fused_attempt", True))
+        return eng
     step_t, jump_t = step_jump_times(o.get("step_t"), o.get("jump_t"), float(p.t_cpu[0]), p.device)
     reduce_fn, n_global, seg_counts_global, agree_fn, exchange = None, None, None, None, None
     pg = o.get("process_group")
@@ -458,7 +467,7 @@ def _solve_rows_event(p, event_fn, ev0, taped=False):
     graph = p.options.get("graph", "auto")
     if graph == "auto" and not isinstance(event_fn, torch.nn.Module):
         graph = False
-    eng = _make_adaptive_engine(p, graph=graph, lockstep=taped)
+    eng = _make_adaptive_engine(p, graph=graph, lockstep=taped, row_tape=taped)
     B = p.shape[0]
     # the bisection tolerance: atol, or with a per-element atol the smallest of the row's own elements
     if p.atol_vec is not None:
@@ -894,7 +903,7 @@ def _odeint_backprop(p, func, y0, t, params, _stats):
 
     def run():
         if p.options.get("independent_rows"):     # options['differentiable'] (_check_independent_rows)
-            eng = _make_adaptive_engine(p, lockstep=True)
+            eng = _make_adaptive_engine(p, lockstep=True, row_tape=True)
             t64 = p.t_cpu.to(torch.float64).to(p.device)
             if p.t_cpu.dim() == 2:
                 sol, tape = eng.solve_taped(p.y0_flat, None, t_start=float(p.t_cpu[0, 0]), grid=t64)
