@@ -1,5 +1,6 @@
 """The whole-attempt kernel (csrc/tdq_attempt.cu) at row counts around its 32-row tile: one partial tile alone, one full tile,
-a full tile plus one row, and more tiles than an H100 has SMs plus a partial tile.  Each k_i, y1, the error prefix and the
+a full tile plus one row, and three tiles per SM plus a partial one ("96P+17", P the device's SM count: CTA 0 runs four
+tiles, the last of them partial, and every other CTA three).  Each k_i, y1, the error prefix and the
 committed candidates must be BITWISE what the 16-row stage kernel (csrc/tdq_linear.cu) writes, and the squared error norm
 agree to float64 summation order."""
 import ctypes as C
@@ -7,6 +8,7 @@ import ctypes as C
 import pytest
 import torch
 
+import grid_stride as G
 from oracle import ode_oracle as O
 from test_gpu_kernels import _engine, _rand
 from test_gpu_linear import DEV, _attempt_reference, _planes, _weight
@@ -15,8 +17,12 @@ pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("method", ["dopri5", "bosh3"])
-@pytest.mark.parametrize("rows", [31, 32, 33, 3 * 132 * 32 + 17])
-def test_attempt_tile_boundaries_equal_stage_sequence(method, rows):
+@pytest.mark.parametrize("size", [31, 32, 33, "96P+17"])
+def test_attempt_tile_boundaries_equal_stage_sequence(method, size):
+    P = G.sm_count()
+    rows = G.rows(size, P)
+    if size == "96P+17":
+        assert G.multi_tile(rows, P)
     n = rows * 128
     eng, _lib, _stream = _engine(method, torch.float32, n, 0.0371, 0.5, 1.0)
     lib = eng.lib

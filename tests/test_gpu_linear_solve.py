@@ -8,6 +8,7 @@ mailbox tick, so its nfe counts no trailing no-op attempts, like the device loop
 import pytest
 import torch
 
+import grid_stride as G
 import problems as P
 
 pytestmark = pytest.mark.gpu
@@ -59,10 +60,22 @@ def _check(W, y0, t, method="dopri5", **opts):
     return got
 
 
+def _rows(size):
+    """size (an int or tests/grid_stride.py's "aP+b") as a row count for this device.  "32P" gives every CTA exactly one
+    full tile; every larger size gives at least one CTA two or more, so each CTA's partial covers several tiles."""
+    P = G.sm_count()
+    B = G.rows(size, P)
+    if size == "32P":
+        assert G.tiles(B) == P
+    elif B > 32 * P:
+        assert G.multi_tile(B, P)
+    return B
+
+
 @pytest.mark.parametrize("method", ["dopri5", "bosh3"])
-@pytest.mark.parametrize("rows", [1, 31, 32, 33, 1000, 132 * 32])
+@pytest.mark.parametrize("rows", [1, 31, 32, 33, 1000, "32P", "32P+1", "64P+17", 65536])
 def test_persistent_solve_bitwise(method, rows):
-    _check(_weight(), _y0(rows), torch.tensor([0.0, 2.0], device=DEV), method)
+    _check(_weight(), _y0(_rows(rows)), torch.tensor([0.0, 2.0], device=DEV), method)
 
 
 @pytest.mark.parametrize("method", ["dopri5", "bosh3"])
@@ -70,12 +83,28 @@ def test_persistent_solve_reverse_time(method):
     _check(_weight(), _y0(33), torch.tensor([2.0, 0.5], device=DEV), method)
 
 
+MANY_OUTPUTS = torch.cat([torch.linspace(0.0, 0.01, 7), torch.linspace(0.02, 3.0, 60)])
+
+
 @pytest.mark.parametrize("method", ["dopri5", "bosh3"])
 def test_persistent_solve_many_outputs(method):
     """outputs inside most steps, several inside one step: the in-kernel fit runs many times"""
-    t = torch.cat([torch.linspace(0.0, 0.01, 7), torch.linspace(0.02, 3.0, 60)]).to(DEV)
+    t = MANY_OUTPUTS.to(DEV)
     out, st = _check(_weight(), _y0(1000), t, method)
     assert out.shape[0] == t.numel()
+
+
+@pytest.mark.parametrize("method", ["dopri5", "bosh3"])
+@pytest.mark.parametrize("case", ["reverse_64P+17", "many_outputs_65536"])
+def test_persistent_solve_several_tiles_per_cta(method, case):
+    """reverse time with a partial tile in CTA 0's third pass, and the in-kernel fit (grid-stride over 8.4 M elements) at
+    nearly every step of the benchmark's batch"""
+    if case.startswith("reverse"):
+        _check(_weight(), _y0(_rows("64P+17")), torch.tensor([2.0, 0.5], device=DEV), method)
+    else:
+        t = MANY_OUTPUTS.to(DEV)
+        out, _ = _check(_weight(), _y0(_rows(65536)), t, method)
+        assert out.shape[0] == t.numel()
 
 
 def test_persistent_solve_reverse_many_outputs():
@@ -127,9 +156,11 @@ def _failure(W, y0, t, **opts):
     return type(e.value), str(e.value)
 
 
-@pytest.mark.parametrize("case", ["max_num_steps", "dt_underflow", "nonfinite"])
+@pytest.mark.parametrize("case", ["max_num_steps", "dt_underflow", "nonfinite", "nonfinite_32P+5", "nonfinite_last"])
 def test_persistent_solve_failures(case):
-    W, y0 = _weight(), _y0(40)
+    """40 rows; and 65,536 with the infinity in row 32P + 5 (CTA 0's second tile) or in the last row"""
+    W = _weight()
+    y0 = _y0(_rows(65536) if case in ("nonfinite_32P+5", "nonfinite_last") else 40)
     t = torch.tensor([0.0, 2.0], device=DEV)
     opts = {}
     if case == "max_num_steps":
@@ -138,10 +169,11 @@ def test_persistent_solve_failures(case):
         t = torch.tensor([1.0, 2.0], device=DEV)
         opts["first_step"] = 1e-20                     # 1 + 1e-20 == 1: the first attempt fails
     else:
-        y0[3, 5] = float("inf")
+        r = {"nonfinite": 3, "nonfinite_32P+5": G.rows("32P+5", G.sm_count()), "nonfinite_last": y0.shape[0] - 1}[case]
+        y0[r, 5] = float("inf")
         opts["first_step"] = 0.01                      # past the initial step selection, which would end in dt 0
     got = _failure(W, y0, t, **opts)
     assert got == _failure(W, y0, t, device_loop=False, **opts)
     assert got == _failure(W, y0, t, run_ahead=0, **opts)
-    assert {"max_num_steps": "max_num_steps exceeded", "dt_underflow": "underflow in dt",
-            "nonfinite": "non-finite values"}[case] in got[1], got
+    assert {"max_num_steps": "max_num_steps exceeded",
+            "dt_underflow": "underflow in dt"}.get(case, "non-finite values") in got[1], got
