@@ -419,6 +419,20 @@ int tdq_fixed_emit_cubic(int32_t dtype, const void *y0, const void *y1, const vo
                          const int32_t *out_idx_dev, const void *coef_dev, int32_t rec_lo, int32_t rec_hi, size_t n,
                          void *stream);
 
+/* The adjoint of tdq_fixed_emit_cubic over the records [rec_lo, rec_hi) of one step (the same out_idx_dev and coef_dev,
+ * n_records entries each), for gradients of the discrete solve: with g_r = grad_sol[out_idx[r]] (row-major [*, n]),
+ *   ybar0 += c0*g_r,  fbar0 += c1*g_r,  ybar1 += c2*g_r,  fbar1 += c3*g_r      r ascending, rounded in the state dtype,
+ * in one pass over the state; the four accumulators are distinct n-element buffers.  With dots != NULL also
+ *   dots[4*(r - rec_lo) + m] = <g_r, x_m>,  x = (y0, f0, y1, f1)      float64,
+ * summed in an order that depends on n only (not on the device, the launch or the pointers' alignment), so a call
+ * repeats bit for bit; `partials` then needs tdq_fixed_emit_cubic_grad_partials_len(dtype, n, rec_hi - rec_lo)
+ * doubles of scratch (no initial value; not shared with a concurrent call).  0 for an unsupported dtype. */
+size_t tdq_fixed_emit_cubic_grad_partials_len(int32_t dtype, size_t n, int32_t n_records);
+int tdq_fixed_emit_cubic_grad(int32_t dtype, const void *y0, const void *y1, const void *f0, const void *f1,
+                              const void *grad_sol, void *ybar0, void *fbar0, void *ybar1, void *fbar1,
+                              const int32_t *out_idx_dev, const void *coef_dev, int32_t n_records, int32_t rec_lo,
+                              int32_t rec_hi, size_t n, double *dots, double *partials, void *stream);
+
 /* ---- implicit fixed-grid Runge-Kutta: Broyden's iteration as low-rank streaming passes (tdq_implicit.cu) --------------
  * rk_common.py:438-459 (FIRK, one solve over every active stage) and :525-547 (DIRK, one solve per stage) keep a dense
  * M x M Jacobian estimate.  J starts at I and only receives rank-1 updates whose vector is the new residual, so

@@ -123,6 +123,19 @@ def _tabulate(grid, t, method, dtype, perturb, t_sign):
                       cubic, (t1.to(T) * t_sign).contiguous(), n_steps)
 
 
+class CubicRecords(NamedTuple):
+    """What the reverse sweep of an interp='cubic' step needs of its outputs: the device tables of the forward's emit
+    (tdq_fixed_emit_cubic), the step's record range in them, and each record's h = (t_j - t0) / dt with the step's dt,
+    float64 in ascending time."""
+    coef: torch.Tensor          # [records, 4] weights of (y0, f0, y1, f1), state dtype, reverse-time sign folded in
+    out_idx: torch.Tensor       # [records] int32 output row of every record
+    n_records: int
+    lo: int
+    hi: int
+    h: list
+    dt: float
+
+
 class Step(NamedTuple):
     """What the driver hands a step: grid step k (None for an event step), start time, step size and end time as the
     reference's loops have them -- t's dtype on a grid (solvers.py:110-112); on an event step t0 in the state dtype,
@@ -385,10 +398,18 @@ class FixedGridEngine:
             sol = self._solve_grid(y0_flat, grid_cpu, t_cpu, tab)
         finally:
             self._taping = None
+        if self.interp == "cubic":
+            # the weights' derivatives need h and dt of every record, in float64 from t's dtype like the weights
+            t64, g64 = t_cpu.to(torch.float64), grid_cpu.to(torch.float64)
         for k, st in enumerate(tape):
             st["k"], st["perturb"] = k, self.perturb
-            st["outs"] = [(int(tab.out_idx[r]), int(tab.mode[r]), float(tab.slope[r]))
-                          for r in range(int(tab.rec_begin[k]), int(tab.rec_begin[k + 1]))]
+            lo, hi = int(tab.rec_begin[k]), int(tab.rec_begin[k + 1])
+            if self.interp == "cubic":
+                dt = float(g64[k + 1] - g64[k])
+                st["cubic"] = CubicRecords(self.cubic_dev, self.out_idx, tab.out_idx.numel(), lo, hi,
+                                           [float(t64[j] - g64[k]) / dt for j in tab.out_idx[lo:hi].tolist()], dt)
+            else:
+                st["outs"] = [(int(tab.out_idx[r]), int(tab.mode[r]), float(tab.slope[r])) for r in range(lo, hi)]
         return sol, tape
 
     # ---- event handling with a fixed step (solvers.py:130-164) ------------------------------------------------

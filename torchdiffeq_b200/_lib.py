@@ -160,6 +160,9 @@ _SIGNATURES = {
     "tdq_linear_solve_scratch_len": (_sz, []),
     "tdq_linear_solve": (C.c_int, [_vp, _ptab, _i32, _pp, _vp, _vp, _vp, _i32, _sz, _vp, _sz, _vp, _vp, _vp]),
     "tdq_fixed_emit_cubic": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _sz, _vp]),
+    "tdq_fixed_emit_cubic_grad_partials_len": (_sz, [_i32, _sz, _i32]),
+    "tdq_fixed_emit_cubic_grad": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32,
+                                            _i32, _sz, _vp, _vp, _vp]),
     "tdq_pack_segments": (C.c_int, [_i32, _vp, _pp, _pi64, _pi64, _pdbl, _i32, _vp]),
     "tdq_implicit_partials_len": (_sz, [_i32]),
     "tdq_implicit_state_len": (_sz, [_i32]),

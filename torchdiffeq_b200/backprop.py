@@ -28,7 +28,7 @@ import ctypes as C
 import torch
 
 from . import _lib
-from ._engine import _stream, on_solver_stream
+from ._engine import _DTYPES, _stream, on_solver_stream
 from ._fixed import stage_times
 
 
@@ -109,12 +109,18 @@ class StepAdjoint:
         self.F, self.params, self.need_t = F, tuple(params), need_t
         self.pbar = [None] * len(self.params)
 
-    def vjp(self, t_val, y_val, g):
-        """(y_bar, t_bar) of f(t, y) against g; parameter gradients accumulate in self.pbar."""
+    def record(self, t_val, y_val):
+        """f(t, y) evaluated with its graph, for a later vjp(..., rec=) that needs the value too."""
         with torch.enable_grad():
             tr = t_val.detach().clone().requires_grad_(self.need_t)
             yr = y_val.detach().requires_grad_(True)
-            out = self.F(tr, yr)
+            return tr, yr, self.F(tr, yr)
+
+    def vjp(self, t_val, y_val, g, rec=None):
+        """(y_bar, t_bar) of f(t, y) against g; parameter gradients accumulate in self.pbar.  rec: what record(t_val,
+        y_val) returned, instead of a fresh evaluation."""
+        tr, yr, out = self.record(t_val, y_val) if rec is None else rec
+        with torch.enable_grad():
             if not out.requires_grad:
                 return None, None
             inputs = [yr] + ([tr] if self.need_t else []) + list(self.params)
@@ -412,8 +418,58 @@ def rows_backward(p, tape, t, grad_sol, params, need_t, event=False):
     return tbar, y0bar, sa.pbar
 
 
+def cubic_weight_grads(h, dt):
+    """Derivatives of the cubic Hermite weights (h00, h10 dt, h01, h11 dt) of solvers.py:166-173 w.r.t. (t_j, t0, t1):
+    float64 [R, 3, 4] for the records' h = (t_j - t0) / dt and their step's dt = t1 - t0, by the chain rule through
+    dh/dt_j = 1/dt, dh/dt0 = (h - 1)/dt, dh/dt1 = -h/dt, ddt/dt0 = -1 and ddt/dt1 = 1."""
+    h = torch.as_tensor(h, dtype=torch.float64)
+    z = torch.zeros_like(h)
+    dw_dh = torch.stack([6 * h * h - 6 * h, (3 * h * h - 4 * h + 1) * dt, 6 * h - 6 * h * h, (3 * h * h - 2 * h) * dt], 1)
+    dw_ddt = torch.stack([z, h * (1 - h) * (1 - h), z, h * h * (h - 1)], 1)
+    return torch.stack([dw_dh / dt, dw_dh * ((h - 1) / dt)[:, None] - dw_ddt, dw_dh * (-h / dt)[:, None] + dw_ddt], 1)
+
+
+def _cubic_emit_backward(sa, cub, k, y0, y1, f0, t1_dev, grad_sol, ybar1, sign, gbar, obar):
+    """Adjoint of the interp='cubic' outputs of grid step k (solvers.py:120-122, :166-173), in the ascending time of
+    fixed_backward: y0, y1 and f0 = k_1 as that sweep has them (f0 reference-sense, sign * the raw func output).  Returns
+    (ybar0, ybar1, f0bar); f(t1, y1)'s VJP is taken here, its time part and the weights' time derivatives go into gbar
+    and obar (when the times need gradients)."""
+    lib, T, dev, n = _lib.load(), y0.dtype, y0.device, y0.numel()
+    # f1 = f(t1, y1) once, with its graph.  The reference evaluates f1 again for every output time of the step; the VJP
+    # of the summed cotangent is the sum of those per-output VJPs up to rounding.
+    rec = sa.record(t1_dev, y1)
+    f1 = rec[2].detach().to(T).contiguous()
+    acc = torch.zeros(4, n, dtype=T, device=dev)                       # ybar0, fbar0, ybar1, fbar1
+    R = cub.hi - cub.lo
+    dots = partials = None
+    if sa.need_t:
+        dots = torch.empty(R, 4, dtype=torch.float64, device=dev)
+        partials = torch.empty(lib.tdq_fixed_emit_cubic_grad_partials_len(_DTYPES[T], n, R), dtype=torch.float64,
+                               device=dev)
+    y1c, f0c = y1.contiguous(), f0.to(T).contiguous()
+    _lib.check(lib.tdq_fixed_emit_cubic_grad(
+        _DTYPES[T], y0.data_ptr(), y1c.data_ptr(), f0c.data_ptr(), f1.data_ptr(), grad_sol.data_ptr(), acc[0].data_ptr(),
+        acc[1].data_ptr(), acc[2].data_ptr(), acc[3].data_ptr(), cub.out_idx.data_ptr(), cub.coef.data_ptr(),
+        cub.n_records, cub.lo, cub.hi, n, dots.data_ptr() if dots is not None else None,
+        partials.data_ptr() if partials is not None else None, _stream()))
+    # the table folds the reverse-time sign into the dt*f weights, which multiply RAW func outputs: a reference-sense
+    # f's cotangent is sign * the kernel's, while the dots with reference-sense f0 / f1 need no sign
+    f0bar, f1bar = (acc[1], acc[3]) if sign == 1.0 else (acc[1] * sign, acc[3] * sign)
+    gy1, tb = sa.vjp(t1_dev, y1, f1bar.to(rec[2].dtype), rec=rec)
+    ybar1 = _acc(_acc(ybar1, acc[2]), gy1)
+    if sa.need_t:
+        if tb is not None:
+            gbar[k + 1] += tb.double()
+        c = torch.einsum("rqm,rm->rq", cubic_weight_grads(cub.h, cub.dt).to(dev), dots)
+        obar.index_add_(0, cub.out_idx[cub.lo:cub.hi].long(), c[:, 0])
+        gbar[k] += c[:, 1].sum()
+        gbar[k + 1] += c[:, 2].sum()
+    return acc[0], ybar1, f0bar
+
+
 def fixed_backward(p, method, tape, grid, t_cpu, grad_sol, params, need_t):
-    """Reverse sweep over the steps of a fixed-grid solve (solvers.py:102-128, linear interpolation :175-181).
+    """Reverse sweep over the steps of a fixed-grid solve (solvers.py:102-128, linear interpolation :175-181, cubic
+    Hermite :166-173).
     grid / t_cpu: ascending CPU tensors.  Returns (grid_bar, t_out_bar) as float64 device tensors (or None), y0_bar,
     [param_bar]."""
     dev, T, sign = p.device, p.dtype, p.t_sign
@@ -447,9 +503,13 @@ def fixed_backward(p, method, tape, grid, t_cpu, grad_sol, params, need_t):
             if w != 0.0:
                 incr = _acc(incr, kk, w)                               # dy / dt
         y1 = y0 + incr * dtf
-        ybar1, ybar0 = gy, None
+        ybar1, ybar0, f0bar = gy, None, None
+        cub = st.get("cubic")
+        if cub is not None and cub.hi > cub.lo:
+            ybar0, ybar1, f0bar = _cubic_emit_backward(sa, cub, k, y0, y1, k1, _dev(g1.to(T), dev), grad_sol, ybar1,
+                                                       sign, gbar, obar)
         h = float(g1 - g0)
-        for (j, mode, slope) in st["outs"]:                            # solvers.py:175-181
+        for (j, mode, slope) in st.get("outs", ()):                    # solvers.py:175-181
             G = grad_sol[j]
             if mode == 0:
                 ybar0 = _acc(ybar0, G)
@@ -466,6 +526,7 @@ def fixed_backward(p, method, tape, grid, t_cpu, grad_sol, params, need_t):
                     gbar[k] += sb * (-1.0 / h + frac / h)
                     gbar[k + 1] += sb * (-frac / h)
         kbar = [None] * (len(alpha) + 1)
+        kbar[0] = f0bar                                                # the cubic outputs' f0 is the step's k_1
         dtbar = None
         if ybar1 is not None:
             ybar0 = _acc(ybar0, ybar1)
@@ -531,7 +592,9 @@ class _BackpropFunction(torch.autograd.Function):
                     # the grid as a differentiable function of the (ascending) output times, whatever constructor made it
                     tb = obar.to("cpu")
                     if grid_req.requires_grad:
-                        (gt,) = torch.autograd.grad(grid_req, t_req, gbar.to("cpu").to(grid_req.dtype), allow_unused=True)
+                        # the grid's graph is kept for every backward through this solve (gradcheck runs several)
+                        (gt,) = torch.autograd.grad(grid_req, t_req, gbar.to("cpu").to(grid_req.dtype), allow_unused=True,
+                                                    retain_graph=True)
                         if gt is not None:
                             tb = tb + gt.double()
                     tbar = (tb * p.t_sign).to(t.dtype).to(t.device)

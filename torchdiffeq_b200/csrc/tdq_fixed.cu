@@ -2,6 +2,7 @@
 //
 //   k_rk4        stage values and the final update of rk4_alt_step_func   rk_common.py:110-118, fixed_grid.py:24-29, solvers.py:115
 //   k_fixed_emit outputs of one grid step by linear interpolation         solvers.py:117-125, :175-181
+//   k_fixed_emit_cubic(_grad)  cubic Hermite outputs of one step, and their adjoint   solvers.py:120-122, :166-173
 //   k_pack       concat + per-segment scale of the augmented dynamics     misc.py:137-145, :158-165, adjoint.py:94-105
 //
 // The step size comes from a device array indexed by a device step counter so that one captured
@@ -188,6 +189,112 @@ k_fixed_emit_cubic(const T *__restrict__ y0, const T *__restrict__ y1, const T *
     }
 }
 
+// Adjoint of k_fixed_emit_cubic over records [lo, hi) of one step, in one pass over the state:
+//   ybar0 += c0*g_r,  fbar0 += c1*g_r,  ybar1 += c2*g_r,  fbar1 += c3*g_r      g_r = grad_sol[out_idx[r]], r ascending
+// and, with DOTS, the float64 partial sums of <g_r, y0>, <g_r, f0>, <g_r, y1>, <g_r, f1> of this block at
+// partials[(4*(r - lo) + m) * gridDim.x + blockIdx.x].  Thread x of block b owns the Vec<T>::N consecutive elements
+// from (b*kThreads + x)*Vec<T>::N; they are moved with one 128-bit access when the pointer is aligned and the group lies
+// inside [0, n), element by element otherwise.  The owner of an element, and so every partial, depends on n alone: not
+// on the alignment, the device or the schedule.
+template <typename T>
+__device__ __forceinline__ Vec<T> ld_group(const T *p, bool aligned, size_t i0, size_t n) {
+    Vec<T> r;
+    if (aligned && i0 + Vec<T>::N <= n) return ld_stream<T>(p + i0);
+#pragma unroll
+    for (int e = 0; e < Vec<T>::N; ++e) r.v[e] = (i0 + e < n) ? p[i0 + e] : (T)0;
+    return r;
+}
+
+template <typename T>
+__device__ __forceinline__ void st_group(T *p, bool aligned, size_t i0, size_t n, const Vec<T> &x) {
+    if (aligned && i0 + Vec<T>::N <= n) {
+        st_vec<T>(p + i0, x);
+        return;
+    }
+#pragma unroll
+    for (int e = 0; e < Vec<T>::N; ++e)
+        if (i0 + e < n) p[i0 + e] = x.v[e];
+}
+
+__device__ __forceinline__ bool tdq_dev_aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+template <typename T, bool DOTS>
+__global__ void __launch_bounds__(kThreads)
+k_fixed_emit_cubic_grad(const T *__restrict__ y0, const T *__restrict__ y1, const T *__restrict__ f0,
+                        const T *__restrict__ f1, const T *__restrict__ grad_sol, T *__restrict__ ybar0,
+                        T *__restrict__ fbar0, T *__restrict__ ybar1, T *__restrict__ fbar1,
+                        const int32_t *__restrict__ out_idx, const T *__restrict__ coef, int lo, int hi, size_t n,
+                        double *__restrict__ partials) {
+    using A = Ar<T>;
+    using V = Vec<T>;
+    __shared__ double red[kThreads / 32];
+    const size_t i0 = ((size_t)blockIdx.x * kThreads + threadIdx.x) * V::N;
+    V a, b, fa, fb;
+    if (DOTS) {
+        a = ld_group(y0, tdq_dev_aligned16(y0), i0, n);
+        b = ld_group(y1, tdq_dev_aligned16(y1), i0, n);
+        fa = ld_group(f0, tdq_dev_aligned16(f0), i0, n);
+        fb = ld_group(f1, tdq_dev_aligned16(f1), i0, n);
+    }
+    V ga = ld_group<T>(ybar0, tdq_dev_aligned16(ybar0), i0, n), gfa = ld_group<T>(fbar0, tdq_dev_aligned16(fbar0), i0, n),
+      gb = ld_group<T>(ybar1, tdq_dev_aligned16(ybar1), i0, n), gfb = ld_group<T>(fbar1, tdq_dev_aligned16(fbar1), i0, n);
+    for (int r = lo; r < hi; ++r) {
+        const T c0 = coef[4 * (size_t)r], c1 = coef[4 * (size_t)r + 1], c2 = coef[4 * (size_t)r + 2],
+                c3 = coef[4 * (size_t)r + 3];
+        const T *g = grad_sol + (size_t)out_idx[r] * n;
+        const V gv = ld_group(g, tdq_dev_aligned16(g), i0, n);
+        double d0 = 0.0, d1 = 0.0, d2 = 0.0, d3 = 0.0;
+#pragma unroll
+        for (int e = 0; e < V::N; ++e) {
+            const T x = gv.v[e];
+            ga.v[e] = A::add(ga.v[e], A::mul(c0, x));
+            gfa.v[e] = A::add(gfa.v[e], A::mul(c1, x));
+            gb.v[e] = A::add(gb.v[e], A::mul(c2, x));
+            gfb.v[e] = A::add(gfb.v[e], A::mul(c3, x));
+            if (DOTS) {                             // elements past n were loaded as zeros and add nothing
+                d0 += (double)x * (double)a.v[e];
+                d1 += (double)x * (double)fa.v[e];
+                d2 += (double)x * (double)b.v[e];
+                d3 += (double)x * (double)fb.v[e];
+            }
+        }
+        if (DOTS) {
+            double *p = partials + (size_t)4 * (r - lo) * gridDim.x + blockIdx.x;
+            const double s0 = block_sum<kThreads>(d0, red);
+            if (threadIdx.x == 0) p[0] = s0;
+            const double s1 = block_sum<kThreads>(d1, red);
+            if (threadIdx.x == 0) p[gridDim.x] = s1;
+            const double s2 = block_sum<kThreads>(d2, red);
+            if (threadIdx.x == 0) p[2 * (size_t)gridDim.x] = s2;
+            const double s3 = block_sum<kThreads>(d3, red);
+            if (threadIdx.x == 0) p[3 * (size_t)gridDim.x] = s3;
+        }
+    }
+    st_group(ybar0, tdq_dev_aligned16(ybar0), i0, n, ga);
+    st_group(fbar0, tdq_dev_aligned16(fbar0), i0, n, gfa);
+    st_group(ybar1, tdq_dev_aligned16(ybar1), i0, n, gb);
+    st_group(fbar1, tdq_dev_aligned16(fbar1), i0, n, gfb);
+}
+
+// dots[q] = sum over the blocks of partials[q * parts + .]: one warp per dot, lanes strided in block order, then the
+// fixed shuffle tree of warp_sum.
+__global__ void __launch_bounds__(128)
+k_fixed_emit_cubic_dots(const double *__restrict__ partials, int parts, int n_dots, double *__restrict__ dots) {
+    const int q = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (q >= n_dots) return;
+    double v = 0.0;
+    for (int i = lane; i < parts; i += 32) v += partials[(size_t)q * parts + i];
+    v = warp_sum(v);
+    if (lane == 0) dots[q] = v;
+}
+
+// blocks of k_fixed_emit_cubic_grad for n elements: a function of n and the dtype only
+inline size_t cubic_grad_blocks(size_t n, int vn) {
+    const size_t per_block = (size_t)kThreads * vn;
+    const size_t b = (n + per_block - 1) / per_block;
+    return b ? b : 1;
+}
+
 // Generic linear combination for the multistep (Adams) predictor / corrector of fixed_adams.py:198-215:
 //   out = [base +] ((x_0*c_0 + x_1*c_1) + x_2*c_2) + ...      products and sums rounded separately, ascending order,
 // the first product initialises the sum (Python's sum() starts from 0 + x_0*c_0 = x_0*c_0 exactly).
@@ -324,6 +431,41 @@ int tdq_fixed_emit_cubic(int32_t dtype, const void *y0, const void *y1, const vo
                                (const T *)y0, (const T *)y1, (const T *)f0, (const T *)f1, (T *)solution, out_idx_dev,
                                (const T *)coef_dev, rec_lo, rec_hi, n)));
     TDQ_CHECK_CUDA(cudaGetLastError());
+    return TDQ_OK;
+}
+
+size_t tdq_fixed_emit_cubic_grad_partials_len(int32_t dtype, size_t n, int32_t n_records) {
+    if ((dtype != TDQ_F32 && dtype != TDQ_F64) || n_records < 0) return 0;
+    return 4 * (size_t)n_records * cubic_grad_blocks(n, dtype == TDQ_F32 ? Vec<float>::N : Vec<double>::N);
+}
+
+int tdq_fixed_emit_cubic_grad(int32_t dtype, const void *y0, const void *y1, const void *f0, const void *f1,
+                              const void *grad_sol, void *ybar0, void *fbar0, void *ybar1, void *fbar1,
+                              const int32_t *out_idx_dev, const void *coef_dev, int32_t n_records, int32_t rec_lo,
+                              int32_t rec_hi, size_t n, double *dots, double *partials, void *stream) {
+    TDQ_REQUIRE(y0 && y1 && f0 && f1 && grad_sol && ybar0 && fbar0 && ybar1 && fbar1 && out_idx_dev && coef_dev,
+                "null argument");
+    TDQ_REQUIRE(dots == nullptr || partials != nullptr,
+                "dots need tdq_fixed_emit_cubic_grad_partials_len(dtype, n, rec_hi - rec_lo) doubles of partials");
+    TDQ_REQUIRE(rec_lo >= 0 && rec_lo <= rec_hi && rec_hi <= n_records, "bad record range");
+    TDQ_REQUIRE(dtype == TDQ_F32 || dtype == TDQ_F64, "unsupported dtype");
+    const size_t blocks = cubic_grad_blocks(n, dtype == TDQ_F32 ? Vec<float>::N : Vec<double>::N);
+    TDQ_REQUIRE(n > 0 && blocks <= 0x7fffffffu, "n out of range");
+    if (rec_hi == rec_lo) return TDQ_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    TDQ_DISPATCH_T(dtype, tdq_dispatch(TdqBool{}, dots != nullptr, [&](auto D) {
+                       k_fixed_emit_cubic_grad<T, D><<<(unsigned)blocks, kThreads, 0, st>>>(
+                           (const T *)y0, (const T *)y1, (const T *)f0, (const T *)f1, (const T *)grad_sol, (T *)ybar0,
+                           (T *)fbar0, (T *)ybar1, (T *)fbar1, out_idx_dev, (const T *)coef_dev, rec_lo, rec_hi, n,
+                           partials);
+                       return 0;
+                   }));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    if (dots) {
+        const int n_dots = 4 * (rec_hi - rec_lo);
+        k_fixed_emit_cubic_dots<<<(n_dots + 3) / 4, 128, 0, st>>>(partials, (int)blocks, n_dots, dots);
+        TDQ_CHECK_CUDA(cudaGetLastError());
+    }
     return TDQ_OK;
 }
 

@@ -924,9 +924,6 @@ def _odeint_backprop(p, func, y0, t, params, _stats):
         if p.method in IMPLICIT_METHODS:
             raise NotImplementedError("gradients through the discrete implicit solve (Broyden's iteration) are not "
                                       "implemented; use odeint_adjoint with the implicit methods")
-        if o.get("interp", "linear") != "linear":
-            raise NotImplementedError("gradients through interp='cubic' are not implemented (use the default linear "
-                                      "interpolation, or odeint_adjoint)")
         y0_view = p.layout.views(p.y0_flat) if p.is_tuple else p.y0_flat.view(p.shape)
         with torch.enable_grad():                     # the grid as a differentiable function of the output times
             t_req = p.t_cpu.detach().clone().requires_grad_(True)
