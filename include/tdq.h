@@ -47,7 +47,9 @@ typedef enum {
     TDQ_RUN_NONFINITE = 2,      /* rk_common.py:287  assert isfinite(y0).all()                     */
     TDQ_RUN_MAX_STEPS = 3,      /* rk_common.py:247  assert n_steps < max_num_steps                */
     TDQ_RUN_EXCHANGE_TIMEOUT = 4, /* a peer rank never delivered its norm partials (sharded solves) */
-    TDQ_RUN_BARRIER_TIMEOUT = 5 /* a CTA of tdq_linear_solve missed a grid barrier by 10 s          */
+    TDQ_RUN_BARRIER_TIMEOUT = 5, /* a CTA of tdq_linear_solve missed a grid barrier by 10 s         */
+    TDQ_RUN_EXCHANGE_SEGMENTS = 6 /* armed exchange (world > 1) and n_seg > TDQ_MAX_SEGS: the peer    */
+                                  /* buffers cannot carry the partials, so nothing is decided         */
 } tdq_run_status;
 
 /* Butcher tableau of an explicit embedded RK method, float64 as in the reference
@@ -114,8 +116,9 @@ typedef struct {
 
 /* ---- library ------------------------------------------------------------------------------ */
 int tdq_abi_version(void);
-/* sizeof the ABI structs as compiled (0: tdq_tableau, 1: tdq_options, 2: tdq_mailbox); lets a foreign
- * binding verify its own struct definitions. */
+/* sizeof the ABI structs as compiled (0: tdq_tableau, 1: tdq_options, 2: tdq_mailbox, 3: one rank's exchange
+ * buffer of tdq_xchg_create -- double vals[4][TDQ_MAX_RANKS][TDQ_MAX_SEGS + 2] then uint64_t flags[4][TDQ_MAX_RANKS],
+ * slot ((epoch & 1) << 1) | (attempt & 1)); lets a foreign binding verify its own struct definitions. */
 size_t tdq_sizeof(int32_t which);
 const char *tdq_last_error(void);
 /* Number of SMs of the current device (grid sizing). */
@@ -491,7 +494,9 @@ int tdq_xchg_open(const tdq_ipc_handle *handle, void **peer_ptr);
 int tdq_xchg_close(void *peer_ptr);
 int tdq_xchg_destroy(void *dev_ptr);
 /* After tdq_ctrl_init: peer_ptrs[r] = rank r's exchange buffer as mapped in THIS process (own buffer at
- * index `rank`); epoch must be the same on all ranks and differ from solve to solve. */
+ * index `rank`); epoch must be the same on all ranks and differ from solve to solve.  With world > 1 every
+ * tdq_controller call that passes norm sums (no ratio_dev) must have n_seg <= TDQ_MAX_SEGS; otherwise the controller
+ * halts the solve with TDQ_RUN_EXCHANGE_SEGMENTS and writes nothing to the peers. */
 int tdq_ctrl_set_exchange(void *ctrl_dev, const void *const *peer_ptrs, int32_t rank, int32_t world,
                           uint64_t epoch, void *stream);
 

@@ -36,6 +36,10 @@ def test_struct_sizes(lib):
     assert C.sizeof(lib.Tableau) == L.tdq_sizeof(0) == 16 + 8 * (16 + 16 * 17 + 3 * 17)
     assert C.sizeof(lib.Options) == L.tdq_sizeof(1)
     assert C.sizeof(lib.Mailbox) == L.tdq_sizeof(2)
+    # one rank's exchange buffer: 4 slots x 16 ranks x (64 segments + non-finite count + pad) doubles, then 4 x 16 flags
+    assert C.sizeof(lib.XBuf) == L.tdq_sizeof(3) == 34304
+    assert lib.XBuf.flags.offset == 4 * lib.TDQ_MAX_RANKS * (lib.TDQ_MAX_SEGS + 2) * 8
+    assert L.tdq_sizeof(4) == 0
     assert lib.load().tdq_ctrl_size() % 256 == 0
     assert lib.load().tdq_ctrl_tstage_offset() % 16 == 0
 
@@ -237,3 +241,44 @@ def test_stage_launchers_host_side_contract(lib):
     refused(lc(0, P, P, lib.ptr_array([P, None, P]), cf, 3, 4096, None), fn, "null term")
     for nt in (1, 17):
         assert lc(nt % 2, P, None, lib.ptr_array([P] * 17), cf, nt, 0, None) == 0
+
+
+def test_exchange_host_side_contract(lib):
+    """tdq_ctrl_set_exchange, tdq_xchg_create / _open refuse bad arguments before any CUDA call, with a message naming the
+    entry point; tdq_xchg_close / _destroy of NULL are no-ops.  Every pointer is fake: none of these calls may use one."""
+    import ctypes as C
+    L = lib.load()
+    P = 16
+
+    def refused(rc, fn, msg):
+        assert rc != 0 and L.tdq_last_error().decode() == "%s: %s" % (fn, msg)
+
+    se, fn = L.tdq_ctrl_set_exchange, "tdq_ctrl_set_exchange"
+    peers = lib.ptr_array([P + 256 * r for r in range(lib.TDQ_MAX_RANKS + 1)])
+    refused(se(None, peers, 0, 2, 1, None), fn, "null argument")
+    refused(se(P, None, 0, 2, 1, None), fn, "null argument")
+    for rank, world in ((0, 0), (0, lib.TDQ_MAX_RANKS + 1), (2, 2), (16, 16), (-1, 2), (0, -1)):
+        refused(se(P, peers, rank, world, 1, None), fn, "rank/world out of range")
+    for hole in (0, 1, 15):                                       # a NULL among the first `world` peer pointers
+        holed = lib.ptr_array([None if r == hole else P for r in range(16)])
+        refused(se(P, holed, 0, 16, 1, None), fn, "missing peer buffer")
+    refused(se(P, lib.ptr_array([P, None]), 0, 2, 1, None), fn, "missing peer buffer")
+
+    h = lib.IpcHandle()
+    ptr = C.c_void_p()
+    refused(L.tdq_xchg_create(None, C.byref(h)), "tdq_xchg_create", "null argument")
+    refused(L.tdq_xchg_create(C.byref(ptr), None), "tdq_xchg_create", "null argument")
+    refused(L.tdq_xchg_open(None, C.byref(ptr)), "tdq_xchg_open", "null argument")
+    refused(L.tdq_xchg_open(C.byref(h), None), "tdq_xchg_open", "null argument")
+    assert L.tdq_xchg_close(None) == 0 and L.tdq_xchg_destroy(None) == 0
+
+
+def test_exchange_segments_status(lib):
+    """An armed controller with more norm segments than the peer buffers carry halts with its own status, and the engine
+    turns it into an error that names the limit."""
+    from torchdiffeq_b200._engine import AdaptiveEngine
+    assert lib.RUN_EXCHANGE_SEGMENTS == 6 and lib.TDQ_MAX_SEGS == 64
+    hdr = open(os.path.join(ROOT, "include", "tdq.h")).read()
+    assert re.search(r"TDQ_RUN_EXCHANGE_SEGMENTS\s*=\s*6\b", hdr)
+    with pytest.raises(lib.TdqError, match="at most 64 norm segments"):
+        AdaptiveEngine._raise_status(None, lib.RUN_EXCHANGE_SEGMENTS, 0.01, None)

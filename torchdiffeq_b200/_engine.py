@@ -566,6 +566,9 @@ class AdaptiveEngine:
             raise SolverFailure("non-finite values in state `y`: {}".format(y) + where)
         if s == _lib.RUN_EXCHANGE_TIMEOUT:
             raise _lib.TdqError("a peer rank did not deliver its norm partials within 10 s (sharded solve)")
+        if s == _lib.RUN_EXCHANGE_SEGMENTS:
+            raise _lib.TdqError("the peer exchange of a sharded solve carries at most %d norm segments; this solve has more"
+                                % _lib.TDQ_MAX_SEGS)
         if s == _lib.RUN_BARRIER_TIMEOUT:
             raise _lib.TdqError("a block of the persistent linear solve missed a grid barrier by 10 s")
         if s == _lib.RUN_MAX_STEPS:

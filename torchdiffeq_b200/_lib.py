@@ -11,7 +11,8 @@ TDQ_MAX_K = TDQ_MAX_STAGES + 1
 TDQ_MAX_SEGS = 64
 TDQ_F32, TDQ_F64 = 0, 1
 TDQ_ERR_UNSUPPORTED = 3
-RUN_OK, RUN_DT_UNDERFLOW, RUN_NONFINITE, RUN_MAX_STEPS, RUN_EXCHANGE_TIMEOUT, RUN_BARRIER_TIMEOUT = 0, 1, 2, 3, 4, 5
+(RUN_OK, RUN_DT_UNDERFLOW, RUN_NONFINITE, RUN_MAX_STEPS, RUN_EXCHANGE_TIMEOUT, RUN_BARRIER_TIMEOUT,
+ RUN_EXCHANGE_SEGMENTS) = range(7)
 TDQ_MAX_RANKS = 16
 # tdq_rows_field (include/tdq.h)
 (ROWS_T0, ROWS_T1, ROWS_DT, ROWS_RATIO, ROWS_ATT_T0, ROWS_ATT_DT, ROWS_ATT_T1, ROWS_FIT_DT, ROWS_H0, ROWS_D1, ROWS_PAR,
@@ -60,6 +61,14 @@ class Mailbox(C.Structure):
         ("next_t0", C.c_double), ("next_dt", C.c_double),
         ("on_jump_t", C.c_int32), ("on_step_t", C.c_int32), ("par", C.c_int32),
     ]
+
+
+class XBuf(C.Structure):
+    """One rank's exchange buffer of a sharded solve (tdq_xchg_create, tdq_sizeof(3)): slot
+    ((epoch & 1) << 1) | (attempt & 1) holds every rank's n_seg + 1 norm partials and its flag
+    (epoch << 32) | (attempt + 1)."""
+    _fields_ = [("vals", ((C.c_double * (TDQ_MAX_SEGS + 2)) * TDQ_MAX_RANKS) * 4),
+                ("flags", (C.c_uint64 * TDQ_MAX_RANKS) * 4)]
 
 
 class RowsTape(C.Structure):
@@ -247,7 +256,7 @@ def load():
         fn.argtypes = args
     if lib.tdq_abi_version() != ABI_VERSION:
         raise TdqError("libtdq.so ABI version mismatch")
-    for which, st in ((0, Tableau), (1, Options), (2, Mailbox)):
+    for which, st in ((0, Tableau), (1, Options), (2, Mailbox), (3, XBuf)):
         if lib.tdq_sizeof(which) != C.sizeof(st):
             raise TdqError("libtdq.so struct layout mismatch for %s; rebuild it" % st.__name__)
     _lib = lib

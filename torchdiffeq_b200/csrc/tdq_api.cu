@@ -226,6 +226,7 @@ size_t tdq_sizeof(int32_t which) {
         case 0: return sizeof(tdq_tableau);
         case 1: return sizeof(tdq_options);
         case 2: return sizeof(tdq_mailbox);
+        case 3: return sizeof(TdqXBuf);
     }
     return 0;
 }

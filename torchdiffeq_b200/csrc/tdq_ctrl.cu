@@ -32,7 +32,17 @@ k_controller(TdqCtrl *c, const double *norm_in, const int64_t *cnt, int n_seg, c
     TdqCtrl &sc = *reinterpret_cast<TdqCtrl *>(raw);
     __shared__ double xsum[TDQ_MAX_SEGS + 2];
     __shared__ int xfail;
-    if (sc.xworld > 1 && !sc.halt && norm_in != nullptr && ratio_dev == nullptr && n_seg <= TDQ_MAX_SEGS) {
+    const bool exchange = sc.xworld > 1 && !sc.halt && norm_in != nullptr && ratio_dev == nullptr;
+    if (exchange && n_seg > TDQ_MAX_SEGS) {
+        // The peer buffers hold the partials of at most TDQ_MAX_SEGS segments: deciding on this rank's local sums would give
+        // it a step size of its own.  Halt instead; the mailbox still ticks (ctrl_decide's halted path) and reports the status.
+        __syncthreads();                                                   // every thread has read sc.halt above
+        if (threadIdx.x == 0) {
+            sc.status = TDQ_RUN_EXCHANGE_SEGMENTS;
+            sc.halt = 1;
+        }
+        __syncthreads();
+    } else if (exchange) {
         // Fused all-reduce over NVLink peer memory: thread t talks to rank t.
         const int R = sc.xworld, me = sc.xrank, nv = n_seg + 1;
         const int par = (int)(((sc.xepoch & 1ull) << 1) | (sc.seq & 1ull));
