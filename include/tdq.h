@@ -436,6 +436,22 @@ int tdq_fixed_emit_cubic_grad(int32_t dtype, const void *y0, const void *y1, con
                               const int32_t *out_idx_dev, const void *coef_dev, int32_t n_records, int32_t rec_lo,
                               int32_t rec_hi, size_t n, double *dots, double *partials, void *stream);
 
+/* The adjoint of one Adams step's history sums (the tdq_lincomb predictor dy0 = sum_j T(cp_j) f_j and corrector
+ * delta = sum_j T(cc_j) f_j of fixed_adams.py:200-215), for gradients of the discrete solve, in one pass over the state:
+ *   fbar[j] <- (fbar[j] + T(cp[j])*dy0bar) + T(cc[j])*deltabar      j = 0 .. p-1, 1 <= p <= 11,
+ * every product and sum rounded in the state dtype; the cc term only when deltabar != NULL (the explicit method has no
+ * corrector).  fbar: HOST array of p distinct n-element device accumulators; cp, cc, wp, wc: HOST float64 arrays of p.
+ * With dots != NULL also
+ *   dots[0] = <dy0bar, sum_j wp[j] f[j]>,   dots[1] = <deltabar, sum_j wc[j] f[j]>  (only with deltabar)    float64,
+ * each element's sum over j formed in float64, j ascending, and the elements summed in an order that depends on n only,
+ * so a call repeats bit for bit; f is then a HOST array of the p history values and `partials` needs
+ * tdq_adams_grad_hist_partials_len(dtype, n) doubles of scratch (no initial value; not shared with a concurrent call).
+ * 0 for an unsupported dtype. */
+size_t tdq_adams_grad_hist_partials_len(int32_t dtype, size_t n);
+int tdq_adams_grad_hist(int32_t dtype, const void *dy0bar, const void *deltabar, void *const *fbar, const void *const *f,
+                        const double *cp, const double *cc, const double *wp, const double *wc, int32_t p, size_t n,
+                        double *dots, double *partials, void *stream);
+
 /* ---- implicit fixed-grid Runge-Kutta: Broyden's iteration as low-rank streaming passes (tdq_implicit.cu) --------------
  * rk_common.py:438-459 (FIRK, one solve over every active stage) and :525-547 (DIRK, one solve per stage) keep a dense
  * M x M Jacobian estimate.  J starts at I and only receives rank-1 updates whose vector is the new residual, so

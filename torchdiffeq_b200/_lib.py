@@ -172,6 +172,8 @@ _SIGNATURES = {
     "tdq_fixed_emit_cubic_grad_partials_len": (_sz, [_i32, _sz, _i32]),
     "tdq_fixed_emit_cubic_grad": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32,
                                             _i32, _sz, _vp, _vp, _vp]),
+    "tdq_adams_grad_hist_partials_len": (_sz, [_i32, _sz]),
+    "tdq_adams_grad_hist": (C.c_int, [_i32, _vp, _vp, _pp, _pp, _pdbl, _pdbl, _pdbl, _pdbl, _i32, _sz, _vp, _vp, _vp]),
     "tdq_pack_segments": (C.c_int, [_i32, _vp, _pp, _pi64, _pi64, _pdbl, _i32, _vp]),
     "tdq_implicit_partials_len": (_sz, [_i32]),
     "tdq_implicit_state_len": (_sz, [_i32]),

@@ -467,13 +467,9 @@ def _cubic_emit_backward(sa, cub, k, y0, y1, f0, t1_dev, grad_sol, ybar1, sign, 
     return acc[0], ybar1, f0bar
 
 
-def fixed_backward(p, method, tape, grid, t_cpu, grad_sol, params, need_t):
-    """Reverse sweep over the steps of a fixed-grid solve (solvers.py:102-128, linear interpolation :175-181, cubic
-    Hermite :166-173).
-    grid / t_cpu: ascending CPU tensors.  Returns (grid_bar, t_out_bar) as float64 device tensors (or None), y0_bar,
-    [param_bar]."""
-    dev, T, sign = p.device, p.dtype, p.t_sign
-    alpha, beta, wts = FIXED_TABLEAUS[method]
+def _ascending_field(p):
+    """Reference-sense dynamics in the ascending engine time s = sign * t (misc.py:158-165), flat."""
+    sign = p.t_sign
 
     def F(s_, y_):
         out = p.fn(s_ * sign, y_)
@@ -481,70 +477,236 @@ def fixed_backward(p, method, tape, grid, t_cpu, grad_sol, params, need_t):
             out = p.layout.flatten(list(out))
         out = out.reshape(-1)
         return out * sign if sign != 1.0 else out
-    sa = StepAdjoint(F, params, need_t)
+    return F
+
+
+def _outputs_backward(sa, st, k, g0, g1, y0, y1, f0, t_cpu, grad_sol, ybar1, sign, gbar, obar):
+    """Adjoint of the outputs grid step k produced: linear interpolation (solvers.py:175-181) or cubic Hermite
+    (:166-173, _cubic_emit_backward), for fixed_backward and adams_backward alike.  f0: the step's f(t0, y0),
+    reference-sense.  Returns (ybar0, ybar1, f0bar); the time terms go into gbar and obar."""
+    T, dev, need_t = y0.dtype, y0.device, sa.need_t
+    ybar0, f0bar = None, None
+    cub = st.get("cubic")
+    if cub is not None and cub.hi > cub.lo:
+        ybar0, ybar1, f0bar = _cubic_emit_backward(sa, cub, k, y0, y1, f0, _dev(g1.to(T), dev), grad_sol, ybar1, sign,
+                                                   gbar, obar)
+    h = float(g1 - g0)
+    for (j, mode, slope) in st.get("outs", ()):                        # solvers.py:175-181
+        G = grad_sol[j]
+        if mode == 0:
+            ybar0 = _acc(ybar0, G)
+        elif mode == 1:
+            ybar1 = _acc(ybar1, G)
+        else:
+            sl = float(torch.as_tensor(slope).to(T))
+            ybar0 = _acc(ybar0, G, 1.0 - sl)
+            ybar1 = _acc(ybar1, G, sl)
+            if need_t:
+                sb = torch.dot(G.double(), (y1 - y0).double())
+                frac = float(t_cpu[j] - g0) / h
+                obar[j] += sb / h
+                gbar[k] += sb * (-1.0 / h + frac / h)
+                gbar[k + 1] += sb * (-frac / h)
+    return ybar0, ybar1, f0bar
+
+
+class _RkStep:
+    """One explicit fixed-grid step (fixed_grid.py:6-60) recomputed from its y0 for the reverse sweep, and its adjoint.
+    k1 = f(t0, y0) unless given: an Adams bootstrap step's k1 is its newest history entry (fixed_adams.py:196-197)."""
+
+    def __init__(self, sa, method, g0, g1, y0, perturb, k1=None):
+        T, dev = y0.dtype, y0.device
+        self.sa, self.y0 = sa, y0
+        self.alpha, beta, self.wts = FIXED_TABLEAUS[method]
+        dt = g1 - g0                                                   # t's dtype, like the reference (solvers.py:112)
+        self.dtf = dtf = float(dt.to(T))
+        ts = stage_times(method, g0, dt, g1, perturb, T)              # the forward step's func times
+        self.times = [_dev(tt, dev) for tt in ts[1:1 + len(self.alpha)]]
+        self.t0_dev = _dev(ts[0], dev)
+        if k1 is None:
+            with torch.no_grad():
+                k1 = sa.F(self.t0_dev, y0)
+        self.coefs = [[b * dtf for b in row] for row in beta]
+        self.Ys, self.ks = sa.stages(self.times, y0, k1, self.coefs)
+        incr = None
+        for kk, w in zip(self.ks, self.wts):
+            if w != 0.0:
+                incr = _acc(incr, kk, w)                               # dy / dt
+        self.incr = incr
+        self.y1 = y0 + incr * dtf
+
+    def backward(self, k, ybar0, ybar1, f0bar, gbar):
+        """Adjoint of the stages and of y1 = y0 + dt sum_j w_j k_j; f0bar joins k_1's cotangent.  The stage times'
+        parts go into gbar[k].  Returns (ybar0, kbar0, dtbar): k_1's cotangent and dt's adjoint for the caller."""
+        sa, dtf, y0 = self.sa, self.dtf, self.y0
+        kbar = [None] * (len(self.alpha) + 1)
+        kbar[0] = f0bar
+        dtbar = None
+        if ybar1 is not None:
+            ybar0 = _acc(ybar0, ybar1)
+            for j, w in enumerate(self.wts):
+                if w != 0.0:
+                    kbar[j] = _acc(kbar[j], ybar1, w * dtf)
+            if sa.need_t:
+                dtbar = _acc(dtbar, torch.dot(ybar1.double(), self.incr.double()))
+        ybar0, kbar0, tsum, per_stage = sa.sweep(self.times, self.Ys, self.coefs, kbar, ybar0, None)
+        if sa.need_t:
+            for i, (Yb, tb) in enumerate(per_stage):
+                if Yb is not None and dtf != 0.0:
+                    dtbar = _acc(dtbar, torch.dot(Yb.double(), ((self.Ys[i] - y0) / dtf).double()))
+                if tb is not None:
+                    gbar[k] += tb.double()
+                    dtbar = _acc(dtbar, tb.double(), self.alpha[i])
+        return ybar0, kbar0, dtbar
+
+
+def fixed_backward(p, method, tape, grid, t_cpu, grad_sol, params, need_t):
+    """Reverse sweep over the steps of a fixed-grid solve (solvers.py:102-128, linear interpolation :175-181, cubic
+    Hermite :166-173).
+    grid / t_cpu: ascending CPU tensors.  Returns (grid_bar, t_out_bar) as float64 device tensors (or None), y0_bar,
+    [param_bar]."""
+    dev, sign = p.device, p.t_sign
+    sa = StepAdjoint(_ascending_field(p), params, need_t)
     gbar = torch.zeros(grid.numel(), dtype=torch.float64, device=dev) if need_t else None
     obar = torch.zeros(t_cpu.numel(), dtype=torch.float64, device=dev) if need_t else None
     gy = None
     for st in reversed(tape):
         k = st["k"]
         g0, g1 = grid[k], grid[k + 1]
-        dt = g1 - g0                                                   # t's dtype, like the reference (solvers.py:112)
-        dtf = float(dt.to(T))
         y0 = st["y0"]
-        ts = stage_times(method, g0, dt, g1, st["perturb"], T)        # the forward step's func times
-        times = [_dev(tt, dev) for tt in ts[1:1 + len(alpha)]]
-        t0_dev = _dev(ts[0], dev)
-        with torch.no_grad():
-            k1 = F(t0_dev, y0)
-        coefs = [[b * dtf for b in row] for row in beta]
-        Ys, ks = sa.stages(times, y0, k1, coefs)
-        incr = None
-        for kk, w in zip(ks, wts):
-            if w != 0.0:
-                incr = _acc(incr, kk, w)                               # dy / dt
-        y1 = y0 + incr * dtf
-        ybar1, ybar0, f0bar = gy, None, None
-        cub = st.get("cubic")
-        if cub is not None and cub.hi > cub.lo:
-            ybar0, ybar1, f0bar = _cubic_emit_backward(sa, cub, k, y0, y1, k1, _dev(g1.to(T), dev), grad_sol, ybar1,
-                                                       sign, gbar, obar)
-        h = float(g1 - g0)
-        for (j, mode, slope) in st.get("outs", ()):                    # solvers.py:175-181
-            G = grad_sol[j]
-            if mode == 0:
-                ybar0 = _acc(ybar0, G)
-            elif mode == 1:
-                ybar1 = _acc(ybar1, G)
-            else:
-                sl = float(torch.as_tensor(slope).to(T))
-                ybar0 = _acc(ybar0, G, 1.0 - sl)
-                ybar1 = _acc(ybar1, G, sl)
-                if need_t:
-                    sb = torch.dot(G.double(), (y1 - y0).double())
-                    frac = float(t_cpu[j] - g0) / h
-                    obar[j] += sb / h
-                    gbar[k] += sb * (-1.0 / h + frac / h)
-                    gbar[k + 1] += sb * (-frac / h)
-        kbar = [None] * (len(alpha) + 1)
-        kbar[0] = f0bar                                                # the cubic outputs' f0 is the step's k_1
-        dtbar = None
-        if ybar1 is not None:
-            ybar0 = _acc(ybar0, ybar1)
-            for j, w in enumerate(wts):
-                if w != 0.0:
-                    kbar[j] = _acc(kbar[j], ybar1, w * dtf)
-            if need_t:
-                dtbar = _acc(dtbar, torch.dot(ybar1.double(), incr.double()))
-        ybar0, kbar0, tsum, per_stage = sa.sweep(times, Ys, coefs, kbar, ybar0, None)
-        if need_t:
-            for i, (Yb, tb) in enumerate(per_stage):
-                if Yb is not None and dtf != 0.0:
-                    dtbar = _acc(dtbar, torch.dot(Yb.double(), ((Ys[i] - y0) / dtf).double()))
-                if tb is not None:
-                    gbar[k] += tb.double()
-                    dtbar = _acc(dtbar, tb.double(), alpha[i])
+        rk = _RkStep(sa, method, g0, g1, y0, st["perturb"])
+        ybar0, ybar1, f0bar = _outputs_backward(sa, st, k, g0, g1, y0, rk.y1, rk.ks[0], t_cpu, grad_sol, gy, sign, gbar,
+                                                obar)
+        ybar0, kbar0, dtbar = rk.backward(k, ybar0, ybar1, f0bar, gbar)   # the cubic outputs' f0 is the step's k_1
         if kbar0 is not None:                                          # k_1 = f(t0, y0), a fresh evaluation every step
-            gyk, tb = sa.vjp(t0_dev, y0, kbar0)
+            gyk, tb = sa.vjp(rk.t0_dev, y0, kbar0)
+            ybar0 = _acc(ybar0, gyk)
+            if need_t and tb is not None:
+                gbar[k] += tb.double()
+        if need_t and dtbar is not None:
+            gbar[k + 1] += dtbar
+            gbar[k] -= dtbar
+        gy = ybar0
+    y0bar = _acc(gy, grad_sol[0])
+    return gbar, obar, y0bar, sa.pbar
+
+
+def adams_hist_grad(dy0bar, deltabar, fbars, fs, cp, cc, wp, wc, need_dots):
+    """The adjoint of one Adams step's history sums (tdq_adams_grad_hist): fbars[j] += T(cp_j) dy0bar + T(cc_j) deltabar
+    in place (deltabar None for the explicit method); with need_dots also dt's adjoint <dy0bar, sum_j wp_j fs_j> +
+    <deltabar, sum_j wc_j fs_j>, a float64 0-dim device tensor (else None)."""
+    lib, T, n = _lib.load(), dy0bar.dtype, dy0bar.numel()
+    dc = _DTYPES[T]
+    dots = partials = None
+    if need_dots:
+        dots = torch.empty(2, dtype=torch.float64, device=dy0bar.device)
+        partials = torch.empty(lib.tdq_adams_grad_hist_partials_len(dc, n), dtype=torch.float64, device=dy0bar.device)
+    has_delta = deltabar is not None
+    _lib.check(lib.tdq_adams_grad_hist(
+        dc, dy0bar.data_ptr(), deltabar.data_ptr() if has_delta else None, _lib.ptr_array([b.data_ptr() for b in fbars]),
+        _lib.ptr_array([f.data_ptr() for f in fs]), _lib.dbl_array(cp), _lib.dbl_array(cc) if has_delta else None,
+        _lib.dbl_array(wp), _lib.dbl_array(wc) if has_delta else None, len(fbars), n,
+        dots.data_ptr() if need_dots else None, partials.data_ptr() if need_dots else None, _stream()))
+    if not need_dots:
+        return None
+    return dots[0] + dots[1] if has_delta else dots[0]
+
+
+def adams_backward(p, method, tape, grid, t_cpu, grad_sol, params, need_t, lc=None, hist_grad=adams_hist_grad):
+    """Reverse sweep over the steps of an Adams solve (AdamsBashforthMoulton._step_func, fixed_adams.py:193-222, inside
+    solvers.py:102-128), on the tape of AdamsEngine: every step's y0, its raw f0 = func(t0, y0) and an AdamsTape.
+    Arguments and result as fixed_backward.  lc / hist_grad: the state-sized sums, the forward's tdq_lincomb and
+    tdq_adams_grad_hist unless given (a CPU restatement can stand in for both).
+
+    A history entry's cotangent collects the contributions of up to 11 later steps and is complete when the sweep
+    reaches its own step; then one VJP of f(t0, y0) takes it into y0, t0 and the parameters.  The cotangents are kept
+    for RAW func outputs, so the kernel's coefficients are the forward's own; a reference-sense f's is sign * that."""
+    from ._adams import _BASHFORTH, _MOULTON, ADAMS_METHODS, AdamsSums, lincomb
+    dev, T, sign, n = p.device, p.dtype, p.t_sign, p.n
+    implicit = ADAMS_METHODS[method]
+    if lc is None:
+        lib, dc = _lib.load(), _DTYPES[T]
+        lc = lambda out, base, terms: lincomb(lib, dc, n, out, base, terms)
+    sa = StepAdjoint(_ascending_field(p), params, need_t)
+    gbar = torch.zeros(grid.numel(), dtype=torch.float64, device=dev) if need_t else None
+    obar = torch.zeros(t_cpu.numel(), dtype=torch.float64, device=dev) if need_t else None
+    # tape index -> cotangent of that step's raw f0, for the entries a later step still reads (at most max_order).  A
+    # buffer is dropped after its VJP, never reused: autograd may return the cotangent it was given as a parameter's
+    # gradient (a func output that is a parameter plus something), and StepAdjoint keeps that tensor.
+    fbar = {}
+
+    def fb(j):
+        b = fbar.get(j)
+        if b is None:
+            b = fbar[j] = torch.zeros(n, dtype=T, device=dev)
+        return b
+    gy = None
+    for st in reversed(tape):
+        k, ad, y0 = st["k"], st["adams"], st["y0"]
+        g0, g1 = grid[k], grid[k + 1]
+        dt = g1 - g0                                                   # t's dtype (solvers.py:112)
+        ts = stage_times("rk4", g0, dt, g1, st["perturb"], T)          # f0 at t0 (Perturb.NEXT), the corrector at t1 (PREV)
+        t0_dev, t1_dev = _dev(ts[0], dev), _dev(ts[3], dev)
+        f0 = st["f"] * sign if sign != 1.0 else st["f"]
+        # ---- recompute: y1, and the corrector's evaluations with their graphs -------------------------------------
+        recs = []
+        if ad.bootstrap:
+            k1 = tape[ad.hist[0]]["f"]
+            rk = _RkStep(sa, "rk4", g0, g1, y0, st["perturb"], k1=k1 * sign if sign != 1.0 else k1)
+            y1 = rk.y1
+        else:
+            sums = AdamsSums(lc, ad.order, dt, sign, T, implicit)
+            hist = [tape[j]["f"] for j in ad.hist]
+            dy = sums.predict(hist, y0)
+            if implicit:
+                delta = sums.delta(hist, y0)
+                for _ in range(ad.iters):                              # the forward's points, bit for bit
+                    Y = torch.empty_like(y0)
+                    sums.point(Y, y0, dy)
+                    recs.append(sa.record(t1_dev, Y))
+                    phi = recs[-1][2].detach()
+                    dy = sums.correct((phi * sign if sign != 1.0 else phi).to(T).contiguous(), delta)
+            y1 = torch.empty_like(y0)
+            sums.point(y1, y0, dy)
+        # ---- outputs of the step ------------------------------------------------------------------------------------
+        ybar0, ybar1, f0bar = _outputs_backward(sa, st, k, g0, g1, y0, y1, f0, t_cpu, grad_sol, gy, sign, gbar, obar)
+        if f0bar is not None:
+            fb(k).add_(f0bar, alpha=sign)
+        # ---- the step -----------------------------------------------------------------------------------------------
+        dtbar = None
+        if ad.bootstrap:
+            ybar0, kbar0, dtbar = rk.backward(k, ybar0, ybar1, None, gbar)
+            if kbar0 is not None:
+                fb(ad.hist[0]).add_(kbar0, alpha=sign)
+        elif ybar1 is not None:
+            ybar0 = _acc(ybar0, ybar1)
+            ddy, dbar = ybar1, None                                    # cotangents of dy_i and of delta
+            if implicit:
+                m0, cphi = _MOULTON[ad.order + 1][0], sums.c0 * sign              # dy's weight of f(t1, .): T(dt m_0)
+            for rec in reversed(recs):                                 # dy_{i+1} = T(dt m_0) f(t1, y0 + dy_i) + delta
+                dbar = _acc(dbar, ddy)
+                if need_t:
+                    dtbar = _acc(dtbar, torch.dot(ddy.double(), rec[2].detach().double()) * m0)
+                gY, tb = sa.vjp(t1_dev, None, (ddy * cphi).to(rec[2].dtype), rec=rec)
+                if need_t and tb is not None:
+                    gbar[k + 1] += tb.double()
+                if gY is None:
+                    ddy = None
+                    break
+                ybar0 = _acc(ybar0, gY)
+                ddy = gY
+            if ddy is None:
+                ddy = torch.zeros_like(y0)
+            wp = [sign * b for b in _BASHFORTH[ad.order]]
+            cc = [sums.dt_T * c for c in sums.cs] if dbar is not None else None
+            dots = hist_grad(ddy.to(T).contiguous(), dbar.to(T).contiguous() if dbar is not None else None,
+                             [fb(j) for j in ad.hist], hist, sums.cp, cc, wp, sums.cs if dbar is not None else None,
+                             need_t)
+            dtbar = _acc(dtbar, dots)
+        # ---- f0 = f(t0, y0): its cotangent is complete --------------------------------------------------------------
+        b = fbar.pop(k, None)
+        if b is not None:
+            gyk, tb = sa.vjp(t0_dev, y0, b * sign if sign != 1.0 else b)
             ybar0 = _acc(ybar0, gyk)
             if need_t and tb is not None:
                 gbar[k] += tb.double()
@@ -584,9 +746,10 @@ class _BackpropFunction(torch.autograd.Function):
                                                           ctx.need_t)
             else:
                 grid_req, grid, t_req = ctx.aux["grid_req"], ctx.aux["grid"], ctx.aux["t_req"]
+                sweep = adams_backward if ctx.aux.get("adams") else fixed_backward
                 with torch.no_grad():
-                    gbar, obar, y0bar, pbar = fixed_backward(p, p.method, ctx.aux["tape"], grid, p.t_cpu, grad_sol, params,
-                                                             ctx.need_t)
+                    gbar, obar, y0bar, pbar = sweep(p, p.method, ctx.aux["tape"], grid, p.t_cpu, grad_sol, params,
+                                                    ctx.need_t)
                 tbar = None
                 if ctx.need_t:
                     # the grid as a differentiable function of the (ascending) output times, whatever constructor made it

@@ -3,6 +3,7 @@
 //   k_rk4        stage values and the final update of rk4_alt_step_func   rk_common.py:110-118, fixed_grid.py:24-29, solvers.py:115
 //   k_fixed_emit outputs of one grid step by linear interpolation         solvers.py:117-125, :175-181
 //   k_fixed_emit_cubic(_grad)  cubic Hermite outputs of one step, and their adjoint   solvers.py:120-122, :166-173
+//   k_adams_grad_hist  adjoint of one Adams step's predictor / corrector history sums  fixed_adams.py:200-215
 //   k_pack       concat + per-segment scale of the augmented dynamics     misc.py:137-145, :158-165, adjoint.py:94-105
 //
 // The step size comes from a device array indexed by a device step counter so that one captured
@@ -295,6 +296,76 @@ inline size_t cubic_grad_blocks(size_t n, int vn) {
     return b ? b : 1;
 }
 
+// Adjoint of the history sums of one Adams step (fixed_adams.py:200-215), in one pass over the state:
+//   fbar_j <- (fbar_j + cp_j*dy0bar) + cc_j*deltabar      j = 0 .. p-1, every product and sum rounded in T
+// (the cc term only with DELTA) and, with DOTS, the float64 partial sums of this block at partials[q * gridDim.x +
+// blockIdx.x] of
+//   q = 0: <dy0bar, sum_j wp_j f_j>,   q = 1: <deltabar, sum_j wc_j f_j>      (q = 1 only with DELTA)
+// where each element's sum over j is formed in float64, j ascending.  Element ownership is that of
+// k_fixed_emit_cubic_grad (ld_group / st_group), so the partials depend on n alone.  The p <= 11 terms are unrolled so
+// the by-value arrays are only indexed by constants.
+constexpr int kAdamsHist = 11;                  // the deque of fixed_adams.py:179 holds at most _MAX_ORDER - 1 entries
+
+struct AdamsHistArgs {
+    void *fbar[kAdamsHist];
+    const void *f[kAdamsHist];
+    double cp[kAdamsHist], cc[kAdamsHist], wp[kAdamsHist], wc[kAdamsHist];
+};
+
+template <typename T, bool DELTA, bool DOTS>
+__global__ void __launch_bounds__(kThreads)
+k_adams_grad_hist(const T *__restrict__ dy0bar, const T *__restrict__ deltabar, const AdamsHistArgs a, int p, size_t n,
+                  double *__restrict__ partials) {
+    using A = Ar<T>;
+    using V = Vec<T>;
+    __shared__ double red[kThreads / 32];
+    const size_t i0 = ((size_t)blockIdx.x * kThreads + threadIdx.x) * V::N;
+    const V g = ld_group(dy0bar, tdq_dev_aligned16(dy0bar), i0, n);
+    V d;
+    if (DELTA) d = ld_group(deltabar, tdq_dev_aligned16(deltabar), i0, n);
+    double sp[V::N], sc[V::N];
+#pragma unroll
+    for (int e = 0; e < V::N; ++e) sp[e] = sc[e] = 0.0;
+#pragma unroll
+    for (int j = 0; j < kAdamsHist; ++j) {
+        if (j < p) {
+            T *fb = reinterpret_cast<T *>(a.fbar[j]);
+            const bool al = tdq_dev_aligned16(fb);
+            V acc = ld_group<T>(fb, al, i0, n);
+            const T cp = (T)a.cp[j], cc = (T)a.cc[j];
+#pragma unroll
+            for (int e = 0; e < V::N; ++e) {
+                acc.v[e] = A::add(acc.v[e], A::mul(cp, g.v[e]));
+                if (DELTA) acc.v[e] = A::add(acc.v[e], A::mul(cc, d.v[e]));
+            }
+            st_group(fb, al, i0, n, acc);
+            if (DOTS) {
+                const T *f = reinterpret_cast<const T *>(a.f[j]);
+                const V fv = ld_group(f, tdq_dev_aligned16(f), i0, n);
+#pragma unroll
+                for (int e = 0; e < V::N; ++e) {
+                    sp[e] += a.wp[j] * (double)fv.v[e];
+                    if (DELTA) sc[e] += a.wc[j] * (double)fv.v[e];
+                }
+            }
+        }
+    }
+    if (DOTS) {                                 // elements past n were loaded as zeros and add nothing
+        double dp = 0.0, dc = 0.0;
+#pragma unroll
+        for (int e = 0; e < V::N; ++e) {
+            dp += (double)g.v[e] * sp[e];
+            if (DELTA) dc += (double)d.v[e] * sc[e];
+        }
+        const double s0 = block_sum<kThreads>(dp, red);
+        if (threadIdx.x == 0) partials[blockIdx.x] = s0;
+        if (DELTA) {
+            const double s1 = block_sum<kThreads>(dc, red);
+            if (threadIdx.x == 0) partials[gridDim.x + blockIdx.x] = s1;
+        }
+    }
+}
+
 // Generic linear combination for the multistep (Adams) predictor / corrector of fixed_adams.py:198-215:
 //   out = [base +] ((x_0*c_0 + x_1*c_1) + x_2*c_2) + ...      products and sums rounded separately, ascending order,
 // the first product initialises the sum (Python's sum() starts from 0 + x_0*c_0 = x_0*c_0 exactly).
@@ -464,6 +535,50 @@ int tdq_fixed_emit_cubic_grad(int32_t dtype, const void *y0, const void *y1, con
     if (dots) {
         const int n_dots = 4 * (rec_hi - rec_lo);
         k_fixed_emit_cubic_dots<<<(n_dots + 3) / 4, 128, 0, st>>>(partials, (int)blocks, n_dots, dots);
+        TDQ_CHECK_CUDA(cudaGetLastError());
+    }
+    return TDQ_OK;
+}
+
+size_t tdq_adams_grad_hist_partials_len(int32_t dtype, size_t n) {
+    if (dtype != TDQ_F32 && dtype != TDQ_F64) return 0;
+    return 2 * cubic_grad_blocks(n, dtype == TDQ_F32 ? Vec<float>::N : Vec<double>::N);
+}
+
+int tdq_adams_grad_hist(int32_t dtype, const void *dy0bar, const void *deltabar, void *const *fbar, const void *const *f,
+                        const double *cp, const double *cc, const double *wp, const double *wc, int32_t p, size_t n,
+                        double *dots, double *partials, void *stream) {
+    TDQ_REQUIRE(dy0bar && fbar && cp, "null argument");
+    TDQ_REQUIRE(p >= 1 && p <= kAdamsHist, "p out of range");
+    TDQ_REQUIRE(deltabar == nullptr || cc != nullptr, "deltabar needs cc");
+    TDQ_REQUIRE(dots == nullptr || (partials && f && wp && (deltabar == nullptr || wc)),
+                "dots need f, wp (and wc with deltabar) and tdq_adams_grad_hist_partials_len(dtype, n) doubles of partials");
+    TDQ_REQUIRE(dtype == TDQ_F32 || dtype == TDQ_F64, "unsupported dtype");
+    const size_t blocks = cubic_grad_blocks(n, dtype == TDQ_F32 ? Vec<float>::N : Vec<double>::N);
+    TDQ_REQUIRE(n > 0 && blocks <= 0x7fffffffu, "n out of range");
+    AdamsHistArgs a;
+    memset(&a, 0, sizeof(a));
+    for (int j = 0; j < p; ++j) {
+        TDQ_REQUIRE(fbar[j] != nullptr, "null accumulator");
+        TDQ_REQUIRE(dots == nullptr || f[j] != nullptr, "null history value");
+        a.fbar[j] = fbar[j];
+        a.f[j] = dots ? f[j] : nullptr;
+        a.cp[j] = cp[j];
+        a.cc[j] = deltabar ? cc[j] : 0.0;
+        a.wp[j] = dots ? wp[j] : 0.0;
+        a.wc[j] = dots && deltabar ? wc[j] : 0.0;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    TDQ_DISPATCH_T(dtype, tdq_dispatch(TdqBool{}, deltabar != nullptr, [&](auto E) {
+                       return tdq_dispatch(TdqBool{}, dots != nullptr, [&](auto D) {
+                           k_adams_grad_hist<T, E, D><<<(unsigned)blocks, kThreads, 0, st>>>(
+                               (const T *)dy0bar, (const T *)deltabar, a, p, n, partials);
+                           return 0;
+                       });
+                   }));
+    TDQ_CHECK_CUDA(cudaGetLastError());
+    if (dots) {
+        k_fixed_emit_cubic_dots<<<1, 128, 0, st>>>(partials, (int)blocks, deltabar ? 2 : 1, dots);
         TDQ_CHECK_CUDA(cudaGetLastError());
     }
     return TDQ_OK;

@@ -918,9 +918,6 @@ def _odeint_backprop(p, func, y0, t, params, _stats):
             holder["eng"] = eng
             return sol.clone(), {"kind": "adaptive", "tape": tape, "tab": adaptive_tableau(p.method)}
         o = p.options
-        if p.method in ADAMS_METHODS:
-            raise NotImplementedError("gradients of the discrete solve are implemented for the explicit Runge-Kutta "
-                                      "methods; use odeint_adjoint with the Adams methods")
         if p.method in IMPLICIT_METHODS:
             raise NotImplementedError("gradients through the discrete implicit solve (Broyden's iteration) are not "
                                       "implemented; use odeint_adjoint with the implicit methods")
@@ -932,7 +929,8 @@ def _odeint_backprop(p, func, y0, t, params, _stats):
         eng = _make_fixed_engine(p, graph=False)
         sol, tape = eng.solve_taped(p.y0_flat, grid, p.t_cpu)
         holder["eng"] = eng
-        return sol, {"kind": "fixed", "tape": tape, "grid": grid, "grid_req": grid_req, "t_req": t_req}
+        return sol, {"kind": "fixed", "tape": tape, "grid": grid, "grid_req": grid_req, "t_req": t_req,
+                     "adams": p.method in ADAMS_METHODS}
     with on_solver_stream(p.device) as ss:
         sol = _BackpropFunction.apply(p, run, t, y0_flat, *params)
         ss.publish(sol)
@@ -991,7 +989,8 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
     accepts `graph` (True/False/'auto'), `run_ahead` (int; 0 reproduces the reference's exact func
     call sequence) and `process_group` (batch-sharded solve with a common step size).
     Under autograd the result carries the gradient of the discrete solve w.r.t. y0, t and func's parameters
-    (backprop.py); odeint_adjoint gives the continuous adjoint instead.
+    (backprop.py) for the adaptive, explicit fixed-grid and Adams methods (linear or cubic outputs); the implicit
+    Runge-Kutta methods refuse it.  odeint_adjoint gives the continuous adjoint instead.
 
     options={'independent_rows': True} (adaptive methods, tensor y0 of shape [B, *rest]): every row y0[r] gets its own step
     size control, so row r's result is the reference's odeint(func, y0[r:r+1], t) for a row-wise func and does not depend
