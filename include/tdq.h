@@ -496,6 +496,41 @@ int tdq_implicit_update(int32_t dtype, void *x, int32_t n_stages, size_t n, cons
                         const void *f0, void *y_out, const void *y0, const void *const *k, const double *coefs,
                         int32_t n_terms, double *partials, double *out, void *stream);
 
+/* The reverse of one Broyden solve, for gradients of the discrete implicit solve (DESIGN.md section 5b).  With the
+ * forward's banks U (slot j+1 = R_{j+1}) and S (slot j = s_j), its raw dot matrix in `state`, and a bank L of
+ * lambda_m = J_m^-T sbar_m in the same chunking, reverse iteration m = m*-1 .. 0 is:
+ * tdq_implicit_grad_combine: out = T(base + sum_{q < n_terms} coefs_dev[q] * v_{v_lo+q}) over M = n_stages*n elements,
+ *   accumulated in float64 (base first, q ascending) and rounded once; base may be NULL.  Then float64 dots
+ *   out_dots[q] = out . d_{d_lo+q} for q < n_dots and out_dots[n_dots+q] = v_{g_slot} . v_q for q < n_gram, reduced as
+ *   the forward's (partials: tdq_implicit_partials_len(n_dots + n_gram) doubles, zeroed once).  coefs_dev is DEVICE
+ *   memory (a row of the workspace below), so the sweep makes no host read.  Moves
+ *   (1 + n_terms + n_dots + n_gram + [n_gram > 0] + 1 + (sweeps - 1)) * M * sizeof(T) bytes, sweeps = ceil((n_dots +
+ *   n_gram) / 8): base, the terms, the dot and Gram vectors and the Gram row's own vector read, out written, and out
+ *   read again by every further sweep of 8 dots.
+ * tdq_implicit_grad_solve: one CTA, float64.  Solves (diag(sigma) + U^T S) v = U^T sbar_m (dots[0..m): U^T sbar_m from
+ *   the combine, dots[m..2m): s_m . s_j), the transpose of diag(sigma) C, from the forward's state; then with
+ *   mu_j = lambda_m . R_{j+1} = dots[j] - (U^T S v)_j it writes, in ws (tdq_implicit_grad_ws_len(max_iters) doubles):
+ *   vneg = -v, Acoef[j][m] = -mu_j/sigma_j, Acoef[j][j] += 2 mu_j G_j / sigma_j^2, Qcoef[j][m] = G_j/sigma_j + [j = m-1]
+ *   (j < m).  Row j of Acoef: s_j's cotangent is Xbar + sum_q Acoef[j][q] s_q; row j of Qcoef: -R_{j+1}'s cotangent is
+ *   sum_q Qcoef[j][q] lambda_q.  Both tables are zeroed when m == m_star - 1.  ws = [Acoef | Qcoef | vneg | scratch].
+ * tdq_implicit_grad_stage: the adjoint of stage values y_r = y0 + sum_j T(coefs[r][j]) k_j (and of y1 = y0 + sum_j
+ *   T(c_j) k_j with one row): xbar -= q over x_rows*n elements when xbar != NULL, then per element
+ *   y0bar += sum_r ybar_r and kbar_j += T(coefs[r][j]) * ybar_r (r ascending, in T); kbar pointers may alias one
+ *   another and xbar.  With dot != NULL also dot[0] = sum_e sum_{r,j} w[r][j] ybar_r[e] k_j[e] in float64 (partials:
+ *   tdq_implicit_partials_len(1)).  coefs, w: HOST n_rows*n_terms float64.  Moves
+ *   (3 x_rows + n_rows + 2 + 2 n_terms [+ n_terms with dot]) * n * sizeof(T) bytes. */
+size_t tdq_implicit_grad_ws_len(int32_t max_iters);
+int tdq_implicit_grad_combine(int32_t dtype, void *out, const void *base, int32_t n_stages, size_t n,
+                              const void *const *v_chunks, const void *const *d_chunks, int32_t n_chunks,
+                              int64_t per_chunk, const double *coefs_dev, int32_t v_lo, int32_t n_terms, int32_t d_lo,
+                              int32_t n_dots, int32_t g_slot, int32_t n_gram, double *partials, double *out_dots,
+                              void *stream);
+int tdq_implicit_grad_solve(const double *state, const double *dots, double *ws, int32_t m, int32_t m_star,
+                            int32_t max_iters, void *stream);
+int tdq_implicit_grad_stage(int32_t dtype, const void *const *ybar, int32_t n_rows, size_t n, void *const *kbar,
+                            const void *const *k, const double *coefs, const double *w, int32_t n_terms, void *y0bar,
+                            void *xbar, const void *q, int32_t x_rows, double *partials, double *dot, void *stream);
+
 /* ---- sharded solves: norm partials exchanged over NVLink peer memory INSIDE tdq_controller ----- */
 /* The reference has no multi-GPU path; its RMS norm is a mean over the whole batch (misc.py:22-23), so
  * batch-sharded ranks must sum their n_seg+1 float64 partials before every accept/reject decision.

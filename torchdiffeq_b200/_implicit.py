@@ -16,7 +16,7 @@ import warnings
 import torch
 
 from . import _lib
-from ._engine import _stream
+from ._engine import _RetryWithCopies, _stream
 from ._fixed import FixedGridEngine
 
 _CONVERGED, _SINGULAR, _EXHAUSTED = 1, 2, 3
@@ -56,6 +56,16 @@ TABLEAUS = _tableaus()
 IMPLICIT_METHODS = tuple(TABLEAUS)
 
 
+def stage_time(a, t0, dt, t1):
+    """The func time of a stage with alpha = a (a tensor of the state dtype), from t0, dt and t1 of that dtype in the
+    engine's ascending time (rk_common.py:471-481)."""
+    if bool(a == 1.):
+        return torch.nextafter(t1, t1 - 1)                        # Perturb.PREV (misc.py:190-192)
+    if bool(a == 0.):
+        return t0
+    return t0 + a * dt
+
+
 class ImplicitEngine(FixedGridEngine):
     """FixedGridFIRKODESolver / FixedGridDIRKODESolver._step_func (rk_common.py:415-466, :488-554) as the step of the
     fixed-grid engine."""
@@ -82,6 +92,7 @@ class ImplicitEngine(FixedGridEngine):
         # banks: chunks of per_chunk M-vectors, at most TDQ_IMPL_MAX_CHUNKS of them, grown on demand
         self._per_chunk = max(4, -(-(self.max_iters + 1) // 64))
         self._u_chunks, self._s_chunks = [], []
+        self._replaying = False
 
     # ---- buffers --------------------------------------------------------------------------------------------------
     def _alloc(self):
@@ -119,16 +130,21 @@ class ImplicitEngine(FixedGridEngine):
         self._bufs = None
 
     def _stage_time(self, i, t0, dt, t1):
-        a = self.alpha_T[i]
-        if bool(a == 1.):
-            return torch.nextafter(t1, t1 - 1)                    # Perturb.PREV (misc.py:190-192)
-        if bool(a == 0.):
-            return t0
-        return t0 + a * dt
+        return stage_time(self.alpha_T[i], t0, dt, t1)
 
     # ---- one step ---------------------------------------------------------------------------------------------------
     def _step_once(self, rec, emit):
         """One implicit step: y1 into self.y1, then the emit; returns [f0]."""
+        if self._taping is not None:
+            self._taping[-1].pop("broyden", None)                # a retried step tapes its solves again
+        f0 = self._solve_step(rec, self.tcur[0], None)
+        if emit:
+            self._emit_step(rec.k, f0)
+        return [f0]
+
+    def _solve_step(self, rec, t_f0, traces):
+        """f0 = func(t_f0, y0), the Broyden solve(s) and y1 = y0 + sum_j K_j fl(dt c_j) into self.y1; returns f0.
+        traces: None, or a list that gets one dict per Broyden solve (see replay_step)."""
         b = self._alloc()
         T, dev, n, sgn = self.dtype, self.device, self.n, self.t_sign
         # (t0, dt, t1) as 0-dim tensors of the state dtype (rk_common.py:416-433)
@@ -136,7 +152,7 @@ class ImplicitEngine(FixedGridEngine):
         t0, dt, t1 = t0.to(T), dt.to(T), t1.to(T)
         S = len(self.alpha_T)
         self._taken = set()
-        f0 = self._call_fn(self.tcur[0], self.y0w, None)          # Perturb.NEXT when perturb (in tcur)
+        f0 = self._call_fn(t_f0, self.y0w, None)                 # Perturb.NEXT when perturb (in tcur)
         times = torch.stack([self._stage_time(i, t0, dt, t1) for i in range(S)]) * sgn
         times = times.to(dev)
         coef = [[float(bij * dt) * sgn for bij in self.beta_T[i]] for i in range(S)]   # fl_T(beta_ij * dt), signed
@@ -146,25 +162,58 @@ class ImplicitEngine(FixedGridEngine):
             for i in range(S):
                 if self.skipped[i]:
                     continue
-                self._broyden(b, f0, [times[i]], b["K"][i], Kp[:i + 1], [coef[i]])
+                self._broyden(b, f0, [times[i]], b["K"][i], Kp[:i + 1], [coef[i]], traces, [i])
         else:
             act = [i for i in range(S) if not self.skipped[i]]
             X = b["K"][0]
             pos = {i: a for a, i in enumerate(act)}
             Kp = [X.data_ptr() + pos[j] * n * esz if j in pos else f0.data_ptr() for j in range(S)]
-            self._broyden(b, f0, [times[i] for i in act], X, Kp, [coef[i] for i in act])
+            self._broyden(b, f0, [times[i] for i in act], X, Kp, [coef[i] for i in act], traces, act)
         # y1 = y0 + sum_j K_j * fl(dt * c_sol_j)  (rk_common.py:464 / :552, solvers.py:115), one launch
         cs = [float(dt * c) * sgn for c in self.c_T]
         _lib.check(self.lib.tdq_lincomb(self.dc, self.y1.data_ptr(), self.y0w.data_ptr(), _lib.ptr_array(Kp),
                                         _lib.dbl_array(cs), S, n, _stream()))
         self.launches += 1
         self._taken = {f0.data_ptr()}
-        if emit:
-            self._emit_step(rec.k, f0)
-        return [f0]
+        return f0
 
-    def _broyden(self, b, f0, times, X, Kp, coefs):
-        """Broyden's method from K = f0 for the rows of one solve (rk_common.py:435-462 / :523-550)."""
+    # ---- replay for the reverse sweep (backprop.implicit_backward) -------------------------------------------------
+    def replay_step(self, rec, y0):
+        """Grid step `rec` again from the taped y0 with the forward's own launches, so every iterate is bitwise the
+        forward's, keeping what its reverse sweep needs.  Returns (f0, y1, K, traces): K the step's final stage
+        vectors (K[j] is f0 for a skipped stage), one trace per Broyden solve (DIRK: per stage) with
+            stages   the tableau stages it solves for (its rows), coefs their signed fl(beta_ij dt) rows
+            m, code  the updates made and the final status
+            U, S     the residual and step banks (lists of chunks), state the raw dot matrix
+            X, Y     every iterate X_0 .. X_m and its stage values, rows * n elements each.
+        Counters, warnings and results of the solve are left as the forward left them."""
+        nfe, launches, iters, warned = self.nfe, self.launches, self.iterations, self.n_warnings
+        self._alloc()
+        self.y0w.copy_(y0)
+        traces = []
+        self._replaying = True
+        try:
+            try:
+                f0 = self._solve_step(rec, self.ts_all[rec.k, 0], traces)
+            except _RetryWithCopies:
+                traces.clear()
+                f0 = self._solve_step(rec, self.ts_all[rec.k, 0], traces)
+        finally:
+            self._replaying = False
+            self.nfe, self.launches, self.iterations, self.n_warnings = nfe, launches, iters, warned
+        n, b = self.n, self._bufs
+        if self.dirk:
+            K = [f0 if self.skipped[j] else b["K"][j].clone() for j in range(len(self.alpha_T))]
+        else:
+            X = traces[0]["X"][-1]
+            act = traces[0]["stages"]
+            K = [X[act.index(j) * n:(act.index(j) + 1) * n] if j in act else f0 for j in range(len(self.alpha_T))]
+        return f0, self.y1.clone(), K, traces
+
+    def _broyden(self, b, f0, times, X, Kp, coefs, traces=None, stages=None):
+        """Broyden's method from K = f0 for the rows of one solve (rk_common.py:435-462 / :523-550).  On a taped
+        solve the number of updates and the final status go on the step's tape; with traces (replay_step) the solve's
+        banks, dot matrix and iterates go into a new trace."""
         lib, dc, n, st = self.lib, self.dc, self.n, _stream()
         rows = len(times)
         Y = b["Y"]
@@ -184,10 +233,21 @@ class ImplicitEngine(FixedGridEngine):
                                                  u, s, nc, self._per_chunk, slot, slot, part, res_out, st))
             self.launches += 1
 
+        tr = None
+        if traces is not None:
+            self._u_chunks, self._s_chunks = [], []                   # the banks stay with the trace
+            tr = dict(stages=list(stages), coefs=[list(r) for r in coefs], X=[], Y=[])
+            traces.append(tr)
+
+        def keep():
+            if tr is not None:
+                tr["X"].append(X.reshape(-1)[:rows * n].clone())
+                tr["Y"].append(Y[:rows * n].clone())
         # init: K = f0 in every row, first stage values
         _lib.check(lib.tdq_implicit_update(dc, X.data_ptr(), rows, n, None, None, 0, 1, -1, None, f0.data_ptr(),
                                            Y.data_ptr(), self.y0w.data_ptr(), kp, cf, nt, None, None, st))
         self.launches += 1
+        keep()
         residual(0)
         m = 0
         while True:
@@ -198,8 +258,9 @@ class ImplicitEngine(FixedGridEngine):
             if code == _CONVERGED:
                 break
             if code in (_SINGULAR, _EXHAUSTED):
-                warnings.warn(_MSG)
-                self.n_warnings += 1
+                if not self._replaying:
+                    warnings.warn(_MSG)
+                    self.n_warnings += 1
                 break
             u, s, nc = self._bank(m + 2)
             _lib.check(lib.tdq_implicit_update(dc, X.data_ptr(), rows, n, u, s, nc, self._per_chunk, m,
@@ -208,4 +269,10 @@ class ImplicitEngine(FixedGridEngine):
             self.launches += 1
             m += 1
             self.iterations += 1
+            keep()
             residual(m)
+        if tr is not None:
+            tr.update(m=m, code=code, U=self._u_chunks, S=self._s_chunks, state=state.clone())
+            self._u_chunks, self._s_chunks = [], []
+        elif self._taping is not None:
+            self._taping[-1].setdefault("broyden", []).append((m, code))

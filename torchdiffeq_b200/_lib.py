@@ -181,6 +181,12 @@ _SIGNATURES = {
     "tdq_implicit_solve": (C.c_int, [_i32, _vp, _vp, _vp, _vp, _i32, _i32, _dbl, _vp]),
     "tdq_implicit_update": (C.c_int, [_i32, _vp, _i32, _sz, _pp, _pp, _i32, _i64, _i32, _vp, _vp, _vp, _vp, _pp, _pdbl,
                                       _i32, _vp, _vp, _vp]),
+    "tdq_implicit_grad_ws_len": (_sz, [_i32]),
+    "tdq_implicit_grad_combine": (C.c_int, [_i32, _vp, _vp, _i32, _sz, _pp, _pp, _i32, _i64, _vp, _i32, _i32, _i32, _i32,
+                                            _i32, _i32, _vp, _vp, _vp]),
+    "tdq_implicit_grad_solve": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "tdq_implicit_grad_stage": (C.c_int, [_i32, _pp, _i32, _sz, _pp, _pp, _pdbl, _pdbl, _i32, _vp, _vp, _vp, _i32, _vp,
+                                          _vp, _vp]),
     "tdq_rows_size": (_sz, [_sz]),
     "tdq_rows_offset": (_sz, [_i32, _sz]),
     "tdq_rows_partials_len": (_sz, [_sz, _sz]),

@@ -718,6 +718,200 @@ def adams_backward(p, method, tape, grid, t_cpu, grad_sol, params, need_t, lc=No
     return gbar, obar, y0bar, sa.pbar
 
 
+class Bank:
+    """M-vectors in chunks, as the Broyden kernels take them: vector j is row j % per_chunk of chunks[j // per_chunk]."""
+
+    def __init__(self, chunks):
+        self.chunks, self.per_chunk = list(chunks), chunks[0].shape[0]
+
+    def vec(self, j):
+        return self.chunks[j // self.per_chunk][j % self.per_chunk]
+
+    def like(self):
+        return Bank([torch.empty_like(c) for c in self.chunks])
+
+    def ptrs(self):
+        return _lib.ptr_array([c.data_ptr() for c in self.chunks])
+
+
+def _ws_rows(ws, mx):
+    """Views of the reverse Broyden workspace (tdq_implicit_grad_solve): (Acoef row m, Qcoef row m, vneg)."""
+    return (lambda m: ws[m * mx:(m + 1) * mx]), (lambda m: ws[(mx + m) * mx:(mx + m + 1) * mx]), ws[2 * mx * mx:][:mx]
+
+
+class ImplicitGradOps:
+    """The state-sized and small passes of implicit_backward: libtdq's tdq_implicit_grad_* (a CPU restatement with the
+    same methods can stand in).  mx: the solve's max_iters."""
+
+    def __init__(self, dtype, device, mx):
+        self.lib, self.dc, self.mx, self.device = _lib.load(), _DTYPES[dtype], mx, device
+        self.partials = torch.zeros(self.lib.tdq_implicit_partials_len(2 * mx), dtype=torch.float64, device=device)
+
+    def workspace(self):
+        return torch.zeros(self.lib.tdq_implicit_grad_ws_len(self.mx), dtype=torch.float64, device=self.device)
+
+    def combine(self, out, base, v, v_lo, coefs, n_terms, rows, d=None, d_lo=0, n_dots=0, g_slot=0, n_gram=0,
+                dots=None):
+        """out = T(base + sum_q coefs[q] v_{v_lo+q}); dots[:n_dots] = out . d_{d_lo+q}, dots[n_dots:] = v_{g_slot} . v_q.
+        v and d share one chunking, as the engine grows its banks."""
+        if d is not None and (len(d.chunks), d.per_chunk) != (len(v.chunks), v.per_chunk):
+            raise ValueError("the dot bank must be chunked as the combination bank")
+        n = out.numel() // rows
+        _lib.check(self.lib.tdq_implicit_grad_combine(
+            self.dc, out.data_ptr(), base.data_ptr() if base is not None else None, rows, n, v.ptrs(),
+            d.ptrs() if d is not None else None, len(v.chunks), v.per_chunk, coefs.data_ptr() if n_terms else None, v_lo,
+            n_terms, d_lo, n_dots, g_slot, n_gram, self.partials.data_ptr(), dots.data_ptr() if dots is not None else None,
+            _stream()))
+
+    def solve(self, state, dots, ws, m, m_star):
+        _lib.check(self.lib.tdq_implicit_grad_solve(state.data_ptr(), dots.data_ptr(), ws.data_ptr(), m, m_star, self.mx,
+                                                    _stream()))
+
+    def stage(self, ybars, kbars, ks, coefs, w, y0bar, xbar, q, need_dot):
+        """Adjoint of y_r = y0 + sum_j T(coefs[r][j]) k_j (and xbar -= q): returns the float64 0-dim dot
+        sum_rj w[r][j] <ybar_r, k_j> with need_dot, else None."""
+        n = y0bar.numel()
+        dot = torch.empty(1, dtype=torch.float64, device=y0bar.device) if need_dot else None
+        flat = lambda rows: [c for r in rows for c in r]
+        _lib.check(self.lib.tdq_implicit_grad_stage(
+            self.dc, _lib.ptr_array([y.data_ptr() for y in ybars]), len(ybars), n,
+            _lib.ptr_array([b.data_ptr() for b in kbars]), _lib.ptr_array([x.data_ptr() for x in ks]),
+            _lib.dbl_array(flat(coefs)), _lib.dbl_array(flat(w)), len(kbars), y0bar.data_ptr(),
+            xbar.data_ptr() if xbar is not None else None, q.data_ptr() if q is not None else None,
+            xbar.numel() // n if xbar is not None else 0, self.partials.data_ptr() if need_dot else None,
+            dot.data_ptr() if need_dot else None, _stream()))
+        return dot[0] if need_dot else None
+
+
+def implicit_backward(p, method, tape, grid, t_cpu, grad_sol, params, need_t, replay, ops):
+    """Reverse sweep over the steps of an implicit Runge-Kutta solve (FixedGridFIRKODESolver / FixedGridDIRKODESolver,
+    rk_common.py:415-558, inside solvers.py:102-128): the gradient autograd gives the reference through every Broyden
+    iteration its forward took.  Arguments and result as fixed_backward, plus replay(Step, y0) -> (f0, y1, K, traces)
+    (ImplicitEngine.replay_step: the step again, bitwise, with its banks and iterates) and ops (ImplicitGradOps).
+
+    One Broyden solve, X_0 = f0, R_m = X_m - F(X_m), s_m = -J_m^-1 R_m, X_{m+1} = X_m + s_m,
+    J_m = I + sum_{j<m} R_{j+1} s_j^T / sigma_j, reversed for m = m*-1 .. 0 (DESIGN.md section 5b):
+      R_{m+1}'s cotangent is complete: Xbar += Rbar - (dF/dX)^T Rbar, one func VJP per stage at X_{m+1}'s stage values;
+      sbar_m = Xbar + the later iterations' terms; lambda_m = J_m^-T sbar_m by the transposed m x m system;
+      Rbar_m -= lambda_m; Rbar_{j+1} -= lambda_m (s_m.s_j)/sigma_j and sbar_j gets s_m and s_j terms (j < m).
+    Cotangents of stage values and of the K's are kept for the RAW func outputs (the engine's signed coefficients)."""
+    from ._fixed import Step
+    from ._implicit import TABLEAUS, stage_time
+    dev, T, sign, n = p.device, p.dtype, p.t_sign, p.n
+    dirk, alpha, beta, c_sol = TABLEAUS[method]
+    cast = lambda v: torch.tensor(v, dtype=torch.float64).to(T)          # the engine's tableau (rk_common.py:410-413)
+    alpha_T, beta_T, c_T = [cast(a) for a in alpha], [cast(b) for b in beta], cast(c_sol)
+    S = len(alpha)
+    sa = StepAdjoint(_ascending_field(p), params, need_t)
+    gbar = torch.zeros(grid.numel(), dtype=torch.float64, device=dev) if need_t else None
+    obar = torch.zeros(t_cpu.numel(), dtype=torch.float64, device=dev) if need_t else None
+    mx = ops.mx
+    gy = None
+    for st in reversed(tape):
+        k, y0 = st["k"], st["y0"]
+        g0, g1 = grid[k], grid[k + 1]
+        dt = g1 - g0                                                   # t's dtype (solvers.py:112)
+        f0, y1, K, traces = replay(Step(k, g0, dt, g1), y0)
+        if [(tr["m"], tr["code"]) for tr in traces] != st["broyden"]:
+            raise RuntimeError("the replay of implicit step %d made (updates, status) %s, the forward %s"
+                               % (k, [(tr["m"], tr["code"]) for tr in traces], st["broyden"]))
+        t0T, dtT, t1T = g0.to(T), dt.to(T), g1.to(T)
+        s_stage = [_dev(stage_time(a, t0T, dtT, t1T), dev) for a in alpha_T]
+        dtbar = None
+
+        def time_bar(i, tb):                                           # a stage time's cotangent into t0, dt or t1
+            nonlocal dtbar
+            if bool(alpha_T[i] == 1.):
+                gbar[k + 1] += tb.double()
+            else:
+                gbar[k] += tb.double()
+                if not bool(alpha_T[i] == 0.):
+                    dtbar = _acc(dtbar, tb.double(), float(alpha_T[i]))
+        # ---- outputs of the step, then y1 = y0 + sum_j K_j fl(dt c_j) ---------------------------------------------------
+        ybar0, ybar1, f0bar_ref = _outputs_backward(sa, st, k, g0, g1, y0, y1, f0 * sign if sign != 1.0 else f0, t_cpu,
+                                                    grad_sol, gy, sign, gbar, obar)
+        y0bar = torch.zeros(n, dtype=T, device=dev) if ybar0 is None else ybar0.to(T).clone()
+        f0bar = torch.zeros(n, dtype=T, device=dev)
+        if f0bar_ref is not None:
+            f0bar.add_(f0bar_ref.to(T), alpha=sign)
+        if dirk:
+            Kbar = [torch.zeros(n, dtype=T, device=dev) for _ in range(S)]
+            for j in range(S):
+                if not any(j in tr["stages"] for tr in traces):
+                    Kbar[j] = f0bar                                    # a skipped stage keeps f0
+        else:
+            act = traces[0]["stages"]
+            Xbar = torch.zeros(len(act) * n, dtype=T, device=dev)
+            Kbar = [Xbar[act.index(j) * n:(act.index(j) + 1) * n] if j in act else f0bar for j in range(S)]
+        if ybar1 is not None:
+            cs = [float(dtT * c) * sign for c in c_T]
+            d = ops.stage([ybar1.to(T).contiguous()], Kbar, K, [cs], [[sign * float(c) for c in c_T]], y0bar, None,
+                          None, need_t)
+            dtbar = _acc(dtbar, d)
+        # ---- the Broyden solves, last first --------------------------------------------------------------------------
+        for tr in reversed(traces):
+            stages, m_star = tr["stages"], tr["m"]
+            rows, nt = len(stages), len(tr["coefs"][0])
+            xbar = Kbar[stages[0]] if dirk else Xbar
+            kbars = Kbar[:nt]
+            w = [[sign * float(b) for b in beta_T[i][:nt]] for i in stages]
+
+            def terms(i):                                              # the stage-value formula's K's at iterate i
+                X = tr["X"][i]
+                if dirk:
+                    return K[:nt - 1] + [X]
+                return [X[stages.index(j) * n:(stages.index(j) + 1) * n] if j in stages else f0 for j in range(S)]
+
+            def resid_bar(i, q):
+                """R_i's cotangent -q: Xbar -= q, and (dF/dX)^T q through one VJP per stage at iterate i."""
+                nonlocal dtbar
+                Y, ybars = tr["Y"][i], []
+                for a, s in enumerate(stages):
+                    qa = q[a * n:(a + 1) * n]
+                    gY, tb = sa.vjp(s_stage[s], Y[a * n:(a + 1) * n], qa * sign if sign != 1.0 else qa)
+                    ybars.append(gY.to(T).contiguous() if gY is not None else torch.zeros(n, dtype=T, device=dev))
+                    if need_t and tb is not None:
+                        time_bar(s, tb)
+                    del gY, tb
+                dtbar = _acc(dtbar, ops.stage(ybars, kbars, terms(i), tr["coefs"], w, y0bar, xbar, q, need_t))
+
+            if m_star > 0:
+                U, Sb = Bank(tr["U"]), Bank(tr["S"])
+                L = Sb.like()                                          # lambda_m in slot m
+                ws = ops.workspace()
+                arow, qrow, vneg = _ws_rows(ws, mx)
+                sbar, q = torch.empty_like(xbar), torch.empty_like(xbar)
+                dots = torch.empty(2 * mx, dtype=torch.float64, device=dev)
+                for m in reversed(range(m_star)):
+                    if m + 1 < m_star:
+                        ops.combine(q, None, L, m + 1, qrow(m)[m + 1:], m_star - m - 1, rows)
+                        resid_bar(m + 1, q)
+                    last = m + 1 == m_star                             # nothing later left terms for s_m
+                    ops.combine(sbar, xbar, Sb, m, arow(m)[m:], 0 if last else m_star - m, rows, d=U, d_lo=1, n_dots=m,
+                                g_slot=m, n_gram=m, dots=dots)
+                    ops.solve(tr["state"], dots, ws, m, m_star)
+                    ops.combine(L.vec(m), sbar, Sb, 0, vneg, m, rows)
+                resid_bar(0, L.vec(0))                                 # R_0's cotangent is -lambda_0
+                del U, Sb, L
+            for a in range(rows):                                      # X_0 = f0 in every stage of the solve
+                f0bar.add_(xbar[a * n:(a + 1) * n])
+        # ---- f0 = func(t0, y0): its cotangent is complete -----------------------------------------------------------------
+        ts = stage_times("rk4", g0, dt, g1, st["perturb"], T)
+        gyk, tb = sa.vjp(_dev(ts[0], dev), y0, f0bar * sign if sign != 1.0 else f0bar)
+        if gyk is not None:
+            y0bar = y0bar + gyk
+        if need_t:
+            if tb is not None:
+                gbar[k] += tb.double()
+            if dtbar is not None:
+                gbar[k + 1] += dtbar
+                gbar[k] -= dtbar
+        del traces, K
+        gy = y0bar
+    y0bar = _acc(gy, grad_sol[0])
+    return gbar, obar, y0bar, sa.pbar
+
+
 class _BackpropFunction(torch.autograd.Function):
     """odeint with gradients of the discrete solve (see the module docstring)."""
 
@@ -747,6 +941,10 @@ class _BackpropFunction(torch.autograd.Function):
             else:
                 grid_req, grid, t_req = ctx.aux["grid_req"], ctx.aux["grid"], ctx.aux["t_req"]
                 sweep = adams_backward if ctx.aux.get("adams") else fixed_backward
+                eng = ctx.aux.get("implicit")
+                if eng is not None:
+                    ops = ImplicitGradOps(p.dtype, p.device, eng.max_iters)
+                    sweep = lambda *a: implicit_backward(*a, replay=eng.replay_step, ops=ops)
                 with torch.no_grad():
                     gbar, obar, y0bar, pbar = sweep(p, p.method, ctx.aux["tape"], grid, p.t_cpu, grad_sol, params,
                                                     ctx.need_t)

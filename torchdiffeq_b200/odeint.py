@@ -35,7 +35,7 @@ _FIXED_OPTIONS = {"step_size", "grid_constructor", "interp", "perturb", "norm"}
 _ADAMS_OPTIONS = _FIXED_OPTIONS | {"max_iters", "max_order"}
 _IMPLICIT_OPTIONS = _FIXED_OPTIONS | {"max_iters"}                                  # rk_common.py:382-388
 _OUR_OPTIONS = {"graph", "run_ahead", "process_group", "cache", "exchange", "device_loop", "fused_linear", "fused_attempt",
-                 "independent_rows", "differentiable", "event_gradient", "compact_rows"}
+                 "independent_rows", "differentiable", "event_gradient", "compact_rows", "implicit_gradient"}
 
 
 def _rms_norm(tensor):
@@ -390,6 +390,17 @@ def check_event_gradient(options, rows=True):
         raise NotImplementedError("options['event_gradient'] is implemented for options={'independent_rows': True, "
                                   "'differentiable': True} only; a shared-batch event solve gets its gradients from "
                                   "odeint_adjoint")
+
+
+def check_implicit_gradient(options, method):
+    """options['implicit_gradient']: 'discrete' (plain odeint under autograd differentiates the implicit methods' Broyden
+    iteration as the reference's autograd does) is the only value, and only the implicit methods take it."""
+    v = options.get("implicit_gradient")
+    if not (isinstance(v, str) and v == "discrete"):
+        raise ValueError("options['implicit_gradient'] must be 'discrete', got %r" % (v,))
+    if method not in IMPLICIT_METHODS:
+        raise ValueError("options['implicit_gradient'] applies to the implicit methods %s, not to method %r"
+                         % (", ".join(IMPLICIT_METHODS), method or "dopri5"))
 
 
 def check_compact_rows(options):
@@ -918,9 +929,11 @@ def _odeint_backprop(p, func, y0, t, params, _stats):
             holder["eng"] = eng
             return sol.clone(), {"kind": "adaptive", "tape": tape, "tab": adaptive_tableau(p.method)}
         o = p.options
-        if p.method in IMPLICIT_METHODS:
-            raise NotImplementedError("gradients through the discrete implicit solve (Broyden's iteration) are not "
-                                      "implemented; use odeint_adjoint with the implicit methods")
+        if p.method in IMPLICIT_METHODS and o.get("implicit_gradient") is None:
+            raise NotImplementedError("gradients through the discrete implicit solve (Broyden's iteration) are opt-in: "
+                                      "pass options['implicit_gradient'] = 'discrete' (its backward replays every step "
+                                      "and costs several forward solves), or use odeint_adjoint (one backward solve, "
+                                      "the continuous adjoint)")
         y0_view = p.layout.views(p.y0_flat) if p.is_tuple else p.y0_flat.view(p.shape)
         with torch.enable_grad():                     # the grid as a differentiable function of the output times
             t_req = p.t_cpu.detach().clone().requires_grad_(True)
@@ -930,7 +943,7 @@ def _odeint_backprop(p, func, y0, t, params, _stats):
         sol, tape = eng.solve_taped(p.y0_flat, grid, p.t_cpu)
         holder["eng"] = eng
         return sol, {"kind": "fixed", "tape": tape, "grid": grid, "grid_req": grid_req, "t_req": t_req,
-                     "adams": p.method in ADAMS_METHODS}
+                     "adams": p.method in ADAMS_METHODS, "implicit": eng if p.method in IMPLICIT_METHODS else None}
     with on_solver_stream(p.device) as ss:
         sol = _BackpropFunction.apply(p, run, t, y0_flat, *params)
         ss.publish(sol)
@@ -989,8 +1002,16 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
     accepts `graph` (True/False/'auto'), `run_ahead` (int; 0 reproduces the reference's exact func
     call sequence) and `process_group` (batch-sharded solve with a common step size).
     Under autograd the result carries the gradient of the discrete solve w.r.t. y0, t and func's parameters
-    (backprop.py) for the adaptive, explicit fixed-grid and Adams methods (linear or cubic outputs); the implicit
-    Runge-Kutta methods refuse it.  odeint_adjoint gives the continuous adjoint instead.
+    (backprop.py) for the adaptive, explicit fixed-grid and Adams methods (linear or cubic outputs).  odeint_adjoint
+    gives the continuous adjoint instead.
+
+    The implicit Runge-Kutta methods ('implicit_euler', 'implicit_midpoint', 'trapezoid', 'gl4', 'gl6', 'radauIIA3',
+    'radauIIA5', 'sdirk2', 'trbdf2') give it with options['implicit_gradient'] = 'discrete' (the only value; ValueError
+    for another value or another method) and raise NotImplementedError under autograd without it.  The gradient is then
+    the one the reference's autograd gives, through every Broyden iteration the forward took; the convergence test, the
+    singular break and max_iters are decisions, so constants.  It is opt-in because of its cost: the backward replays
+    every step bit for bit and takes one func VJP per active stage per Broyden iteration, several forward solves of
+    work, while odeint_adjoint's backward is one solve.  Without anything that needs a gradient the key does nothing.
 
     options={'independent_rows': True} (adaptive methods, tensor y0 of shape [B, *rest]): every row y0[r] gets its own step
     size control, so row r's result is the reference's odeint(func, y0[r:r+1], t) for a row-wise func and does not depend
@@ -1045,6 +1066,8 @@ def odeint(func, y0, t, *, rtol=1e-7, atol=1e-9, method=None, options=None, even
         check_compact_rows(options)
     if options and "event_gradient" in options:
         check_event_gradient(options, rows=bool(options.get("independent_rows")))
+    if options and "implicit_gradient" in options:
+        check_implicit_gradient(options, method)
     if options and options.get("independent_rows"):
         row_ev0 = _check_independent_rows(func, y0, t, method, options, event_fn)
         if row_ev0 is not None:
